@@ -2,7 +2,8 @@
 """Headline benchmark: ResNet-50 fp16 batch-8 inferences/sec (+ p50/p99 request latency) through the
 per-request hot path, N replicas on N GPUs of one node (no collective: requests are independent).
 
-  python bench.py --gpus N --steps K --warmup W            # this repo's sm_100a path
+  python bench.py --gpus N --steps K --warmup W            # this repo's sm_90a path
+  python bench.py ... --dump-outputs DIR                   # also write the last timed step's output as DIR/*.npy
   python bench.py --impl reference --gpus N --steps K ...  # CPU arm: the oracle port of the reference path
 
 A "step" is one pass of the hot path over one batch of 8 synthetic 3x224x224 images.
@@ -32,7 +33,7 @@ sys.path.insert(0, ROOT)
 BATCH = 8
 CONTEXTS = 4          # BASELINE.json configs[1]: 4 concurrent ExecutionContexts / streams
 BUFFERS = 8           # 2x contexts, reference examples/00_TensorRT/infer.cc:88
-RING = 32             # 32 x 4.82 MB = 154 MB of distinct inputs > 126 MB L2
+RING = 32             # 32 x 4.82 MB = 154 MB of distinct inputs > 50 MB L2
 METRIC = "ResNet-50 fp16 b=8 inferences/sec"
 UNIT = "inferences/s"
 ALGO_BYTES_PER_STEP = 470.9e6   # SURVEY.md 8(d): fp16 weights + conv in/out + residual reads, batch 8
@@ -184,7 +185,7 @@ def run_reference(args):
     print(json.dumps(line), flush=True)
 
 
-def run_config2(capi, builder, peaks_int8_tops: float = 4500.0):
+def run_config2(capi, builder, peaks_int8_tops: float = 1979.0):
     """BASELINE.json configs[2]: ResNet-152 INT8, batch 32, dynamic batching (examples/03_Batching), 8 streams, 1 GPU.
     Device-resident throughput of 8 execution contexts + the end-to-end rate of single-image requests merged by
     BatchedInferRunner (2 ms window) -- a SECONDARY line; the headline stays on configs[1]."""
@@ -207,7 +208,7 @@ def run_config2(capi, builder, peaks_int8_tops: float = 4500.0):
     finally:
         mgr.close()
     return {
-        "workload": "ResNet-152 int8 batch=32, dynamic batching, 8 streams, 1xB200 (BASELINE.json configs[2])",
+        "workload": "ResNet-152 int8 batch=32, dynamic batching, 8 streams, 1xH100 (BASELINE.json configs[2])",
         "metric": "ResNet-152 int8 b=32 inferences/sec", "value": value, "unit": UNIT, "ms_per_step": ms / steps, "steps": steps,
         "contexts": contexts, "dtype": "s8 (bottleneck convolutions; fp16 stem and classifier)", "gpu_launches": launches * steps,
         "e2e": {"value": steady, "unit": UNIT, "requests": n_img - warm - cool, "warm_requests": warm, "cool_requests": cool,
@@ -218,9 +219,7 @@ def run_config2(capi, builder, peaks_int8_tops: float = 4500.0):
         "roofline": {"bound": "tensor", "kernel": "conv_i8_tcgen05 (the 154 INT8 convolutions of one forward pass)",
                      "achieved": ops * steps / (ms * 1e-3) / 1e12, "peak": peaks_int8_tops, "unit": "TOP/s",
                      "frac": ops * steps / (ms * 1e-3) / 1e12 / peaks_int8_tops,
-                     # DRAM bytes (read + write) of the 155 conv launches of one batch-32 forward pass, committed ncu pass
-                     "traffic": 1171.1e6, "traffic_source": "profiles/ncu_metrics_r2_int8.csv",
-                     "peak_source": "NOMINAL dense int8 4.5 POP/s (B200_PROFILING.md table; MEASURED_PEAKS.json has no int8 entry)"},
+                     "peak_source": "H100 SXM data sheet, dense int8 at 700 W (not a measured peak)"},
     }
 
 
@@ -271,12 +270,16 @@ def run_b200(args):
     sampler = ClockSampler(local)
     barrier()
     sampler.start()
-    elapsed_ms, launches_per_step = capi.device_throughput(blob, CONTEXTS, BATCH, args.steps, max(args.warmup, 3), ring)
+    last_out = np.empty((BATCH, 1000), np.float32)  # softmax output of the last timed step
+    elapsed_ms, launches_per_step = capi.device_throughput(blob, CONTEXTS, BATCH, args.steps, max(args.warmup, 3), ring, last_out)
     barrier()
     clocks = sampler.stop()
     elapsed_ms = max_over_ranks(elapsed_ms)
     ms_per_step = elapsed_ms / args.steps
     value = world * args.steps * BATCH / (elapsed_ms * 1e-3)
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "probabilities.npy"), last_out)
 
     # ---- e2e: InferenceManager / InferRunner / InferBench with pinned host buffers -------------------------
     # Tactics are timed at RegisterModel and every (lane-pinned context, batch) plan + graph is built in
@@ -358,16 +361,13 @@ def run_b200(args):
         peak_tf, peak_src = float(peaks["bf16_tflops_sustained"]), "MEASURED_PEAKS.json bf16_tflops_sustained (kernel timed inside a long step)"
         peak_hbm = float(peaks["hbm_gbs"])
     except Exception:
-        peak_tf, peak_src, peak_hbm = 1400.0, "fallback 1.4 PFLOP/s sustained (B200_PROFILING.md)", 6650.0
+        peak_tf, peak_src, peak_hbm = 989.0, "H100 SXM data sheet, dense fp16 at 700 W (not a measured peak)", 3350.0
     # the conv kernel's time inside one step of the timed region = step time x its share of the forward pass
     conv_ms_per_step = ms_per_step * conv_share
     achieved_tf = conv_flops / (conv_ms_per_step * 1e-3) / 1e12
     roofline = {
         "bound": "tensor", "kernel": "conv_f16_tcgen05 (all %d conv launches of one forward pass)" % n_conv,
         "achieved": achieved_tf, "peak": peak_tf, "unit": "TFLOP/s", "frac": achieved_tf / peak_tf,
-        # DRAM bytes (read+write) of the 53 conv launches of ONE forward pass = one step, from the committed ncu pass
-        # profiles/ncu_metrics_r2l.csv (cold L2; outputs stay L2-resident inside each kernel)
-        "traffic": 267.3e6, "traffic_source": "profiles/ncu_metrics_r2l.csv",
         "peak_source": peak_src,
         "flops_per_step": conv_flops, "conv_share_of_step": conv_share,
         # aggregate over 4 overlapping contexts (above) vs the kernels in isolation on ONE stream: conv FLOPs / (single-
@@ -378,23 +378,6 @@ def run_b200(args):
         "hbm_view": {"algorithmic_bytes_per_step": ALGO_BYTES_PER_STEP,
                      "achieved_gbs": ALGO_BYTES_PER_STEP / (ms_per_step * 1e-3) / 1e9, "peak_gbs": peak_hbm},
     }
-    try:
-        # every convolution against the roof that binds IT: the tensor peak, or -- for the wide short-K layers whose
-        # activations live in L2 -- the read / write bandwidth of L2 for unique streaming data (tensorrt_laboratory_b200/roofs.py)
-        from tensorrt_laboratory_b200 import graph, roofs, weights
-        net = graph.resnet_caffe(50)
-        floors = roofs.conv_floors(graph.lower(net, weights.random_weights(net, 0)), BATCH, peak_tf)
-        floor_us = sum(f["floor_us"] for f in floors)
-        roofline["per_layer_roofs"] = {
-            "floor_us_per_step": floor_us, "frac": floor_us / (conv_ms_per_step * 1e3),
-            "tensor_bound_layers": sum(f["roof"] == "tensor" for f in floors), "memory_bound_layers": sum(f["roof"] == "memory" for f in floors),
-            "tensor_floor_us": sum(f["tensor_floor_us"] for f in floors), "memory_floor_us": sum(f["memory_floor_us"] for f in floors),
-            "l2_read_tbs": roofs.L2_READ_BPS / 1e12, "l2_write_tbs": roofs.L2_WRITE_BPS / 1e12,
-            "source": "per layer max(2MNK / tensor peak, reads / L2 read bw + writes / L2 write bw); L2 figures: tools/micro/l2_stream.cu, "
-                      "profiles/l2_stream_r2.log; per-layer table: profiles/roofline_r2_saturated.md"}
-    except Exception as ex:  # an explanatory view must never take the line down
-        roofline["per_layer_roofs"] = {"error": f"{type(ex).__name__}: {ex}"}
-
     config2 = None
     if world == 1 and not args.no_config2:
         try:
@@ -419,7 +402,7 @@ def run_b200(args):
         "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3),
         "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
         "dtype": "f16", "data": "synthetic",
-        "config": {"workload": "ResNet-50 fp16 batch=8, 1xB200 per replica, 4 concurrent ExecutionContexts/streams, synthetic 3x224x224 (BASELINE.json configs[1])",
+        "config": {"workload": "ResNet-50 fp16 batch=8, 1xH100 per replica, 4 concurrent ExecutionContexts/streams, synthetic 3x224x224 (BASELINE.json configs[1])",
                    "global_batch": BATCH * world, "contexts": CONTEXTS, "buffers": BUFFERS,
                    "l2_policy": f"inputs larger than L2: ring of {RING} distinct batches = {RING * in_bytes / 1e6:.0f} MB",
                    "parallelism": f"replicas x{world} (no collective)",
@@ -459,9 +442,11 @@ def main():
     ap.add_argument("--cpu-batches", type=int, default=20)
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg (profiling runs)")
     ap.add_argument("--no-config2", action="store_true", help="skip the secondary ResNet-152 INT8 line (BASELINE configs[2])")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the output of the last timed step (softmax probabilities, [8, 1000] float32) as DIR/probabilities.npy")
     args = ap.parse_args()
     if args.gpus > 1 and "WORLD_SIZE" not in os.environ:
-        # convenience: re-launch ourselves one rank per GPU (the driver does this itself via torchrun)
+        # convenience: re-launch ourselves one rank per GPU
         cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={args.gpus}",
                "--master-addr", "127.0.0.1", "--master-port", "29517", os.path.abspath(__file__)] + sys.argv[1:]
         raise SystemExit(subprocess.call(cmd))

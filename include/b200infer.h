@@ -1,5 +1,5 @@
 /*
- * b200infer.h -- C ABI of the B200-native inference engine that replaces TensorRT underneath
+ * b200infer.h -- C ABI of the H100-native inference engine that replaces TensorRT underneath
  * trtlab/tensorrt (NVIDIA/tensorrt-laboratory).  Plain C, plain pointers and sizes; no C++/torch types.
  *
  * Every entry point mirrors 1:1 one nvinfer1:: call the reference makes on its per-request hot path.
@@ -11,7 +11,7 @@
  * same contract as nvinfer1::IExecutionContext.  All work is asynchronous on the caller's stream.
  *
  * There is NO CPU fallback: b2_engine_deserialize fails with B2_ENODEVICE if the current device is not
- * an sm_100 part or no CUDA device is present.
+ * an sm_90 part or no CUDA device is present.
  */
 #ifndef B200INFER_H_
 #define B200INFER_H_
@@ -28,7 +28,7 @@ extern "C" {
 enum {
     B2_OK = 0,
     B2_EINVAL = 1,    /* bad argument / malformed blob            */
-    B2_ENODEVICE = 2, /* no CUDA device, or not sm_100            */
+    B2_ENODEVICE = 2, /* no CUDA device, or not sm_90             */
     B2_ECUDA = 3,     /* a CUDA runtime / driver call failed      */
     B2_ENOMEM = 4,    /* allocation failed                        */
     B2_ESTATE = 5     /* call sequence error (e.g. no device memory set) */

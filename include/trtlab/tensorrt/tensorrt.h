@@ -1,5 +1,5 @@
 // trtlab::TensorRT -- the reference's C++ surface for the per-request inference hot path, re-hosted on
-// the B200-native engine (include/b200infer.h) instead of nvinfer1.  No NvInfer.h is included anywhere.
+// the H100-native engine (include/b200infer.h) instead of nvinfer1.  No NvInfer.h is included anywhere.
 //
 // v1 ("legacy", the drop-in contract named by the north star; reference include root
 // tensorrt/laboratory/*.h):  Runtime/StandardRuntime/ManagedRuntime, Model, Buffers/FixedBuffers,

@@ -66,9 +66,11 @@ int trt_workspace_infer(const void* blob, size_t nbytes, const void* input, size
  * requests cut from a 3-segment ring (which therefore wraps); output and device time of the last request */
 int trt_cyclic_infer(const void* blob, size_t nbytes, int batch, const void* input, size_t input_bytes, void* output,
                      size_t output_bytes, int managed_runtime, int rounds, double* compute_seconds);
-/* device-resident throughput of `contexts` concurrent execution contexts (inputs cycled through a device ring) */
+/* device-resident throughput of `contexts` concurrent execution contexts (inputs cycled through a device ring);
+ * `last_output` (nullable) receives the first output binding of the last timed step */
 int trt_device_throughput(const void* blob, size_t nbytes, int contexts, int batch, int steps, int warmup,
-                          const void* host_ring, int ring_batches, double* elapsed_ms, int* launches_per_step);
+                          const void* host_ring, int ring_batches, double* elapsed_ms, int* launches_per_step,
+                          void* last_output);
 
 #ifdef __cplusplus
 }

@@ -69,7 +69,7 @@ def pack_weights_sw128(W: np.ndarray) -> np.ndarray:
     exactly what the kernel wants in shared memory for a 64-K weight sub-tile under the 128-byte swizzle (16-byte
     chunk j of row r sits at chunk j ^ (r % 8)).  The N tile of ANY width BN in {32, 64, 128} for k-block kb is then
     ONE contiguous run of BN*128 bytes = one `cp.async.bulk` instruction (instruction issue, ~200 cycles per TMA op
-    from a single thread, is what paces the main loop -- profiles/phase_timing)."""
+    from a single thread, is what paces the main loop)."""
     cout, K = W.shape
     assert cout % 32 == 0 and K % 64 == 0 and W.dtype == np.float16
     blk = W.reshape(cout // 32, 32, K // 64, 8, 8)            # [nb, r, kb, chunk, elem]

@@ -101,7 +101,7 @@ SYMBOLS = [
     ("trt_manager_bench_window", _I, [_VP, _S, _I, _SZ, _SZ, _SZ, C.POINTER(_D), C.POINTER(_D), _SZ, C.POINTER(_SZ)]),
     ("trt_manager_bench_windows", _I, [_VP, _S, _I, _SZ, _SZ, _SZ, _SZ, C.POINTER(_D), C.POINTER(_D), _SZ, C.POINTER(_SZ)]),
     ("trt_timed_pipeline", _I, [_VP, _SZ, _I, C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_float)]),
-    ("trt_device_throughput", _I, [_VP, _SZ, _I, _I, _I, _I, _VP, _I, C.POINTER(_D), C.POINTER(_I)]),
+    ("trt_device_throughput", _I, [_VP, _SZ, _I, _I, _I, _I, _VP, _I, C.POINTER(_D), C.POINTER(_I), _VP]),
     ("trt_workspace_infer", _I, [_VP, _SZ, _VP, _SZ, _VP, _SZ, _I, _I]),
     ("trt_cyclic_infer", _I, [_VP, _SZ, _I, _VP, _SZ, _VP, _SZ, _I, _I, C.POINTER(_D)]),
 ]
@@ -588,13 +588,18 @@ def timed_pipeline(blob: bytes, iters: int = 20):
     return dict(h2d_ms=a.value, compute_ms=b.value, d2h_ms=c.value)
 
 
-def device_throughput(blob: bytes, contexts: int, batch: int, steps: int, warmup: int, ring: np.ndarray):
-    """-> (elapsed_ms, kernel launches per step).  ``ring``: [R, batch, C, H, W] host array (cast to the input dtype)."""
+def device_throughput(blob: bytes, contexts: int, batch: int, steps: int, warmup: int, ring: np.ndarray,
+                      last_output: np.ndarray | None = None):
+    """-> (elapsed_ms, kernel launches per step).  ``ring``: [R, batch, C, H, W] host array (cast to the input dtype).
+    ``last_output``: optional C-contiguous array that receives the output binding of the last timed step."""
     ring = np.ascontiguousarray(ring, dtype=input_np_dtype(blob))
+    if last_output is not None and not last_output.flags["C_CONTIGUOUS"]:
+        raise ValueError("last_output must be C-contiguous")
     ms = _D()
     nl = _I()
     check(load().trt_device_throughput(blob, len(blob), contexts, batch, steps, warmup, ring.ctypes.data,
-                                       ring.shape[0], C.byref(ms), C.byref(nl)))
+                                       ring.shape[0], C.byref(ms), C.byref(nl),
+                                       None if last_output is None else last_output.ctypes.data))
     return ms.value, nl.value
 
 

@@ -291,11 +291,11 @@ struct b2_context {
     int no_fold = 0;    // 1: run the stem through the generic 8-channel tap path instead of the row-folded one
     int autotune = 4;  // 0 off (cost model), 1 latency mode, N>=2 throughput mode over N streams
     int fork = 0;      // 1: run side branches (Op::side_join) on a forked stream / a parallel graph branch.  Off by default:
-                       // measured neutral on B200 (0.476 ms either way, 4-context throughput within noise) -- the fork and
+                       // measured neutral (4-context throughput within noise) -- the fork and
                        // join turn the programmatic (PDL) edges around them into full dependencies, which eats the overlap
     int net = 0;       // 1: runs of 64-channel-block tcgen05 convolutions execute as ONE persistent kernel (net_kernel.cu).
-                       // Opt-in: bit-identical, but measured slower than the per-layer kernels at batch 8 (profiles/README.md, r2a-c)
-    int net_ctas = 0;  // CTAs of that kernel (0 = one per SM); a server running N contexts gives each about 148 / N
+                       // Opt-in: bit-identical; not the default
+    int net_ctas = 0;  // CTAs of that kernel (0 = one per SM); a server running N contexts gives each about 1 / N of the SMs
     int net_bn = 0;    // force its N tile (64 / 128); 0 = 128 wherever the channel count allows
     int net_stages = 0;  // force its shared-memory ring depth (2..4); 0 = the deepest that lets two CTAs share an SM
     int i8_bn = 0;       // INT8 convolutions: force the N tile (128 / 256); 0 = 128
@@ -599,8 +599,11 @@ int make_map_im2col(CUtensorMap* map, const void* base, int C, int W, int H, int
     return B2_OK;
 }
 
+// SMs of the device the engine runs on (set when an engine is created for a device; 132 = H100 SXM until then)
+static int g_sms = 132;
+
 // Analytic cost model (microseconds) over the instantiated (N tile, pipeline depth, split-K) space.  The
-// constants are rough B200 figures: ~70 KB/us of L2->SM bandwidth per SM, ~1 us TMA round trip, ~5 TB/s of
+// constants are rough figures: ~70 KB/us of L2->SM bandwidth per SM, ~1 us TMA round trip, ~5 TB/s of
 // aggregate L2 bandwidth, ~2 us of fixed per-CTA cost.  It only has to rank configurations sensibly.
 ConvConfig pick_conv_config(int M, int cout_phys, int kblocks, int kb, bool residual, const b2_context* c, bool honor_forced) {
     const int m_tiles = (M + 127) / 128;
@@ -625,11 +628,11 @@ ConvConfig pick_conv_config(int M, int cout_phys, int kblocks, int kb, bool resi
                 if (!(honor_forced && c->force_stages) && !stage_depth_useful(bn, kb, st, kpc)) continue;
                 const double smem = b2k::conv_smem_bytes(bn, st, residual);
                 int per_sm = int(227.0 * 1024 / smem);
-                per_sm = std::min(per_sm, 512 / std::max(32, bn));
+                per_sm = std::min(per_sm, bn <= 64 ? 2 : 1);  // 384-thread CTAs: the register file holds two only for BN <= 64
                 per_sm = std::max(1, std::min(per_sm, 8));
                 const int ctas = tiles * splits;
-                const int waves = (ctas + 148 * per_sm - 1) / (148 * per_sm);
-                const int sharing = std::max(1, std::min(per_sm, (ctas + 147) / 148));
+                const int waves = (ctas + g_sms * per_sm - 1) / (g_sms * per_sm);
+                const int sharing = std::max(1, std::min(per_sm, (ctas + g_sms - 1) / g_sms));
                 const double stage_bytes = 16384.0 + bn * 128.0;
                 const double t_kb = std::max(stage_bytes / (70000.0 / sharing), 1.0 / st);
                 double t_epi = 0.6 + bn / 64.0 * 0.4 + (residual ? 0.4 : 0.0);
@@ -881,10 +884,8 @@ int autotune_conv(b2_context* c, const Op& op, int batch, int fixed_splits, int 
             }
             const int kpc = (nkb + sp - 1) / sp;
             if (ws) {
-                candidates.push_back(ConvConfig{bn, st, 1, 0.0, sps, std::min(tiles, 148), 1});
-                if (tiles > 74) candidates.push_back(ConvConfig{bn, st, 1, 0.0, sps, 74, 1});  // half the SMs per stream
-                if (tiles >= 592 && b2k::conv_ws_smem(bn, st, sps, r.res >= 0) <= 113 * 1024)
-                    candidates.push_back(ConvConfig{bn, st, 1, 0.0, sps, 296, 1});  // two co-resident CTAs per SM
+                candidates.push_back(ConvConfig{bn, st, 1, 0.0, sps, std::min(tiles, g_sms), 1});
+                if (tiles > g_sms / 2) candidates.push_back(ConvConfig{bn, st, 1, 0.0, sps, g_sms / 2, 1});  // half the SMs per stream
                 continue;
             }
             if (sps == 2 && kpc < 4) continue;  // double-width stages only pay on long K loops
@@ -897,7 +898,7 @@ int autotune_conv(b2_context* c, const Op& op, int batch, int fixed_splits, int 
             const bool cn_forced_here = c->force_cn > 1 && kbsz == 64 && (int(r.cout_phys) / bn) % c->force_cn == 0 &&
                                         b2k::conv_cluster_config_exists(bn, st, sps, c->force_cn);
             if (!cn_forced_here) candidates.push_back(ConvConfig{bn, st, sp, 0.0, sps, 0, 1});
-            // clusters along N that multicast the activation tile: never won a timing on B200 (the L2 read is shared but
+            // clusters along N that multicast the activation tile: never won a timing (the L2 read is shared but
             // every SM still ingests the whole tile, and the cluster barriers cost latency) -> tried only on request
             if (kbsz == 64 && c->force_cn > 0)
                 for (int cn = 2; cn <= 4; cn *= 2)
@@ -1156,7 +1157,7 @@ int tune_engine_batch(b2_context* c, int batch) {
         // persistent -- adds the same products in the same order), so letting the timing pick it would make the BITS of a
         // model depend on the load-time measurement of that process: seen once as a 4e-3 relative difference between a tuned
         // manager and an untuned session of the same plan.  It never won a serving-regime timing anyway (the closest
-        // candidate is 40 % behind, profiles/tune_dump_r2_rn50_b8_4streams.log), so the tuner leaves it alone unless
+        // candidate was 40 % behind), so the tuner leaves it alone unless
         // B2_TUNE_SPLITK=1; `splits` stays available as an explicit option.
         static const bool tune_splitk = env_int("B2_TUNE_SPLITK", 0) != 0;
         int splits = (side || !tune_splitk) ? 1 : 0;
@@ -1298,13 +1299,13 @@ int fuse_net_runs(b2_context* c, Plan* plan, int batch) {
         run->args.layer_done = reinterpret_cast<int*>(d + off_ld);
         run->args.ctrl = reinterpret_cast<int*>(d + off_ctrl);
         run->args.n_layers = n, run->args.total_tiles = tile_cursor, run->args.n_flags = flag_cursor;
-        // ring depth: the deepest that still lets two CTAs share an SM (227 KiB less 1 KiB of system use per CTA)
-        int stages = c->net_stages > 0 ? c->net_stages : 4;
-        while (c->net_stages <= 0 && stages > 2 && 2 * (b2k::net_smem_bytes(n, stages) + 1024) > 227 * 1024) --stages;
+        // ring depth 4: one CTA per SM (the consumer warpgroups' accumulators fill the register file)
+        const int stages = c->net_stages > 0 ? c->net_stages : 4;
         run->args.stages = std::max(2, std::min(stages, 4));
-        const int per_sm = 2 * (b2k::net_smem_bytes(n, run->args.stages) + 1024) <= 227 * 1024 ? 2 : 1;
-        run->ctas = c->net_ctas > 0 ? c->net_ctas : 148 * per_sm;
-        run->ctas = std::max(1, std::min(run->ctas, std::min(148 * per_sm, tile_cursor)));
+        const int per_sm = 1;
+        run->ctas = c->net_ctas > 0 ? c->net_ctas : g_sms * per_sm;
+        // an explicit count may exceed one CTA per SM: later CTAs start as earlier ones retire (tickets are drawn by running CTAs)
+        run->ctas = std::max(1, std::min(run->ctas, std::min(2 * g_sms, tile_cursor)));
         run->first_op = int(i), run->last_op = int(j);
         Launch L;
         L.kind = L_NET;
@@ -1430,11 +1431,11 @@ int build_plan(b2_context* c, int batch, Plan** out) {
                 if (r.relu & 4) {  // INT8 tensor path
                     L.kind = L_CONV_I8;
                     // one tactic, by rule: the 128-wide N tile with a ring no deeper than the K loop, shallow enough (2-3
-                    // stages) that two CTAs share an SM (measured: profiles/probe_r2_int8_*.log); "i8_bn" / "i8_stages" override
+                    // stages) that two CTAs share an SM (measured); "i8_bn" / "i8_stages" override
                     // tactic = (N tile, ring depth): timed at load (b2_engine_tune) or carried by the plan; untuned engines use
-                    // a rule -- many CTAs want shallow rings (more CTAs per SM), few CTAs a 2-deep one (profiles/probe_r2_int8*)
+                    // a rule -- many CTAs want shallow rings (more CTAs per SM), few CTAs a 2-deep one (probe_r2_int8*)
                     const int m_tiles = (batch * int(e->tensors[r.out].h * e->tensors[r.out].w) + 127) / 128;
-                    int bn = 128, st = m_tiles * (int(r.cout_phys) / 128) >= 2 * 148 ? 1 : 2;
+                    int bn = 128, st = m_tiles * (int(r.cout_phys) / 128) >= 2 * g_sms ? 1 : 2;
                     if (c->autotune) {
                         std::lock_guard<std::mutex> lock(e->tune_mutex);
                         tune_cache_load(e);
@@ -1463,7 +1464,7 @@ int build_plan(b2_context* c, int batch, Plan** out) {
                     if (c->force_ws > 0 && kbsz == 64 && (r.relu & 2) && cfg.splits == 1 &&
                         b2k::conv_ws_config_exists(cfg.bn, cfg.stages, cfg.sps) &&
                         b2k::conv_ws_smem(cfg.bn, cfg.stages, cfg.sps, r.res >= 0) <= 227 * 1024)
-                        cfg.ws = std::min(((M + 127) / 128) * (int(r.cout_phys) / cfg.bn), c->force_ws > 1 ? c->force_ws : 148);
+                        cfg.ws = std::min(((M + 127) / 128) * (int(r.cout_phys) / cfg.bn), c->force_ws > 1 ? c->force_ws : g_sms);
                     if (c->force_halo > 0 && conv_halo_rows(c, op) && b2k::conv_halo_config_exists(cfg.bn) && cfg.splits == 1 &&
                         int(r.cin_phys) / 64 <= 8 && b2k::conv_halo_smem(cfg.bn, int(to.w), conv_halo_rows(c, op), int(r.cin_phys) / 64) <= 227 * 1024)
                         cfg.halo = 1, cfg.ws = 0, cfg.cn = 1;
@@ -1870,9 +1871,10 @@ static int deserialize_impl(b2_runtime* rt, const void* blob, size_t nbytes, boo
         }
         cudaDeviceProp prop;
         B2_CUDA(cudaGetDeviceProperties(&prop, dev));
-        if (prop.major != 10)
-            return fail(B2_ENODEVICE, "device %d is sm_%d%d; this library only carries sm_100a code", dev, prop.major, prop.minor);
+        if (prop.major != 9 || prop.minor != 0)
+            return fail(B2_ENODEVICE, "device %d is sm_%d%d; this library only carries sm_90a code", dev, prop.major, prop.minor);
         e->device = dev;
+        g_sms = prop.multiProcessorCount;
         rc = b2k::init_conv_kernels();
         if (!rc) rc = b2k::init_net_kernel();
         if (!rc) rc = b2k::init_conv_i8_kernels();

@@ -1,38 +1,24 @@
-// INT8 kernels of the B200-native engine (BASELINE configs[2]: ResNet-152 int8; reference examples/ONNX/resnet50/int8.py,
+// INT8 kernels of the H100-native engine (BASELINE configs[2]: ResNet-152 int8; reference examples/ONNX/resnet50/int8.py,
 // build.py:63-65 reach INT8 through TensorRT's builder).
 //
 //  * conv_i8_tcgen05<BN> -- implicit-GEMM convolution on the INT8 tensor path: TMA (tiled or im2col mode, 1-byte elements,
-//    one 128-byte swizzle row = 128 channels) -> tcgen05.mma.kind::i8 (UMMA 128 x BN x 32, s8 x s8 -> s32 in TMEM, exact)
+//    one 128-byte swizzle row = 128 channels) -> wgmma (64 x BN x 32 per warpgroup, s8 x s8 -> s32 in registers, exact)
 //    -> requantising epilogue in fp32, two fused multiply-adds (quantize.py: the CPU oracle reproduces it bit for bit)
 //        t = fma(float(acc), m[c], b[c]);  t = fma(float(q_res), r, t);  t = max(t, 0);  q = clip(rint(t), +-127)
 //    -> int8 -> 128-byte-swizzled staging tile -> TMA store.  Same warp roles as conv_f16_tcgen05 (warp 0 activation
-//    producer, warp 1 MMA issuer, warp 2 TMEM owner, warp 3 weight producer, all four = epilogue), PDL throughout.
+//    producer, warp 3 weight producer, warps 4-11 = two consumer warpgroups doing wgmma and the epilogue), PDL throughout.
 //  * quantize_h_to_i8_kernel -- fp16 NHWC -> int8 NHWC (channels zero-padded to the 128-channel rows of the INT8 layout)
 //  * avgpool_i8_kernel       -- global average pool: int8 NHWC -> fp16 [N][C]  (exact integer sums)
 //  * output_cast_i8_kernel   -- int8 NHWC -> fp32 NCHW binding (dequantised)
 #include "kernels.h"
-#include "ptx_sm100.cuh"
+#include "ptx_sm90.cuh"
+#include "wgmma_sm90.cuh"
 
 namespace b2k {
 
 namespace {
 
-// D[tmem] (+)= A[smem desc] * B[smem desc], s8 x s8 -> s32; issued by ONE thread on behalf of the CTA.
-__device__ __forceinline__ void umma_i8(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// instruction descriptor, kind::i8: D = s32 (c_format 2 @4), A = B = signed 8 bit (1 @7, 1 @10), both K-major, N>>3 @17, M>>4 @24
-__host__ __device__ constexpr uint32_t make_idesc_i8(int m, int n) {
-    return (2u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(n >> 3) << 17) | (static_cast<uint32_t>(m >> 4) << 24);
-}
-
+constexpr int kI8Threads = 384;  // warps 0-3: producers, warps 4-11: two consumer warpgroups (rows 0-63 / 64-127)
 constexpr int kI8ASub = 128 * 128;  // 128 rows x 128 K-bytes
 
 __host__ __device__ constexpr int conv_i8_smem_layout_bytes(int bn, int stages, bool residual) {
@@ -41,23 +27,14 @@ __host__ __device__ constexpr int conv_i8_smem_layout_bytes(int bn, int stages, 
 
 }  // namespace
 
-// four s32 -> one word of four s8 (byte i = sat_s8(q_i)): two saturating pack conversions
-__device__ __forceinline__ uint32_t pack4_sat_s8(int q0, int q1, int q2, int q3) {
-    uint32_t hi, out;
-    asm("cvt.pack.sat.s8.s32.b32 %0, %1, %2, %3;" : "=r"(hi) : "r"(q3), "r"(q2), "r"(0));
-    asm("cvt.pack.sat.s8.s32.b32 %0, %1, %2, %3;" : "=r"(out) : "r"(q1), "r"(q0), "r"(hi));
-    return out;
-}
-
 template <int BN, int STAGES>
-__global__ void __launch_bounds__(128)
+__global__ void __launch_bounds__(kI8Threads, 1)
 conv_i8_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapOut,
                 const __grid_constant__ CUtensorMap mapRes, const I8ConvArgs p) {
     constexpr int A_STAGE = kI8ASub, B_STAGE = BN * 128;
     constexpr int PIPE_BYTES = STAGES * (A_STAGE + B_STAGE);
     constexpr int TILE_BYTES = 128 * BN;     // int8 output / residual tile
     constexpr int NBOX = BN / 128;           // 128-column TMA boxes per tile row
-    constexpr int NG = BN / 32;
     static_assert(TILE_BYTES <= PIPE_BYTES, "the output staging tile reuses the pipeline buffers");
 
     extern __shared__ uint8_t smem_raw[];
@@ -72,7 +49,6 @@ conv_i8_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
     uint64_t* empty_bar = full_bar + STAGES;
     uint64_t* accum_bar = empty_bar + STAGES;
     uint64_t* res_bar = accum_bar + 1;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(res_bar + 1);
     float* s_m = reinterpret_cast<float*>(tail + 256);
     float* s_b = s_m + BN;
 
@@ -81,8 +57,8 @@ conv_i8_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
     const int n0 = blockIdx.x * BN;
     const int m0 = blockIdx.y * 128;
     const int nk = p.num_kblocks;
-    // real output channels of this N tile, rounded up to the MMA's granularity: the instruction is issued N = nv wide, only
-    // nv weight rows are fetched, and the epilogue writes zeros for the rest (what the padded weights would have produced)
+    // real output channels of this N tile, rounded up to 32: only nv weight rows are fetched, and the epilogue writes zeros
+    // for the rest (what the padded weights would have produced; the MMA's columns >= nv read unfetched rows and are dropped)
     int nv = p.cout_real - n0;
     nv = nv >= BN ? BN : (nv <= 0 ? 32 : ((nv + 31) / 32) * 32);
     const uint32_t b_bytes = static_cast<uint32_t>(nv) * 128u;
@@ -94,18 +70,13 @@ conv_i8_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
         if (has_res) tma_prefetch_desc(&mapRes);
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], 1);
+            mbar_init(&empty_bar[s], 8);  // one arrival per consumer warp
         }
-        mbar_init(accum_bar, 1);
         mbar_init(res_bar, 1);
         fence_barrier_init();
         fence_proxy_async();
     }
-    if (warp == 2) tmem_alloc(tmem_slot, BN);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     if (warp == 3) {  // requantisation constants -> smem (published by the pre-epilogue barrier)
         for (int i = lane; i < BN; i += 32) {
             s_m[i] = __ldg(p.m + n0 + i);
@@ -113,6 +84,7 @@ conv_i8_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
         }
     }
 
+    int32_t acc[BN / 2];
     if (warp == 0) {
         // ================= activation producer =================
         int img0 = 0, p0 = 0, q0 = 0;
@@ -153,34 +125,43 @@ conv_i8_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
                 }
             }
         }
-    } else if (warp == 1) {
-        // ================= MMA issuer =================
-        const uint32_t idesc = make_idesc_i8(128, nv);
+    } else if (warp >= 4) {
+        // ================= consumers: wgmma over the ring, s32 accumulators in registers =================
+        const uint32_t wg = static_cast<uint32_t>((warp - 4) >> 2);
         int cur_cb = 0;
         for (int i = 0; i < nk; ++i) {
             const int s = i % STAGES;
             mbar_wait(&full_bar[s], (i / STAGES) & 1);
-            tc_fence_after();
-            const uint32_t a_addr = smem_u32(sA + s * A_STAGE);
+            const uint32_t a_addr = smem_u32(sA + s * A_STAGE) + wg * 8192;
             const uint32_t b_addr = smem_u32(sB + s * B_STAGE);
             // all-zero 32-byte slices at the end of a tap's last channel block contribute nothing: not issued
             const int nj = (cur_cb == p.cblocks - 1) ? p.last_cb_mmas : 4;
-            if (elect_one_sync()) {
+            wgmma_fence();
 #pragma unroll
-                for (int j = 0; j < 4; ++j) {  // 4 x (K = 32 bytes) inside one 128-byte swizzle row
-                    if (j < nj) {
-                        const uint64_t ad = make_smem_desc(a_addr + j * 32, 16, 1024, 2);
-                        const uint64_t bd = make_smem_desc(b_addr + j * 32, 16, 1024, 2);
-                        umma_i8(tmem_base, ad, bd, idesc, (i > 0 || j > 0) ? 1u : 0u);
-                    }
+            for (int j = 0; j < 4; ++j) {  // 4 x (K = 32 bytes) inside one 128-byte swizzle row
+                if (j < nj) {
+                    const uint64_t ad = make_wgmma_desc(a_addr + j * 32, 16, 1024, WG_SW128);
+                    const uint64_t bd = make_wgmma_desc(b_addr + j * 32, 16, 1024, WG_SW128);
+                    wgmma_i8<BN>(acc, ad, bd, (i > 0 || j > 0) ? 1u : 0u);
                 }
-                umma_commit(&empty_bar[s]);
             }
-            __syncwarp();
+            wgmma_commit();
+            if constexpr (STAGES == 1) {  // the only stage is refilled for step i+1: retire step i first
+                wgmma_wait<0>();
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty_bar[0]);
+            } else {
+                wgmma_wait<1>();  // step i-1 has retired: its stage goes back to the producers
+                __syncwarp();
+                if (i > 0 && lane == 0) mbar_arrive(&empty_bar[(i - 1) % STAGES]);
+            }
             if (++cur_cb == p.cblocks) cur_cb = 0;
         }
-        if (elect_one_sync()) umma_commit(accum_bar);
-        __syncwarp();
+        if constexpr (STAGES > 1) {
+            wgmma_wait<0>();
+            __syncwarp();
+            if (nk > 0 && lane == 0) mbar_arrive(&empty_bar[(nk - 1) % STAGES]);
+        }
     } else if (warp == 3) {
         // ================= weight producer (constants: no dependency wait) =================
         const uint8_t* src = p.wpacked + static_cast<size_t>(n0 >> 5) * 4096;
@@ -193,64 +174,43 @@ conv_i8_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
         }
     }
 
-    // ====== epilogue: TMEM (s32) -> requantise -> int8 -> swizzled staging tile -> TMA store ======
+    // ====== epilogue (consumer warpgroups): s32 registers -> requantise -> int8 -> swizzled staging tile -> TMA store ======
     pdl_wait();
-    const int row = warp * 32 + lane;
-    mbar_wait(accum_bar, 0);
-    tc_fence_after();
     __syncthreads();  // s_m / s_b visible; every role has left its loop: the pipeline buffers are free
     pdl_launch_dependents();
-    if (has_res) mbar_wait(res_bar, 0);
-    const uint32_t taddr = tmem_base + (static_cast<uint32_t>(warp * 32) << 16);
-    const float r = p.r;
-    const bool relu = p.relu != 0;
+    if (warp >= 4) {
+        if (has_res) mbar_wait(res_bar, 0);
+        const int row0 = 64 * ((warp - 4) >> 2) + 16 * ((warp - 4) & 3) + (lane >> 2);
+        const float r = p.r;
+        // q = clip(rint(max(t, relu ? 0 : -inf)), -127, 127): the lower clamp and the ReLU are ONE fp32 max before the
+        // conversion (rint is monotonic and rint(-127) = -127)
+        const float lo = p.relu != 0 ? 0.0f : -127.0f;
 #pragma unroll
-    for (int g = 0; g < NG; ++g) {
-        if (g * 32 >= nv) {  // padding channels (CTA-uniform): the result is zero by construction, nothing to read or compute
+        for (int j = 0; j < BN / 8; ++j) {
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-                const int col = g * 32 + h * 16;
-                *reinterpret_cast<uint4*>(sOut + static_cast<uint32_t>((col >> 7) * (128 * 128)) + swz_off<128>(row, (col & 127) >> 4)) =
-                    make_uint4(0u, 0u, 0u, 0u);
-            }
-            continue;
-        }
-        uint32_t acc[32];
-        tmem_ld32(taddr + g * 32, acc);
-        tmem_wait_ld();
+                const int row = row0 + 8 * h;
+                const int col = 8 * j + 2 * (lane & 3);
+                const uint32_t so = static_cast<uint32_t>((col >> 7) * (128 * 128)) + swz_off<128>(row, (col & 127) >> 4) + (col & 15);
+                uint16_t packed = 0;  // padding channels (col >= nv): zero by construction
+                if (col < nv) {
+                    char2 rq = make_char2(0, 0);
+                    if (has_res) rq = *reinterpret_cast<const char2*>(sRes + so);
+                    int q[2];
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {  // 16 columns = one 16-byte chunk of the int8 row
-            const int col = g * 32 + h * 16;
-            const int box = col >> 7;
-            const int chunk = (col & 127) >> 4;
-            const uint32_t so = static_cast<uint32_t>(box * (128 * 128)) + swz_off<128>(row, chunk);
-            uint4 rv = make_uint4(0u, 0u, 0u, 0u);
-            if (has_res) rv = *reinterpret_cast<const uint4*>(sRes + so);
-            const int8_t* rq = reinterpret_cast<const int8_t*>(&rv);
-            // q = clip(rint(max(t, relu ? 0 : -inf)), -127, 127) with as few issue slots as the contract allows (this loop is
-            // what bounds the wide, short-K layers): the lower clamp and the ReLU are ONE fp32 max before the conversion
-            // (rint is monotonic and rint(-127) = -127), the upper clamp is the saturation of the s32 -> s8 pack.
-            const float lo = relu ? 0.0f : -127.0f;
-            int q[16];
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-                const int c = col + i;
-                float t = __fmaf_rn(__int2float_rn(static_cast<int>(acc[h * 16 + i])), s_m[c], s_b[c]);
-                if (has_res) t = __fmaf_rn(__int2float_rn(static_cast<int>(rq[i])), r, t);
-                q[i] = __float2int_rn(fmaxf(t, lo));  // > 127 (up to INT_MAX for huge t) saturates in the pack
+                    for (int e = 0; e < 2; ++e) {
+                        float t = __fmaf_rn(__int2float_rn(acc[4 * j + 2 * h + e]), s_m[col + e], s_b[col + e]);
+                        if (has_res) t = __fmaf_rn(__int2float_rn(e ? rq.y : rq.x), r, t);
+                        q[e] = min(__float2int_rn(fmaxf(t, lo)), 127);  // > 127 (up to INT_MAX for huge t) saturates
+                    }
+                    packed = static_cast<uint16_t>((q[0] & 0xFF) | ((q[1] & 0xFF) << 8));
+                }
+                *reinterpret_cast<uint16_t*>(sOut + so) = packed;
             }
-            uint4 o;
-            o.x = pack4_sat_s8(q[0], q[1], q[2], q[3]);
-            o.y = pack4_sat_s8(q[4], q[5], q[6], q[7]);
-            o.z = pack4_sat_s8(q[8], q[9], q[10], q[11]);
-            o.w = pack4_sat_s8(q[12], q[13], q[14], q[15]);
-            *reinterpret_cast<uint4*>(sOut + so) = o;
         }
     }
     fence_proxy_async();
-    tc_fence_before();
     __syncthreads();
-    if (warp == 2) tmem_dealloc(tmem_base, BN);
     if (threadIdx.x == 0) {
 #pragma unroll
         for (int b = 0; b < NBOX; ++b) tma_store_2d(&mapOut, sOut + b * (128 * 128), n0 + b * 128, m0);
@@ -279,7 +239,7 @@ int init_conv_i8_kernels() {
 int launch_conv_i8_tcgen05(const I8ConvLaunch& L, cudaStream_t stream) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(static_cast<unsigned>(L.grid_n), static_cast<unsigned>(L.grid_m), 1);
-    cfg.blockDim = dim3(128);
+    cfg.blockDim = dim3(kI8Threads);
     cfg.dynamicSmemBytes = static_cast<size_t>(conv_i8_smem_layout_bytes(L.bn, L.stages, L.args.has_res != 0));
     cfg.stream = stream;
     cudaLaunchAttribute attr[1];

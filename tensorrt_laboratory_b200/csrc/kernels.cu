@@ -1,9 +1,10 @@
-// sm_100a kernels of the B200-native inference engine.
+// sm_90a kernels of the H100-native inference engine.
 //
 //  * conv_f16_tcgen05 -- implicit-GEMM convolution: TMA (tiled or im2col mode) -> 128B-swizzled smem ->
-//    tcgen05.mma (UMMA 128xBNx16, fp16 x fp16 -> fp32 in TMEM) -> tcgen05.ld epilogue with
-//    bias / residual / ReLU fused -> 128-bit NHWC stores.  One 128xBN output tile per CTA,
-//    warp 0 = TMA producer, warp 1 = MMA issuer, warp 2 = TMEM allocator, all 4 warps = epilogue.
+//    wgmma (64xBNx16 per warpgroup, fp16 x fp16 -> fp32 in registers) -> epilogue with bias / residual / ReLU
+//    fused -> swizzled smem tile -> TMA store.  One 128xBN output tile per CTA of 12 warps: warp 0 = activation
+//    producer, warp 3 = weight producer (64-wide K-blocks), warps 4-7 and 8-11 = the two consumer warpgroups
+//    (output rows 0-63 and 64-127: wgmma + epilogue).
 //  * SIMT kernels -- fp32-engine reference path (fp64 accumulate) and the non-GEMM operators
 //    (layout casts, max/avg pool, FC, softmax).
 //
@@ -15,7 +16,8 @@
 #include <stdlib.h>
 #include <string.h>
 
-#include "ptx_sm100.cuh"
+#include "ptx_sm90.cuh"
+#include "wgmma_sm90.cuh"
 
 namespace b2k {
 
@@ -27,7 +29,6 @@ struct ConvCfg {
     static constexpr int B_SUBBLK = BN * 64 * 2;
     static constexpr int A_STAGE = SPS * A_SUBBLK;
     static constexpr int B_STAGE = SPS * B_SUBBLK;
-    static constexpr int TMEM_COLS = BN < 32 ? 32 : BN;
     static constexpr int PIPE_BYTES = STAGES * (A_STAGE + B_STAGE);
     static constexpr int TILE_BYTES = 128 * BN * 2;  // one fp16 output (or residual) tile
     static_assert(TILE_BYTES <= PIPE_BYTES, "the output staging tile reuses the pipeline buffers");
@@ -41,8 +42,19 @@ __host__ __device__ constexpr int conv_smem_layout_bytes(int bn, int stages, boo
 // AV resolves the operand paths at compile time for the production instantiations: 1 = im2col-mode activations + packed
 // weights, 2 = tiled activations + packed weights, 0 = decided at run time from ConvArgs (thin-K paths, unpacked plans,
 // clusters, debug).
+constexpr int kConvThreads = 384;
+constexpr int kConsumerWarps = 8;  // warps 4..11: two warpgroups of 64 output rows each
+
+// Thread (warp w of its warpgroup, lane l) of consumer warpgroup `wg` owns rows 64 wg + 16 w + l/4 (+8) and columns
+// 8j + 2(l%4) (+1) of the 128 x BN tile (wgmma fragment layout, wgmma_sm90.cuh).
+struct FragPos {
+    int row0, col0;
+    __device__ FragPos(int consumer_warp, int lane)
+        : row0(64 * (consumer_warp >> 2) + 16 * (consumer_warp & 3) + (lane >> 2)), col0(2 * (lane & 3)) {}
+};
+
 template <int BN, int KB, int STAGES, int SPS, int CN = 1, bool DBG = false, int AV = 0>
-__global__ void __launch_bounds__(128)
+__global__ void __launch_bounds__(kConvThreads, BN <= 64 ? 2 : 1)
 conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
                  const __grid_constant__ CUtensorMap mapOut, const __grid_constant__ CUtensorMap mapRes,
                  const ConvArgs p) {
@@ -51,11 +63,9 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
     constexpr int TPS = 64 / KB;            // TMA sub-tiles per stage: 1 (KB=64), 2 (KB=32 row-folded stem), 8 (KB=8)
     constexpr int A_SUB = 128 * KB * 2;     // bytes of one A sub-tile
     constexpr int B_SUB = BN * KB * 2;
-    constexpr int NG = BN / 32;             // 32-column groups of the accumulator
     constexpr int OW = BN >= 64 ? 64 : 32;  // columns per output TMA box
     constexpr int OROWB = OW * 2;           // bytes per staged output row (128 or 64)
     constexpr int NBOX = BN / OW;
-    constexpr uint32_t IDESC = make_idesc_f16(128, BN);
 
     extern __shared__ uint8_t smem_raw[];
     // 1 KiB alignment by OFFSETTING the __shared__ array (a uintptr_t round trip would turn every later access into a
@@ -71,8 +81,7 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
     uint64_t* empty_bar = full_bar + STAGES;
     uint64_t* accum_bar = empty_bar + STAGES;
     uint64_t* res_bar = accum_bar + 1;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(res_bar + 1);
-    uint32_t* last_flag = tmem_slot + 1;
+    uint32_t* last_flag = reinterpret_cast<uint32_t*>(res_bar + 1);
     float* s_bias = reinterpret_cast<float*>(tail + 256);
 
     const int warp = threadIdx.x >> 5;
@@ -80,7 +89,7 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
     const int n0 = blockIdx.x * BN;
     const int m0 = blockIdx.y * 128;
     // phase timestamps / bottleneck-isolation switches exist only in the DBG instantiations: even never-taken uniform
-    // branches inside the single-thread producer and MMA loops are measurable (see profiles/README.md, A/B runs)
+    // branches inside the single-thread producer and MMA loops are measurable (A/B runs)
     long long* dbg = (DBG && p.dbg) ? p.dbg + 16ll * ((blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) : nullptr;
     if (dbg && threadIdx.x == 0) {
         dbg[0] = clock64();
@@ -120,19 +129,14 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
         if (has_res) tma_prefetch_desc(&mapRes);
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], static_cast<uint32_t>(cn));
+            mbar_init(&empty_bar[s], static_cast<uint32_t>(kConsumerWarps * cn));
         }
-        mbar_init(accum_bar, 1);
         mbar_init(res_bar, 1);
         fence_barrier_init();
         fence_proxy_async();
     }
-    if (warp == 2) tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-    tc_fence_before();
     __syncthreads();
     if (cn > 1) cluster_sync_all();  // peers' barriers exist before anything is multicast at them
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     if (warp == 3) {  // bias -> smem while the pipeline spins up; published by the pre-epilogue barrier
 #pragma unroll
         for (int i = 0; i < BN / 32; ++i) s_bias[lane + 32 * i] = __ldg(p.bias + n0 + lane + 32 * i);
@@ -283,33 +287,47 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
             if (dbg && lane == 0) dbg[11] = tw, dbg[12] = te, dbg[13] = tl;
         }
         __syncwarp();
-    } else if (warp == 1) {
-        {
-            // ================= MMA issuer (whole warp converged, one elected lane issues) =================
-            long long mw = 0, mi = 0;
-            for (int i = 0; i < nk; ++i) {
-                const int s = i % STAGES;
-                const uint32_t ph = (i / STAGES) & 1;
-                long long m0c = 0, m1c = 0;
-                if (dbg) m0c = clock64();
-                mbar_wait(&full_bar[s], ph);
-                tc_fence_after();
-                if (dbg) m1c = clock64(), mw += m1c - m0c;
-                if (dbg && i == 0 && lane == 0) dbg[3] = clock64();
-                const uint32_t a_addr = smem_u32(sA + s * Cfg::A_STAGE);
-                const uint32_t b_addr = smem_u32(sB + s * Cfg::B_STAGE);
-                if (elect_one_sync()) {
-                if (skip_mma) {
-                } else if (KB == 64) {
+    }
+
+    // ================= consumers: wgmma over the ring, accumulators in registers =================
+    const int cw = warp - 4;  // consumer warp 0..7 (warpgroup cw / 4)
+    float acc[BN / 2];
+    if (warp >= 4) {
+        const uint32_t wg = static_cast<uint32_t>(cw >> 2);
+        // one arrival per consumer warp (on every CTA of the cluster: a peer refills its slice of our stage)
+        auto release_stage = [&](int st) {
+            __syncwarp();
+            if (lane == 0) {
+                if (cn > 1) {
+                    for (uint32_t r = 0; r < static_cast<uint32_t>(cn); ++r) mbar_arrive_cluster(&empty_bar[st], r);
+                } else {
+                    mbar_arrive(&empty_bar[st]);
+                }
+            }
+        };
+        long long mw = 0, mi = 0;
+        for (int i = 0; i < nk; ++i) {
+            const int s = i % STAGES;
+            const uint32_t ph = (i / STAGES) & 1;
+            long long m0c = 0, m1c = 0;
+            if (dbg) m0c = clock64();
+            mbar_wait(&full_bar[s], ph);
+            if (dbg) m1c = clock64(), mw += m1c - m0c;
+            if (dbg && i == 0 && cw == 0 && lane == 0) dbg[3] = clock64();
+            const uint32_t a_addr = smem_u32(sA + s * Cfg::A_STAGE);
+            const uint32_t b_addr = smem_u32(sB + s * Cfg::B_STAGE);
+            if (!skip_mma) {
+                wgmma_fence();
+                if (KB == 64) {
                     const int ns = subs_in_step(i);
 #pragma unroll
                     for (int u = 0; u < SPS; ++u) {
                         if (u < ns) {
 #pragma unroll
                             for (int j = 0; j < 4; ++j) {  // 4 x (K = 16) inside one 128-byte swizzle row
-                                const uint64_t ad = make_smem_desc(a_addr + u * Cfg::A_SUBBLK + j * 32, 16, 1024, 2);
-                                const uint64_t bd = make_smem_desc(b_addr + u * Cfg::B_SUBBLK + j * 32, 16, 1024, 2);
-                                umma_f16(tmem_base, ad, bd, IDESC, (i > 0 || u > 0 || j > 0) ? 1u : 0u);
+                                const uint64_t ad = make_wgmma_desc(a_addr + u * Cfg::A_SUBBLK + wg * 8192 + j * 32, 16, 1024, WG_SW128);
+                                const uint64_t bd = make_wgmma_desc(b_addr + u * Cfg::B_SUBBLK + j * 32, 16, 1024, WG_SW128);
+                                wgmma_f16<BN>(acc, ad, bd, (i > 0 || u > 0 || j > 0) ? 1u : 0u);
                             }
                         }
                     }
@@ -319,33 +337,38 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
                     for (int t = 0; t < nt; ++t) {
 #pragma unroll
                         for (int j = 0; j < 2; ++j) {
-                            const uint64_t ad = make_smem_desc(a_addr + t * A_SUB + j * 32, 16, 512, 4);
-                            const uint64_t bd = make_smem_desc(b_addr + t * B_SUB + j * 32, 16, 512, 4);
-                            umma_f16(tmem_base, ad, bd, IDESC, (i > 0 || t > 0 || j > 0) ? 1u : 0u);
+                            const uint64_t ad = make_wgmma_desc(a_addr + t * A_SUB + wg * 4096 + j * 32, 16, 512, WG_SW64);
+                            const uint64_t bd = make_wgmma_desc(b_addr + t * B_SUB + j * 32, 16, 512, WG_SW64);
+                            wgmma_f16<BN>(acc, ad, bd, (i > 0 || t > 0 || j > 0) ? 1u : 0u);
                         }
                     }
                 } else {
                     const int nt = sub_tiles(kb_begin + i);
                     for (int j = 0; j < nt / 2; ++j) {  // one K=16 step = two 8-channel taps
-                        const uint64_t ad = make_smem_desc(a_addr + 2 * j * A_SUB, A_SUB, 128, 0);
-                        const uint64_t bd = make_smem_desc(b_addr + 2 * j * B_SUB, B_SUB, 128, 0);
-                        umma_f16(tmem_base, ad, bd, IDESC, (i > 0 || j > 0) ? 1u : 0u);
+                        const uint64_t ad = make_wgmma_desc(a_addr + 2 * j * A_SUB + wg * 1024, A_SUB, 128, WG_NOSWZ);
+                        const uint64_t bd = make_wgmma_desc(b_addr + 2 * j * B_SUB, B_SUB, 128, WG_NOSWZ);
+                        wgmma_f16<BN>(acc, ad, bd, (i > 0 || j > 0) ? 1u : 0u);
                     }
                 }
-                if (cn > 1) umma_commit_mc(&empty_bar[s], cmask);  // every producer of the cluster hears it
-                else umma_commit(&empty_bar[s]);                   // frees the smem stage when these MMAs retire
-                }
-                __syncwarp();
-                if (dbg) mi += clock64() - m1c;
             }
-            if (elect_one_sync()) umma_commit(accum_bar);  // accumulator complete
-            __syncwarp();
-            if (dbg && lane == 0) dbg[4] = clock64(), dbg[14] = mw, dbg[15] = mi;
+            wgmma_commit();
+            if constexpr (STAGES == 1) {  // the only stage is refilled for step i+1: retire step i first
+                wgmma_wait<0>();
+                release_stage(0);
+            } else {
+                wgmma_wait<1>();  // step i-1 has retired: its stage goes back to the producers
+                if (i > 0) release_stage((i - 1) % STAGES);
+            }
+            if (dbg) mi += clock64() - m1c;
         }
-        __syncwarp();
+        if constexpr (STAGES > 1) {
+            wgmma_wait<0>();
+            if (nk > 0) release_stage((nk - 1) % STAGES);
+        }
+        if (dbg && cw == 0 && lane == 0) dbg[4] = clock64(), dbg[14] = mw, dbg[15] = mi;
     }
 
-    else if (warp == 3 && KB == 64) {
+    if (warp == 3 && KB == 64) {
         // ================= weight producer: constants, so no dependency wait; only the ring's empty barriers ====
         for (int i = 0; i < nk; ++i) {
             const int s = i % STAGES;
@@ -355,81 +378,53 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
         }
     }
 
-    // ====== epilogue: TMEM -> registers -> bias/residual/ReLU -> fp16 -> swizzled smem tile -> TMA store ======
+    // ====== epilogue (consumer warpgroups): registers -> bias/residual/ReLU -> fp16 -> swizzled smem tile -> TMA store ======
     pdl_wait();  // every global access below depends on the previous kernel
-    const int row = warp * 32 + lane;
-
-    mbar_wait(accum_bar, 0);  // all MMAs retired: the pipeline buffers are free to become the output staging tile
-    tc_fence_after();
-    __syncthreads();          // s_bias visible; every role has left its loop
-    if (dbg && threadIdx.x == 64) dbg[5] = clock64();
+    __syncthreads();  // every role has left its loop: the pipeline buffers are free to become the output staging tile; s_bias visible
+    if (dbg && threadIdx.x == 128) dbg[5] = clock64();
     if (p.pdl_trigger == 1) pdl_launch_dependents();
-    const uint32_t taddr = tmem_base + (static_cast<uint32_t>(warp * 32) << 16);
+    const FragPos fp(cw, lane);
 
-    // bias + residual + relu for 32 columns of this thread's row, packed into the staging tile
-    auto finish_group = [&](int g, float (&f)[32]) {
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-            const int col = g * 32 + q * 8;       // column inside the BN-wide tile
-            const int box = col / OW;             // which 64- (or 32-) column TMA box
-            const int chunk = (col % OW) / 8;     // 16-byte chunk inside the box row
-            const uint32_t so = static_cast<uint32_t>(box * (128 * OROWB)) + swz_off<OROWB>(row, chunk);
-            float v[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) v[i] = f[q * 8 + i] + s_bias[col + i];
-            if (has_res) {
-                const uint4 rv = *reinterpret_cast<const uint4*>(sRes + so);
-                const __half2* r2 = reinterpret_cast<const __half2*>(&rv);
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    const float2 rf = __half22float2(r2[i]);
-                    v[2 * i] += rf.x;
-                    v[2 * i + 1] += rf.y;
-                }
-            }
-            if (p.relu) {
-#pragma unroll
-                for (int i = 0; i < 8; ++i) v[i] = fmaxf(v[i], 0.0f);
-            }
-            uint4 o;
-            __half2* o2 = reinterpret_cast<__half2*>(&o);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) o2[i] = __floats2half2_rn(v[2 * i], v[2 * i + 1]);
-            *reinterpret_cast<uint4*>(sOut + so) = o;
+    // bias + residual + relu for columns (col, col + 1) of one row, packed into the staging tile
+    auto finish_pair = [&](int row, int col, float v0, float v1) {
+        const int box = col / OW;          // which 64- (or 32-) column TMA box
+        const int chunk = (col % OW) / 8;  // 16-byte chunk inside the box row
+        const uint32_t so = static_cast<uint32_t>(box * (128 * OROWB)) + swz_off<OROWB>(row, chunk) + (col % 8) * 2;
+        v0 += s_bias[col];
+        v1 += s_bias[col + 1];
+        if (has_res) {
+            const float2 rf = __half22float2(*reinterpret_cast<const __half2*>(sRes + so));
+            v0 += rf.x;
+            v1 += rf.y;
         }
+        if (p.relu) {
+            v0 = fmaxf(v0, 0.0f);
+            v1 = fmaxf(v1, 0.0f);
+        }
+        *reinterpret_cast<__half2*>(sOut + so) = __floats2half2_rn(v0, v1);
     };
 
     bool do_store = true;
     if (!split) {
-        if (has_res) mbar_wait(res_bar, 0);
-        constexpr int GP = NG >= 2 ? 2 : 1;  // groups per TMEM round trip
+        if (warp >= 4) {
+            if (has_res) mbar_wait(res_bar, 0);
 #pragma unroll
-        for (int g0 = 0; g0 < NG; g0 += GP) {
-            uint32_t acc[GP][32];
+            for (int j = 0; j < BN / 8; ++j)
 #pragma unroll
-            for (int j = 0; j < GP; ++j) tmem_ld32(taddr + (g0 + j) * 32, acc[j]);
-            tmem_wait_ld();
-#pragma unroll
-            for (int j = 0; j < GP; ++j) {
-                float f[32];
-#pragma unroll
-                for (int i = 0; i < 32; ++i) f[i] = __uint_as_float(acc[j][i]);
-                finish_group(g0 + j, f);
-            }
+                for (int h = 0; h < 2; ++h) finish_pair(fp.row0 + 8 * h, 8 * j + fp.col0, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
         }
     } else {
         // ---- split-K: publish the fp32 partial tile, the last CTA of the tile reduces IN FIXED ORDER ----
         const int tile = blockIdx.y * gridDim.x + blockIdx.x;
         float* ws_tile = p.workspace + static_cast<size_t>(tile) * p.splits * (128 * BN);
-        float* mine = ws_tile + static_cast<size_t>(blockIdx.z) * (128 * BN) + static_cast<size_t>(row) * BN;
+        if (warp >= 4) {
+            float* mine = ws_tile + static_cast<size_t>(blockIdx.z) * (128 * BN);
 #pragma unroll
-        for (int g = 0; g < NG; ++g) {
-            uint32_t acc[32];
-            tmem_ld32(taddr + g * 32, acc);
-            tmem_wait_ld();
+            for (int j = 0; j < BN / 8; ++j)
 #pragma unroll
-            for (int q = 0; q < 8; ++q)
-                __stcg(reinterpret_cast<uint4*>(mine + g * 32) + q, make_uint4(acc[4 * q], acc[4 * q + 1], acc[4 * q + 2], acc[4 * q + 3]));
+                for (int h = 0; h < 2; ++h)
+                    __stcg(reinterpret_cast<float2*>(mine + (fp.row0 + 8 * h) * BN + 8 * j + fp.col0),
+                           make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]));
         }
         __syncthreads();
         if (threadIdx.x == 0) {
@@ -444,42 +439,29 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
         }
         __syncthreads();
         do_store = *last_flag != 0;
-        if (do_store) {
+        if (do_store && warp >= 4) {
             __threadfence();
             if (has_res) mbar_wait(res_bar, 0);
+#pragma unroll 4
+            for (int j = 0; j < BN / 8; ++j) {
 #pragma unroll
-            for (int g = 0; g < NG; ++g) {
-                float f[32];
-#pragma unroll
-                for (int i = 0; i < 32; ++i) f[i] = 0.f;
-                for (int sp = 0; sp < p.splits; sp += 2) {  // two partial tiles (16 x 16 B) in flight per step
-                    const float4* s0 = reinterpret_cast<const float4*>(ws_tile + static_cast<size_t>(sp) * (128 * BN) +
-                                                                       static_cast<size_t>(row) * BN + g * 32);
-                    const bool two = sp + 1 < p.splits;
-                    const float4* s1 = two ? s0 + (128 * BN) / 4 : s0;
-                    float4 t0[8], t1[8];
-#pragma unroll
-                    for (int q = 0; q < 8; ++q) t0[q] = __ldcg(s0 + q);
-#pragma unroll
-                    for (int q = 0; q < 8; ++q) t1[q] = two ? __ldcg(s1 + q) : make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-                    for (int q = 0; q < 8; ++q) {  // fixed order: split sp, then split sp+1
-                        f[4 * q] = (f[4 * q] + t0[q].x) + t1[q].x;
-                        f[4 * q + 1] = (f[4 * q + 1] + t0[q].y) + t1[q].y;
-                        f[4 * q + 2] = (f[4 * q + 2] + t0[q].z) + t1[q].z;
-                        f[4 * q + 3] = (f[4 * q + 3] + t0[q].w) + t1[q].w;
+                for (int h = 0; h < 2; ++h) {
+                    const int row = fp.row0 + 8 * h, col = 8 * j + fp.col0;
+                    float f0 = 0.f, f1 = 0.f;
+                    for (int sp = 0; sp < p.splits; ++sp) {  // fixed order: split 0, 1, ...
+                        const float2 t = __ldcg(reinterpret_cast<const float2*>(ws_tile + static_cast<size_t>(sp) * (128 * BN) + row * BN + col));
+                        f0 += t.x;
+                        f1 += t.y;
                     }
+                    finish_pair(row, col, f0, f1);
                 }
-                finish_group(g, f);
             }
         }
     }
-    if (dbg && threadIdx.x == 64) dbg[6] = clock64();
+    if (dbg && threadIdx.x == 128) dbg[6] = clock64();
     if (p.pdl_trigger == 2) pdl_launch_dependents();  // latest useful point: only the output store is left
     fence_proxy_async();  // generic-proxy smem writes -> visible to the TMA (async proxy)
-    tc_fence_before();
     __syncthreads();
-    if (warp == 2) tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
     if (threadIdx.x == 0 && do_store) {
         // rows >= M and nothing else are clipped by the tensor map; one bulk store per 64-column box
 #pragma unroll
@@ -496,7 +478,7 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
         __syncthreads();
         cluster_sync_all();
     }
-    if (dbg && threadIdx.x == 64) {
+    if (dbg && threadIdx.x == 128) {
         dbg[7] = clock64();
         unsigned long long gt;
         asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt));
@@ -507,26 +489,22 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
 // =================================================================================================
 // conv_f16_tcgen05_ws -- persistent, warp-specialised variant (a TACTIC next to the one-tile-per-CTA kernel).
 //   gridDim.x CTAs walk the tile list with a static stride.  12 warps:
-//     warp 0  activation producer (TMA)                              warp 1  MMA issuer
-//     warp 2  weight producer (cp.async.bulk) + TMEM owner           warp 3  residual producer (TMA)
-//     warps 4-7   epilogue group 0: the CTA's even tiles, accumulator 0, staging / residual buffer 0
-//     warps 8-11  epilogue group 1: the odd tiles, accumulator 1, staging / residual buffer 1
-//   (TMEM lane quadrant of an epilogue warp = warp % 4.)
-//   Everything a tile needs is double-buffered, so the stream never drains: while group g turns tile i into fp16
-//   (TMEM -> regs -> +bias +residual, ReLU -> swizzled smem -> TMA store), the other group does the same for tile i+1,
-//   the MMA warp fills the accumulator of tile i+2's parity as soon as it is drained, the producers run STAGES K-blocks
-//   and one residual tile ahead, and the TMA store of a staging buffer is awaited only right before that buffer is
-//   written again (two tiles later).  For the wide, short-K 1x1 convolutions with a residual -- memory-shaped layers
-//   whose roofline is the L2 read+write stream (tools/micro/l2_stream.cu) -- this keeps loads, math and stores of
-//   three tiles in flight per CTA.  The prologue (barrier init, TMEM alloc) and the first TMA round trip are paid once
-//   per CTA instead of once per tile.  64-channel K-blocks with packed weights only; no split-K.
+//     warp 0  activation producer (TMA)          warp 2  weight producer (cp.async.bulk)
+//     warp 3  residual producer (TMA)            warps 4-7 / 8-11  consumer warpgroups: rows 0-63 / 64-127 of every
+//                                                tile (wgmma, then the epilogue straight from the registers)
+//   The producers run STAGES K-blocks and one residual tile ahead across tile boundaries, and staging / residual buffers
+//   are double-buffered by tile parity: the TMA store of a staging buffer is awaited only right before that buffer is
+//   written again (two tiles later).  For the wide, short-K 1x1 convolutions with a residual -- memory-shaped layers --
+//   this keeps loads of the next tile in flight while the current one is finished.  The prologue (barrier init) and the
+//   first TMA round trip are paid once per CTA instead of once per tile.  64-channel K-blocks with packed weights only;
+//   no split-K.
 // =================================================================================================
 __host__ __device__ constexpr int conv_ws_smem_bytes(int bn, int stages, int sps, bool residual) {
     return stages * sps * (128 * 64 * 2 + bn * 64 * 2) + 2 * 128 * bn * 2 + (residual ? 2 * 128 * bn * 2 : 0) + 256 + 1024;
 }
 
 template <int BN, int STAGES, int SPS>
-__global__ void __launch_bounds__(384)
+__global__ void __launch_bounds__(kConvThreads, 1)
 conv_f16_tcgen05_ws(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapOut,
                     const __grid_constant__ CUtensorMap mapRes, const ConvArgs p) {
     constexpr int A_SUBBLK = 128 * 64 * 2;
@@ -535,12 +513,9 @@ conv_f16_tcgen05_ws(const __grid_constant__ CUtensorMap mapA, const __grid_const
     constexpr int B_STAGE = SPS * B_SUBBLK;
     constexpr int PIPE_BYTES = STAGES * (A_STAGE + B_STAGE);
     constexpr int TILE_BYTES = 128 * BN * 2;
-    constexpr int NG = BN / 32;
     constexpr int OW = BN >= 64 ? 64 : 32;
     constexpr int OROWB = OW * 2;
     constexpr int NBOX = BN / OW;
-    constexpr int TMEM_COLS = 2 * BN < 32 ? 32 : 2 * BN;  // two accumulators (power of two for BN in {32..256})
-    constexpr uint32_t IDESC = make_idesc_f16(128, BN);
 
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -552,11 +527,8 @@ conv_f16_tcgen05_ws(const __grid_constant__ CUtensorMap mapA, const __grid_const
     uint8_t* tail = sRes + (has_res ? 2 * TILE_BYTES : 0);
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(tail);
     uint64_t* empty_bar = full_bar + STAGES;
-    uint64_t* acc_full = empty_bar + STAGES;   // [2]
-    uint64_t* acc_empty = acc_full + 2;        // [2]
-    uint64_t* res_full = acc_empty + 2;        // [2]
+    uint64_t* res_full = empty_bar + STAGES;   // [2]
     uint64_t* res_empty = res_full + 2;        // [2]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(res_empty + 2);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -574,28 +546,21 @@ conv_f16_tcgen05_ws(const __grid_constant__ CUtensorMap mapA, const __grid_const
         if (has_res) tma_prefetch_desc(&mapRes);
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], 1);
+            mbar_init(&empty_bar[s], kConsumerWarps);
         }
         for (int b = 0; b < 2; ++b) {
-            mbar_init(&acc_full[b], 1);
-            mbar_init(&acc_empty[b], 1);
             mbar_init(&res_full[b], 1);
             mbar_init(&res_empty[b], 1);
         }
         fence_barrier_init();
         fence_proxy_async();
     }
-    if (warp == 2) tmem_alloc(tmem_slot, TMEM_COLS);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     if (p.pdl_trigger == 0) pdl_launch_dependents();
     // optional phase accounting (debug aid, b2_context_debug_conv_timing): 16 int64 per CTA
-    //  0 start  1 roles begin  2 epilogue group 0 done  3 tiles of group 0   group 0, summed over its tiles: 4 wait accumulator
-    //  5 wait residual  6 wait own previous store + barrier A  7 TMEM -> regs -> smem  8 barrier B + store issue
-    //  9 MMA warp: wait accumulator free  10 MMA warp: wait operands  11 producer: wait residual buffer  12 producer: wait stage
-    //  13 MMA warp done
+    //  0 start  1 roles begin  2 consumers done  3 tiles   consumer warp 4, summed over its tiles: 4 wgmma main loop
+    //  5 wait residual  6 wait previous store of the buffer + barrier A  7 registers -> smem  8 barrier B + store issue
+    //  10 consumers: wait operands  11 producer: wait residual buffer  12 producer: wait stage
     long long* const dbg = p.dbg ? p.dbg + static_cast<size_t>(blockIdx.x) * 16 : nullptr;
     if (dbg && threadIdx.x == 0) dbg[1] = clock64();
 
@@ -687,146 +652,101 @@ conv_f16_tcgen05_ws(const __grid_constant__ CUtensorMap mapA, const __grid_const
                 __syncwarp();
             }
         }
-    } else if (warp == 1) {
-        // ================= MMA issuer =================
-        int g = 0, lt = 0;
-        long long w_acc = 0, w_ops = 0;
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++lt) {
-            const int b = lt & 1;
-            const long long t0 = dbg ? clock64() : 0;
-            mbar_wait(&acc_empty[b], ((lt >> 1) & 1) ^ 1);  // the epilogue has drained this accumulator
-            if (dbg) w_acc += clock64() - t0;
-            tc_fence_after();
-            const uint32_t tmem_d = tmem_base + static_cast<uint32_t>(b * BN);
-            for (int i = 0; i < nsteps; ++i, ++g) {
-                const int s = g % STAGES;
-                const long long t1 = dbg ? clock64() : 0;
-                mbar_wait(&full_bar[s], (g / STAGES) & 1);
-                if (dbg) w_ops += clock64() - t1;
-                tc_fence_after();
-                const uint32_t a_addr = smem_u32(sA + s * A_STAGE);
-                const uint32_t b_addr = smem_u32(sB + s * B_STAGE);
-                if (elect_one_sync()) {
-                    const int ns = subs_in_step(i);
-#pragma unroll
-                    for (int u = 0; u < SPS; ++u) {
-                        if (u < ns) {
-#pragma unroll
-                            for (int j = 0; j < 4; ++j) {
-                                const uint64_t ad = make_smem_desc(a_addr + u * A_SUBBLK + j * 32, 16, 1024, 2);
-                                const uint64_t bd = make_smem_desc(b_addr + u * B_SUBBLK + j * 32, 16, 1024, 2);
-                                umma_f16(tmem_d, ad, bd, IDESC, (i > 0 || u > 0 || j > 0) ? 1u : 0u);
-                            }
-                        }
-                    }
-                    umma_commit(&empty_bar[s]);
-                    if (i == nsteps - 1) umma_commit(&acc_full[b]);
-                }
-                __syncwarp();
-            }
-        }
-        if (p.pdl_trigger == 1) pdl_launch_dependents();
-        if (dbg && lane == 0) dbg[9] = w_acc, dbg[10] = w_ops, dbg[13] = clock64();
     } else if (warp >= 4) {
-        // ================= epilogue: two groups of 4 warps (128 threads, one accumulator row each) =================
+        // ================= consumers: wgmma + epilogue, every tile =================
         pdl_wait();
-        const int grp = (warp - 4) >> 2;  // == accumulator / staging / residual buffer index == parity of the local tile
-        const int q = warp & 3;           // TMEM lane quadrant this warp may access
-        const int row = q * 32 + lane;
-        const bool e0 = (threadIdx.x == 128 + grp * 128);
-        uint8_t* const my_out = sOut + grp * TILE_BYTES;
-        const uint8_t* const my_res = sRes + grp * TILE_BYTES;
-        const uint32_t bar_a = 1 + 2 * grp, bar_b = 2 + 2 * grp;
-        int lt = grp;
-        const bool rec = dbg && e0 && grp == 0;
-        long long d_acc = 0, d_res = 0, d_a = 0, d_math = 0, d_b = 0, d_tiles = 0;
-        for (int tile = blockIdx.x + grp * static_cast<int>(gridDim.x); tile < num_tiles; tile += 2 * gridDim.x, lt += 2) {
+        const int cw = warp - 4;
+        const uint32_t wg_off = static_cast<uint32_t>(cw >> 2) * 8192u;
+        const FragPos fp(cw, lane);
+        const bool e0 = threadIdx.x == 128;
+        const bool rec = dbg && e0;
+        long long d_mma = 0, d_res = 0, d_a = 0, d_math = 0, d_b = 0, d_tiles = 0, w_ops = 0;
+        float acc[BN / 2];
+        int g = 0, lt = 0;
+        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++lt) {
             const int mt = tile / p.tiles_n;
             const int nt = tile - mt * p.tiles_n;
             const int m0 = mt * 128, n0 = nt * BN;
-            const uint32_t par = (lt >> 1) & 1;
+            const int buf = lt & 1;
             const long long c0 = rec ? clock64() : 0;
-            mbar_wait(&acc_full[grp], par);
-            tc_fence_after();
-            const long long c1 = rec ? clock64() : 0;
-            if (has_res) mbar_wait(&res_full[grp], par);
-            const long long c2 = rec ? clock64() : 0;
-            // (A) this group's previous TMA store has finished READING the staging buffer
-            if (e0) tma_store_wait_read0();
-            named_bar_sync(bar_a, 128);
-            const long long c3 = rec ? clock64() : 0;
-            const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(grp * BN);
-            const float4* bias4 = reinterpret_cast<const float4*>(p.bias + n0);
-            constexpr int GP = NG >= 2 ? 2 : 1;
+            for (int i = 0; i < nsteps; ++i, ++g) {
+                const int s = g % STAGES;
+                const long long t1 = rec ? clock64() : 0;
+                mbar_wait(&full_bar[s], (g / STAGES) & 1);
+                if (rec) w_ops += clock64() - t1;
+                const uint32_t a_addr = smem_u32(sA + s * A_STAGE) + wg_off;
+                const uint32_t b_addr = smem_u32(sB + s * B_STAGE);
+                const int ns = subs_in_step(i);
+                wgmma_fence();
 #pragma unroll
-            for (int g0 = 0; g0 < NG; g0 += GP) {
-                uint32_t acc[GP][32];
+                for (int u = 0; u < SPS; ++u) {
+                    if (u < ns) {
 #pragma unroll
-                for (int j = 0; j < GP; ++j) tmem_ld32(taddr + (g0 + j) * 32, acc[j]);
-                tmem_wait_ld();
-#pragma unroll
-                for (int j = 0; j < GP; ++j) {
-#pragma unroll
-                    for (int qq = 0; qq < 4; ++qq) {
-                        const int col = (g0 + j) * 32 + qq * 8;
-                        const int box = col / OW;
-                        const int chunk = (col % OW) / 8;
-                        const uint32_t so = static_cast<uint32_t>(box * (128 * OROWB)) + swz_off<OROWB>(row, chunk);
-                        const float4 b0 = __ldg(bias4 + col / 4), b1 = __ldg(bias4 + col / 4 + 1);
-                        float v[8];
-                        v[0] = __uint_as_float(acc[j][qq * 8 + 0]) + b0.x;
-                        v[1] = __uint_as_float(acc[j][qq * 8 + 1]) + b0.y;
-                        v[2] = __uint_as_float(acc[j][qq * 8 + 2]) + b0.z;
-                        v[3] = __uint_as_float(acc[j][qq * 8 + 3]) + b0.w;
-                        v[4] = __uint_as_float(acc[j][qq * 8 + 4]) + b1.x;
-                        v[5] = __uint_as_float(acc[j][qq * 8 + 5]) + b1.y;
-                        v[6] = __uint_as_float(acc[j][qq * 8 + 6]) + b1.z;
-                        v[7] = __uint_as_float(acc[j][qq * 8 + 7]) + b1.w;
-                        if (has_res) {
-                            const uint4 rv = *reinterpret_cast<const uint4*>(my_res + so);
-                            const __half2* r2 = reinterpret_cast<const __half2*>(&rv);
-#pragma unroll
-                            for (int i = 0; i < 4; ++i) {
-                                const float2 rf = __half22float2(r2[i]);
-                                v[2 * i] += rf.x;
-                                v[2 * i + 1] += rf.y;
-                            }
+                        for (int j = 0; j < 4; ++j) {
+                            const uint64_t ad = make_wgmma_desc(a_addr + u * A_SUBBLK + j * 32, 16, 1024, WG_SW128);
+                            const uint64_t bd = make_wgmma_desc(b_addr + u * B_SUBBLK + j * 32, 16, 1024, WG_SW128);
+                            wgmma_f16<BN>(acc, ad, bd, (i > 0 || u > 0 || j > 0) ? 1u : 0u);
                         }
-                        if (p.relu) {
-#pragma unroll
-                            for (int i = 0; i < 8; ++i) v[i] = fmaxf(v[i], 0.0f);
-                        }
-                        uint4 o;
-                        __half2* o2 = reinterpret_cast<__half2*>(&o);
-#pragma unroll
-                        for (int i = 0; i < 4; ++i) o2[i] = __floats2half2_rn(v[2 * i], v[2 * i + 1]);
-                        *reinterpret_cast<uint4*>(my_out + so) = o;
                     }
                 }
+                wgmma_commit();
+                wgmma_wait<1>();  // step g-1 has retired: its stage goes back to the producers
+                __syncwarp();
+                if (i > 0 && lane == 0) mbar_arrive(&empty_bar[(g - 1) % STAGES]);
             }
-            tc_fence_before();
+            wgmma_wait<0>();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty_bar[(g - 1) % STAGES]);
+            const long long c1 = rec ? clock64() : 0;
+            if (has_res) mbar_wait(&res_full[buf], (lt >> 1) & 1);
+            const long long c2 = rec ? clock64() : 0;
+            // (A) the store issued from this staging buffer two tiles ago has finished READING it
+            if (e0) tma_store_wait_read1();
+            named_bar_sync(1, 256);
+            const long long c3 = rec ? clock64() : 0;
+            uint8_t* const my_out = sOut + buf * TILE_BYTES;
+            const uint8_t* const my_res = sRes + buf * TILE_BYTES;
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+                const int col = 8 * j + fp.col0;
+                const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias + n0 + col));
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int row = fp.row0 + 8 * h;
+                    const uint32_t so = static_cast<uint32_t>((col / OW) * (128 * OROWB)) + swz_off<OROWB>(row, (col % OW) / 8) + (col % 8) * 2;
+                    float v0 = acc[4 * j + 2 * h] + bb.x, v1 = acc[4 * j + 2 * h + 1] + bb.y;
+                    if (has_res) {
+                        const float2 rf = __half22float2(*reinterpret_cast<const __half2*>(my_res + so));
+                        v0 += rf.x;
+                        v1 += rf.y;
+                    }
+                    if (p.relu) {
+                        v0 = fmaxf(v0, 0.0f);
+                        v1 = fmaxf(v1, 0.0f);
+                    }
+                    *reinterpret_cast<__half2*>(my_out + so) = __floats2half2_rn(v0, v1);
+                }
+            }
             fence_proxy_async();
             const long long c4 = rec ? clock64() : 0;
-            // (B) every thread of the group has drained its TMEM rows, read its residual row and staged its output row
-            named_bar_sync(bar_b, 128);
+            // (B) every consumer has read its residual rows and staged its output rows
+            named_bar_sync(2, 256);
             if (e0) {
-                mbar_arrive(&acc_empty[grp]);              // the accumulator may be overwritten by tile lt+2
-                if (has_res) mbar_arrive(&res_empty[grp]);  // the residual buffer may be refilled
+                if (has_res) mbar_arrive(&res_empty[buf]);  // the residual buffer may be refilled
 #pragma unroll
                 for (int bx = 0; bx < NBOX; ++bx) tma_store_2d(&mapOut, my_out + bx * (128 * OROWB), n0 + bx * OW, m0);
-                tma_store_commit();  // awaited at (A) of this group's next tile, or below before the CTA retires
+                tma_store_commit();  // awaited at (A) two tiles later, or below before the CTA retires
             }
             if (rec) {
                 const long long c5 = clock64();
-                d_acc += c1 - c0, d_res += c2 - c1, d_a += c3 - c2, d_math += c4 - c3, d_b += c5 - c4, ++d_tiles;
+                d_mma += c1 - c0, d_res += c2 - c1, d_a += c3 - c2, d_math += c4 - c3, d_b += c5 - c4, ++d_tiles;
             }
         }
+        if (p.pdl_trigger == 1) pdl_launch_dependents();
         if (e0) tma_store_wait_read0();  // shared memory must outlive the last bulk store's read
-        if (rec) dbg[2] = clock64(), dbg[3] = d_tiles, dbg[4] = d_acc, dbg[5] = d_res, dbg[6] = d_a, dbg[7] = d_math, dbg[8] = d_b;
+        if (rec) dbg[2] = clock64(), dbg[3] = d_tiles, dbg[4] = d_mma, dbg[5] = d_res, dbg[6] = d_a, dbg[7] = d_math, dbg[8] = d_b, dbg[10] = w_ops;
     }
-    tc_fence_before();
     __syncthreads();
-    if (warp == 2) tmem_dealloc(tmem_base, TMEM_COLS);
 }
 
 // =================================================================================================
@@ -836,12 +756,12 @@ conv_f16_tcgen05_ws(const __grid_constant__ CUtensorMap mapA, const __grid_const
 //   The tile is R whole output rows of one image in PADDED coordinates: accumulator row m' = hh*(W+2) + ww.  One 4-D
 //   TMA box {64 ch, W+2, R+2, 1} starting at (w = -1, h = h0-1) lands the halo block in smem as (R+2)*(W+2) pixel rows
 //   of 128 B (SWIZZLE_128B); out-of-image pixels are zero-filled by the TMA, which IS the convolution's padding.  The A
-//   operand of tap (r, s) is the same block read from pixel row r*(W+2)+s on: a start-address offset in the UMMA
+//   operand of tap (r, s) is the same block read from pixel row r*(W+2)+s on: a start-address offset in the wgmma
 //   descriptor (the 128B swizzle is a function of the absolute smem address, so a row shift keeps it consistent).
 //   Columns ww = W, W+1 of every row compute garbage that the output TMA store (box {BN, W+2, R, 1} at w = 0) clips.
 //   A traffic per tile and channel block: (R+2)(W+2) pixel rows instead of 9 x 128.
 //
-//   warp 0 = halo producer, warp 1 = MMA issuer, warp 2 = TMEM owner, warp 3 = weight producer, all 4 = epilogue.
+//   warp 0 = halo producer, warp 3 = weight producer, warps 4-11 = two consumer warpgroups (wgmma + epilogue).
 //   The halo blocks of ALL channel blocks stay resident, so the K loop runs tap outer / channel block inner exactly
 //   like the im2col kernel: same products in the same fp32 summation order -> bit-identical results, whichever of the
 //   two tactics the tuner picks.
@@ -860,14 +780,12 @@ __host__ __device__ constexpr int halo_smem_bytes(int bn, int w, int r, int cblo
 }
 
 template <int BN>
-__global__ void __launch_bounds__(128)
+__global__ void __launch_bounds__(kConvThreads, 1)
 conv3x3_halo_tcgen05(const __grid_constant__ CUtensorMap mapIn, const __grid_constant__ CUtensorMap mapOut, const ConvArgs p) {
     constexpr int NB = halo_b_stages(BN);
     constexpr int B_BLK = BN * 128;  // one tap of one 64-channel block: BN rows of 128 B (pre-swizzled)
-    constexpr int NG = BN / 32;
     constexpr int OW = 64;
     constexpr int NBOX = BN / OW;
-    constexpr uint32_t IDESC = make_idesc_f16(128, BN);
 
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -881,8 +799,6 @@ conv3x3_halo_tcgen05(const __grid_constant__ CUtensorMap mapIn, const __grid_con
     uint64_t* a_full = reinterpret_cast<uint64_t*>(tail);
     uint64_t* b_full = a_full + kHaloMaxCBlocks;
     uint64_t* b_empty = b_full + NB;
-    uint64_t* accum_bar = b_empty + NB;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accum_bar + 1);
     float* s_bias = reinterpret_cast<float*>(tail + 256);
 
     const int warp = threadIdx.x >> 5;
@@ -900,19 +816,15 @@ conv3x3_halo_tcgen05(const __grid_constant__ CUtensorMap mapIn, const __grid_con
         for (int s = 0; s < cblocks; ++s) mbar_init(&a_full[s], 1);
         for (int s = 0; s < NB; ++s) {
             mbar_init(&b_full[s], 1);
-            mbar_init(&b_empty[s], 1);
+            mbar_init(&b_empty[s], kConsumerWarps);
         }
-        mbar_init(accum_bar, 1);
         fence_barrier_init();
         fence_proxy_async();
     }
-    if (warp == 2) tmem_alloc(tmem_slot, BN);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     if (p.pdl_trigger == 0) pdl_launch_dependents();
 
+    float acc[BN / 2];
     if (warp == 0) {
         // ================= halo producer =================
         const uint32_t halo_bytes = static_cast<uint32_t>((R + 2) * Wp * 128);
@@ -924,8 +836,9 @@ conv3x3_halo_tcgen05(const __grid_constant__ CUtensorMap mapIn, const __grid_con
             }
         }
         __syncwarp();
-    } else if (warp == 1) {
-        // ================= MMA issuer =================
+    } else if (warp >= 4) {
+        // ================= consumers: wgmma, accumulators in registers =================
+        const uint32_t wg_off = static_cast<uint32_t>((warp - 4) >> 2) * 8192u;  // 64 pixel rows of 128 B
         int i = 0;
 #pragma unroll 1
         for (int tap = 0; tap < 9; ++tap) {
@@ -936,25 +849,25 @@ conv3x3_halo_tcgen05(const __grid_constant__ CUtensorMap mapIn, const __grid_con
                 const int sb = i % NB;
                 if (tap == 0) mbar_wait(&a_full[cb], 0);
                 mbar_wait(&b_full[sb], (i / NB) & 1);
-                tc_fence_after();
-                const uint32_t a_addr = smem_u32(sA + cb * a_stage) + tap_off;
+                const uint32_t a_addr = smem_u32(sA + cb * a_stage) + tap_off + wg_off;
                 const uint32_t b_addr = smem_u32(sB + sb * B_BLK);
-                if (elect_one_sync()) {
+                wgmma_fence();
 #pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        // descriptor "base offset" stays 0: the swizzle pattern is anchored at the 1024-aligned stage base
-                        // (measured: setting it to (addr >> 7) & 7 for the shifted start gives wrong results)
-                        const uint64_t ad = make_smem_desc(a_addr + j * 32, 16, 1024, 2);
-                        const uint64_t bd = make_smem_desc(b_addr + j * 32, 16, 1024, 2);
-                        umma_f16(tmem_base, ad, bd, IDESC, (i > 0 || j > 0) ? 1u : 0u);
-                    }
-                    umma_commit(&b_empty[sb]);
+                for (int j = 0; j < 4; ++j) {
+                    // descriptor "base offset" stays 0: the swizzle pattern is anchored at the 1024-aligned stage base
+                    const uint64_t ad = make_wgmma_desc(a_addr + j * 32, 16, 1024, WG_SW128);
+                    const uint64_t bd = make_wgmma_desc(b_addr + j * 32, 16, 1024, WG_SW128);
+                    wgmma_f16<BN>(acc, ad, bd, (i > 0 || j > 0) ? 1u : 0u);
                 }
+                wgmma_commit();
+                wgmma_wait<1>();  // step i-1 has retired: its weight block goes back to the producer
                 __syncwarp();
+                if (i > 0 && lane == 0) mbar_arrive(&b_empty[(i - 1) % NB]);
             }
         }
-        if (elect_one_sync()) umma_commit(accum_bar);
+        wgmma_wait<0>();
         __syncwarp();
+        if (lane == 0) mbar_arrive(&b_empty[(nsteps - 1) % NB]);
     } else if (warp == 3) {
         // ================= weight producer (constants: no dependency wait) =================
         for (int i = lane; i < BN; i += 32) s_bias[i] = __ldg(p.bias + n0 + i);
@@ -970,42 +883,29 @@ conv3x3_halo_tcgen05(const __grid_constant__ CUtensorMap mapIn, const __grid_con
         }
     }
 
-    // ====== epilogue: TMEM -> registers -> bias/ReLU -> fp16 -> swizzled smem tile -> 4-D TMA store ======
+    // ====== epilogue (consumer warpgroups): registers -> bias/ReLU -> fp16 -> swizzled smem tile -> 4-D TMA store ======
     pdl_wait();
-    const int row = warp * 32 + lane;
-    mbar_wait(accum_bar, 0);
-    tc_fence_after();
     __syncthreads();
     if (p.pdl_trigger == 1) pdl_launch_dependents();
-    const uint32_t taddr = tmem_base + (static_cast<uint32_t>(warp * 32) << 16);
+    if (warp >= 4) {
+        const FragPos fp(warp - 4, lane);
 #pragma unroll
-    for (int g = 0; g < NG; ++g) {
-        uint32_t acc[32];
-        tmem_ld32(taddr + g * 32, acc);
-        tmem_wait_ld();
+        for (int j = 0; j < BN / 8; ++j) {
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-            const int col = g * 32 + q * 8;
-            const int box = col / OW;
-            const int chunk = (col % OW) / 8;
-            const uint32_t so = static_cast<uint32_t>(box * (128 * 128)) + swz_off<128>(row, chunk);
-            float v[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                v[i] = __uint_as_float(acc[q * 8 + i]) + s_bias[col + i];
-                if (p.relu) v[i] = fmaxf(v[i], 0.0f);
+            for (int h = 0; h < 2; ++h) {
+                const int row = fp.row0 + 8 * h, col = 8 * j + fp.col0;
+                const uint32_t so = static_cast<uint32_t>((col / OW) * (128 * 128)) + swz_off<128>(row, (col % OW) / 8) + (col % 8) * 2;
+                float v0 = acc[4 * j + 2 * h] + s_bias[col], v1 = acc[4 * j + 2 * h + 1] + s_bias[col + 1];
+                if (p.relu) {
+                    v0 = fmaxf(v0, 0.0f);
+                    v1 = fmaxf(v1, 0.0f);
+                }
+                *reinterpret_cast<__half2*>(sOut + so) = __floats2half2_rn(v0, v1);
             }
-            uint4 o;
-            __half2* o2 = reinterpret_cast<__half2*>(&o);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) o2[i] = __floats2half2_rn(v[2 * i], v[2 * i + 1]);
-            *reinterpret_cast<uint4*>(sOut + so) = o;
         }
     }
     fence_proxy_async();
-    tc_fence_before();
     __syncthreads();
-    if (warp == 2) tmem_dealloc(tmem_base, BN);
     if (threadIdx.x == 0) {
         // box {64 ch, W+2, R, 1} at w = 0: the two garbage columns of every row and rows past H are clipped
 #pragma unroll
@@ -1055,18 +955,18 @@ static int launch_one(const ConvLaunch& L, cudaStream_t stream) {
     const size_t smem = size_t(conv_smem_layout_bytes(BN, STAGES, L.args.residual != nullptr, SPS));
     if (CN > 1 && (KB != 64 || L.grid_n % CN != 0 || L.args.cn != CN)) return static_cast<int>(cudaErrorInvalidValue);
     if (CN == 1 && (L.args.dbg != nullptr || L.args.dbg_mode != 0))
-        return launch_kernel_cluster(conv_f16_tcgen05<BN, KB, STAGES, SPS, 1, true>, grid, dim3(128), smem, stream, true, 1u, L.mapA,
+        return launch_kernel_cluster(conv_f16_tcgen05<BN, KB, STAGES, SPS, 1, true>, grid, dim3(kConvThreads), smem, stream, true, 1u, L.mapA,
                                      L.mapB, L.mapOut, L.mapRes, L.args);
     if constexpr (CN == 1 && KB == 64) {
         if (L.args.wpacked != nullptr) {
             if (L.args.a_mode == A_TILED)
-                return launch_kernel_cluster(conv_f16_tcgen05<BN, KB, STAGES, SPS, 1, false, 2>, grid, dim3(128), smem, stream, true, 1u,
+                return launch_kernel_cluster(conv_f16_tcgen05<BN, KB, STAGES, SPS, 1, false, 2>, grid, dim3(kConvThreads), smem, stream, true, 1u,
                                              L.mapA, L.mapB, L.mapOut, L.mapRes, L.args);
-            return launch_kernel_cluster(conv_f16_tcgen05<BN, KB, STAGES, SPS, 1, false, 1>, grid, dim3(128), smem, stream, true, 1u,
+            return launch_kernel_cluster(conv_f16_tcgen05<BN, KB, STAGES, SPS, 1, false, 1>, grid, dim3(kConvThreads), smem, stream, true, 1u,
                                          L.mapA, L.mapB, L.mapOut, L.mapRes, L.args);
         }
     }
-    return launch_kernel_cluster(conv_f16_tcgen05<BN, KB, STAGES, SPS, CN>, grid, dim3(128), smem, stream, true,
+    return launch_kernel_cluster(conv_f16_tcgen05<BN, KB, STAGES, SPS, CN>, grid, dim3(kConvThreads), smem, stream, true,
                                  static_cast<unsigned>(CN), L.mapA, L.mapB, L.mapOut, L.mapRes, L.args);
 }
 
@@ -1114,9 +1014,9 @@ static int launch_conv_halo(const ConvLaunch& L, cudaStream_t stream) {
     if (smem > 227 * 1024 || R < 1 || R * (L.args.Wo + 2) > 128 || L.args.cblocks > kHaloMaxCBlocks) return static_cast<int>(cudaErrorInvalidValue);
     dim3 grid(L.grid_n, L.grid_m, 1);
     switch (L.bn) {
-        case 64: return launch_kernel(conv3x3_halo_tcgen05<64>, grid, dim3(128), smem, stream, true, L.mapA, L.mapOut, L.args);
-        case 128: return launch_kernel(conv3x3_halo_tcgen05<128>, grid, dim3(128), smem, stream, true, L.mapA, L.mapOut, L.args);
-        case 256: return launch_kernel(conv3x3_halo_tcgen05<256>, grid, dim3(128), smem, stream, true, L.mapA, L.mapOut, L.args);
+        case 64: return launch_kernel(conv3x3_halo_tcgen05<64>, grid, dim3(kConvThreads), smem, stream, true, L.mapA, L.mapOut, L.args);
+        case 128: return launch_kernel(conv3x3_halo_tcgen05<128>, grid, dim3(kConvThreads), smem, stream, true, L.mapA, L.mapOut, L.args);
+        case 256: return launch_kernel(conv3x3_halo_tcgen05<256>, grid, dim3(kConvThreads), smem, stream, true, L.mapA, L.mapOut, L.args);
     }
     return static_cast<int>(cudaErrorInvalidValue);
 }
@@ -1168,7 +1068,7 @@ int launch_conv_f16_tcgen05(const ConvLaunch& L, cudaStream_t stream) {
 template <int BN, int STAGES, int SPS>
 static int launch_one_ws(const ConvLaunch& L, cudaStream_t stream) {
     const size_t smem = size_t(conv_ws_smem_bytes(BN, STAGES, SPS, L.args.residual != nullptr));
-    return launch_kernel(conv_f16_tcgen05_ws<BN, STAGES, SPS>, dim3(L.ws_ctas), dim3(384), smem, stream, true, L.mapA, L.mapOut,
+    return launch_kernel(conv_f16_tcgen05_ws<BN, STAGES, SPS>, dim3(L.ws_ctas), dim3(kConvThreads), smem, stream, true, L.mapA, L.mapOut,
                          L.mapRes, L.args);
 }
 
@@ -2038,7 +1938,10 @@ int launch_tail_f16(const TailArgs& a, cudaStream_t stream) {
     static int cap = -1, use_pdl = -1;
     if (cap < 0) {
         const char* v = getenv("B2_TAIL_CTAS");
-        cap = v ? atoi(v) : 148;  // one wave: every FC item (8 neurons) gets its own CTA, so the weight rows stream in one round
+        int sms = 0, dev = 0;
+        cudaGetDevice(&dev);
+        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+        cap = v ? atoi(v) : sms;  // one wave: every FC item (8 neurons) gets its own CTA, so the weight rows stream in one round
         if (cap < 1) cap = 1;
         v = getenv("B2_TAIL_PDL");
         use_pdl = v ? atoi(v) : 1;

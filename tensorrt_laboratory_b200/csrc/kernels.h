@@ -1,4 +1,4 @@
-// Host-visible launch API of the sm_100a kernels (implemented in kernels.cu).
+// Host-visible launch API of the sm_90a kernels (implemented in kernels.cu).
 // Internal to libb200infer.so -- the public boundary is include/b200infer.h.
 #pragma once
 #include <cuda.h>
@@ -9,8 +9,8 @@
 namespace b2k {
 
 // ---------------------------------------------------------------------------------------------
-// implicit-GEMM convolution on tcgen05 tensor cores
-//   D[M = batch*Ho*Wo, N = Cout] = A[M, K = taps*Cin] * B[N, K]^T,  fp16 in, fp32 accumulate in TMEM,
+// implicit-GEMM convolution on the tensor cores (wgmma)
+//   D[M = batch*Ho*Wo, N = Cout] = A[M, K = taps*Cin] * B[N, K]^T,  fp16 in, fp32 accumulate in registers,
 //   epilogue: + bias[n] (+ residual[m][n]) -> relu -> fp16 -> NHWC store.
 // ---------------------------------------------------------------------------------------------
 enum { A_TILED = 0, A_IM2COL = 1 };
@@ -125,7 +125,7 @@ int net_smem_bytes(int n_layers, int stages);
 int launch_net_f16_tcgen05(const NetArgs& a, int ctas, cudaStream_t stream);
 
 // ---------------------------------------------------------------------------------------------
-// INT8 path (i8_kernels.cu): tcgen05.mma.kind::i8 convolution with a requantising epilogue + its SIMT helpers
+// INT8 path (i8_kernels.cu): wgmma s8 convolution with a requantising epilogue + its SIMT helpers
 // ---------------------------------------------------------------------------------------------
 struct I8ConvArgs {
     const uint8_t* wpacked;  // int8 weights as pre-swizzled blocks [num_kblocks][Cout/32][32][128 B] (K-block = 128 bytes)

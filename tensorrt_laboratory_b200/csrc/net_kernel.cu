@@ -1,17 +1,15 @@
-// net_f16_tcgen05 -- the forward pass of a run of convolution layers as ONE persistent sm_100a kernel.
+// net_f16_tcgen05 -- the forward pass of a run of convolution layers as ONE persistent sm_90a kernel.
 //
-// Why: at batch 8 a ResNet layer is 13..800 output tiles whose CTAs live ~2 us of fixed cost (launch, barrier init, TMEM
-// allocation, first TMA round trip, epilogue, teardown) around a 0.2..2 us main loop, and every layer boundary is a
-// grid-wide dependency.  Here the CTAs are persistent, the tiles of ALL layers form one ordered work list that CTAs draw
-// tickets from, the epilogue of tile i overlaps the main loop of tile i+1 (two TMEM accumulators), weights of the next
-// tile stream in while the current one computes, and a tile of layer L+1 starts as soon as the M tiles of layer L it
-// reads have been stored (arrival counters in global memory, release/acquire at gpu scope).
+// Why: at batch 8 a ResNet layer is 13..800 output tiles whose CTAs pay a fixed cost (launch, barrier init, first TMA
+// round trip, epilogue, teardown) around a short main loop, and every layer boundary is a grid-wide dependency.  Here the
+// CTAs are persistent, the tiles of ALL layers form one ordered work list that CTAs draw tickets from, operands of the
+// next tile stream in while the current one computes and is stored, and a tile of layer L+1 starts as soon as the M tiles
+// of layer L it reads have been stored (arrival counters in global memory, release/acquire at gpu scope).
 //
 // The chain "tile finished -> dependent tile's first MMA" is what bounds a forward pass at this batch size, so it is kept
-// short: the epilogue goes straight from TMEM through registers to global memory (8 warps, 16-byte stores, residual read
-// directly from global -- no shared-memory staging, no TMA store, no store-side barriers), the last epilogue warp to
-// finish publishes the tile, and waiters poll without back-off.  Without staging tiles the CTA needs only its operand
-// ring, so TWO CTAs (normally of two different forward passes) share an SM and fill each other's dependency stalls.
+// short: the epilogue goes straight from the wgmma registers to global memory (8 warps, residual read directly from
+// global -- no shared-memory staging, no TMA store, no store-side barriers), the last consumer warp to finish publishes
+// the tile, and waiters poll without back-off.
 //
 // Deadlock freedom: tickets are drawn in list order by RUNNING CTAs only, a CTA works through its tickets in order, and
 // a tile only ever waits for tiles with smaller tickets -- so the smallest unfinished ticket always belongs to a running
@@ -19,17 +17,19 @@
 // ExecutionContext).  Every wait is bounded and traps instead of hanging.
 //
 // Warp roles (12 warps):  0 activation producer (dependency waits, TMA tiled / im2col loads)
-//                         1 MMA issuer (tcgen05.mma 128 x BN x 16, fp32 accumulators in TMEM)
-//                         2 weight producer (cp.async.bulk of pre-swizzled blocks) + TMEM owner
+//                         1 idle
+//                         2 weight producer (cp.async.bulk of pre-swizzled blocks)
 //                         3 scheduler (ticket counter -> tile ring in shared memory)
-//                         4-11 epilogue: warp w owns TMEM lane quadrant w % 4 and column half (w - 4) / 4 of the tile
+//                         4-11 two consumer warpgroups: wgmma 64 x BN x 16 each (rows 0-63 / 64-127), fp32 accumulators
+//                              in registers, then the epilogue
 //
 // Same products in the same fp32 order as conv_f16_tcgen05 (tap outer, channel block inner, K=16 steps in order), same
 // epilogue arithmetic: results are bit-identical to the per-layer kernels.
 //
 // Replaces the forward pass the reference delegates to TensorRT: trtlab/tensorrt/src/workspace.cc:47,52 (enqueueV2).
 #include "kernels.h"
-#include "ptx_sm100.cuh"
+#include "ptx_sm90.cuh"
+#include "wgmma_sm90.cuh"
 
 namespace b2k {
 
@@ -40,9 +40,8 @@ constexpr int kASub = 128 * 64 * 2;           // 16 KiB
 constexpr int kBSubMax = 128 * 64 * 2;        // BN <= 128
 constexpr int kSchedSlots = 4;
 constexpr int kEpiWarps = 8;
-constexpr int kSchedConsumers = 3 + kEpiWarps;  // A, B, MMA, epilogue warps
+constexpr int kSchedConsumers = 2 + kEpiWarps;  // A, B, consumer warps
 constexpr int kThreads = (4 + kEpiWarps) * 32;
-constexpr int kTmemCols = 256;                // two 128-column accumulators
 
 __device__ __forceinline__ int ld_acquire(const int* p) {
     int v;
@@ -54,20 +53,11 @@ __device__ __forceinline__ void red_relaxed_add(int* p, int v) {
 }
 __device__ __forceinline__ void fence_acq_rel_gpu() { asm volatile("fence.acq_rel.gpu;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
-__device__ __forceinline__ uint4 ld_global_v4(const void* p) {
-    uint4 v;
-    asm volatile("ld.global.cg.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p) : "memory");
-    return v;
-}
-
 struct Smem {
     uint64_t full[kMaxStages], empty[kMaxStages];
-    uint64_t acc_full[2], acc_empty[2];
     uint64_t sched_full[kSchedSlots], sched_empty[kSchedSlots];
     int4 sched[kSchedSlots];  // {layer (-1 = no more work), mt, nt, ticket}
-    int pub_cnt[2];           // epilogue warps that have stored their part of the tile in accumulator b
-    uint32_t tmem_slot;
-    uint32_t pad;
+    int pub_cnt[8];           // consumer warps that have stored their part of tile it (slot it & 7)
 };
 
 }  // namespace
@@ -79,7 +69,7 @@ __host__ __device__ constexpr int net_smem_layout_bytes(int n_layers, int stages
 // DBG: per-role wait / busy cycle counters into a.dbg (8 roles x 8 int64 per CTA) -- a separate instantiation, the
 // production kernel carries none of it.
 template <bool DBG>
-__global__ void __launch_bounds__(kThreads, 2) net_f16_tcgen05(const NetArgs a) {
+__global__ void __launch_bounds__(kThreads, 1) net_f16_tcgen05(const NetArgs a) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     const int stages = a.stages;
@@ -102,13 +92,9 @@ __global__ void __launch_bounds__(kThreads, 2) net_f16_tcgen05(const NetArgs a) 
     if (threadIdx.x == 0) {
         for (int s = 0; s < kMaxStages; ++s) {
             mbar_init(&sm.full[s], 1);
-            mbar_init(&sm.empty[s], 1);
+            mbar_init(&sm.empty[s], kEpiWarps);
         }
-        for (int b = 0; b < 2; ++b) {
-            mbar_init(&sm.acc_full[b], 1);
-            mbar_init(&sm.acc_empty[b], kEpiWarps);
-            sm.pub_cnt[b] = 0;
-        }
+        for (int b = 0; b < 8; ++b) sm.pub_cnt[b] = 0;
         for (int s = 0; s < kSchedSlots; ++s) {
             mbar_init(&sm.sched_full[s], 1);
             mbar_init(&sm.sched_empty[s], kSchedConsumers);
@@ -116,11 +102,7 @@ __global__ void __launch_bounds__(kThreads, 2) net_f16_tcgen05(const NetArgs a) 
         fence_barrier_init();
         fence_proxy_async();
     }
-    if (warp == 2) tmem_alloc(&sm.tmem_slot, kTmemCols);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = sm.tmem_slot;
 
     long long dbg_acc[6] = {0, 0, 0, 0, 0, 0};  // this thread's counters (meaning depends on the role)
     const long long dbg_t0 = DBG ? clock64() : 0;
@@ -298,112 +280,82 @@ __global__ void __launch_bounds__(kThreads, 2) net_f16_tcgen05(const NetArgs a) 
             }
         }
         dbg_flush(2);
-    } else if (warp == 1) {
-        // ================= MMA issuer =================
+    } else if (warp >= 4) {
+        // ================= consumers: wgmma -> registers -> bias / residual / ReLU -> fp16 -> global =================
+        // 8 warps, two warpgroups: warpgroup h computes rows 64h..64h+63 of the tile; a thread owns two rows and two
+        // adjacent columns of every 8-column block (wgmma fragment layout) and stores them as 4-byte pairs.
+        const int cw = warp - 4;
+        const uint32_t wg_off = static_cast<uint32_t>(cw >> 2) * 8192u;
+        const int row0 = 64 * (cw >> 2) + 16 * (cw & 3) + (lane >> 2);
+        const int col0 = 2 * (lane & 3);
+        float acc[64];
         int s = 0;
         uint32_t ph = 0;
         for (int it = 0;; ++it) {
             const int4 t = next_tile(it);
             if (t.x < 0) break;
             const NetLayerInfo& L = s_layers[t.x];
-            const int b = it & 1;
-            wait_t(&sm.acc_empty[b], ((it >> 1) & 1) ^ 1, 2);  // the epilogue has drained this accumulator
-            tc_fence_after();
-            const uint32_t tmem_d = tmem_base + static_cast<uint32_t>(b * 128);
-            const uint32_t idesc = make_idesc_f16(128, L.bn);
             const int nkb = L.num_kblocks;
+            const bool wide = L.bn == 128;
+            int prev_s = 0;
             for (int i = 0; i < nkb; ++i) {
                 wait_t(&sm.full[s], ph, 1);
-                tc_fence_after();
-                const uint32_t a_addr = smem_u32(sA + s * kASub);
+                const uint32_t a_addr = smem_u32(sA + s * kASub) + wg_off;
                 const uint32_t b_addr = smem_u32(sB + s * kBSubMax);
-                if (elect_one_sync()) {
+                wgmma_fence();
 #pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        const uint64_t ad = make_smem_desc(a_addr + j * 32, 16, 1024, 2);
-                        const uint64_t bd = make_smem_desc(b_addr + j * 32, 16, 1024, 2);
-                        umma_f16(tmem_d, ad, bd, idesc, (i > 0 || j > 0) ? 1u : 0u);
-                    }
-                    umma_commit(&sm.empty[s]);
-                    if (i == nkb - 1) umma_commit(&sm.acc_full[b]);
+                for (int j = 0; j < 4; ++j) {
+                    const uint64_t ad = make_wgmma_desc(a_addr + j * 32, 16, 1024, WG_SW128);
+                    const uint64_t bd = make_wgmma_desc(b_addr + j * 32, 16, 1024, WG_SW128);
+                    if (wide) wgmma_f16<128>(acc, ad, bd, (i > 0 || j > 0) ? 1u : 0u);
+                    else wgmma_f16<64>(*reinterpret_cast<float(*)[32]>(acc), ad, bd, (i > 0 || j > 0) ? 1u : 0u);
                 }
+                wgmma_commit();
+                wgmma_wait<1>();  // step i-1 has retired: its stage goes back to the producers
                 __syncwarp();
+                if (i > 0 && lane == 0) mbar_arrive(&sm.empty[prev_s]);
+                prev_s = s;
                 if (++s == stages) s = 0, ph ^= 1;
             }
-        }
-        dbg_flush(1);
-    } else {
-        // ================= epilogue: TMEM -> registers -> bias / residual / ReLU -> fp16 -> global =================
-        // 8 warps: warp w reads TMEM lane quadrant w % 4 (hardware rule) and the column half (w - 4) / 4 of the tile; a
-        // thread owns one output pixel (row) and streams its columns 32 at a time as four 16-byte stores.
-        const int q = warp & 3;
-        const int half = (warp - 4) >> 2;
-        const int row = q * 32 + lane;
-        for (int it = 0;; ++it) {
-            const int4 t = next_tile(it);
-            if (t.x < 0) break;
-            const NetLayerInfo& L = s_layers[t.x];
-            const int b = it & 1;
-            const int hw = L.bn >> 1;                       // columns of this warp: 32 (BN = 64) or 64 (BN = 128)
-            const int c0 = t.z * L.bn + half * hw;          // first output channel of this warp
-            const int m = t.y * 128 + row;
-            const bool valid = m < L.M;
-            const bool relu = L.relu != 0;
-            const __half* res = L.residual ? L.residual + static_cast<size_t>(m) * L.Cout + c0 : nullptr;
-            __half* out = L.out + static_cast<size_t>(m) * L.Cout + c0;
-            const float4* bias4 = reinterpret_cast<const float4*>(L.bias + c0);
-            wait_t(&sm.acc_full[b], (it >> 1) & 1, 1);
-            tc_fence_after();
+            wgmma_wait<0>();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&sm.empty[prev_s]);
             const long long cb = tick();
-            const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(b * 128 + half * hw);
-            for (int cc = 0; cc < hw; cc += 32) {
-                uint4 rv[4];
-                if (res != nullptr && valid) {  // issued ahead of the TMEM load; both are in flight together
+            const int n0 = t.z * L.bn;
+            const bool relu = L.relu != 0;
+            const int nblk = L.bn >> 3;
 #pragma unroll
-                    for (int i = 0; i < 4; ++i) rv[i] = ld_global_v4(res + cc + i * 8);
-                }
-                uint32_t acc[32];
-                tmem_ld32(taddr + cc, acc);
-                tmem_wait_ld();
+            for (int h = 0; h < 2; ++h) {
+                const int m = t.y * 128 + row0 + 8 * h;
+                if (m >= L.M) continue;
+                const __half* res = L.residual ? L.residual + static_cast<size_t>(m) * L.Cout + n0 : nullptr;
+                __half* out = L.out + static_cast<size_t>(m) * L.Cout + n0;
 #pragma unroll
-                for (int qq = 0; qq < 4; ++qq) {
-                    const float4 b0 = __ldg(bias4 + ((cc + qq * 8) >> 2)), b1 = __ldg(bias4 + ((cc + qq * 8) >> 2) + 1);
-                    float v[8];
-                    v[0] = __uint_as_float(acc[qq * 8 + 0]) + b0.x;
-                    v[1] = __uint_as_float(acc[qq * 8 + 1]) + b0.y;
-                    v[2] = __uint_as_float(acc[qq * 8 + 2]) + b0.z;
-                    v[3] = __uint_as_float(acc[qq * 8 + 3]) + b0.w;
-                    v[4] = __uint_as_float(acc[qq * 8 + 4]) + b1.x;
-                    v[5] = __uint_as_float(acc[qq * 8 + 5]) + b1.y;
-                    v[6] = __uint_as_float(acc[qq * 8 + 6]) + b1.z;
-                    v[7] = __uint_as_float(acc[qq * 8 + 7]) + b1.w;
-                    if (res != nullptr && valid) {
-                        const __half2* r2 = reinterpret_cast<const __half2*>(&rv[qq]);
-#pragma unroll
-                        for (int i = 0; i < 4; ++i) {
-                            const float2 rf = __half22float2(r2[i]);
-                            v[2 * i] += rf.x;
-                            v[2 * i + 1] += rf.y;
+                for (int j = 0; j < 16; ++j) {
+                    if (j < nblk) {
+                        const int col = 8 * j + col0;
+                        const float2 bb = __ldg(reinterpret_cast<const float2*>(L.bias + n0 + col));
+                        float v0 = acc[4 * j + 2 * h] + bb.x, v1 = acc[4 * j + 2 * h + 1] + bb.y;
+                        if (res != nullptr) {
+                            const float2 rf = __half22float2(__ldcg(reinterpret_cast<const __half2*>(res + col)));
+                            v0 += rf.x;
+                            v1 += rf.y;
                         }
+                        if (relu) {
+                            v0 = fmaxf(v0, 0.0f);
+                            v1 = fmaxf(v1, 0.0f);
+                        }
+                        *reinterpret_cast<__half2*>(out + col) = __floats2half2_rn(v0, v1);
                     }
-                    if (relu) {
-#pragma unroll
-                        for (int i = 0; i < 8; ++i) v[i] = fmaxf(v[i], 0.0f);
-                    }
-                    uint4 o;
-                    __half2* o2 = reinterpret_cast<__half2*>(&o);
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) o2[i] = __floats2half2_rn(v[2 * i], v[2 * i + 1]);
-                    if (valid) *reinterpret_cast<uint4*>(out + cc + qq * 8) = o;
                 }
             }
             const long long cf = tick();
-            tc_fence_before();
             fence_acq_rel_gpu();  // this thread's stores are performed before anything that follows the warp barrier below
             __syncwarp();
             if (lane == 0) {
-                // The eighth warp to get here publishes the tile.  Counting BEFORE releasing the accumulator keeps tile
-                // it and tile it + 2 (same accumulator, same counter) apart: the MMA of it + 2 cannot start earlier.
+                // The eighth warp to get here publishes the tile.  A warp runs at most kSchedSlots (4) tiles ahead of
+                // the slowest one (the scheduler ring), so eight counter slots never mix two tiles.
+                const int b = it & 7;
                 const int prev = atomicAdd(&sm.pub_cnt[b], 1);
                 if (prev == kEpiWarps - 1) {
                     sm.pub_cnt[b] = 0;
@@ -411,7 +363,6 @@ __global__ void __launch_bounds__(kThreads, 2) net_f16_tcgen05(const NetArgs a) 
                     red_relaxed_add(a.mt_done + L.out_flag_off + t.y, 1);
                     red_relaxed_add(a.layer_done + t.x, 1);
                 }
-                mbar_arrive(&sm.acc_empty[b]);  // accumulator b may be overwritten (tile it + 2)
             }
             if (DBG) dbg_acc[2] += cf - cb, dbg_acc[3] += clock64() - cf;
         }
@@ -419,9 +370,7 @@ __global__ void __launch_bounds__(kThreads, 2) net_f16_tcgen05(const NetArgs a) 
     }
 
     // ---------------- teardown; the last CTA re-arms the counters for the next launch ----------------
-    tc_fence_before();
     __syncthreads();
-    if (warp == 2) tmem_dealloc(tmem_base, kTmemCols);
     __shared__ int s_last;
     if (threadIdx.x == 0) {
         __threadfence();

@@ -162,7 +162,7 @@ class PyInferenceManager : public InferenceManager {
 }  // namespace
 
 PYBIND11_MODULE(trtlab, m) {
-    m.doc() = "trtlab Python surface (InferenceManager / InferRunner / InferFuture) on the B200-native runtime";
+    m.doc() = "trtlab Python surface (InferenceManager / InferRunner / InferFuture) on the H100-native runtime";
     py::class_<PyInferenceManager, std::shared_ptr<PyInferenceManager>>(m, "InferenceManager")
         .def(py::init<int, int, int, int, int>(), py::arg("max_exec_concurrency") = 1, py::arg("max_copy_concurrency") = 0,
              py::arg("pre_threads") = 1, py::arg("cuda_threads") = 1, py::arg("post_threads") = 3)

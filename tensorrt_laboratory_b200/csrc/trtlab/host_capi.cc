@@ -365,7 +365,7 @@ int trt_cyclic_infer(const void* blob, size_t nbytes, int batch, const void* inp
 }
 
 int trt_device_throughput(const void* blob, size_t nbytes, int contexts, int batch, int steps, int warmup,
-                          const void* host_ring, int ring_batches, double* elapsed_ms, int* launches_per_step) {
+                          const void* host_ring, int ring_batches, double* elapsed_ms, int* launches_per_step, void* last_output) {
     if (!blob || contexts < 1 || steps < 1 || !host_ring || ring_batches < 1 || !elapsed_ms) return fail(B2_EINVAL, "bad arguments");
     b2_runtime* rt = nullptr;
     b2_engine* eng = nullptr;
@@ -421,8 +421,13 @@ int trt_device_throughput(const void* blob, size_t nbytes, int contexts, int bat
     for (auto& x : ctx) {
         if (status != B2_OK) break;
         if ((status = b2_context_create(eng, &x.c))) break;
-        // the contexts share the GPU: each persistent network kernel gets its share of the 2 x 148 CTA slots (B2_NET_CTAS overrides)
-        if (!getenv("B2_NET_CTAS")) b2_context_set_option(x.c, "net_ctas", std::max(1, 296 / contexts));
+        // the contexts share the GPU: each persistent network kernel gets its share of the SMs (one CTA each; B2_NET_CTAS overrides)
+        if (!getenv("B2_NET_CTAS")) {
+            int dev = 0, sms = 0;
+            cudaGetDevice(&dev);
+            cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+            b2_context_set_option(x.c, "net_ctas", std::max(1, sms / contexts));
+        }
         if (!cuda_ok(cudaMalloc(&x.scratch, std::max<size_t>(b2_engine_device_memory_size(eng), 1024)), "cudaMalloc scratch")) break;
         if ((status = b2_context_set_device_memory(x.c, x.scratch))) break;
         x.bind.assign(nb, nullptr);
@@ -501,6 +506,13 @@ int trt_device_throughput(const void* blob, size_t nbytes, int contexts, int bat
         float ms = 0.f;
         if (status == B2_OK && cuda_ok(cudaEventElapsedTime(&ms, start, stop), "elapsed")) *elapsed_ms = ms;
         if (launches_per_step) *launches_per_step = b2_context_nb_launches(ctx[0].c, batch);
+        // optional: the first output binding of the last timed step (`batch` rows), as the caller's host buffer
+        for (int i = 0; last_output && status == B2_OK && i < nb; ++i) {
+            if (i == in_id) continue;
+            const size_t out_bytes = bytes[i] / size_t(b2_engine_max_batch(eng)) * size_t(batch);
+            cuda_ok(cudaMemcpy(last_output, ctx[size_t((steps - 1) % contexts)].bind[i], out_bytes, cudaMemcpyDeviceToHost), "last output");
+            break;
+        }
     }
     bg_stop = true;
     if (bg.joinable()) bg.join();

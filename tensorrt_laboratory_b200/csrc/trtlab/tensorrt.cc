@@ -34,6 +34,9 @@ void* CudaPinnedHostMemory::Allocate(size_t bytes) {
         cudaGetLastError();
         throw std::bad_alloc();
     }
+    // touch every page now, on the allocating thread: otherwise the first request to use a stack pays a page fault
+    // per 4 KiB of its input and output
+    memset(p, 0, bytes ? bytes : 1);
     return p;
 }
 void CudaPinnedHostMemory::Free(void* ptr) {
@@ -452,6 +455,9 @@ void InferenceManager::PrepareModel(const Model* model) {
     const std::string mode = env ? env : "all";
     if (mode == "0") return;
     const int max_batch = model->GetMaxBatchSize();
+    int dev = 0, sms = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     for (size_t lane = 0; lane < m_Lanes.size(); lane++) {
         auto& pool = item->second[lane];
         std::vector<std::shared_ptr<IExecutionContext>> held;
@@ -459,10 +465,10 @@ void InferenceManager::PrepareModel(const Model* model) {
         for (size_t k = 0; k < n; k++) held.push_back(pool->PopWithoutReturn());
         for (auto& ctx : held) {
             TRT_CHECK_B2(b2_context_set_device_memory(ctx->handle, m_Lanes[lane]->workspace));
-            if (!getenv("B2_NET_CTAS")) b2_context_set_option(ctx->handle, "net_ctas", std::max(1, 296 / std::max(1, m_MaxExecutions)));
+            if (!getenv("B2_NET_CTAS")) b2_context_set_option(ctx->handle, "net_ctas", std::max(1, sms / std::max(1, m_MaxExecutions)));
             if (ZeroCopyInput() && !getenv("B2_INPUT_CTAS")) {  // a PCIe-paced cast must not hold every thread slot of the GPU
                 const char* v = getenv("TRTLAB_ZERO_COPY_CTAS");
-                b2_context_set_option(ctx->handle, "input_ctas", v ? atoi(v) : 74);
+                b2_context_set_option(ctx->handle, "input_ctas", v ? atoi(v) : std::max(1, sms / 2));
             }
             for (int b = (mode == "max" || max_batch > 64) ? max_batch : 1; b <= max_batch; b++)
                 TRT_CHECK_B2(b2_context_prepare(ctx->handle, b, nullptr));

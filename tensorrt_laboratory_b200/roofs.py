@@ -2,20 +2,15 @@
 
 For each convolution at a given batch: the tensor-core floor (2*M*N*K over the sustained fp16/bf16 peak) and the memory
 floor for L2-resident activations -- algorithmic bytes (activations in + weights + residual read, output written, fp16)
-over the bandwidth the memory system gives UNIQUE streaming data, which differs for reads and writes
-(tools/micro/l2_stream.cu on this pool's B200s, profiles/l2_stream_r2.log: 17.5 TB/s read, 7.3 TB/s write).  A layer's
-floor is the larger of the two; the sum over layers is what a forward pass costs if every kernel sat on its own roof.
-Used by bench.py (`roofline.per_layer_roofs`) and tools/roofline_saturated.py."""
+over the bandwidth the memory system gives UNIQUE streaming data, which differs for reads and writes (measure it with
+tools/micro/l2_stream.cu on the GPU in question).  A layer's floor is the larger of the two; the sum over layers is what a
+forward pass costs if every kernel sat on its own roof.  Used by tools/roofline_saturated.py."""
 from __future__ import annotations
 
 from typing import Dict, List
 
-L2_READ_BPS = 17.5e12
-L2_WRITE_BPS = 7.3e12
-
-
-def conv_floors(lowered: dict, batch: int, peak_tflops: float, l2_read_bps: float = L2_READ_BPS,
-                l2_write_bps: float = L2_WRITE_BPS, elt_bytes: int = 2) -> List[Dict]:
+def conv_floors(lowered: dict, batch: int, peak_tflops: float, l2_read_bps: float, l2_write_bps: float,
+                elt_bytes: int = 2) -> List[Dict]:
     T = lowered["tensors"]
     out = []
     for op in lowered["ops"]:

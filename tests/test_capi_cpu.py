@@ -233,7 +233,7 @@ def test_per_layer_roofs_of_resnet50():
     wide short-K layers with a residual are memory-bound and the 3x3 layers tensor-bound."""
     from tensorrt_laboratory_b200 import graph, roofs, weights
     net = graph.resnet_caffe(50)
-    fl = roofs.conv_floors(graph.lower(net, weights.random_weights(net, 0)), 8, 1429.0)
+    fl = roofs.conv_floors(graph.lower(net, weights.random_weights(net, 0)), 8, 1429.0, 17.5e12, 7.3e12)
     assert len(fl) == 53
     by = {f["name"]: f for f in fl}
     assert abs(sum(f["flops"] for f in fl) / 61.69e9 - 1) < 0.01

@@ -78,10 +78,10 @@ def test_double_width_pipeline_stages(gpu, bn, stages):
 
 @pytest.mark.parametrize("bn,stages,sps", [(32, 4, 1), (64, 2, 1), (64, 4, 2), (128, 2, 1), (128, 2, 2), (256, 2, 1)])
 def test_persistent_warp_specialised_tactic(gpu, bn, stages, sps):
-    """conv_f16_tcgen05_ws: persistent CTAs, separate epilogue warps, double-buffered TMEM.  Same K order as the
+    """conv_f16_tcgen05_ws: persistent CTAs, producers running ahead across tiles, double-buffered staging.  Same K order as the
     one-tile-per-CTA kernel -> bit-identical results."""
     opts = {"bn": bn, "stages": stages, "sps": sps}
-    # many tiles per CTA (M = 4*56*56 = 12544 -> 98 m-tiles x n-tiles on <= 148 CTAs), 1x1 tiled A, fused residual
+    # many tiles per CTA (M = 4*56*56 = 12544 -> 98 m-tiles x n-tiles on <= one CTA per SM), 1x1 tiled A, fused residual
     a = _check(64, 56, 256, 1, 1, batch=4, residual=True, options=dict(opts, ws=1))
     b = _check(64, 56, 256, 1, 1, batch=4, residual=True, options=dict(opts, ws=-1))
     np.testing.assert_array_equal(a, b)
@@ -89,7 +89,7 @@ def test_persistent_warp_specialised_tactic(gpu, bn, stages, sps):
     a = _check(128, 14, 256, 3, 1, batch=3, options=dict(opts, ws=1))
     b = _check(128, 14, 256, 3, 1, batch=3, options=dict(opts, ws=-1))
     np.testing.assert_array_equal(a, b)
-    # forced small grid: every CTA walks several tiles, both TMEM accumulators and barrier phases wrap many times
+    # forced small grid: every CTA walks several tiles, both staging buffers and barrier phases wrap many times
     _check(256, 28, 256, 1, 2, batch=4, relu=False, options=dict(opts, ws=7))
 
 

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Pivot an `ncu --csv --metrics ...` log (one row per launch x metric) into one row per launch, labelled with the
 engine's launch names (gpurun_out/launch_names.txt written by tools/profile_forward.py).
-usage: python tools/condense_ncu.py raw.csv launch_names.txt > profiles/ncu_metrics_<tag>.csv"""
+usage: python tools/condense_ncu.py raw.csv launch_names.txt > ncu_metrics_<tag>.csv"""
 import csv
 import sys
 

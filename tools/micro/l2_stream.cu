@@ -1,15 +1,14 @@
-// Microbenchmark: what bandwidth does B200's memory system give UNIQUE streaming data of a given footprint?
+// Microbenchmark: what bandwidth does the GPU's memory system give UNIQUE streaming data of a given footprint?
 //
-// The conv stack at batch 8 keeps its activations in the 126 MB L2 (DRAM traffic is 0.57x the algorithmic bytes,
-// profiles/roofline_r1i.md), so the roofline of its memory-shaped layers (wide 1x1 convolutions with a residual: read A,
-// read residual, write output) is the L2 <-> SM bandwidth for data every CTA touches ONCE -- not the 30 TB/s that
-// l2_feed.cu reaches with a handful of tiles shared by all CTAs.  Three access mixes over a buffer of S MB, all SMs:
+// The conv stack at batch 8 keeps much of its activations in L2, so the roofline of its memory-shaped layers (wide 1x1 convolutions with a residual: read A,
+// read residual, write output) is the L2 <-> SM bandwidth for data every CTA touches ONCE -- not the rate a handful
+// of tiles shared by all CTAs reaches.  Three access mixes over a buffer of S MB, all SMs:
 //   read   : ld.global.v4 (or cp.async.bulk global->smem, `tma`) of the whole buffer, repeated
 //   write  : st.global.v4 of the whole buffer
 //   rrw    : read 2 streams + write 1 stream (the residual-conv mix), S split 2:1
 // Footprints from 8 MB (L2 resident, near+far partitions) to 512 MB (HBM).
 //
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o l2_stream.x l2_stream.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o l2_stream.x l2_stream.cu
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>

@@ -1,5 +1,5 @@
-// Microbenchmark: how fast can B200 retire chains of tiny dependent kernels, as a function of the number of
-// concurrent streams?  (Is a 58-kernel forward pass launch-bound?)   nvcc -arch=sm_100a -o launch_bound launch_bound.cu
+// Microbenchmark: how fast can the GPU retire chains of tiny dependent kernels, as a function of the number of
+// concurrent streams?  (Is a 58-kernel forward pass launch-bound?)   nvcc -arch=sm_90a -o launch_bound launch_bound.cu
 #include <cuda_runtime.h>
 #include <cstdio>
 #include <vector>
@@ -15,7 +15,7 @@ __global__ void tiny(float* p, int work) {
 int main() {
     const int chain = 58, iters = 200;
     for (int pdl = 0; pdl < 2; ++pdl)
-        for (int ctas : {1, 148, 296})
+        for (int ctas : {1, 132, 264})
             for (int ns : {1, 2, 4, 8}) {
                 std::vector<cudaStream_t> s(ns);
                 std::vector<cudaGraphExec_t> g(ns);

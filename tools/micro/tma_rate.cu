@@ -1,7 +1,6 @@
 // Microbenchmark: what limits the rate at which ONE SM can start TMA transfers -- the issuing thread, or the unit?
 //
-// The conv main loops run at ~460-510 cycles per 64-wide K-block whatever the tile width (l2_feed.cu), i.e. ~230 cycles per
-// TMA request.  This probe separates the candidates on L2-hot operands, without MMAs (stage release = plain arrive):
+// This probe separates the candidates on L2-hot operands, without MMAs (stage release = plain arrive):
 //   mode 0  one producer warp issues A (tensor tile 128x64, 16 KB) and B (bulk copy, BN x 128 B) of every K-block
 //   mode 1  A and B from two different warps (what the conv kernels do)
 //   mode 2  two producer warps alternate K-blocks (each issues A and B of its own blocks)
@@ -9,7 +8,7 @@
 //   mode 4  four producer warps alternate K-blocks
 // each for 1..4 co-resident CTAs per SM (2-stage rings).  Reported: cycles per K-block per CTA and K-blocks per 1000 cycles
 // per SM.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tma_rate.x tma_rate.cu -lcuda
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tma_rate.x tma_rate.cu -lcuda
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -179,7 +178,9 @@ static void run(int per_sm, int mode, void* dA, const uint8_t* dW, int m_tiles, 
         return;
     }
     Params p{iters, mode, m_tiles, k_blocks, dW, d_out};
-    const int grid = 148 * per_sm;
+    int sms = 0;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+    const int grid = sms * per_sm;
     cudaEvent_t e0, e1;
     cudaEventCreate(&e0);
     cudaEventCreate(&e1);

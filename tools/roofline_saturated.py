@@ -1,11 +1,11 @@
 #!/usr/bin/env python
 """Per-layer roofline in the SERVING regime, from the load-time tuner's dump (tools/gpu_tune_dump.py, B2_TUNE_VERBOSE):
 time per launch of each convolution's winning tactic with N concurrent copies of the layer, against BOTH roofs --
-  tensor:  2*M*N*K / 1429 TFLOP/s (MEASURED_PEAKS.json bf16_tflops_sustained)
+  tensor:  2*M*N*K / the sustained fp16 tensor peak (TFLOP/s, measured on the same GPU)
   memory:  algorithmic bytes (activations in + weights + residual + output, fp16) / the L2 bandwidth tools/micro/l2_stream.cu
-           measures for unique streaming data: reads 17.5 TB/s, writes 7.3 TB/s (time = reads/17.5 + writes/7.3)
+           measures for unique streaming data, separately for reads and writes (TB/s)
 and names the roof that binds each layer.  The sum of the winners is the forward pass's cost in that regime.
-usage: python tools/roofline_saturated.py profiles/tune_dump_r2_rn50_b8_4streams.log [step_us] > profiles/roofline_r2_saturated.md"""
+usage: python tools/roofline_saturated.py TUNE_DUMP PEAK_TFLOPS L2_READ_TBS L2_WRITE_TBS [step_us]"""
 import os
 import re
 import sys
@@ -13,7 +13,6 @@ import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from tensorrt_laboratory_b200 import graph, roofs, weights  # noqa: E402
 
-PEAK_TF = 1429.0
 BATCH = 8
 
 
@@ -25,10 +24,11 @@ def main():
         if m:
             best[m.group(1)] = dict(M=int(m.group(3)), N=int(m.group(4)), K=int(m.group(5)), bn=int(m.group(6)), st=int(m.group(7)),
                                     sps=int(m.group(9)), ws=int(m.group(10)), us=float(m.group(13)), streams=int(m.group(14)))
-    step_us = float(sys.argv[2]) if len(sys.argv) > 2 else None
+    peak_tf, l2_read, l2_write = float(sys.argv[2]), float(sys.argv[3]) * 1e12, float(sys.argv[4]) * 1e12
+    step_us = float(sys.argv[5]) if len(sys.argv) > 5 else None
     net = graph.resnet_caffe(50)
     low = graph.lower(net, weights.random_weights(net, 0))
-    floors = {f["name"]: f for f in roofs.conv_floors(low, BATCH, PEAK_TF)}
+    floors = {f["name"]: f for f in roofs.conv_floors(low, BATCH, peak_tf, l2_read, l2_write)}
     print("| layer | GEMM M×N×K | tactic | µs per launch (saturated) | TFLOP/s | tensor floor µs | bytes MB (rd / wr) | memory floor µs | binding roof | floor / measured |")
     print("|---|---|---|---|---|---|---|---|---|---|")
     tot = tot_tensor = tot_mem = tot_floor = flops_all = 0.0
@@ -44,7 +44,7 @@ def main():
               f"{f['read_bytes'] / 1e6:.1f} / {f['write_bytes'] / 1e6:.1f} | {f['memory_floor_us']:.2f} | {f['roof']} | {f['floor_us'] / b['us']:.2f} |")
     print()
     print(f"Sum of the {len(best)} winners: **{tot:.1f} µs** per forward pass" + (f" (measured step of the whole network: {step_us:.0f} µs)" if step_us else "")
-          + f"; {flops_all / tot * 1e-6:.0f} TFLOP/s = {flops_all / tot * 1e-6 / PEAK_TF:.2f} of the sustained tensor peak.")
+          + f"; {flops_all / tot * 1e-6:.0f} TFLOP/s = {flops_all / tot * 1e-6 / peak_tf:.2f} of the sustained tensor peak.")
     print(f"Floors: tensor {tot_tensor:.1f} µs, memory (L2 stream) {tot_mem:.1f} µs, per-layer max of the two {tot_floor:.1f} µs "
           f"= {tot_floor / tot:.2f} of the measured sum.")
     for roof, (us, fl) in by_roof.items():

@@ -2,7 +2,7 @@
 """Per-kernel roofline table from a condensed ncu metrics file (tools/condense_ncu.py) and the layer FLOPs of the graph:
 the three numbers SURVEY.md 8(d) asks for -- tensor-pipe % per kernel with the FLOP-weighted network average, achieved
 DRAM GB/s per kernel, and the end-to-end rate against the PCIe ceiling.
-usage: python tools/roofline_table.py profiles/ncu_metrics_r1i.csv [profiles/bench_r1i.json] > profiles/roofline_r1i.md"""
+usage: python tools/roofline_table.py ncu_metrics.csv [bench.json] > roofline.md"""
 import csv
 import json
 import os
@@ -11,7 +11,7 @@ import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from tensorrt_laboratory_b200 import graph, weights  # noqa: E402
 
-PEAK_TF = 1429.0     # MEASURED_PEAKS.json bf16_tflops_sustained on this pool's B200s
+PEAK_TF = float(os.environ.get("PEAK_TFLOPS", "989"))  # sustained tensor peak of the GPU; default: H100 SXM data sheet, dense fp16
 PEAK_HBM = 6587.7    # GB/s, measured copy bandwidth
 BATCH = 8
 

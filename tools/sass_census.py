@@ -1,6 +1,6 @@
-"""Opcode census of the shipped library: per kernel, how many tensor-core / TMEM / TMA instructions its SASS holds.
-    python tools/sass_census.py [tensorrt_laboratory_b200/libb200infer.so] > profiles/sass_census_rNN.txt
-UTCHMMA = tcgen05.mma kind::f16, UTCIMMA = kind::i8, LDTM = tcgen05.ld, UTMALDG / UTMASTG = TMA tensor load / store,
+"""Opcode census of the shipped library: per kernel, how many tensor-core / TMA instructions its SASS holds.
+    python tools/sass_census.py [tensorrt_laboratory_b200/libb200infer.so] > sass_census.txt
+HGMMA = wgmma f16, IGMMA = wgmma s8, WARPSYNC/WARPGROUP = warpgroup fences, UTMALDG / UTMASTG = TMA tensor load / store,
 UBLKCP = cp.async.bulk, HMMA = the legacy mma.sync path (must be absent)."""
 import collections
 import os
@@ -8,7 +8,7 @@ import re
 import subprocess
 import sys
 
-OPS = ["UTCHMMA", "UTCIMMA", "UTCQMMA", "LDTM", "STTM", "UTMALDG", "UTMASTG", "UBLKCP", "UTCBAR", "SYNCS", "HMMA", "IMMA", "ATOMG", "REDG", "MEMBAR"]
+OPS = ["HGMMA", "IGMMA", "WARPGROUP", "UTMALDG", "UTMASTG", "UBLKCP", "SYNCS", "HMMA", "IMMA", "ATOMG", "REDG", "MEMBAR"]
 
 
 def main():
