@@ -136,16 +136,11 @@ conv_i8_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
             const uint32_t b_addr = smem_u32(sB + s * B_STAGE);
             // all-zero 32-byte slices at the end of a tap's last channel block contribute nothing: not issued
             const int nj = (cur_cb == p.cblocks - 1) ? p.last_cb_mmas : 4;
-            wgmma_fence();
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {  // 4 x (K = 32 bytes) inside one 128-byte swizzle row
-                if (j < nj) {
-                    const uint64_t ad = make_wgmma_desc(a_addr + j * 32, 16, 1024, WG_SW128);
-                    const uint64_t bd = make_wgmma_desc(b_addr + j * 32, 16, 1024, WG_SW128);
-                    wgmma_i8<BN>(acc, ad, bd, (i > 0 || j > 0) ? 1u : 0u);
-                }
-            }
-            wgmma_commit();
+            wgmma_group_upto<4>(nj, [&](int j) {  // up to 4 x (K = 32 bytes) inside one 128-byte swizzle row
+                const uint64_t ad = make_wgmma_desc(a_addr + j * 32, 16, 1024, WG_SW128);
+                const uint64_t bd = make_wgmma_desc(b_addr + j * 32, 16, 1024, WG_SW128);
+                wgmma_i8<BN>(acc, ad, bd, (i > 0 || j > 0) ? 1u : 0u);
+            });
             if constexpr (STAGES == 1) {  // the only stage is refilled for step i+1: retire step i first
                 wgmma_wait<0>();
                 __syncwarp();

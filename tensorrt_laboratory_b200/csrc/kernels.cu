@@ -149,8 +149,7 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
         const int n = p.taps_phys - kb * TPS;
         return n > TPS ? TPS : n;
     };
-    const bool skip_mma = DBG && (p.dbg_mode & 1), skip_a = DBG && KB == 64 && (p.dbg_mode & 2),
-               skip_b = DBG && KB == 64 && (p.dbg_mode & 4);
+    const bool skip_a = DBG && KB == 64 && (p.dbg_mode & 2), skip_b = DBG && KB == 64 && (p.dbg_mode & 4);
     // step i of the pipeline covers K-blocks kb_begin + i*SPS ... ; `kb` below is always the FIRST K-block of a step
     auto stage_bytes = [&](int kb) -> uint32_t {
         if (KB == 64) {
@@ -316,42 +315,34 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
             if (dbg && i == 0 && cw == 0 && lane == 0) dbg[3] = clock64();
             const uint32_t a_addr = smem_u32(sA + s * Cfg::A_STAGE);
             const uint32_t b_addr = smem_u32(sB + s * Cfg::B_STAGE);
-            if (!skip_mma) {
-                wgmma_fence();
-                if (KB == 64) {
-                    const int ns = subs_in_step(i);
-#pragma unroll
-                    for (int u = 0; u < SPS; ++u) {
-                        if (u < ns) {
-#pragma unroll
-                            for (int j = 0; j < 4; ++j) {  // 4 x (K = 16) inside one 128-byte swizzle row
-                                const uint64_t ad = make_wgmma_desc(a_addr + u * Cfg::A_SUBBLK + wg * 8192 + j * 32, 16, 1024, WG_SW128);
-                                const uint64_t bd = make_wgmma_desc(b_addr + u * Cfg::B_SUBBLK + j * 32, 16, 1024, WG_SW128);
-                                wgmma_f16<BN>(acc, ad, bd, (i > 0 || u > 0 || j > 0) ? 1u : 0u);
-                            }
-                        }
-                    }
-                } else if (KB == 32) {
-                    // row-folded stem: each sub-tile is one filter row = 32 K-elements in 64-byte swizzled rows
-                    const int nt = sub_tiles(kb_begin + i);
-                    for (int t = 0; t < nt; ++t) {
-#pragma unroll
-                        for (int j = 0; j < 2; ++j) {
-                            const uint64_t ad = make_wgmma_desc(a_addr + t * A_SUB + wg * 4096 + j * 32, 16, 512, WG_SW64);
-                            const uint64_t bd = make_wgmma_desc(b_addr + t * B_SUB + j * 32, 16, 512, WG_SW64);
-                            wgmma_f16<BN>(acc, ad, bd, (i > 0 || t > 0 || j > 0) ? 1u : 0u);
-                        }
-                    }
-                } else {
-                    const int nt = sub_tiles(kb_begin + i);
-                    for (int j = 0; j < nt / 2; ++j) {  // one K=16 step = two 8-channel taps
-                        const uint64_t ad = make_wgmma_desc(a_addr + 2 * j * A_SUB + wg * 1024, A_SUB, 128, WG_NOSWZ);
-                        const uint64_t bd = make_wgmma_desc(b_addr + 2 * j * B_SUB, B_SUB, 128, WG_NOSWZ);
-                        wgmma_f16<BN>(acc, ad, bd, (i > 0 || j > 0) ? 1u : 0u);
-                    }
-                }
+            // one wgmma per K = 16; the number of them in a step is resolved outside the group (wgmma_group)
+            if constexpr (KB == 64) {
+                auto mma = [&](int t) {  // K-block u = t / 4, then 4 x (K = 16) inside its 128-byte swizzle row
+                    const int u = t >> 2, j = t & 3;
+                    const uint64_t ad = make_wgmma_desc(a_addr + u * Cfg::A_SUBBLK + wg * 8192 + j * 32, 16, 1024, WG_SW128);
+                    const uint64_t bd = make_wgmma_desc(b_addr + u * Cfg::B_SUBBLK + j * 32, 16, 1024, WG_SW128);
+                    wgmma_f16<BN>(acc, ad, bd, (i > 0 || t > 0) ? 1u : 0u);
+                };
+                if (SPS == 1 || subs_in_step(i) == SPS) wgmma_group<4 * SPS>(mma);
+                else wgmma_group<4>(mma);  // SPS = 2, odd K-block count: the last step holds one K-block
+            } else if constexpr (KB == 32) {
+                // row-folded stem: each sub-tile is one filter row = 32 K-elements in 64-byte swizzled rows
+                auto mma = [&](int t) {
+                    const int st = t >> 1, j = t & 1;
+                    const uint64_t ad = make_wgmma_desc(a_addr + st * A_SUB + wg * 4096 + j * 32, 16, 512, WG_SW64);
+                    const uint64_t bd = make_wgmma_desc(b_addr + st * B_SUB + j * 32, 16, 512, WG_SW64);
+                    wgmma_f16<BN>(acc, ad, bd, (i > 0 || t > 0) ? 1u : 0u);
+                };
+                if (sub_tiles(kb_begin + i) == TPS) wgmma_group<2 * TPS>(mma);
+                else wgmma_group<2>(mma);
+            } else {
+                auto mma = [&](int j) {  // one K=16 step = two 8-channel taps
+                    const uint64_t ad = make_wgmma_desc(a_addr + 2 * j * A_SUB + wg * 1024, A_SUB, 128, WG_NOSWZ);
+                    const uint64_t bd = make_wgmma_desc(b_addr + 2 * j * B_SUB, B_SUB, 128, WG_NOSWZ);
+                    wgmma_f16<BN>(acc, ad, bd, (i > 0 || j > 0) ? 1u : 0u);
+                };
+                wgmma_group_upto<TPS / 2>(sub_tiles(kb_begin + i) / 2, mma);  // taps_phys is even
             }
-            wgmma_commit();
             if constexpr (STAGES == 1) {  // the only stage is refilled for step i+1: retire step i first
                 wgmma_wait<0>();
                 release_stage(0);
@@ -676,20 +667,14 @@ conv_f16_tcgen05_ws(const __grid_constant__ CUtensorMap mapA, const __grid_const
                 if (rec) w_ops += clock64() - t1;
                 const uint32_t a_addr = smem_u32(sA + s * A_STAGE) + wg_off;
                 const uint32_t b_addr = smem_u32(sB + s * B_STAGE);
-                const int ns = subs_in_step(i);
-                wgmma_fence();
-#pragma unroll
-                for (int u = 0; u < SPS; ++u) {
-                    if (u < ns) {
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            const uint64_t ad = make_wgmma_desc(a_addr + u * A_SUBBLK + j * 32, 16, 1024, WG_SW128);
-                            const uint64_t bd = make_wgmma_desc(b_addr + u * B_SUBBLK + j * 32, 16, 1024, WG_SW128);
-                            wgmma_f16<BN>(acc, ad, bd, (i > 0 || u > 0 || j > 0) ? 1u : 0u);
-                        }
-                    }
-                }
-                wgmma_commit();
+                auto mma = [&](int t) {  // K-block u = t / 4, then 4 x (K = 16) inside its 128-byte swizzle row
+                    const int u = t >> 2, j = t & 3;
+                    const uint64_t ad = make_wgmma_desc(a_addr + u * A_SUBBLK + j * 32, 16, 1024, WG_SW128);
+                    const uint64_t bd = make_wgmma_desc(b_addr + u * B_SUBBLK + j * 32, 16, 1024, WG_SW128);
+                    wgmma_f16<BN>(acc, ad, bd, (i > 0 || t > 0) ? 1u : 0u);
+                };
+                if (SPS == 1 || subs_in_step(i) == SPS) wgmma_group<4 * SPS>(mma);
+                else wgmma_group<4>(mma);  // SPS = 2, odd K-block count: the last step holds one K-block
                 wgmma_wait<1>();  // step g-1 has retired: its stage goes back to the producers
                 __syncwarp();
                 if (i > 0 && lane == 0) mbar_arrive(&empty_bar[(g - 1) % STAGES]);
@@ -1061,9 +1046,10 @@ int launch_conv_f16_tcgen05(const ConvLaunch& L, cudaStream_t stream) {
     return static_cast<int>(cudaErrorInvalidValue);
 }
 
-// instantiated persistent (BN, STAGES, SPS) configurations
+// instantiated persistent (BN, STAGES, SPS) configurations; none with BN = 256: its 128 accumulators per thread plus the
+// double-buffered epilogue spill at 384 threads
 #define B2_FOR_EACH_CONV_WS(X) \
-    X(32, 4, 1) X(64, 2, 1) X(64, 4, 1) X(64, 2, 2) X(64, 4, 2) X(128, 2, 1) X(128, 4, 1) X(128, 2, 2) X(256, 2, 1)
+    X(32, 4, 1) X(64, 2, 1) X(64, 4, 1) X(64, 2, 2) X(64, 4, 2) X(128, 2, 1) X(128, 4, 1) X(128, 2, 2)
 
 template <int BN, int STAGES, int SPS>
 static int launch_one_ws(const ConvLaunch& L, cudaStream_t stream) {

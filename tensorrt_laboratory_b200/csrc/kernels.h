@@ -41,7 +41,7 @@ struct ConvArgs {
     int halo_rows;           // halo variant: output rows R per tile (tile = R rows x (Wo+2) padded columns of one image)
     int cn;                  // CTAs per cluster along N sharing one activation tile by TMA multicast (1 = no cluster)
     int tiles_m, tiles_n;    // persistent variant: output tile grid (128-row x BN-column tiles)
-    int dbg_mode;            // bottleneck isolation (debug only): bit0 skip MMA issue, bit1 skip A loads, bit2 skip B loads
+    int dbg_mode;            // bottleneck isolation (debug only): bit1 skip A loads, bit2 skip B loads
     long long* dbg;          // optional per-CTA phase timestamps (16 x int64 per CTA), nullptr in production
 };
 

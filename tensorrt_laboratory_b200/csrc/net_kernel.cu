@@ -302,15 +302,15 @@ __global__ void __launch_bounds__(kThreads, 1) net_f16_tcgen05(const NetArgs a) 
                 wait_t(&sm.full[s], ph, 1);
                 const uint32_t a_addr = smem_u32(sA + s * kASub) + wg_off;
                 const uint32_t b_addr = smem_u32(sB + s * kBSubMax);
-                wgmma_fence();
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    const uint64_t ad = make_wgmma_desc(a_addr + j * 32, 16, 1024, WG_SW128);
-                    const uint64_t bd = make_wgmma_desc(b_addr + j * 32, 16, 1024, WG_SW128);
-                    if (wide) wgmma_f16<128>(acc, ad, bd, (i > 0 || j > 0) ? 1u : 0u);
-                    else wgmma_f16<64>(*reinterpret_cast<float(*)[32]>(acc), ad, bd, (i > 0 || j > 0) ? 1u : 0u);
-                }
-                wgmma_commit();
+                // 4 x (K = 16) inside one 128-byte swizzle row; the tile width is chosen outside the wgmma group
+                auto ad = [&](int j) { return make_wgmma_desc(a_addr + j * 32, 16, 1024, WG_SW128); };
+                auto bd = [&](int j) { return make_wgmma_desc(b_addr + j * 32, 16, 1024, WG_SW128); };
+                if (wide)
+                    wgmma_group<4>([&](int j) { wgmma_f16<128>(acc, ad(j), bd(j), (i > 0 || j > 0) ? 1u : 0u); });
+                else
+                    wgmma_group<4>([&](int j) {
+                        wgmma_f16<64>(*reinterpret_cast<float(*)[32]>(acc), ad(j), bd(j), (i > 0 || j > 0) ? 1u : 0u);
+                    });
                 wgmma_wait<1>();  // step i-1 has retired: its stage goes back to the producers
                 __syncwarp();
                 if (i > 0 && lane == 0) mbar_arrive(&sm.empty[prev_s]);

@@ -97,4 +97,27 @@ __device__ __forceinline__ void wgmma_i8(int32_t (&d)[N / 2], uint64_t a, uint64
     else wgmma_i8_n256(d, a, b, accumulate);
 }
 
+// One wgmma group: fence, mma(0) ... mma(N-1), commit.  No wgmma between fence and commit may sit under a run-time
+// branch: ptxas then inserts a warpgroup arrive/wait around EVERY wgmma of the kernel (warning C7520), so each K = 16 step
+// waits for the previous one and nothing stays in flight across commit / wait_group.  Run-time choices between groups of
+// different length are made outside the group (wgmma_group_upto).
+template <int N, class F>
+__device__ __forceinline__ void wgmma_group(F&& mma) {
+    wgmma_fence();
+#pragma unroll
+    for (int t = 0; t < N; ++t) mma(t);
+    wgmma_commit();
+}
+// wgmma_group<n> for a run-time n in [1, MAX]
+template <int MAX, class F>
+__device__ __forceinline__ void wgmma_group_upto(int n, F&& mma) {
+    if constexpr (MAX > 1) {
+        if (n < MAX) {
+            wgmma_group_upto<MAX - 1>(n, mma);
+            return;
+        }
+    }
+    wgmma_group<MAX>(mma);
+}
+
 }  // namespace b2k
