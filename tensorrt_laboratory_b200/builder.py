@@ -18,13 +18,39 @@ PREC_FP32, PREC_FP16, PREC_INT8 = 0, 1, 2
 OP_INPUT_CAST, OP_CONV, OP_MAXPOOL, OP_AVGPOOL, OP_FC, OP_SOFTMAX, OP_OUTPUT_CAST, OP_QUANTIZE = range(8)
 T_ACT, T_VEC = 0, 1
 MAGIC = b"B2ENGINE"
-VERSION = 1
+VERSION = 1           # plans without grouped convolutions: 176-byte op records
+VERSION_GROUPED = 2   # a plan with at least one grouped convolution: 192-byte op records (+ groups)
 
 _HEADER = struct.Struct("<8sIIIIIIQQ64s16x")
 _TENSOR = struct.Struct("<64sIIIIIif4x")  # ... binding, scale (INT8 tensors: real value = q * scale; 0 = fp16 / fp32 tensor)
 _OP = struct.Struct("<64sIiiiiIIIIIIIIIIIQQQQIIII")
+_OP_V2 = struct.Struct("<64sIiiiiIIIIIIIIIIIQQQQIIIII12x")  # version 2: _OP + groups + 12 reserved bytes
 _BINDING = struct.Struct("<64sIIiI8i16x")
-assert _HEADER.size == 128 and _TENSOR.size == 96 and _OP.size == 176 and _BINDING.size == 128
+assert _HEADER.size == 128 and _TENSOR.size == 96 and _OP.size == 176 and _OP_V2.size == 192 and _BINDING.size == 128
+
+
+def grouped_tc_span(cin: int, cout: int, groups: int, cin_phys: int, cout_phys: int) -> int:
+    """K elements per filter tap in the weight row of a grouped fp16 convolution that runs on the tensor cores, or 0 when
+    its geometry runs on the SIMT convolution.  Tensor-core geometries have Cin/g == Cout/g == cpg with cpg | 64 (a group
+    lies inside one 64-channel block: span 64) or 64 | cpg (span cpg)."""
+    if groups <= 1 or cin != cout or cin_phys != cout_phys or cin_phys % 64 or cout_phys % 32:
+        return 0
+    cpg = cin // groups
+    if 64 % cpg and cpg % 64:
+        return 0
+    return max(cpg, 64)
+
+
+def expand_grouped_weights(W: np.ndarray, groups: int, span: int, cout_phys: int) -> np.ndarray:
+    """Block-diagonal weight rows of a tensor-core grouped convolution: W [Cout, taps, cpg] -> [Cout_phys, taps, span].
+    Row o is read against the `span` input channels starting at channel (o // span) * span, so its cpg real weights sit
+    at columns g*cpg - (o // span)*span ... (g = o's group) and every other column is zero."""
+    cout, taps, cpg = W.shape
+    out = np.zeros((cout_phys, taps, span), dtype=W.dtype)
+    o = np.arange(cout)
+    col = (o // cpg) * cpg - (o // span) * span
+    out[o[:, None, None], np.arange(taps)[None, :, None], (col[:, None] + np.arange(cpg)[None, :])[:, None, :]] = W
+    return out
 
 
 def _roundup(v: int, m: int) -> int:
@@ -170,7 +196,7 @@ def build_plan(lowered: dict, precision: int = PREC_FP16, max_batch: int = 8,
     s2d_op = None
     if (precision_fp == PREC_FP16 and stem_s2d and len(readers) == 1 and readers[0]["type"] == G.OP_CONV
             and readers[0]["stride"] == 2 and cin <= 4 and win % 2 == 0 and lowered["input"] not in outputs
-            and readers[0]["k"] >= 3):
+            and readers[0]["k"] >= 3 and readers[0].get("groups", 1) == 1):
         s2d_op = readers[0]
         _, _, s2d_lo, s2d_hi = stem_s2d_transform(s2d_op["W"], s2d_op["k"], s2d_op["pad"], win)
         # the horizontal padding is made PHYSICAL (zero pixels written by the cast), so the conv has pad_w = 0 and its
@@ -200,6 +226,33 @@ def build_plan(lowered: dict, precision: int = PREC_FP16, max_batch: int = 8,
             rec.update(type=OP_CONV, k=k, stride=op["stride"], pad=op["pad"], relu=int(op["relu"]) | 2 | 4,
                        cin=op["cin"], cout=op["cout"], cin_phys=cin_phys, cout_phys=cout_phys, taps=taps, taps_phys=taps,
                        w_off=w_off, w_bytes=w_bytes, b_off=b_off, b_bytes=b_bytes)
+            if op["residual"] is not None:
+                rec["res"] = add_tensor(op["residual"])
+        elif t == G.OP_CONV and op.get("groups", 1) > 1:
+            if "W" not in op:
+                raise ValueError(f"conv {op['name']}: lowered graph carries no weights")
+            # tensor-core geometry: packed block-diagonal rows [Cout_phys][taps][span]; otherwise (SIMT, fp32 engines)
+            # row-major [Cout_phys][taps][Cin/groups]
+            groups = op["groups"]
+            cin_phys, cout_phys = tensors[ti]["c_phys"], tensors[to]["c_phys"]
+            k = op["k"]
+            taps, cpg_in = k * k, op["cin"] // groups
+            Wg = op["W"].reshape(op["cout"], taps, cpg_in)
+            span = grouped_tc_span(op["cin"], op["cout"], groups, cin_phys, cout_phys)
+            packed = precision_fp == PREC_FP16 and pack_weights and span > 0
+            if packed:
+                Wx = expand_grouped_weights(Wg.astype(np.float16), groups, span, cout_phys)
+                w_off, w_bytes = add_payload(pack_weights_sw128(Wx.reshape(cout_phys, taps * span)))
+            else:
+                W = np.zeros((cout_phys, taps, cpg_in), dtype=np.float32)
+                W[:op["cout"]] = Wg
+                w_off, w_bytes = add_payload(W.astype(wdtype))
+            bias = np.zeros(cout_phys, dtype=np.float32)
+            bias[:op["cout"]] = op["bias"]
+            b_off, b_bytes = add_payload(bias)
+            rec.update(type=OP_CONV, k=k, stride=op["stride"], pad=op["pad"], relu=int(op["relu"]) | (2 if packed else 0),
+                       cin=op["cin"], cout=op["cout"], cin_phys=cin_phys, cout_phys=cout_phys, taps=taps, taps_phys=taps,
+                       w_off=w_off, w_bytes=w_bytes, b_off=b_off, b_bytes=b_bytes, groups=groups)
             if op["residual"] is not None:
                 rec["res"] = add_tensor(op["residual"])
         elif t == G.OP_CONV:
@@ -265,26 +318,38 @@ def build_plan(lowered: dict, precision: int = PREC_FP16, max_batch: int = 8,
             bindings.append(dict(name=oname, is_input=0, dtype=0, tensor=ti, dims=[trec["c"], trec["h"], trec["w"]]))
             ops.append(dict(name="cast:" + oname, type=OP_OUTPUT_CAST, inp=ti, res=-1, out=-1, binding=bidx))
 
-    tables = _HEADER.size + len(tensors) * _TENSOR.size + len(ops) * _OP.size + len(bindings) * _BINDING.size
+    # version 1 unless a convolution is grouped: every plan without one stays byte-identical to what older builders wrote
+    grouped = any(o.get("groups", 1) > 1 for o in ops)
+    op_struct = _OP_V2 if grouped else _OP
+    tables = _HEADER.size + len(tensors) * _TENSOR.size + len(ops) * op_struct.size + len(bindings) * _BINDING.size
     payload_offset = _roundup(tables, 256)
     blob = bytearray()
-    blob += _HEADER.pack(MAGIC, VERSION, precision, max_batch, len(tensors), len(ops), len(bindings),
-                         payload_offset, len(payload), _name(name or lowered["name"]))
+    blob += _HEADER.pack(MAGIC, VERSION_GROUPED if grouped else VERSION, precision, max_batch, len(tensors), len(ops),
+                         len(bindings), payload_offset, len(payload), _name(name or lowered["name"]))
     for t in tensors:
         blob += _TENSOR.pack(_name(t["name"]), t["kind"], t["h"], t["w"], t["c"], t["c_phys"], t["binding"], t.get("scale", 0.0))
     for o in ops:
-        blob += _OP.pack(_name(o["name"]), o["type"], o["inp"], o["res"], o["out"], o["binding"],
-                         o.get("k", 0), o.get("stride", 0), o.get("pad", 0), o.get("relu", 0), o.get("ceil_mode", 0),
-                         o.get("cin", 0), o.get("cout", 0), o.get("cin_phys", 0), o.get("cout_phys", 0),
-                         o.get("taps", 0), o.get("taps_phys", 0),
-                         o.get("w_off", 0), o.get("w_bytes", 0), o.get("b_off", 0), o.get("b_bytes", 0),
-                         o.get("kw", 0), o.get("stride_w", 0), o.get("pad_w_lo", 0), o.get("pad_w_hi", 0))
+        fields = (_name(o["name"]), o["type"], o["inp"], o["res"], o["out"], o["binding"],
+                  o.get("k", 0), o.get("stride", 0), o.get("pad", 0), o.get("relu", 0), o.get("ceil_mode", 0),
+                  o.get("cin", 0), o.get("cout", 0), o.get("cin_phys", 0), o.get("cout_phys", 0),
+                  o.get("taps", 0), o.get("taps_phys", 0),
+                  o.get("w_off", 0), o.get("w_bytes", 0), o.get("b_off", 0), o.get("b_bytes", 0),
+                  o.get("kw", 0), o.get("stride_w", 0), o.get("pad_w_lo", 0), o.get("pad_w_hi", 0))
+        blob += op_struct.pack(*fields, o.get("groups", 1)) if grouped else op_struct.pack(*fields)
     for b in bindings:
         dims = list(b["dims"]) + [0] * (8 - len(b["dims"]))
         blob += _BINDING.pack(_name(b["name"]), b["is_input"], b["dtype"], b["tensor"], len(b["dims"]), *dims)
     blob += b"\0" * (payload_offset - len(blob))
     blob += payload
     return bytes(blob)
+
+
+def build_resnext_plan(depth: int = 50, precision: int = PREC_FP16, max_batch: int = 8, seed: int = 0,
+                       input_dtype: str = "f32", groups: int = 32, width_per_group: int = 4) -> bytes:
+    """Convenience: generated ResNeXt (:func:`graph.resnext_caffe`) + deterministic weights -> plan (fp16 or fp32)."""
+    from . import weights as Wt
+    net = G.resnext_caffe(depth, groups, width_per_group)
+    return build_plan(G.lower(net, Wt.random_weights(net, seed)), precision, max_batch, input_dtype=input_dtype)
 
 
 def build_resnet_plan(depth: int = 50, precision: int = PREC_FP16, max_batch: int = 8, seed: int = 0,
@@ -301,22 +366,26 @@ def build_resnet_plan(depth: int = 50, precision: int = PREC_FP16, max_batch: in
 
 
 def single_conv_net(cin: int, h: int, w: int, cout: int, k: int, stride: int, pad: int, relu: bool = True,
-                    residual: bool = False, bias: bool = True) -> dict:
+                    residual: bool = False, bias: bool = True, group: int = 1) -> dict:
     """Raw layer list of a one-convolution network (kernel-level parity tests go through the public ABI).
-    With ``residual`` the net is  y = relu(conv_b(x) + conv_a(x))  so the fused add path is exercised."""
+    With ``residual`` the net is  y = relu(conv_b(x) + conv_a(x))  so the fused add path is exercised; ``group`` applies
+    to conv_b (the fused one) only."""
     L = []
     if residual:
         L.append(dict(name="short", type="Convolution", bottoms=["data"], tops=["short"], num_output=cout,
                       kernel_size=k, pad=pad, stride=stride, bias_term=bias))
     L.append(dict(name="conv", type="Convolution", bottoms=["data"], tops=["conv"], num_output=cout,
                   kernel_size=k, pad=pad, stride=stride, bias_term=bias))
+    if group != 1:
+        L[-1]["group"] = group
     top = "conv"
     if residual:
         L.append(dict(name="sum", type="Eltwise", bottoms=["short", "conv"], tops=["sum"], operation="SUM"))
         top = "sum"
     if relu:
         L.append(dict(name="relu", type="ReLU", bottoms=[top], tops=[top]))
-    return {"name": f"conv{k}x{k}s{stride}_{cin}x{h}x{w}_{cout}", "input": "data", "input_dims": [1, cin, h, w],
+    gtag = f"g{group}" if group != 1 else ""
+    return {"name": f"conv{k}x{k}s{stride}{gtag}_{cin}x{h}x{w}_{cout}", "input": "data", "input_dims": [1, cin, h, w],
             "layers": L}
 
 

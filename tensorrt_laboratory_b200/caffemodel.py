@@ -10,7 +10,7 @@ learned parameters are needed, so the wire format is decoded by hand (no protobu
                     legacy .num/.channels/.height/.width = 1..4
 
 Blob conventions restated from Caffe's layers:
-    Convolution / InnerProduct   blobs[0] = weights [Cout, Cin, kh, kw] / [Cout, K], blobs[1] = bias (if bias_term)
+    Convolution / InnerProduct   blobs[0] = weights [Cout, Cin/group, kh, kw] / [Cout, K], blobs[1] = bias (if bias_term)
     BatchNorm                    blobs[0] = mean * f, blobs[1] = variance * f, blobs[2] = [f]  (moving-average factor;
                                  the statistics are blobs / f, and 0 when f == 0)
     Scale                        blobs[0] = gamma, blobs[1] = beta (if bias_term)
@@ -26,6 +26,7 @@ from typing import Dict, List
 
 import numpy as np
 
+from .graph import infer_shapes
 from .onnx_lite import _fields, _packed_varints
 
 
@@ -110,6 +111,10 @@ def load_caffemodel(path_or_bytes, net: dict) -> Dict[str, dict]:
                 W = W.reshape(L["num_output"], -1)
             elif W.ndim != 4 or W.shape[2] != L["kernel_size"] or W.shape[3] != L["kernel_size"]:
                 raise ValueError(f"{name}: weight blob {W.shape} does not match kernel_size {L['kernel_size']}")
+            elif L.get("group", 1) != 1:  # a grouped blob is [Cout, Cin/group, k, k]
+                cin = infer_shapes(net)[L["bottoms"][0]][0]
+                if W.shape[1] * L["group"] != cin:
+                    raise ValueError(f"{name}: weight blob {W.shape} does not match {cin} input channels in {L['group']} groups")
             rec = {"W": np.ascontiguousarray(W, np.float32)}
             if need == 2:
                 rec["b"] = blobs[1].reshape(-1).astype(np.float32)

@@ -103,6 +103,7 @@ struct Tensor {
 
 struct Op {
     b2plan::OpRec r;
+    int groups = 1;  // convs: OpRecV2::groups (version-1 plans: 1)
     std::string name;
     // >= 0: this op's only consumer is the residual input of op `side_join`, and nothing in between depends on it (the
     // shortcut convolution of a ResNet "a" block): it may run on a forked stream, concurrently with the ops up to there
@@ -115,7 +116,12 @@ struct Op {
     int ph() const { return int(r.pad_); }
     int pw_lo() const { return int(r.kw ? r.pad_w_lo : r.pad_); }
     int pw_hi() const { return int(r.kw ? r.pad_w_hi : r.pad_); }
-    double algo_k() const { return r.ceil_mode ? double(r.ceil_mode) : double(r.cin) * r.taps; }
+    double algo_k() const { return r.ceil_mode ? double(r.ceil_mode) : double(r.cin / uint32_t(groups)) * r.taps; }
+    // grouped convolution with the packed block-diagonal weight layout (plan_format.h): input channels per N tile, the
+    // K extent of one tap; 0 = dense, or grouped on the SIMT convolution
+    int group_span() const {
+        return groups > 1 && (r.relu & 2) ? std::max(int(r.cin) / groups, 64) : 0;
+    }
 };
 
 struct Binding {
@@ -323,10 +329,12 @@ int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** pa
     Header h;
     memcpy(&h, base, sizeof h);
     if (memcmp(h.magic, kMagic, 8) != 0) return fail(B2_EINVAL, "plan: bad magic (not a B2ENGINE blob)");
-    if (h.version != kVersion) return fail(B2_EINVAL, "plan: version %u, this library reads %u", h.version, kVersion);
+    if (h.version != kVersion && h.version != kVersionGrouped)
+        return fail(B2_EINVAL, "plan: version %u, this library reads %u and %u", h.version, kVersion, kVersionGrouped);
     if (h.precision > 2) return fail(B2_EINVAL, "plan: unknown precision %u", h.precision);
     if (h.max_batch == 0 || h.max_batch > 4096) return fail(B2_EINVAL, "plan: bad max_batch %u", h.max_batch);
-    const size_t tbl = sizeof(Header) + size_t(h.n_tensors) * sizeof(TensorRec) + size_t(h.n_ops) * sizeof(OpRec) +
+    const size_t op_rec_size = h.version == kVersionGrouped ? sizeof(OpRecV2) : sizeof(OpRec);
+    const size_t tbl = sizeof(Header) + size_t(h.n_tensors) * sizeof(TensorRec) + size_t(h.n_ops) * op_rec_size +
                        size_t(h.n_bindings) * sizeof(BindingRec);
     // (overflow-safe: a > n || b > n - a instead of a + b > n)
     if (tbl > nbytes || h.payload_offset < tbl || h.payload_offset > nbytes || h.payload_bytes > nbytes - h.payload_offset)
@@ -361,9 +369,16 @@ int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** pa
         e->tensors.push_back(t);
     }
     auto tensor_ok = [&](int idx, bool optional) { return (optional && idx == -1) || (idx >= 0 && idx < int(h.n_tensors)); };
-    for (uint32_t i = 0; i < h.n_ops; ++i, p += sizeof(OpRec)) {
+    for (uint32_t i = 0; i < h.n_ops; ++i, p += op_rec_size) {
         Op op;
         memcpy(&op.r, p, sizeof(OpRec));
+        if (h.version == kVersionGrouped) {
+            OpRecV2 r2;
+            memcpy(&r2, p, sizeof r2);
+            if (r2.v1.type == OP_CONV && (r2.groups == 0 || r2.groups > 65536))
+                return fail(B2_EINVAL, "plan: conv %s has %u groups", fixed_str(r2.v1.name, 64).c_str(), r2.groups);
+            if (r2.v1.type == OP_CONV) op.groups = int(r2.groups);
+        }
         op.name = fixed_str(op.r.name, 64);
         const OpRec& r = op.r;
         if (r.type > OP_QUANTIZE) return fail(B2_EINVAL, "plan: op %s has unknown type %u", op.name.c_str(), r.type);
@@ -398,7 +413,26 @@ int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** pa
             if (r.k == 0 || r.stride == 0 || int(r.taps) != op.kh() * op.kw() || r.taps_phys < r.taps || op.sw() == 0)
                 return fail(B2_EINVAL, "plan: conv %s has bad geometry", op.name.c_str());
             const bool i8 = (r.relu & 4) != 0;
-            if (i8) {
+            if (op.groups > 1) {  // layouts: plan_format.h (OpRecV2)
+                const uint32_t g = uint32_t(op.groups);
+                if (i8) return fail(B2_EINVAL, "plan: conv %s: INT8 grouped convolution is not supported", op.name.c_str());
+                if (r.cin % g || r.cout % g)
+                    return fail(B2_EINVAL, "plan: conv %s: %u groups do not divide %u -> %u channels", op.name.c_str(), g, r.cin, r.cout);
+                const uint32_t cpg = r.cin / g;
+                size_t want;
+                if (r.relu & 2) {
+                    if (h.precision == B2_PREC_FP32 || r.cin != r.cout || r.cin_phys != r.cout_phys || r.cin_phys % 64 ||
+                        r.cout_phys % 32 || (64 % cpg && cpg % 64) || r.taps_phys != r.taps)
+                        return fail(B2_EINVAL, "plan: conv %s: packed grouped weights need Cin/g == Cout/g dividing or a multiple of 64",
+                                    op.name.c_str());
+                    want = size_t(r.cout_phys) * r.taps * std::max<uint32_t>(cpg, 64) * 2;
+                } else {
+                    want = size_t(r.cout_phys) * r.taps_phys * cpg * elt;
+                }
+                if (r.w_bytes != want || r.b_bytes != size_t(r.cout_phys) * 4)
+                    return fail(B2_EINVAL, "plan: grouped conv %s weight size mismatch (%llu bytes, layout needs %zu)", op.name.c_str(),
+                                (unsigned long long)r.w_bytes, want);
+            } else if (i8) {
                 const Tensor& qi = e->tensors[r.in];
                 const Tensor& qo = e->tensors[r.out];
                 if (h.precision != B2_PREC_INT8 || !(qi.scale > 0.f) || !(qo.scale > 0.f) || (r.res >= 0 && !(e->tensors[r.res].scale > 0.f)) ||
@@ -605,17 +639,19 @@ static int g_sms = 132;
 // Analytic cost model (microseconds) over the instantiated (N tile, pipeline depth, split-K) space.  The
 // constants are rough figures: ~70 KB/us of L2->SM bandwidth per SM, ~1 us TMA round trip, ~5 TB/s of
 // aggregate L2 bandwidth, ~2 us of fixed per-CTA cost.  It only has to rank configurations sensibly.
-ConvConfig pick_conv_config(int M, int cout_phys, int kblocks, int kb, bool residual, const b2_context* c, bool honor_forced) {
+// group_span > 0 (grouped convolution): only N tiles that divide it, and no split-K.
+ConvConfig pick_conv_config(int M, int cout_phys, int kblocks, int kb, bool residual, const b2_context* c, bool honor_forced,
+                            int group_span = 0) {
     const int m_tiles = (M + 127) / 128;
     ConvConfig best{0, 0, 1, 1e30};
     const int bns[4] = {256, 128, 64, 32};
     const int stgs[4] = {1, 2, 4, 8};
     for (int bn : bns) {
-        if (cout_phys % bn) continue;
+        if (cout_phys % bn || (group_span && group_span % bn)) continue;
         if (honor_forced && c->force_bn && bn != c->force_bn) continue;
         const int tiles = m_tiles * (cout_phys / bn);
         for (int splits = 1; splits <= 8; ++splits) {
-            if (c->force_splits ? splits != c->force_splits : splits != 1) continue;  // split-K is opt-in (measured slower)
+            if (c->force_splits && !group_span ? splits != c->force_splits : splits != 1) continue;  // split-K is opt-in (measured slower)
             if (splits > 1 && (kb != 64 || kblocks / splits < 4 || tiles * splits > 160 || tiles > kMaxSplitTiles ||
                                size_t(tiles) * splits * 128 * bn * 4 > kSplitWorkspaceBytes))
                 continue;
@@ -660,18 +696,20 @@ int conv_kb(const b2_context* c, const Op& op) {
 }
 int conv_num_kblocks(const b2_context* c, const Op& op) {
     const b2plan::OpRec& r = op.r;
+    if (op.group_span()) return int(r.taps) * (op.group_span() / 64);  // one tap x the tile's own channel blocks
     if (r.cin_phys % 64 == 0) return int(r.taps) * (int(r.cin_phys) / 64);
     if (conv_is_row_folded(c, op)) return (op.kh() + 1) / 2;  // two filter rows (2 x 32 K) per 64-wide k-block
     return (int(r.taps_phys) + 7) / 8;
 }
 
 // 3x3 / stride 1 / pad 1 on 64-channel blocks with packed weights and no fused residual: the halo kernel applies.
-// Returns the rows per tile R (0 = not applicable).
+// Returns the rows per tile R (0 = not applicable).  Never for a grouped convolution (its tiles read channel blocks
+// that depend on the N tile).
 int conv_halo_rows(const b2_context* c, const Op& op) {
     const b2plan::OpRec& r = op.r;
     const Tensor& ti = c->e->tensors[r.in];
     const Tensor& to = c->e->tensors[r.out];
-    if (r.cin_phys % 64 || r.cout_phys % 64 || op.kh() != 3 || op.kw() != 3 || op.sh() != 1 || op.sw() != 1 || op.ph() != 1 ||
+    if (op.groups > 1 || r.cin_phys % 64 || r.cout_phys % 64 || op.kh() != 3 || op.kw() != 3 || op.sh() != 1 || op.sw() != 1 || op.ph() != 1 ||
         op.pw_lo() != 1 || op.pw_hi() != 1 || r.res >= 0 || !(r.relu & 2) || c->no_pack || ti.h != to.h || ti.w != to.w)
         return 0;
     const int wp = int(to.w) + 2;
@@ -690,6 +728,11 @@ int make_conv_launch(b2_context* c, const Op& op, int batch, const ConvConfig& c
     const int M = batch * int(to.h) * int(to.w);
     const bool kb64 = r.cin_phys % 64 == 0;
     const bool fold = conv_is_row_folded(c, op);
+    const int span = op.group_span();
+    // grouped: the one-tile-per-CTA kernel only, and N tiles that stay inside one span of input channels
+    if (op.groups > 1 && (!span || cfg.ws || cfg.splits > 1 || cfg.cn > 1 || cfg.halo || span % cfg.bn))
+        return fail(B2_EINVAL, "conv %s: grouped convolutions run one tile per CTA with an N tile dividing %d (bn=%d ws=%d splits=%d cn=%d halo=%d)",
+                    op.name.c_str(), span, cfg.bn, cfg.ws, cfg.splits, cfg.cn, cfg.halo);
     b2k::ConvLaunch& cl = *out;
     memset(&cl, 0, sizeof cl);
     cl.kb = conv_kb(c, op);
@@ -719,7 +762,8 @@ int make_conv_launch(b2_context* c, const Op& op, int batch, const ConvConfig& c
     a.taps = fold ? op.kh() : int(r.taps);            // folded: one "tap" = one filter row of kw*8 K-elements
     a.taps_phys = fold ? op.kh() : int(r.taps_phys);
     a.kw = fold ? 1 : op.kw();
-    a.cblocks = kb64 ? int(r.cin_phys) / 64 : 1;
+    a.cblocks = span ? span / 64 : kb64 ? int(r.cin_phys) / 64 : 1;
+    a.group_span = span;
     a.num_kblocks = nkb;
     a.HoWo = int(to.h * to.w);
     a.Wo = int(to.w);
@@ -864,21 +908,24 @@ int autotune_conv(b2_context* c, const Op& op, int batch, int fixed_splits, int 
     const int reps = std::max(1, env_int("B2_TUNE_REPS", 2));      // measurements per candidate (the quietest counts)
     const int m_tiles = (M + 127) / 128;
     const int split_cands[4] = {1, 2, 4, 8};
+    // grouped convolution: the one-tile-per-CTA kernel without split-K or clusters, N tiles dividing the group span
+    const int span = op.group_span();
     std::vector<ConvConfig> candidates;
     for (int bn : bns) {
-        if (int(r.cout_phys) % bn) continue;
+        if (int(r.cout_phys) % bn || (span && span % bn)) continue;
         const int tiles = m_tiles * (int(r.cout_phys) / bn);
         for (int ws = 0; ws <= 1; ++ws)
         for (int sp : split_cands)
         for (int sps = 1; sps <= 2; ++sps)
         for (int st : stgs) {
             if (fixed_splits > 0 && sp != fixed_splits) continue;
+            if (span && (ws || sp > 1)) continue;
             if (ws) {  // persistent warp-specialised tactic: 64-wide K, packed weights, no split-K
                 if (c->force_ws < 0 || kbsz != 64 || !(r.relu & 2) || sp != 1) continue;
                 if (!b2k::conv_ws_config_exists(bn, st, sps) || b2k::conv_ws_smem(bn, st, sps, r.res >= 0) > 227 * 1024) continue;
                 if (sps == 2 && nkb < 4) continue;
             } else {
-            if (c->force_ws > 0 && kbsz == 64 && (r.relu & 2)) continue;
+            if (c->force_ws > 0 && kbsz == 64 && (r.relu & 2) && !span) continue;
             if (!b2k::conv_config_exists(bn, kbsz, st, sps)) continue;
             if (b2k::conv_smem_bytes(bn, st, r.res >= 0, sps) > 227 * 1024) continue;
             }
@@ -895,12 +942,12 @@ int autotune_conv(b2_context* c, const Op& op, int batch, int fixed_splits, int 
                            (sp - 1) * kpc >= nkb ||
                            size_t(tiles) * sp * 128 * bn * 4 > kSplitWorkspaceBytes))
                 continue;  // split-K only where the plain grid leaves SMs idle
-            const bool cn_forced_here = c->force_cn > 1 && kbsz == 64 && (int(r.cout_phys) / bn) % c->force_cn == 0 &&
+            const bool cn_forced_here = c->force_cn > 1 && kbsz == 64 && !span && (int(r.cout_phys) / bn) % c->force_cn == 0 &&
                                         b2k::conv_cluster_config_exists(bn, st, sps, c->force_cn);
             if (!cn_forced_here) candidates.push_back(ConvConfig{bn, st, sp, 0.0, sps, 0, 1});
             // clusters along N that multicast the activation tile: never won a timing (the L2 read is shared but
             // every SM still ingests the whole tile, and the cluster barriers cost latency) -> tried only on request
-            if (kbsz == 64 && c->force_cn > 0)
+            if (kbsz == 64 && c->force_cn > 0 && !span)
                 for (int cn = 2; cn <= 4; cn *= 2)
                     if ((int(r.cout_phys) / bn) % cn == 0 && (!c->force_cn || cn == c->force_cn) &&
                         b2k::conv_cluster_config_exists(bn, st, sps, cn))
@@ -1031,6 +1078,11 @@ void tune_cache_append(const b2_engine* e, int op, int batch, const ConvConfig& 
 bool tactic_applies(const b2_context* c, const Op& op, int batch, const ConvConfig& cfg) {
     const b2plan::OpRec& r = op.r;
     if (cfg.bn <= 0 || int(r.cout_phys) % cfg.bn) return false;
+    if (op.groups > 1) {  // grouped: one tile per CTA, no split-K / cluster / halo, N tile inside the group span
+        const int span = op.group_span();
+        return span && span % cfg.bn == 0 && !cfg.halo && !cfg.ws && cfg.splits <= 1 && cfg.cn <= 1 &&
+               b2k::conv_config_exists(cfg.bn, 64, cfg.stages, cfg.sps);
+    }
     const int kbsz = conv_kb(c, op);
     if (cfg.halo) return conv_halo_rows(c, op) > 0 && b2k::conv_halo_config_exists(cfg.bn);
     if (cfg.ws) return kbsz == 64 && b2k::conv_ws_config_exists(cfg.bn, cfg.stages, cfg.sps);
@@ -1146,6 +1198,7 @@ int tune_engine_batch(b2_context* c, int batch) {
         }
         const bool kb64 = r.cin_phys % 64 == 0, kb8 = r.cin_phys == 8;
         if (!((kb64 || kb8) && r.cout_phys % 32 == 0 && (kb64 || r.taps_phys % 2 == 0))) continue;
+        if (op.groups > 1 && !op.group_span()) continue;  // grouped on the SIMT convolution: nothing to tune
         {
             std::lock_guard<std::mutex> lock(e->tune_mutex);
             if (e->tuned.count({int(i), batch})) continue;
@@ -1153,6 +1206,7 @@ int tune_engine_batch(b2_context* c, int batch) {
         const Tensor& to = e->tensors[r.out];
         const int kbsz = conv_kb(c, op), nkb = conv_num_kblocks(c, op);
         const bool side = op.side_join >= 0;
+        const bool no_split = side || op.groups > 1;  // side branches and grouped convolutions never split K
         // Split-K is the ONE tactic that changes the fp32 summation order (every other one -- N tile, ring depth, halo,
         // persistent -- adds the same products in the same order), so letting the timing pick it would make the BITS of a
         // model depend on the load-time measurement of that process: seen once as a 4e-3 relative difference between a tuned
@@ -1160,13 +1214,14 @@ int tune_engine_batch(b2_context* c, int batch) {
         // candidate was 40 % behind), so the tuner leaves it alone unless
         // B2_TUNE_SPLITK=1; `splits` stays available as an explicit option.
         static const bool tune_splitk = env_int("B2_TUNE_SPLITK", 0) != 0;
-        int splits = (side || !tune_splitk) ? 1 : 0;
-        if (batch != e->max_batch && !side && tune_splitk) {
+        int splits = (no_split || !tune_splitk) ? 1 : 0;
+        if (batch != e->max_batch && !no_split && tune_splitk) {
             std::lock_guard<std::mutex> lock(e->tune_mutex);
             auto it = e->tuned.find({int(i), e->max_batch});
             if (it != e->tuned.end()) splits = it->second.splits;
         }
-        ConvConfig cfg = pick_conv_config(batch * int(to.h) * int(to.w), int(r.cout_phys), nkb, kbsz, r.res >= 0, c, false);
+        ConvConfig cfg = pick_conv_config(batch * int(to.h) * int(to.w), int(r.cout_phys), nkb, kbsz, r.res >= 0, c, false,
+                                          op.group_span());
         int rc = autotune_conv(c, op, batch, splits, -1, &cfg);
         if (rc) return rc;
         std::lock_guard<std::mutex> lock(e->tune_mutex);
@@ -1426,8 +1481,10 @@ int build_plan(b2_context* c, int batch, Plan** out) {
                 L.bytes = double(batch) * (ti.item_bytes + to.item_bytes * (r.res >= 0 ? 2 : 1)) + double(r.w_bytes);
                 const bool kb64 = r.cin_phys % 64 == 0;
                 const bool kb8 = r.cin_phys == 8;
+                // grouped: the tensor cores take the packed block-diagonal layout; any other grouped geometry is SIMT
+                const int span = op.group_span();
                 const bool tc_ok = half && !c->force_simt && (kb64 || kb8) && r.cout_phys % 32 == 0 &&
-                                   (kb64 || r.taps_phys % 2 == 0);
+                                   (kb64 || r.taps_phys % 2 == 0) && (op.groups == 1 || span > 0);
                 if (r.relu & 4) {  // INT8 tensor path
                     L.kind = L_CONV_I8;
                     // one tactic, by rule: the 128-wide N tile with a ring no deeper than the K loop, shallow enough (2-3
@@ -1454,26 +1511,29 @@ int build_plan(b2_context* c, int batch, Plan** out) {
                     L.kind = L_CONV_TC;
                     const int kbsz = conv_kb(c, op);
                     const int nkb = conv_num_kblocks(c, op);
-                    ConvConfig cfg = pick_conv_config(M, int(r.cout_phys), nkb, kbsz, r.res >= 0, c, true);
+                    ConvConfig cfg = pick_conv_config(M, int(r.cout_phys), nkb, kbsz, r.res >= 0, c, true, span);
                     if (cfg.bn == 0)  // a forced tile that does not divide this layer: fall back to the model
-                        cfg = pick_conv_config(M, int(r.cout_phys), nkb, kbsz, r.res >= 0, c, false);
+                        cfg = pick_conv_config(M, int(r.cout_phys), nkb, kbsz, r.res >= 0, c, false, span);
                     if (cfg.bn == 0) return fail(B2_EINVAL, "conv %s: no kernel configuration", op.name.c_str());
                     if (c->force_sps == 2 && b2k::conv_config_exists(cfg.bn, kbsz, cfg.stages, 2) &&
                         b2k::conv_smem_bytes(cfg.bn, cfg.stages, r.res >= 0, 2) <= 227 * 1024)
                         cfg.sps = 2;
-                    if (c->force_ws > 0 && kbsz == 64 && (r.relu & 2) && cfg.splits == 1 &&
+                    // (the persistent, halo and cluster tactics never take a grouped convolution)
+                    if (c->force_ws > 0 && kbsz == 64 && (r.relu & 2) && cfg.splits == 1 && !span &&
                         b2k::conv_ws_config_exists(cfg.bn, cfg.stages, cfg.sps) &&
                         b2k::conv_ws_smem(cfg.bn, cfg.stages, cfg.sps, r.res >= 0) <= 227 * 1024)
                         cfg.ws = std::min(((M + 127) / 128) * (int(r.cout_phys) / cfg.bn), c->force_ws > 1 ? c->force_ws : g_sms);
                     if (c->force_halo > 0 && conv_halo_rows(c, op) && b2k::conv_halo_config_exists(cfg.bn) && cfg.splits == 1 &&
                         int(r.cin_phys) / 64 <= 8 && b2k::conv_halo_smem(cfg.bn, int(to.w), conv_halo_rows(c, op), int(r.cin_phys) / 64) <= 227 * 1024)
                         cfg.halo = 1, cfg.ws = 0, cfg.cn = 1;
-                    if (c->force_cn > 1 && kbsz == 64 && cfg.ws == 0 && !cfg.halo && (int(r.cout_phys) / cfg.bn) % c->force_cn == 0) cfg.cn = c->force_cn;
+                    if (c->force_cn > 1 && kbsz == 64 && cfg.ws == 0 && !cfg.halo && !span && (int(r.cout_phys) / cfg.bn) % c->force_cn == 0)
+                        cfg.cn = c->force_cn;
                     const bool forced = c->force_bn || c->force_stages || c->force_splits || c->force_sps;
                     const int op_index = int(&op - &e->ops[0]);
-                    // member of a persistent-kernel run: 64-channel K blocks, packed weights, 64 | Cout; no tactic to tune
+                    // member of a persistent-kernel run: 64-channel K blocks, packed weights, 64 | Cout; no tactic to tune.
+                    // A grouped layer is never a member: it ends a run
                     const bool net_ok = c->net && !forced && kbsz == 64 && (r.relu & 2) && !c->no_pack && r.cout_phys % 64 == 0 &&
-                                        c->force_ws <= 0 && c->force_cn <= 0 && c->force_halo <= 0 && !c->force_im2col;
+                                        c->force_ws <= 0 && c->force_cn <= 0 && c->force_halo <= 0 && !c->force_im2col && op.groups == 1;
                     if (net_ok) {
                         int bn = (r.cout_phys % 128 == 0) ? 128 : 64;
                         if (c->net_bn == 64) bn = 64;
@@ -1507,6 +1567,8 @@ int build_plan(b2_context* c, int batch, Plan** out) {
                     a.stride_h = op.sh(), a.stride_w = op.sw(), a.pad_h = op.ph(), a.pad_w = op.pw_lo();
                     a.relu = int(r.relu & 1);
                     a.w_packed = int((r.relu >> 1) & 1);
+                    a.groups = op.groups;
+                    a.wk_tap = op.groups == 1 ? int(r.cin_phys) : span ? span : int(r.cin) / op.groups;
                 }
                 break;
             }
@@ -2202,7 +2264,7 @@ int b2_engine_refine_tactics(b2_engine* e, int streams, int passes, double* gain
             // of SMs; splitting K shortens the link and puts more SMs on it.  The per-layer tuner rejects it (more total
             // work), the chain-bound whole-network rate is where it can pay.  (The split factor fixes the fp32 summation
             // order; it is chosen here, at max batch, and shared by every batch size.)
-            if (env_int("B2_TUNE_SPLITK", 0) != 0 && !(op.side_join >= 0) && cur.splits == 1 && !cur.halo) {  // opt-in: changes bits
+            if (env_int("B2_TUNE_SPLITK", 0) != 0 && !(op.side_join >= 0) && op.groups == 1 && cur.splits == 1 && !cur.halo) {  // opt-in: changes bits
                 const int m_tiles = (batch * int(e->tensors[r.out].h * e->tensors[r.out].w) + 127) / 128;
                 for (int sp : {2, 4}) {
                     const int tiles = m_tiles * (int(r.cout_phys) / cur.bn);
@@ -2225,6 +2287,7 @@ int b2_engine_refine_tactics(b2_engine* e, int streams, int passes, double* gain
                         if (st * sps > nkb + 1 && st > 1) continue;  // a ring deeper than the K loop only costs shared memory
                         if (sps == 2 && nkb < 4) continue;
                         if (bn == cur.bn && st == cur.stages && sps == cur.sps && !cur.halo) continue;
+                        if (op.groups > 1 && !tactic_applies(ctx[0].c, op, batch, ConvConfig{bn, st, 1, 0.0, sps, 0, 1})) continue;
                         cands.push_back(ConvConfig{bn, st, 1, 0.0, sps, 0, 1});
                     }
                 if (conv_halo_rows(ctx[0].c, op) && b2k::conv_halo_config_exists(bn) && int(r.cin_phys) / 64 <= 8 && !(cur.halo && cur.bn == bn) &&
@@ -2442,7 +2505,8 @@ const char* b2_context_launch_name(b2_context* c, int batch, int i) {
              (L->conv.cn > 1 ? " cn=" + std::to_string(L->conv.cn) : std::string()) + (L->conv.halo ? " halo" : "") +
              (L->conv.args.a_mode == b2k::A_TILED ? " tiled" : " im2col") +
              " grid=" + std::to_string(L->conv.grid_n) + "x" + std::to_string(L->conv.grid_m) + "x" +
-             std::to_string(L->conv.args.splits) + " kblk=" + std::to_string(L->conv.args.num_kblocks);
+             std::to_string(L->conv.args.splits) + " kblk=" + std::to_string(L->conv.args.num_kblocks) +
+             (L->conv.args.group_span ? " span=" + std::to_string(L->conv.args.group_span) : std::string());
     if (L->kind == L_CONV_I8)
         s += " bn=" + std::to_string(L->i8.bn) + " st=" + std::to_string(L->i8.stages) + (L->i8.args.a_mode == b2k::A_TILED ? " tiled" : " im2col") + " grid=" +
              std::to_string(L->i8.grid_n) + "x" + std::to_string(L->i8.grid_m) + " kblk=" + std::to_string(L->i8.args.num_kblocks);

@@ -201,11 +201,15 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
             // K-block -> (filter row r, filter column sx, channel block cb), advanced incrementally: integer division
             // by a run-time value costs ~100 cycles and this thread's issue rate paces the whole main loop
             int cur_cb = 0, cur_r = 0, cur_sx = 0;
+            // grouped convolution: the tile's output channels read only the group_span input channels from block cb0 on
+            // (the weights outside a channel's own group are zero); dense layers have cb0 = 0
+            int cb0 = 0;
             if (KB == 64) {
                 const int tap0 = kb_begin / p.cblocks;
                 cur_cb = kb_begin - tap0 * p.cblocks;
                 cur_r = tap0 / p.kw;
                 cur_sx = tap0 - cur_r * p.kw;
+                if (p.group_span) cb0 = (n0 / p.group_span) * (p.group_span >> 6);
             }
             auto load_a = [&](int kb, int s) {  // must be called with consecutive kb starting at kb_begin
                 if (skip_a) return;
@@ -213,17 +217,18 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
                 if (KB == 64) {
                     const int ns = subs_in_step((kb - kb_begin) / SPS);
                     for (int u = 0; u < ns; ++u) {
+                        const int c0 = (cb0 + cur_cb) * 64;
                         if (cn > 1) {
                             if (a_tiled) {
-                                tma_load_2d_mc(&mapA, &full_bar[s], a_dst + u * Cfg::A_SUBBLK + slice_off, cur_cb * 64, ms, cmask);
+                                tma_load_2d_mc(&mapA, &full_bar[s], a_dst + u * Cfg::A_SUBBLK + slice_off, c0, ms, cmask);
                             } else {
-                                tma_load_im2col_4d_mc(&mapA, &full_bar[s], a_dst + u * Cfg::A_SUBBLK + slice_off, cur_cb * 64, base_w,
+                                tma_load_im2col_4d_mc(&mapA, &full_bar[s], a_dst + u * Cfg::A_SUBBLK + slice_off, c0, base_w,
                                                       base_h, img0, static_cast<uint16_t>(cur_sx), static_cast<uint16_t>(cur_r), cmask);
                             }
                         } else if (a_tiled) {
-                            tma_load_2d(&mapA, &full_bar[s], a_dst + u * Cfg::A_SUBBLK, cur_cb * 64, m0);
+                            tma_load_2d(&mapA, &full_bar[s], a_dst + u * Cfg::A_SUBBLK, c0, m0);
                         } else {
-                            tma_load_im2col_4d(&mapA, &full_bar[s], a_dst + u * Cfg::A_SUBBLK, cur_cb * 64, base_w, base_h, img0,
+                            tma_load_im2col_4d(&mapA, &full_bar[s], a_dst + u * Cfg::A_SUBBLK, c0, base_w, base_h, img0,
                                                static_cast<uint16_t>(cur_sx), static_cast<uint16_t>(cur_r));
                         }
                         if (++cur_cb == p.cblocks) {
@@ -1131,7 +1136,7 @@ __device__ __forceinline__ float from_f<float>(float v) { return v; }
 template <>
 __device__ __forceinline__ __half from_f<__half>(float v) { return __float2half_rn(v); }
 
-// direct convolution, one thread per output element (co fastest)
+// direct convolution, one thread per output element (co fastest); grouped convolutions of any geometry
 template <typename T>
 __global__ void conv_simt_kernel(SimtConvArgs a) {
     pdl_launch_dependents();
@@ -1151,8 +1156,12 @@ __global__ void conv_simt_kernel(SimtConvArgs a) {
         out[idx] = from_f<T>(0.0f);
         return;
     }
-    const T* in = reinterpret_cast<const T*>(a.in);
-    const T* w = reinterpret_cast<const T*>(a.w) + static_cast<size_t>(co) * a.taps_phys * a.Cin_phys;
+    // grouped: this channel reads the cin_g input channels from ci0; its weights start at K offset kofs inside each tap
+    const int cin_g = a.Cin / a.groups;
+    const int ci0 = co / (a.Cout / a.groups) * cin_g;
+    const int kofs = (a.groups > 1 && a.w_packed) ? ci0 - co / a.wk_tap * a.wk_tap : 0;
+    const T* in = reinterpret_cast<const T*>(a.in) + ci0;
+    const T* w = reinterpret_cast<const T*>(a.w) + static_cast<size_t>(co) * a.taps_phys * a.wk_tap;
     acc_t acc = 0;
     for (int r = 0; r < a.kh; ++r) {
         const int hi = ho * a.stride_h - a.pad_h + r;
@@ -1161,10 +1170,10 @@ __global__ void conv_simt_kernel(SimtConvArgs a) {
             const int wi = wo * a.stride_w - a.pad_w + s;
             if (wi < 0 || wi >= a.W) continue;
             const T* ip = in + ((static_cast<size_t>(n) * a.H + hi) * a.W + wi) * a.Cin_phys;
-            const T* wp = w + static_cast<size_t>(r * a.kw + s) * a.Cin_phys;
+            const T* wp = w + static_cast<size_t>(r * a.kw + s) * a.wk_tap;
             if (a.w_packed) {
-                const size_t kbase = static_cast<size_t>(r * a.kw + s) * a.Cin_phys;
-                for (int c = 0; c < a.Cin; ++c) {
+                const size_t kbase = static_cast<size_t>(r * a.kw + s) * a.wk_tap + kofs;
+                for (int c = 0; c < cin_g; ++c) {
                     const size_t k = kbase + c;
                     const size_t kk = k & 63;
                     const size_t off = (((k >> 6) * static_cast<size_t>(a.Cout_phys >> 5) + static_cast<size_t>(co >> 5)) << 11) + (static_cast<size_t>(co & 31) << 6) +
@@ -1172,7 +1181,7 @@ __global__ void conv_simt_kernel(SimtConvArgs a) {
                     acc += static_cast<acc_t>(to_f(ip[c])) * static_cast<acc_t>(to_f(reinterpret_cast<const T*>(a.w)[off]));
                 }
             } else {
-                for (int c = 0; c < a.Cin; ++c)
+                for (int c = 0; c < cin_g; ++c)
                     acc += static_cast<acc_t>(to_f(ip[c])) * static_cast<acc_t>(to_f(wp[c]));
             }
         }

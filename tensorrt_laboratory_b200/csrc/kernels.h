@@ -43,6 +43,8 @@ struct ConvArgs {
     int tiles_m, tiles_n;    // persistent variant: output tile grid (128-row x BN-column tiles)
     int dbg_mode;            // bottleneck isolation (debug only): bit1 skip A loads, bit2 skip B loads
     long long* dbg;          // optional per-CTA phase timestamps (16 x int64 per CTA), nullptr in production
+    int group_span;          // grouped convolution (KB==64, one tile per CTA): input channels an N tile reads, max(Cin/g, 64),
+                             // starting at channel (n0 / group_span) * group_span; cblocks = group_span / 64.  0 = dense
 };
 
 struct ConvLaunch {
@@ -170,6 +172,9 @@ struct SimtConvArgs {
     int N, H, W, Cin, Cin_phys, Ho, Wo, Cout, Cout_phys;
     int kh, kw, taps_phys, stride_h, stride_w, pad_h, pad_w, relu;
     int w_packed;          // 1: `w` uses the pre-swizzled block layout (fp16 engines)
+    int groups;            // >= 1; output channel o reads input channels [g * Cin/groups, (g+1) * Cin/groups), g = o / (Cout/groups)
+    int wk_tap;            // K elements per filter tap in a weight row: Cin_phys (dense), Cin/groups (grouped, row-major) or the
+                           // span of a packed grouped layout (plan_format.h), whose row o starts at input channel (o / span) * span
 };
 int launch_conv_simt(const SimtConvArgs& a, bool half_storage, cudaStream_t stream);
 

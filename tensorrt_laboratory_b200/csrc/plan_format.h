@@ -8,7 +8,10 @@
 namespace b2plan {
 
 constexpr char kMagic[8] = {'B', '2', 'E', 'N', 'G', 'I', 'N', 'E'};
+// Version 1: OpRec (176 bytes).  Version 2: OpRecV2 (192 bytes: OpRec + groups), written only when a convolution is
+// grouped, so every plan without one stays version 1.  The engine reads both.
 constexpr uint32_t kVersion = 1;
+constexpr uint32_t kVersionGrouped = 2;
 
 enum OpType : uint32_t {
     OP_INPUT_CAST = 0,   // fp32 NCHW binding -> NHWC activation tensor
@@ -71,6 +74,20 @@ struct OpRec {  // 176 bytes
     // pairs into channels [dw*4 + c]).
     uint32_t kw, stride_w, pad_w_lo, pad_w_hi;
 };
+// Version-2 op record.  `groups` (convs; 1 = dense, 0 is invalid) splits Cin and Cout into `groups` equal groups;
+// output channel o reads only the Cin/groups input channels of its group.  Weight layouts of a grouped convolution:
+//   relu bit 1 set (fp16, tensor-core geometry: Cin/g == Cout/g == cpg with cpg | 64 or 64 | cpg; span = max(cpg, 64)):
+//     builder.pack_weights_sw128 of the block-diagonal matrix [Cout_phys][taps][span].  Row o is multiplied with the
+//     `span` input channels starting at (o / span) * span; its cpg real weights sit at columns
+//     (o / cpg) * cpg - (o / span) * span ... and the other columns are zero.  w_bytes = Cout_phys * taps * span * 2.
+//   relu bit 1 clear (every other geometry, and fp32 engines): row-major [Cout_phys][taps_phys][Cin/groups];
+//     w_bytes = Cout_phys * taps_phys * (Cin / groups) * element size.
+// INT8 grouped convolutions do not exist.
+struct OpRecV2 {  // 192 bytes
+    OpRec v1;
+    uint32_t groups;
+    uint8_t reserved[12];
+};
 struct BindingRec {  // 128 bytes
     char name[64];
     uint32_t is_input;
@@ -86,6 +103,7 @@ static_assert(sizeof(Header) == 128, "Header size");
 static_assert(sizeof(TacticRec) == 40, "TacticRec size");
 static_assert(sizeof(TensorRec) == 96, "TensorRec size");
 static_assert(sizeof(OpRec) == 176, "OpRec size");
+static_assert(sizeof(OpRecV2) == 192, "OpRecV2 size");
 static_assert(sizeof(BindingRec) == 128, "BindingRec size");
 
 }  // namespace b2plan

@@ -127,6 +127,8 @@ def parse_prototxt(text: str) -> dict:
                 stride=_one(p, "stride", 1),
                 bias_term=_one(p, "bias_term", True),
             )
+            if "group" in p:  # absent = 1; read everywhere as L.get("group", 1)
+                rec["group"] = _one(p, "group")
         elif ltype == "BatchNorm":
             p = _one(L, "batch_norm_param", {})
             rec.update(use_global_stats=_one(p, "use_global_stats", True), eps=_one(p, "eps", 1e-5))
@@ -179,11 +181,29 @@ def resnet_caffe(depth: int = 50) -> dict:
     """Generate the raw layer list of ``models/ResNet-{50,152}-deploy.prototxt`` (reference)."""
     if depth not in _RESNET_BLOCKS:
         raise ValueError(f"unsupported ResNet depth {depth}")
+    return _bottleneck_net(f"ResNet-{depth}", depth, [64 << si for si in range(4)], group=1)
+
+
+def resnext_caffe(depth: int = 50, groups: int = 32, width_per_group: int = 4) -> dict:
+    """ResNeXt (Xie et al., "Aggregated Residual Transformations for Deep Neural Networks") in the Caffe conventions of
+    :func:`resnet_caffe`: same stem, block names and BatchNorm + Scale pairs.  The bottleneck's 3x3 convolution has
+    ``groups`` groups of ``width_per_group * 2**stage`` channels (128, 256, 512, 1024 for 32x4d) and carries the stride, as
+    does ``branch1``; the 1x1 ``branch2a`` always has stride 1."""
+    if depth not in _RESNET_BLOCKS:
+        raise ValueError(f"unsupported ResNeXt depth {depth}")
+    widths = [groups * width_per_group << si for si in range(4)]
+    return _bottleneck_net(f"ResNeXt-{depth}-{groups}x{width_per_group}d", depth, widths, group=groups)
+
+
+def _bottleneck_net(name: str, depth: int, widths: List[int], group: int) -> dict:
+    """Bottleneck network with stage widths ``widths``; ``group`` > 1 makes the 3x3 grouped and moves the stride onto it."""
     L: List[dict] = []
 
-    def conv(name, bottom, nout, k, pad, stride, bias):
+    def conv(name, bottom, nout, k, pad, stride, bias, g=1):
         L.append(dict(name=name, type="Convolution", bottoms=[bottom], tops=[name], num_output=nout,
                       kernel_size=k, pad=pad, stride=stride, bias_term=bias))
+        if g != 1:
+            L[-1]["group"] = g
 
     def bn_scale(suffix, blob):
         L.append(dict(name="bn" + suffix, type="BatchNorm", bottoms=[blob], tops=[blob],
@@ -201,21 +221,22 @@ def resnet_caffe(depth: int = 50) -> dict:
     prev = "pool1"
     for si, count in enumerate(_RESNET_BLOCKS[depth]):
         stage = si + 2
-        mid = 64 << si
-        out = mid * 4
+        mid = widths[si]
+        out = 256 << si
         for bi, bname in enumerate(_block_names(count, stage, depth)):
             tag = f"{stage}{bname}"
             stride = 2 if (bi == 0 and stage > 2) else 1
+            s_1x1, s_3x3 = (stride, 1) if group == 1 else (1, stride)
             if bi == 0:
                 conv(f"res{tag}_branch1", prev, out, 1, 0, stride, False)
                 bn_scale(f"{tag}_branch1", f"res{tag}_branch1")
                 shortcut = f"res{tag}_branch1"
             else:
                 shortcut = prev
-            conv(f"res{tag}_branch2a", prev, mid, 1, 0, stride, False)
+            conv(f"res{tag}_branch2a", prev, mid, 1, 0, s_1x1, False)
             bn_scale(f"{tag}_branch2a", f"res{tag}_branch2a")
             relu(f"res{tag}_branch2a_relu", f"res{tag}_branch2a")
-            conv(f"res{tag}_branch2b", f"res{tag}_branch2a", mid, 3, 1, 1, False)
+            conv(f"res{tag}_branch2b", f"res{tag}_branch2a", mid, 3, 1, s_3x3, False, group)
             bn_scale(f"{tag}_branch2b", f"res{tag}_branch2b")
             relu(f"res{tag}_branch2b_relu", f"res{tag}_branch2b")
             conv(f"res{tag}_branch2c", f"res{tag}_branch2b", out, 1, 0, 1, False)
@@ -229,7 +250,7 @@ def resnet_caffe(depth: int = 50) -> dict:
     L.append(dict(name="fc1000", type="InnerProduct", bottoms=["pool5"], tops=["fc1000"],
                   num_output=1000, bias_term=True))
     L.append(dict(name="prob", type="Softmax", bottoms=["fc1000"], tops=["prob"]))
-    return {"name": f"ResNet-{depth}", "input": "data", "input_dims": [1, 3, 224, 224], "layers": L}
+    return {"name": name, "input": "data", "input_dims": [1, 3, 224, 224], "layers": L}
 
 
 # --------------------------------------------------------------------------------------------------
@@ -312,11 +333,14 @@ def lower(net: dict, weights: Optional[dict] = None) -> dict:
         name = L["name"]
         if t == "Convolution":
             cin = tensors[L["bottoms"][0]][0]
+            groups = L.get("group", 1)
+            if groups < 1 or cin % groups or L["num_output"] % groups:
+                raise ValueError(f"Convolution {name}: {groups} groups do not divide {cin} -> {L['num_output']} channels")
             op = dict(type=OP_CONV, name=name, input=L["bottoms"][0], output=L["tops"][0], residual=None,
                       cin=cin, cout=L["num_output"], k=L["kernel_size"], stride=L["stride"], pad=L["pad"],
-                      relu=False)
+                      relu=False, groups=groups)
             if weights is not None:
-                w = np.asarray(weights[name]["W"], dtype=np.float64)  # [Cout, Cin, k, k]
+                w = np.asarray(weights[name]["W"], dtype=np.float64)  # [Cout, Cin/groups, k, k]
                 b = (np.asarray(weights[name]["b"], dtype=np.float64) if L["bias_term"]
                      else np.zeros(L["num_output"], dtype=np.float64))
                 op["_w"], op["_b"] = w, b
@@ -421,12 +445,13 @@ def lower(net: dict, weights: Optional[dict] = None) -> dict:
 
 
 def conv_flops(lowered: dict) -> int:
-    """2*MAC over conv + fc ops, per image (the algorithmic FLOP count used by the roofline)."""
+    """2*MAC over conv + fc ops, per image (the algorithmic FLOP count used by the roofline).  A grouped convolution
+    counts its Cin/groups inputs per output channel, not the zero blocks the tensor-core path multiplies."""
     total = 0
     for op in lowered["ops"]:
         if op["type"] == OP_CONV:
             c, h, w = lowered["tensors"][op["output"]]
-            total += 2 * h * w * op["cout"] * op["cin"] * op["k"] * op["k"]
+            total += 2 * h * w * op["cout"] * (op["cin"] // op.get("groups", 1)) * op["k"] * op["k"]
         elif op["type"] == OP_FC:
             total += 2 * op["cin"] * op["cout"]
     return total

@@ -5,7 +5,7 @@ reference ``examples/ONNX/resnet50/build.py`` hands an ONNX ResNet-50 to ``trtex
 + raw weights the prototxt front-end produces, so everything downstream (lowering / folding, plan builder, oracle) is
 shared.  Supported operators -- the ones ONNX-zoo ResNets and the reference's MNIST model use:
 
-  Conv (group 1, dilation 1, symmetric pads or SAME_UPPER that resolves symmetric) / BatchNormalization / Relu /
+  Conv (any group, dilation 1, symmetric pads or SAME_UPPER that resolves symmetric) / BatchNormalization / Relu /
   Add (two activations -> Eltwise SUM; activation + constant -> bias) / MaxPool (pads, ceil_mode) / AveragePool /
   GlobalAveragePool / Flatten / Reshape (activation flatten or constant reshape) / Gemm (alpha = beta = 1, transB 0|1) /
   MatMul / Softmax.
@@ -79,11 +79,15 @@ def import_onnx(model: dict, input_dims: Optional[List[int]] = None, name: str =
             consts[out] = np.asarray(attrs["value"])
         elif op == "Conv":
             W = np.asarray(const_of(ins[1]), np.float32)
-            if int(attrs.get("group", 1)) != 1 or any(int(d) != 1 for d in attrs.get("dilations", [1, 1])):
-                raise ValueError("onnx import: grouped / dilated Conv is not supported")
+            if any(int(d) != 1 for d in attrs.get("dilations", [1, 1])):
+                raise ValueError("onnx import: dilated Conv is not supported")
+            group = int(attrs.get("group", 1))
             kh, kw = int(W.shape[2]), int(W.shape[3])
             st = [int(s) for s in attrs.get("strides", [1, 1])]
             c, h, w = shapes[ins[0]]
+            if group < 1 or c % group or W.shape[0] % group or W.shape[1] != c // group:
+                raise ValueError(f"onnx import: Conv {node['name'] or out}: weight {tuple(W.shape)} does not fit {c} input "
+                                 f"channels in {group} groups")
             if attrs.get("auto_pad") in ("SAME_UPPER", "SAME_LOWER"):
                 ph, pw = onnx_lite.same_upper_pads(h, kh, st[0]), onnx_lite.same_upper_pads(w, kw, st[1])
                 pads = [ph[0], pw[0], ph[1], pw[1]]
@@ -95,6 +99,8 @@ def import_onnx(model: dict, input_dims: Optional[List[int]] = None, name: str =
             bias = len(ins) > 2
             layers.append(dict(name=lname, type="Convolution", bottoms=[ins[0]], tops=[out], num_output=int(W.shape[0]),
                                kernel_size=kh, pad=pads[0], stride=st[0], bias_term=True))
+            if group != 1:
+                layers[-1]["group"] = group
             weights[lname] = {"W": W, "b": np.asarray(const_of(ins[2]), np.float32).reshape(-1) if bias else np.zeros(W.shape[0], np.float32)}
             shapes[out] = (int(W.shape[0]), conv_out(h, kh, pads[0], pads[2], st[0]), conv_out(w, kw, pads[1], pads[3], st[1]))
         elif op == "BatchNormalization":
@@ -259,7 +265,9 @@ def export_onnx(net: dict, weights: Dict[str, dict], opset: int = 11) -> bytes:
                 ins.append(name + "_b")
                 inits.append(_tensor(name + "_b", np.asarray(weights[name]["b"], np.float32)))
             k, p, s = L["kernel_size"], L["pad"], L["stride"]
-            nodes.append(_node("Conv", ins, [fresh(L["tops"][0])], name, kernel_shape=[k, k], pads=[p, p, p, p], strides=[s, s]))
+            extra = {"group": L["group"]} if L.get("group", 1) != 1 else {}
+            nodes.append(_node("Conv", ins, [fresh(L["tops"][0])], name, kernel_shape=[k, k], pads=[p, p, p, p], strides=[s, s],
+                               **extra))
         elif ty == "BatchNorm":
             nxt = layers[i + 1] if i + 1 < len(layers) else None
             c = len(weights[name]["mean"])

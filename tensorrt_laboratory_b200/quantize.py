@@ -82,7 +82,12 @@ def quantize_lowered(lowered: dict, calib_inputs: np.ndarray, amax: Optional[Dic
     """-> a lowered graph whose eligible convolutions carry INT8 parameters (``Wq`` int8 OHWI, ``m`` / ``b`` fp32 per
     output channel, ``r`` fp32 or None, ``in_scale`` / ``out_scale``), with ``quantize`` ops inserted where an INT8
     convolution reads an fp16 tensor, ``in_scale`` on an average pool that reads INT8, and ``tensor_scales`` {name: s}
-    for every INT8 tensor.  ``lowered`` itself is not modified."""
+    for every INT8 tensor.  ``lowered`` itself is not modified.  Grouped convolutions have no INT8 path: a graph that
+    contains one is rejected before calibration."""
+    for op in lowered["ops"]:
+        if op["type"] == G.OP_CONV and op.get("groups", 1) != 1:
+            raise ValueError(f"conv {op['name']}: INT8 grouped convolution is not supported ({op['groups']} groups); "
+                             "build this model in fp16 or fp32")
     amax = amax or calibrate(lowered, calib_inputs)
     q = copy.copy(lowered)
     q["tensors"] = dict(lowered["tensors"])

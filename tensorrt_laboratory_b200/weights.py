@@ -6,7 +6,8 @@ are DEFINED here, reproducibly, and consumed identically by the CPU oracle and t
 (SURVEY.md section 8(d)):
 
   ``numpy.random.default_rng(seed)``, layers visited in prototxt order;
-  Convolution / InnerProduct  W ~ N(0, sqrt(2/(Cin*k*k)))  (He), bias ~ N(0, 0.01) where present;
+  Convolution / InnerProduct  W ~ N(0, sqrt(2/(Cin*k*k)))  (He; Cin/group for a grouped convolution, whose W is
+              [Cout, Cin/group, k, k]), bias ~ N(0, 0.01) where present;
   BatchNorm   mean ~ N(0, 0.1), var ~ U(0.5, 1.5);
   Scale       gamma ~ U(0.8, 1.2)  (U(0.1, 0.3) on the last BN of a bottleneck, ``*_branch2c``, so the
               residual stream stays bounded in fp16), beta ~ N(0, 0.1).
@@ -30,8 +31,9 @@ def random_weights(net: dict, seed: int = 0) -> dict:
         c, h, w = cur[L["bottoms"][0]]
         if t == "Convolution":
             k = L["kernel_size"]
-            std = np.sqrt(2.0 / (c * k * k))
-            rec = {"W": (rng.standard_normal((L["num_output"], c, k, k)) * std).astype(np.float32)}
+            cg = c // L.get("group", 1)  # inputs per output channel
+            std = np.sqrt(2.0 / (cg * k * k))
+            rec = {"W": (rng.standard_normal((L["num_output"], cg, k, k)) * std).astype(np.float32)}
             if L["bias_term"]:
                 rec["b"] = (rng.standard_normal(L["num_output"]) * 0.01).astype(np.float32)
             out[name] = rec

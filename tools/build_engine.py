@@ -7,6 +7,7 @@ examples/ONNX/resnet50/build.py:35-67).
   python tools/build_engine.py --model mnist --precision fp32 --batch 1 -o mnist.plan
   python tools/build_engine.py --prototxt deploy.prototxt --caffemodel weights.caffemodel --precision int8 --batch 32 -o rn.plan
   python tools/build_engine.py --model resnet50 --batch 8 --tune -o rn50_tuned.plan      (on a GPU box: tactics in the file)
+  python tools/build_engine.py --model resnext50 --precision fp16 --batch 8 --tune -o rx50.plan  (ResNeXt-50 32x4d)
 Weights: deterministic synthetic weights (the reference's benchmark engines are weightless too, models/README.md:6-7),
 unless --caffemodel names a binary NetParameter (trtexec --model=...); MNIST and --onnx carry their own weights.
 --precision int8: post-training quantization, max-abs calibration on --calib (an .npy [N,C,H,W] fp32) or on synthetic images.
@@ -23,7 +24,7 @@ from tensorrt_laboratory_b200 import builder, graph, weights  # noqa: E402
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--model", choices=["resnet50", "resnet152", "mnist"])
+    ap.add_argument("--model", choices=["resnet50", "resnet152", "resnext50", "mnist"])
     ap.add_argument("--prototxt")
     ap.add_argument("--onnx", help="ONNX CNN classifier (Conv / BatchNormalization / Relu / Add / MaxPool / AveragePool / "
                                    "GlobalAveragePool / Flatten / Reshape / Gemm / MatMul / Softmax), e.g. an ONNX-zoo ResNet")
@@ -55,6 +56,9 @@ def main():
         sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
         from tests import helpers
         net, wts, _, _ = helpers.load_mnist_golden()
+    elif a.model == "resnext50":  # 32x4d: grouped 3x3 convolutions (fp16 / fp32 only: INT8 has no grouped convolution)
+        net = graph.resnext_caffe(50)
+        wts = weights_for(net)
     else:
         net = graph.resnet_caffe(int(a.model[6:]))
         wts = weights_for(net)
