@@ -26,6 +26,10 @@ int trt_manager_allocate(trt_manager* m); /* InferenceManager::AllocateResources
 /* one request through InferRunner::Infer(pre, post): pinned H2D -> forward -> D2H, blocking */
 int trt_manager_infer(trt_manager* m, const char* model, int batch, const void* input, size_t input_bytes,
                       float* output, size_t output_bytes, double* compute_seconds);
+/* one request of a model with any number of bindings: `host[i]` / `bytes[i]` for every binding i of the model, in binding
+   order (inputs are read, outputs written; bytes[i] = bytes per item x batch) */
+int trt_manager_infer_bindings(trt_manager* m, const char* model, int batch, void* const* host, const size_t* bytes, int n,
+                               double* compute_seconds);
 /* `n` single-image requests through BatchedInferRunner (Dispatcher<StandardBatcher>, window_us): inputs/outputs are
  * contiguous [n][item]; *batches_executed = number of merged forward passes it took */
 int trt_manager_infer_batched(trt_manager* m, const char* model, int n, const void* inputs, void* outputs, int window_us,

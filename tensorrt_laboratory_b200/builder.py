@@ -16,17 +16,23 @@ from . import graph as G
 
 PREC_FP32, PREC_FP16, PREC_INT8 = 0, 1, 2
 OP_INPUT_CAST, OP_CONV, OP_MAXPOOL, OP_AVGPOOL, OP_FC, OP_SOFTMAX, OP_OUTPUT_CAST, OP_QUANTIZE = range(8)
+OP_EMBED_LN, OP_LAYERNORM, OP_ATTENTION, OP_POOLER = range(8, 12)   # transformer ops (version-3 plans)
+CONV_RELU, CONV_PACKED, CONV_INT8, CONV_GELU = 1, 2, 4, 8            # OpRec.relu bits of a convolution
 T_ACT, T_VEC = 0, 1
 MAGIC = b"B2ENGINE"
 VERSION = 1           # plans without grouped convolutions: 176-byte op records
 VERSION_GROUPED = 2   # a plan with at least one grouped convolution: 192-byte op records (+ groups)
+VERSION_TRANSFORMER = 3  # a plan with transformer ops or a GELU convolution: 224-byte op records (plan_format.h OpRecV3)
 
 _HEADER = struct.Struct("<8sIIIIIIQQ64s16x")
 _TENSOR = struct.Struct("<64sIIIIIif4x")  # ... binding, scale (INT8 tensors: real value = q * scale; 0 = fp16 / fp32 tensor)
 _OP = struct.Struct("<64sIiiiiIIIIIIIIIIIQQQQIIII")
 _OP_V2 = struct.Struct("<64sIiiiiIIIIIIIIIIIQQQQIIIII12x")  # version 2: _OP + groups + 12 reserved bytes
+# version 3: _OP + groups, heads, vocab, positions, types, binding2, binding3, out2, eps, flags + 8 reserved bytes
+_OP_V3 = struct.Struct("<64sIiiiiIIIIIIIIIIIQQQQIIIIIIIIIiiifI8x")
 _BINDING = struct.Struct("<64sIIiI8i16x")
-assert _HEADER.size == 128 and _TENSOR.size == 96 and _OP.size == 176 and _OP_V2.size == 192 and _BINDING.size == 128
+assert _HEADER.size == 128 and _TENSOR.size == 96 and _OP.size == 176 and _OP_V2.size == 192 and _OP_V3.size == 224
+assert _BINDING.size == 128
 
 
 def grouped_tc_span(cin: int, cout: int, groups: int, cin_phys: int, cout_phys: int) -> int:
@@ -318,14 +324,22 @@ def build_plan(lowered: dict, precision: int = PREC_FP16, max_batch: int = 8,
             bindings.append(dict(name=oname, is_input=0, dtype=0, tensor=ti, dims=[trec["c"], trec["h"], trec["w"]]))
             ops.append(dict(name="cast:" + oname, type=OP_OUTPUT_CAST, inp=ti, res=-1, out=-1, binding=bidx))
 
-    # version 1 unless a convolution is grouped: every plan without one stays byte-identical to what older builders wrote
+    return _serialize(tensors, ops, bindings, payload, precision, max_batch, name or lowered["name"])
+
+
+def _serialize(tensors: List[dict], ops: List[dict], bindings: List[dict], payload: bytearray, precision: int, max_batch: int,
+               name: str) -> bytes:
+    # version 1 unless a convolution is grouped (2) or the plan has transformer ops / GELU (3): every plan without them
+    # stays byte-identical to what older builders wrote
+    transformer = any(o["type"] >= OP_EMBED_LN or (o["type"] == OP_CONV and o.get("relu", 0) & CONV_GELU) for o in ops)
     grouped = any(o.get("groups", 1) > 1 for o in ops)
-    op_struct = _OP_V2 if grouped else _OP
+    op_struct = _OP_V3 if transformer else _OP_V2 if grouped else _OP
+    version = VERSION_TRANSFORMER if transformer else VERSION_GROUPED if grouped else VERSION
     tables = _HEADER.size + len(tensors) * _TENSOR.size + len(ops) * op_struct.size + len(bindings) * _BINDING.size
     payload_offset = _roundup(tables, 256)
     blob = bytearray()
-    blob += _HEADER.pack(MAGIC, VERSION_GROUPED if grouped else VERSION, precision, max_batch, len(tensors), len(ops),
-                         len(bindings), payload_offset, len(payload), _name(name or lowered["name"]))
+    blob += _HEADER.pack(MAGIC, version, precision, max_batch, len(tensors), len(ops),
+                         len(bindings), payload_offset, len(payload), _name(name))
     for t in tensors:
         blob += _TENSOR.pack(_name(t["name"]), t["kind"], t["h"], t["w"], t["c"], t["c_phys"], t["binding"], t.get("scale", 0.0))
     for o in ops:
@@ -335,13 +349,125 @@ def build_plan(lowered: dict, precision: int = PREC_FP16, max_batch: int = 8,
                   o.get("taps", 0), o.get("taps_phys", 0),
                   o.get("w_off", 0), o.get("w_bytes", 0), o.get("b_off", 0), o.get("b_bytes", 0),
                   o.get("kw", 0), o.get("stride_w", 0), o.get("pad_w_lo", 0), o.get("pad_w_hi", 0))
-        blob += op_struct.pack(*fields, o.get("groups", 1)) if grouped else op_struct.pack(*fields)
+        if transformer:
+            blob += op_struct.pack(*fields, o.get("groups", 1), o.get("heads", 0), o.get("vocab", 0), o.get("positions", 0),
+                                   o.get("types", 0), o.get("binding2", -1), o.get("binding3", -1), o.get("out2", -1),
+                                   o.get("eps", 0.0), o.get("flags", 0))
+        else:
+            blob += op_struct.pack(*fields, o.get("groups", 1)) if grouped else op_struct.pack(*fields)
     for b in bindings:
         dims = list(b["dims"]) + [0] * (8 - len(b["dims"]))
         blob += _BINDING.pack(_name(b["name"]), b["is_input"], b["dtype"], b["tensor"], len(b["dims"]), *dims)
     blob += b"\0" * (payload_offset - len(blob))
     blob += payload
     return bytes(blob)
+
+
+def build_bert_plan(cfg=None, weights=None, max_batch: int = 16, seed: int = 0, precision: int = PREC_FP16,
+                    name: Optional[str] = None, taps: Sequence[str] = ()) -> bytes:
+    """BERT encoder + pooler (``bert.BertConfig``; default BERT-base at S = 128) -> fp16 plan (version 3).
+
+    ``weights``: a dict or ``.npz`` path in Hugging Face ``BertModel`` names (``bert.load_weights``); default: seeded
+    ``bert.random_weights(cfg, seed)``.  Activations are ``T_ACT`` tensors [N, 1, S, C], so every GEMM is a 1x1
+    convolution on the tensor cores: Q, K and V fused into one layer of 3H output channels, ordered (part, head, d) --
+    channel part * H + 64 * head + d with part 0 = Q, 1 = K, 2 = V; the attention output projection and the second FFN
+    GEMM with the layer input as fused residual; the first FFN GEMM with GELU.  Bindings: int32 ``input_ids``,
+    ``segment_ids``, ``input_mask`` ([S] per item, mask 1 = attend); fp32 ``last_hidden_state`` ([S, H], token-major) and
+    ``pooled_output`` ([H]).  ``taps``: names of intermediate activation tensors (``embeddings``, ``l{i}.qkv``,
+    ``l{i}.context``, ``l{i}.attn_sum``, ``l{i}.attn_ln``, ``l{i}.ffn``, ``l{i}.ffn_sum``, ``l{i}.out``) to expose as
+    extra fp32 [S, C] output bindings of the same names."""
+    from . import bert as Bm
+    cfg = cfg or Bm.BERT_BASE
+    if precision == PREC_FP32:
+        raise ValueError("BERT plans are fp16 only: the attention, LayerNorm and embedding kernels exist for fp16 activations")
+    if precision == PREC_INT8:
+        raise ValueError("BERT plans are fp16 only: INT8 BERT (quantised GEMMs and attention) is not implemented")
+    if precision != PREC_FP16:
+        raise ValueError("precision must be PREC_FP16")
+    S, H, F = cfg.seq, cfg.hidden, cfg.ffn
+    if S % 64 or not 0 < S <= 128:
+        raise ValueError(f"sequence length {S}: a plan is built for S a multiple of 64 and at most 128 "
+                         "(longer sequences need an online softmax)")
+    if cfg.heads * 64 != H:
+        raise ValueError(f"heads * 64 must equal the hidden size ({cfg.heads} * 64 != {H})")
+    if F % 64 or H > 1024 or S > cfg.positions:
+        raise ValueError("the FFN width must be a multiple of 64, the hidden size at most 1024, and S at most the positions")
+    W = Bm.load_weights(weights if weights is not None else Bm.random_weights(cfg, seed), cfg)
+
+    tensors: List[dict] = []
+    ops: List[dict] = []
+    payload = bytearray()
+
+    def add_payload(arr: np.ndarray):
+        while len(payload) % 256:
+            payload.append(0)
+        off = len(payload)
+        raw = np.ascontiguousarray(arr).tobytes()
+        payload.extend(raw)
+        return off, len(raw)
+
+    def act(tname: str, c: int) -> int:
+        tensors.append(dict(name=tname, kind=T_ACT, h=1, w=S, c=c, c_phys=c, binding=-1))
+        return len(tensors) - 1
+
+    def vec(tname: str, c: int, binding: int = -1) -> int:
+        tensors.append(dict(name=tname, kind=T_VEC, h=1, w=1, c=c, c_phys=c, binding=binding))
+        return len(tensors) - 1
+
+    def gemm(oname: str, ti: int, to: int, Wm: np.ndarray, b: np.ndarray, res: int = -1, gelu: bool = False) -> dict:
+        cout, cin = Wm.shape
+        w_off, w_bytes = add_payload(pack_weights_sw128(Wm.astype(np.float16)))
+        b_off, b_bytes = add_payload(b.astype(np.float32))
+        return dict(name=oname, type=OP_CONV, inp=ti, res=res, out=to, binding=-1, k=1, stride=1, pad=0,
+                    relu=CONV_PACKED | (CONV_GELU if gelu else 0), cin=cin, cout=cout, cin_phys=cin, cout_phys=cout, taps=1,
+                    taps_phys=1, w_off=w_off, w_bytes=w_bytes, b_off=b_off, b_bytes=b_bytes)
+
+    def gamma_beta(prefix: str):
+        return add_payload(np.concatenate([W[prefix + ".weight"], W[prefix + ".bias"]]).astype(np.float32))
+
+    # bindings 0..2: int32 inputs, 3: last_hidden_state, 4: pooled_output
+    x = act("embeddings", H)
+    mask = vec("attention_mask_add", S)
+    tables = np.concatenate([W["embeddings.word_embeddings.weight"], W["embeddings.position_embeddings.weight"],
+                             W["embeddings.token_type_embeddings.weight"]]).astype(np.float16)
+    w_off, w_bytes = add_payload(tables)
+    b_off, b_bytes = gamma_beta("embeddings.LayerNorm")
+    ops.append(dict(name="embeddings", type=OP_EMBED_LN, inp=-1, res=-1, out=x, binding=0, binding2=1, binding3=2, out2=mask,
+                    cin=H, cout=H, cin_phys=H, cout_phys=H, vocab=cfg.vocab, positions=cfg.positions, types=cfg.types,
+                    eps=cfg.eps, w_off=w_off, w_bytes=w_bytes, b_off=b_off, b_bytes=b_bytes))
+    for i in range(cfg.layers):
+        p = f"encoder.layer.{i}."
+        qkv, ctx, att, h1 = act(f"l{i}.qkv", 3 * H), act(f"l{i}.context", H), act(f"l{i}.attn_sum", H), act(f"l{i}.attn_ln", H)
+        ffn, fsum, h2 = act(f"l{i}.ffn", F), act(f"l{i}.ffn_sum", H), act(f"l{i}.out", H)
+        Wqkv = np.concatenate([W[p + f"attention.self.{m}.weight"] for m in ("query", "key", "value")])
+        bqkv = np.concatenate([W[p + f"attention.self.{m}.bias"] for m in ("query", "key", "value")])
+        ops.append(gemm(f"l{i}.qkv", x, qkv, Wqkv, bqkv))
+        ops.append(dict(name=f"l{i}.attention", type=OP_ATTENTION, inp=qkv, res=mask, out=ctx, binding=-1, heads=cfg.heads))
+        ops.append(gemm(f"l{i}.attn_out", ctx, att, W[p + "attention.output.dense.weight"], W[p + "attention.output.dense.bias"], res=x))
+        b_off, b_bytes = gamma_beta(p + "attention.output.LayerNorm")
+        ops.append(dict(name=f"l{i}.attn_ln", type=OP_LAYERNORM, inp=att, res=-1, out=h1, binding=-1, eps=cfg.eps, b_off=b_off, b_bytes=b_bytes))
+        ops.append(gemm(f"l{i}.ffn1", h1, ffn, W[p + "intermediate.dense.weight"], W[p + "intermediate.dense.bias"], gelu=True))
+        ops.append(gemm(f"l{i}.ffn2", ffn, fsum, W[p + "output.dense.weight"], W[p + "output.dense.bias"], res=h1))
+        b_off, b_bytes = gamma_beta(p + "output.LayerNorm")
+        ops.append(dict(name=f"l{i}.out_ln", type=OP_LAYERNORM, inp=fsum, res=-1, out=h2, binding=-1, eps=cfg.eps, b_off=b_off, b_bytes=b_bytes))
+        x = h2
+    pooled = vec("pooled_output", H, binding=4)
+    w_off, w_bytes = add_payload(W["pooler.dense.weight"].astype(np.float16))
+    b_off, b_bytes = add_payload(W["pooler.dense.bias"].astype(np.float32))
+    ops.append(dict(name="pooler", type=OP_POOLER, inp=x, res=-1, out=pooled, binding=-1, cin=H, cout=H, cin_phys=H, cout_phys=H,
+                    w_off=w_off, w_bytes=w_bytes, b_off=b_off, b_bytes=b_bytes))
+    ops.append(dict(name="cast:last_hidden_state", type=OP_OUTPUT_CAST, inp=x, res=-1, out=-1, binding=3, flags=1))
+    bindings = [dict(name=n, is_input=1, dtype=3, tensor=0, dims=[S]) for n in ("input_ids", "segment_ids", "input_mask")]
+    bindings.append(dict(name="last_hidden_state", is_input=0, dtype=0, tensor=x, dims=[S, H]))
+    bindings.append(dict(name="pooled_output", is_input=0, dtype=0, tensor=pooled, dims=[H]))
+    for tap in taps:
+        ti = next((k for k, t in enumerate(tensors) if t["name"] == tap and t["kind"] == T_ACT), None)
+        if ti is None:
+            raise ValueError(f"tap {tap!r}: no such activation tensor")
+        bindings.append(dict(name=tap, is_input=0, dtype=0, tensor=ti, dims=[S, tensors[ti]["c"]]))
+        ops.append(dict(name="cast:" + tap, type=OP_OUTPUT_CAST, inp=ti, res=-1, out=-1, binding=len(bindings) - 1, flags=1))
+    default_name = f"bert_l{cfg.layers}_h{H}_s{S}"
+    return _serialize(tensors, ops, bindings, payload, PREC_FP16, max_batch, name or default_name)
 
 
 def build_resnext_plan(depth: int = 50, precision: int = PREC_FP16, max_batch: int = 8, seed: int = 0,

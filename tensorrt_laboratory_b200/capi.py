@@ -92,6 +92,7 @@ SYMBOLS = [
     ("trt_manager_register_model", _I, [_VP, _S, _VP, _SZ, _I]),
     ("trt_manager_allocate", _I, [_VP]),
     ("trt_manager_infer", _I, [_VP, _S, _I, _VP, _SZ, _VP, _SZ, C.POINTER(_D)]),
+    ("trt_manager_infer_bindings", _I, [_VP, _S, _I, _PVP, C.POINTER(_SZ), _I, C.POINTER(_D)]),
     ("trt_manager_infer_batched", _I, [_VP, _S, _I, _VP, _VP, _I, C.POINTER(_I)]),
     ("trt_manager_bench_batched", _I, [_VP, _S, _I, _VP, _I, _VP, _I, _I, _I, C.POINTER(_D), C.POINTER(_D), C.POINTER(_I)]),
     ("trt_manager_metrics_text", _I, [_VP, C.c_char_p, _SZ]),
@@ -406,6 +407,23 @@ class Session:
         return {b["name"]: self.host_array(i, batch).copy()
                 for i, b in enumerate(self.engine.bindings) if not b["is_input"]}
 
+    def infer_bindings(self, inputs: Dict[str, np.ndarray]) -> Dict[str, np.ndarray]:
+        """Synchronous call for engines with any number of bindings: ``inputs`` maps every input binding name to a
+        [batch, ...] array (cast to the binding dtype) -> {output binding name: [batch, ...] array}."""
+        return _infer_bindings(self.engine.bindings, inputs, self.engine.max_batch, self._run_bindings)
+
+    def _run_bindings(self, batch: int, arrays: List[np.ndarray]):
+        for i, b in enumerate(self.engine.bindings):
+            if b["is_input"]:
+                self.host_array(i, batch)[...] = arrays[i]
+        self.h2d(batch)
+        self.enqueue(batch)
+        self.d2h(batch)
+        self.stream.sync()
+        for i, b in enumerate(self.engine.bindings):
+            if not b["is_input"]:
+                arrays[i][...] = self.host_array(i, batch)
+
     def profile(self, batch: int) -> List[dict]:
         """Per-launch device times of one (serialised) forward pass."""
         n = self._lib.b2_context_nb_launches(self.ctx, batch)
@@ -483,6 +501,20 @@ class InferenceManager:
                                           out.ctypes.data, out.nbytes, C.byref(sec)))
         self.last_compute_seconds = sec.value  # device time of the forward pass (ExecutionContext::Synchronize)
         return out
+
+    def infer_bindings(self, name: str, inputs: Dict[str, np.ndarray]) -> Dict[str, np.ndarray]:
+        """One request through the C++ InferenceManager for models with any number of bindings: ``inputs`` maps every
+        input binding name to a [batch, ...] array -> {output binding name: [batch, ...] array}."""
+        meta = self.models[name]
+
+        def run(batch: int, arrays: List[np.ndarray]):
+            ptrs = (C.c_void_p * len(arrays))(*[a.ctypes.data for a in arrays])
+            sizes = (_SZ * len(arrays))(*[a.nbytes for a in arrays])
+            sec = _D()
+            check(self._lib.trt_manager_infer_bindings(self.handle, name.encode(), batch, ptrs, sizes, len(arrays), C.byref(sec)))
+            self.last_compute_seconds = sec.value
+
+        return _infer_bindings(meta.bindings, inputs, meta.max_batch, run)
 
     def infer_timed(self, name: str, x: np.ndarray):
         """-> (output, device seconds of the forward pass), what the reference service reports as compute_time
@@ -580,6 +612,30 @@ class InferenceManager:
             self.close()
         except Exception:
             pass
+
+
+def _infer_bindings(bindings: List[dict], inputs: Dict[str, np.ndarray], max_batch: int, run) -> Dict[str, np.ndarray]:
+    """Checks ``inputs`` against the binding table, allocates the outputs and calls ``run(batch, arrays)`` with one
+    C-contiguous array per binding (binding order)."""
+    names = {b["name"] for b in bindings if b["is_input"]}
+    if set(inputs) != names:
+        raise ValueError(f"inputs {sorted(inputs)} do not match the input bindings {sorted(names)}")
+    batch = None
+    arrays = []
+    for b in bindings:
+        if b["is_input"]:
+            a = np.ascontiguousarray(inputs[b["name"]], dtype=b["np_dtype"])
+            if a.shape[1:] != b["shape"] or (batch is not None and a.shape[0] != batch):
+                raise ValueError(f"binding {b['name']}: shape {a.shape}, expected [batch] + {list(b['shape'])}")
+            batch = a.shape[0]
+        else:
+            a = None
+        arrays.append(a)
+    if not 1 <= batch <= max_batch:
+        raise ValueError(f"batch {batch} outside [1, {max_batch}]")
+    arrays = [a if a is not None else np.empty((batch,) + b["shape"], b["np_dtype"]) for a, b in zip(arrays, bindings)]
+    run(batch, arrays)
+    return {b["name"]: arrays[i] for i, b in enumerate(bindings) if not b["is_input"]}
 
 
 def timed_pipeline(blob: bytes, iters: int = 20):

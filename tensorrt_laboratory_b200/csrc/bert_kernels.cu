@@ -1,0 +1,392 @@
+// sm_90a kernels of the transformer encoder (BERT) path; the six GEMMs of a layer run on conv_f16_tcgen05 as 1x1
+// convolutions, these are the operators between them.
+//
+//  * embed_ln_kernel      -- word + position + token-type rows summed in fp32, LayerNorm, fp16 out; additive mask
+//  * layernorm_h8_kernel  -- LayerNorm over the channels of fp16 rows (16-byte vectors, one row per warp)
+//  * attention_f16_wgmma  -- one CTA (one warpgroup) per (sequence, head, 64 query rows): Q, K, V by TMA, S = Q K^T with
+//                            wgmma into registers, scale + mask + softmax in registers, P fed to P V as the register A
+//                            operand of wgmma, O written at channel 64 * head
+//  * pooler_kernel        -- tanh(W h[CLS] + b), fp32 out
+//
+// Numerics (DESIGN.md, "BERT numerics"): every sum below runs in a fixed order -- a lane adds its own elements in index
+// order, then the warp combines lanes with an xor butterfly -- so a row's result does not depend on the batch, the grid
+// or the other rows.
+#include "kernels.h"
+
+#include "ptx_sm90.cuh"
+#include "wgmma_sm90.cuh"
+
+namespace b2k {
+
+namespace {
+
+template <typename Kern, typename... Args>
+int launch_pdl(Kern kern, dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args... args) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = grid;
+    cfg.blockDim = block;
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = get_pdl() ? 1 : 0;
+    return static_cast<int>(cudaLaunchKernelEx(&cfg, kern, args...));
+}
+
+constexpr int kLnMaxVec = 4;  // 16-byte vectors per lane: rows of up to 32 * 4 * 8 = 1024 channels
+
+__device__ __forceinline__ float warp_sum(float v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+
+__device__ __forceinline__ void unpack8(const uint4& u, float* f) {
+    const __half2* h = reinterpret_cast<const __half2*>(&u);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const float2 t = __half22float2(h[i]);
+        f[2 * i] = t.x;
+        f[2 * i + 1] = t.y;
+    }
+}
+
+// LayerNorm of one row held by a warp: lane l owns 16-byte vectors l, l + 32, ... (nv of them).  mean = (sum x) / C,
+// var = (sum (x - mean)^2) / C, y = fp16(((x - mean) * (1 / sqrt(var + eps))) * gamma + beta).
+__device__ __forceinline__ void ln_row_store(float (&x)[kLnMaxVec][8], int nv, int lane, int C, float eps, const float* gamma,
+                                             const float* beta, __half* out_row, int C_phys) {
+    float s = 0.f;
+#pragma unroll
+    for (int k = 0; k < kLnMaxVec; ++k)
+        if (k < nv)
+#pragma unroll
+            for (int e = 0; e < 8; ++e) s = __fadd_rn(s, x[k][e]);
+    const float mean = __fdiv_rn(warp_sum(s), static_cast<float>(C));
+    float q = 0.f;
+#pragma unroll
+    for (int k = 0; k < kLnMaxVec; ++k)
+        if (k < nv)
+#pragma unroll
+            for (int e = 0; e < 8; ++e) {
+                const float d = __fsub_rn(x[k][e], mean);
+                q = __fadd_rn(q, __fmul_rn(d, d));
+            }
+    const float var = __fdiv_rn(warp_sum(q), static_cast<float>(C));
+    const float rstd = __fdiv_rn(1.0f, __fsqrt_rn(__fadd_rn(var, eps)));
+#pragma unroll
+    for (int k = 0; k < kLnMaxVec; ++k) {
+        if (k >= nv) continue;
+        const int c0 = (lane + 32 * k) * 8;
+        uint4 o;
+        __half2* o2 = reinterpret_cast<__half2*>(&o);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            float y[2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int c = c0 + 2 * i + e;
+                y[e] = __fadd_rn(__fmul_rn(__fmul_rn(__fsub_rn(x[k][2 * i + e], mean), rstd), __ldg(gamma + c)), __ldg(beta + c));
+            }
+            o2[i] = __floats2half2_rn(y[0], y[1]);
+        }
+        *reinterpret_cast<uint4*>(out_row + c0) = o;
+    }
+    for (int c = C + lane; c < C_phys; c += 32) out_row[c] = __float2half_rn(0.f);  // channel padding
+}
+
+constexpr int kRowWarps = 4;  // rows (warps) per CTA of the row kernels
+
+// (the three bindings are separate parameters 0, 1, 2: a captured graph re-points them per request)
+__global__ void __launch_bounds__(32 * kRowWarps) embed_ln_kernel(const int* __restrict__ ids, const int* __restrict__ segs,
+                                                               const int* __restrict__ mask, const EmbedArgs a) {
+    pdl_launch_dependents();
+    pdl_wait();
+    const int lane = threadIdx.x & 31;
+    const long long row = static_cast<long long>(blockIdx.x) * kRowWarps + (threadIdx.x >> 5);
+    if (row >= static_cast<long long>(a.N) * a.S) return;
+    const int s = static_cast<int>(row % a.S);
+    const int id = min(max(__ldg(ids + row), 0), a.vocab - 1);
+    const int seg = min(max(__ldg(segs + row), 0), a.types - 1);
+    if (lane == 0) a.mask_add[row] = __ldg(mask + row) != 0 ? 0.0f : -10000.0f;
+    const uint4* w = reinterpret_cast<const uint4*>(a.tables + static_cast<size_t>(id) * a.C);
+    const uint4* p = reinterpret_cast<const uint4*>(a.tables + static_cast<size_t>(a.vocab + s) * a.C);
+    const uint4* t = reinterpret_cast<const uint4*>(a.tables + static_cast<size_t>(a.vocab + a.positions + seg) * a.C);
+    const int nvec = a.C / 8;
+    const int nv = (nvec - lane + 31) / 32;
+    float x[kLnMaxVec][8];
+#pragma unroll
+    for (int k = 0; k < kLnMaxVec; ++k) {
+        if (k >= nv) continue;
+        const int v = lane + 32 * k;
+        float fw[8], fp[8], ft[8];
+        unpack8(__ldg(w + v), fw);
+        unpack8(__ldg(p + v), fp);
+        unpack8(__ldg(t + v), ft);
+#pragma unroll
+        for (int e = 0; e < 8; ++e) x[k][e] = __fadd_rn(__fadd_rn(fw[e], fp[e]), ft[e]);  // (word + position) + type
+    }
+    ln_row_store(x, nv, lane, a.C, a.eps, a.gamma, a.beta, a.out + row * a.C_phys, a.C_phys);
+}
+
+__global__ void __launch_bounds__(32 * kRowWarps) layernorm_h8_kernel(const __half* __restrict__ in, __half* __restrict__ out,
+                                                                   const float* __restrict__ gamma, const float* __restrict__ beta,
+                                                                   long long rows, int C, int C_phys, float eps) {
+    pdl_launch_dependents();
+    pdl_wait();
+    const int lane = threadIdx.x & 31;
+    const long long row = static_cast<long long>(blockIdx.x) * kRowWarps + (threadIdx.x >> 5);
+    if (row >= rows) return;
+    const uint4* src = reinterpret_cast<const uint4*>(in + row * C_phys);
+    const int nv = (C / 8 - lane + 31) / 32;
+    float x[kLnMaxVec][8];
+#pragma unroll
+    for (int k = 0; k < kLnMaxVec; ++k)
+        if (k < nv) unpack8(src[lane + 32 * k], x[k]);
+    ln_row_store(x, nv, lane, C, eps, gamma, beta, out + row * C_phys, C_phys);
+}
+
+// ---- attention ---------------------------------------------------------------------------------------------------
+// wgmma with the A operand in registers (fragment layout of mma.m16n8k16 per warp: a0 = (r, k..k+1), a1 = (r+8, k..k+1),
+// a2 = (r, k+8..k+9), a3 = (r+8, k+8..k+9) with r = l/4 + 16w, k = 2(l%4)) and B a K-major shared-memory tile
+__device__ __forceinline__ void wgmma_f16_rs_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t b, uint32_t accumulate) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %37, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(accumulate));
+}
+
+__device__ __forceinline__ uint32_t pack_h2(float lo, float hi) {
+    const __half2 h = __floats2half2_rn(lo, hi);
+    return *reinterpret_cast<const uint32_t*>(&h);
+}
+
+template <int S>
+struct AttnSmem {
+    static constexpr int Q = 0;                  // 64 query rows x 128 B (128B swizzle)
+    static constexpr int K = 64 * 128;           // S key rows x 128 B
+    static constexpr int V = K + S * 128;        // S value rows x 128 B, as loaded
+    static constexpr int VT = V + S * 128;       // V^T: S/64 blocks of [64 d rows][64 keys = 128 B], 128B swizzle
+    static constexpr int BAR = VT + S * 128;
+    static constexpr int BYTES = BAR + 64 + 1024;  // + 1 KiB alignment slack
+};
+
+// byte offset of element (row, col) of a [rows][64 fp16] tile stored with the 128-byte swizzle (16-byte chunk j of row r at
+// chunk j ^ (r % 8)); the tile base is 1024-byte aligned
+__device__ __forceinline__ uint32_t sw128(int row, int col) {
+    return static_cast<uint32_t>(row * 128 + ((((col >> 3) ^ row) & 7) << 4) + (col & 7) * 2);
+}
+
+template <int S>
+__global__ void __launch_bounds__(128, 1)
+attention_f16_wgmma(const __grid_constant__ CUtensorMap mapQKV, const float* __restrict__ mask_add, __half* __restrict__ out, int heads,
+                    int H, int out_pitch) {
+    static_assert(S == 64 || S == 128, "sequence lengths 64 and 128");
+    using L = AttnSmem<S>;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+    uint64_t* bar = reinterpret_cast<uint64_t*>(smem + L::BAR);
+    const int n = blockIdx.x / heads, head = blockIdx.x - n * heads;
+    const int q0 = blockIdx.y * 64;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    if (tid == 0) {
+        tma_prefetch_desc(&mapQKV);
+        mbar_init(bar, 1);
+        fence_barrier_init();
+    }
+    __syncthreads();
+    pdl_launch_dependents();
+    pdl_wait();  // Q, K, V and the mask are the previous kernels' output
+    if (tid == 0) {
+        mbar_expect_tx(bar, static_cast<uint32_t>((64 + 2 * S) * 128));
+        const int row0 = n * S;
+        tma_load_2d(&mapQKV, bar, smem + L::Q, head * 64, row0 + q0);
+#pragma unroll
+        for (int b = 0; b < S / 64; ++b) {
+            tma_load_2d(&mapQKV, bar, smem + L::K + b * 8192, H + head * 64, row0 + 64 * b);
+            tma_load_2d(&mapQKV, bar, smem + L::V + b * 8192, 2 * H + head * 64, row0 + 64 * b);
+        }
+    }
+    // this thread's key columns: 8j + 2(l%4) + e
+    float mk[S / 4];
+#pragma unroll
+    for (int j = 0; j < S / 8; ++j) {
+        const float2 m2 = __ldg(reinterpret_cast<const float2*>(mask_add + static_cast<size_t>(n) * S + 8 * j + 2 * (lane & 3)));
+        mk[2 * j] = m2.x;
+        mk[2 * j + 1] = m2.y;
+    }
+    mbar_wait(bar, 0);
+    // V [key][d] -> V^T [d][key] (K-major B operand of P V), 2 keys x 1 d per step
+    for (int e = tid; e < S * 32; e += 128) {
+        const int d = e & 63, key = (e >> 6) * 2;
+        const __half v0 = *reinterpret_cast<const __half*>(smem + L::V + sw128(key, d));
+        const __half v1 = *reinterpret_cast<const __half*>(smem + L::V + sw128(key + 1, d));
+        *reinterpret_cast<__half2*>(smem + L::VT + (key >> 6) * 8192 + sw128(d, key & 63)) = __halves2half2(v0, v1);
+    }
+    fence_proxy_async();  // generic-proxy stores -> visible to wgmma
+    __syncthreads();
+
+    // S = Q K^T: 64 x S, K = 64 (four k16 steps)
+    float sacc[S / 2];
+    const uint32_t q_addr = smem_u32(smem + L::Q), k_addr = smem_u32(smem + L::K);
+    wgmma_group<4>([&](int j) {
+        wgmma_f16<S>(sacc, make_wgmma_desc(q_addr + j * 32, 16, 1024, WG_SW128), make_wgmma_desc(k_addr + j * 32, 16, 1024, WG_SW128),
+                     j > 0 ? 1u : 0u);
+    });
+    wgmma_wait<0>();
+
+    // scores * 0.125 + mask; softmax per row (rows l/4 and l/4 + 8 of this warp's 16): each thread reduces its S/4 values
+    // in column order, then the 4 lanes of the row combine by xor butterfly
+    float mx[2] = {-3.0e38f, -3.0e38f};
+#pragma unroll
+    for (int j = 0; j < S / 8; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                float& v = sacc[4 * j + 2 * h + e];
+                v = __fadd_rn(__fmul_rn(v, 0.125f), mk[2 * j + e]);
+                mx[h] = fmaxf(mx[h], v);
+            }
+    float sum[2] = {0.f, 0.f};
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+        mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+    }
+#pragma unroll
+    for (int j = 0; j < S / 8; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                float& v = sacc[4 * j + 2 * h + e];
+                v = expf(__fsub_rn(v, mx[h]));
+                sum[h] = __fadd_rn(sum[h], v);
+            }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        sum[h] = __fadd_rn(sum[h], __shfl_xor_sync(0xffffffffu, sum[h], 1));
+        sum[h] = __fadd_rn(sum[h], __shfl_xor_sync(0xffffffffu, sum[h], 2));
+    }
+    // P = fp16(p / sum), normalised BEFORE P V; k16 step t of P V reads key columns 16t ... 16t + 15 = accumulator
+    // column blocks j = 2t (a0, a1) and 2t + 1 (a2, a3)
+    uint32_t pa[S / 16][4];
+#pragma unroll
+    for (int t = 0; t < S / 16; ++t)
+#pragma unroll
+        for (int half = 0; half < 2; ++half) {
+            const int j = 2 * t + half;
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+                pa[t][2 * half + h] = pack_h2(__fdiv_rn(sacc[4 * j + 2 * h], sum[h]), __fdiv_rn(sacc[4 * j + 2 * h + 1], sum[h]));
+        }
+
+    // O = P V: 64 x 64, K = S
+    float oacc[32];
+    const uint32_t vt_addr = smem_u32(smem + L::VT);
+    wgmma_group<S / 16>([&](int t) {
+        wgmma_f16_rs_n64(oacc, pa[t], make_wgmma_desc(vt_addr + (t >> 2) * 8192 + (t & 3) * 32, 16, 1024, WG_SW128), t > 0 ? 1u : 0u);
+    });
+    wgmma_wait<0>();
+
+    const int r0 = 16 * warp + (lane >> 2);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        __half* orow = out + static_cast<size_t>(n * S + q0 + r0 + 8 * h) * out_pitch + head * 64 + 2 * (lane & 3);
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+            *reinterpret_cast<__half2*>(orow + 8 * j) = __floats2half2_rn(oacc[4 * j + 2 * h], oacc[4 * j + 2 * h + 1]);
+    }
+}
+
+// pooled[n][j] = tanh(b[j] + W[j] . h[n][0]): one warp per output channel j, its weight row held in registers (loaded
+// before the dependency wait: weights are constants)
+__global__ void __launch_bounds__(256) pooler_kernel(const __half* __restrict__ h, const __half* __restrict__ w, const float* __restrict__ b,
+                                                     float* __restrict__ out, int N, int S, int C, int C_phys) {
+    const int lane = threadIdx.x & 31;
+    const int j = blockIdx.x * 8 + (threadIdx.x >> 5);
+    const int nv = (C / 8 - lane + 31) / 32;
+    float wr[kLnMaxVec][8];
+    if (j < C) {
+        const uint4* wrow = reinterpret_cast<const uint4*>(w + static_cast<size_t>(j) * C);
+#pragma unroll
+        for (int k = 0; k < kLnMaxVec; ++k)
+            if (k < nv) unpack8(__ldg(wrow + lane + 32 * k), wr[k]);
+    }
+    pdl_launch_dependents();
+    pdl_wait();
+    if (j >= C) return;
+    const float bj = __ldg(b + j);
+    for (int n = 0; n < N; ++n) {
+        const uint4* hrow = reinterpret_cast<const uint4*>(h + static_cast<size_t>(n) * S * C_phys);  // token 0 = [CLS]
+        float acc = 0.f;
+#pragma unroll
+        for (int k = 0; k < kLnMaxVec; ++k) {
+            if (k >= nv) continue;
+            float x[8];
+            unpack8(hrow[lane + 32 * k], x);
+#pragma unroll
+            for (int e = 0; e < 8; ++e) acc = __fadd_rn(acc, __fmul_rn(wr[k][e], x[e]));
+        }
+        acc = warp_sum(acc);
+        if (lane == 0) out[static_cast<size_t>(n) * C + j] = tanhf(__fadd_rn(acc, bj));
+    }
+}
+
+__global__ void output_cast_rows_kernel(const __half* __restrict__ src, float* __restrict__ dst, long long rows, int C, int C_phys) {
+    pdl_launch_dependents();
+    pdl_wait();
+    const long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
+    if (idx >= rows * C) return;
+    const long long r = idx / C;
+    dst[idx] = __half2float(src[r * C_phys + (idx - r * C)]);
+}
+
+}  // namespace
+
+int launch_embed_ln(const EmbedArgs& a, cudaStream_t stream) {
+    if (a.C % 8 || a.C > 32 * kLnMaxVec * 8) return static_cast<int>(cudaErrorInvalidValue);
+    const long long rows = static_cast<long long>(a.N) * a.S;
+    return launch_pdl(embed_ln_kernel, dim3(static_cast<unsigned>((rows + kRowWarps - 1) / kRowWarps)), dim3(32 * kRowWarps), 0, stream, a.ids, a.segs,
+                      a.mask, a);
+}
+
+int launch_layernorm(const __half* in, __half* out, const float* gamma, const float* beta, long long rows, int C, int C_phys, float eps,
+                     cudaStream_t stream) {
+    if (C % 8 || C > 32 * kLnMaxVec * 8) return static_cast<int>(cudaErrorInvalidValue);
+    return launch_pdl(layernorm_h8_kernel, dim3(static_cast<unsigned>((rows + kRowWarps - 1) / kRowWarps)), dim3(32 * kRowWarps), 0, stream,
+                      in, out, gamma, beta, rows, C, C_phys, eps);
+}
+
+int init_attention_kernels() {
+    cudaError_t e = cudaFuncSetAttribute(attention_f16_wgmma<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnSmem<64>::BYTES);
+    if (e == cudaSuccess)
+        e = cudaFuncSetAttribute(attention_f16_wgmma<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnSmem<128>::BYTES);
+    return static_cast<int>(e);
+}
+
+int launch_attention(const AttnLaunch& L, cudaStream_t stream) {
+    const dim3 grid(static_cast<unsigned>(L.N * L.heads), static_cast<unsigned>(L.S / 64));
+    if (L.S == 64)
+        return launch_pdl(attention_f16_wgmma<64>, grid, dim3(128), AttnSmem<64>::BYTES, stream, L.mapQKV, L.mask_add, L.out, L.heads, L.H,
+                          L.out_pitch);
+    if (L.S == 128)
+        return launch_pdl(attention_f16_wgmma<128>, grid, dim3(128), AttnSmem<128>::BYTES, stream, L.mapQKV, L.mask_add, L.out, L.heads, L.H,
+                          L.out_pitch);
+    return static_cast<int>(cudaErrorInvalidValue);
+}
+
+int launch_pooler(const __half* h, const __half* w, const float* b, float* out, int N, int S, int C, int C_phys, cudaStream_t stream) {
+    if (C % 8 || C > 32 * kLnMaxVec * 8) return static_cast<int>(cudaErrorInvalidValue);
+    return launch_pdl(pooler_kernel, dim3(static_cast<unsigned>((C + 7) / 8)), dim3(256), 0, stream, h, w, b, out, N, S, C, C_phys);
+}
+
+int launch_output_cast_rows(const __half* src, float* dst, long long rows, int C, int C_phys, cudaStream_t stream) {
+    const long long total = rows * C;
+    return launch_pdl(output_cast_rows_kernel, dim3(static_cast<unsigned>((total + 255) / 256)), dim3(256), 0, stream, src, dst, rows, C, C_phys);
+}
+
+}  // namespace b2k

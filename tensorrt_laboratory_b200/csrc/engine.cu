@@ -104,6 +104,11 @@ struct Tensor {
 struct Op {
     b2plan::OpRec r;
     int groups = 1;  // convs: OpRecV2::groups (version-1 plans: 1)
+    // version-3 fields (plan_format.h OpRecV3); defaults for older plans
+    int heads = 0, vocab = 0, positions = 0, types = 0;
+    int binding2 = -1, binding3 = -1, out2 = -1;
+    float eps = 0.f;
+    uint32_t flags = 0;
     std::string name;
     // >= 0: this op's only consumer is the residual input of op `side_join`, and nothing in between depends on it (the
     // shortcut convolution of a ResNet "a" block): it may run on a forked stream, concurrently with the ops up to there
@@ -134,7 +139,8 @@ struct Binding {
     size_t item_bytes;
 };
 
-enum LKind { L_INPUT_CAST, L_CONV_TC, L_CONV_SIMT, L_MAXPOOL, L_AVGPOOL, L_FC, L_SOFTMAX, L_OUTPUT_CAST, L_NET, L_TAIL, L_QUANTIZE, L_CONV_I8, L_AVGPOOL_I8, L_OUTPUT_CAST_I8 };
+enum LKind { L_INPUT_CAST, L_CONV_TC, L_CONV_SIMT, L_MAXPOOL, L_AVGPOOL, L_FC, L_SOFTMAX, L_OUTPUT_CAST, L_NET, L_TAIL, L_QUANTIZE, L_CONV_I8, L_AVGPOOL_I8, L_OUTPUT_CAST_I8,
+             L_EMBED_LN, L_LAYERNORM, L_ATTENTION, L_POOLER, L_OUTPUT_ROWS };
 
 // A run of consecutive tcgen05 convolution layers executed by ONE persistent kernel (net_kernel.cu): device-side layer
 // table, dependency ranges and arrival counters live in one allocation owned by the plan.
@@ -168,6 +174,10 @@ struct Launch {
     float qscale = 0.f;           // L_QUANTIZE: 1/s; L_AVGPOOL_I8: s/HW; L_OUTPUT_CAST_I8: s
     int C_in_phys = 0;            // L_QUANTIZE / L_AVGPOOL_I8: channel pitch of the source tensor
     bool net_member = false;      // L_CONV_TC that build_plan folds into an L_NET launch
+    b2k::EmbedArgs embed{};       // L_EMBED_LN (ids / segs / mask are the bindings in_binding, in_binding2, in_binding3)
+    int in_binding2 = -1, in_binding3 = -1;
+    b2k::AttnLaunch attn{};       // L_ATTENTION
+    float eps = 0.f;              // L_LAYERNORM
     int N = 0, C = 0, H = 0, W = 0, C_phys = 0, Ho = 0, Wo = 0, k = 0, stride = 0, pad = 0, K = 0, Cout = 0;
 };
 
@@ -187,9 +197,8 @@ struct BindPatch {
     cudaKernelNodeParams np{};    // func / grid / block / smem as captured
     std::vector<void*> params;    // argument pointer array handed to the driver (entries point into the graph's storage ...)
     int n_params = 0;
-    int in_index = -1, out_index = -1;  // ... except these, which point at in_value / out_value below
-    void* in_value = nullptr;
-    void* out_value = nullptr;
+    std::vector<std::pair<int, int>> slots;  // ... except these (kernel-parameter index, binding), which point at values[k]
+    std::vector<void*> values;               // the binding pointer each slot holds now
     b2k::TailArgs tail{};         // fused tail: the whole argument struct is replaced (its `out` field is the binding)
     bool is_tail = false;
 };
@@ -322,6 +331,68 @@ std::string fixed_str(const char* p, size_t n) {
     return std::string(p, len);
 }
 
+// Tensor, size and geometry checks of the transformer ops (plan_format.h OpRecV3); their bindings are checked once the
+// binding table is read.  Adds the op's FLOPs to the engine's count.
+int validate_transformer_op(b2_engine* e, const Op& op) {
+    using namespace b2plan;
+    const OpRec& r = op.r;
+    const char* nm = op.name.c_str();
+    auto act_ok = [&](const Tensor& t) { return t.kind == T_ACT && t.scale == 0.f && t.c % 8 == 0 && t.c <= 1024; };
+    switch (r.type) {
+        case OP_EMBED_LN: {
+            const Tensor& to = e->tensors[r.out];
+            const Tensor& tm = e->tensors[op.out2];
+            if (!act_ok(to) || to.h != 1 || tm.kind != T_VEC || tm.c != to.w || tm.binding >= 0)
+                return fail(B2_EINVAL, "plan: embedding %s: needs an fp16 [1, S, C <= 1024, C %% 8 == 0] output and an fp32 [S] mask tensor", nm);
+            if (op.vocab < 1 || op.types < 1 || op.positions < int(to.w))
+                return fail(B2_EINVAL, "plan: embedding %s: vocab %d / positions %d / types %d do not cover S = %u", nm, op.vocab, op.positions,
+                            op.types, to.w);
+            if (r.w_bytes != uint64_t(op.vocab + op.positions + op.types) * to.c * 2 || r.b_bytes != uint64_t(to.c) * 8)
+                return fail(B2_EINVAL, "plan: embedding %s: table / gamma / beta sizes do not match hidden size %u", nm, to.c);
+            if (!(op.eps >= 0.f && op.eps < 1.f)) return fail(B2_EINVAL, "plan: embedding %s: bad eps", nm);
+            break;
+        }
+        case OP_LAYERNORM: {
+            const Tensor& ti = e->tensors[r.in];
+            const Tensor& to = e->tensors[r.out];
+            if (!act_ok(ti) || !act_ok(to) || ti.h != to.h || ti.w != to.w || ti.c != to.c || ti.c_phys != to.c_phys)
+                return fail(B2_EINVAL, "plan: layernorm %s: needs fp16 input and output of one shape, C %% 8 == 0, C <= 1024", nm);
+            if (r.w_bytes != 0 || r.b_bytes != uint64_t(ti.c) * 8) return fail(B2_EINVAL, "plan: layernorm %s: gamma / beta size mismatch", nm);
+            if (!(op.eps >= 0.f && op.eps < 1.f)) return fail(B2_EINVAL, "plan: layernorm %s: bad eps", nm);
+            break;
+        }
+        case OP_ATTENTION: {
+            const Tensor& ti = e->tensors[r.in];
+            const Tensor& to = e->tensors[r.out];
+            if (r.res < 0) return fail(B2_EINVAL, "plan: attention %s: no mask tensor", nm);
+            const Tensor& tm = e->tensors[r.res];
+            if (op.heads < 1 || uint32_t(op.heads) * 64 != to.c)
+                return fail(B2_EINVAL, "plan: attention %s: heads * 64 (%d * 64) != hidden size %u", nm, op.heads, to.c);
+            if (!act_ok(to) || ti.kind != T_ACT || ti.scale != 0.f || ti.c != 3 * to.c || ti.c_phys != ti.c)
+                return fail(B2_EINVAL, "plan: attention %s: needs a fused fp16 QKV input of 3 x %u channels", nm, to.c);
+            if (ti.h != 1 || to.h != 1 || ti.w != to.w || tm.kind != T_VEC || tm.c != ti.w)
+                return fail(B2_EINVAL, "plan: attention %s: S does not match between QKV, output and mask", nm);
+            if (ti.w % 64 || ti.w > 128) return fail(B2_EINVAL, "plan: attention %s: S = %u (a multiple of 64, at most 128)", nm, ti.w);
+            if (r.w_bytes || r.b_bytes) return fail(B2_EINVAL, "plan: attention %s carries no weights", nm);
+            e->flops_per_item += 4.0 * double(ti.w) * ti.w * to.c;  // Q K^T and P V
+            break;
+        }
+        case OP_POOLER: {
+            const Tensor& ti = e->tensors[r.in];
+            const Tensor& to = e->tensors[r.out];
+            if (!act_ok(ti) || ti.h != 1 || to.kind != T_VEC || to.c != ti.c)
+                return fail(B2_EINVAL, "plan: pooler %s: needs an fp16 [1, S, C] input and an fp32 [C] output", nm);
+            if (r.w_bytes != uint64_t(ti.c) * ti.c * 2 || r.b_bytes != uint64_t(ti.c) * 4)
+                return fail(B2_EINVAL, "plan: pooler %s: weight / bias size mismatch", nm);
+            e->flops_per_item += 2.0 * ti.c * ti.c;
+            break;
+        }
+        default:
+            break;
+    }
+    return B2_OK;
+}
+
 int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** payload) {
     using namespace b2plan;
     if (!blob || nbytes < sizeof(Header)) return fail(B2_EINVAL, "plan: blob too small (%zu bytes)", nbytes);
@@ -329,11 +400,12 @@ int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** pa
     Header h;
     memcpy(&h, base, sizeof h);
     if (memcmp(h.magic, kMagic, 8) != 0) return fail(B2_EINVAL, "plan: bad magic (not a B2ENGINE blob)");
-    if (h.version != kVersion && h.version != kVersionGrouped)
-        return fail(B2_EINVAL, "plan: version %u, this library reads %u and %u", h.version, kVersion, kVersionGrouped);
+    if (h.version != kVersion && h.version != kVersionGrouped && h.version != kVersionTransformer)
+        return fail(B2_EINVAL, "plan: version %u, this library reads %u, %u and %u", h.version, kVersion, kVersionGrouped, kVersionTransformer);
     if (h.precision > 2) return fail(B2_EINVAL, "plan: unknown precision %u", h.precision);
     if (h.max_batch == 0 || h.max_batch > 4096) return fail(B2_EINVAL, "plan: bad max_batch %u", h.max_batch);
-    const size_t op_rec_size = h.version == kVersionGrouped ? sizeof(OpRecV2) : sizeof(OpRec);
+    const bool v3 = h.version == kVersionTransformer;
+    const size_t op_rec_size = v3 ? sizeof(OpRecV3) : h.version == kVersionGrouped ? sizeof(OpRecV2) : sizeof(OpRec);
     const size_t tbl = sizeof(Header) + size_t(h.n_tensors) * sizeof(TensorRec) + size_t(h.n_ops) * op_rec_size +
                        size_t(h.n_bindings) * sizeof(BindingRec);
     // (overflow-safe: a > n || b > n - a instead of a + b > n)
@@ -379,12 +451,30 @@ int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** pa
                 return fail(B2_EINVAL, "plan: conv %s has %u groups", fixed_str(r2.v1.name, 64).c_str(), r2.groups);
             if (r2.v1.type == OP_CONV) op.groups = int(r2.groups);
         }
+        if (v3) {
+            OpRecV3 r3;
+            memcpy(&r3, p, sizeof r3);
+            if (r3.v1.type == OP_CONV && (r3.groups == 0 || r3.groups > 65536))
+                return fail(B2_EINVAL, "plan: conv %s has %u groups", fixed_str(r3.v1.name, 64).c_str(), r3.groups);
+            if (r3.v1.type == OP_CONV) op.groups = int(r3.groups);
+            if (r3.heads > 4096 || r3.vocab > (1u << 24) || r3.positions > (1u << 20) || r3.types > (1u << 20))
+                return fail(B2_EINVAL, "plan: op %s has out-of-range transformer fields", fixed_str(r3.v1.name, 64).c_str());
+            op.heads = int(r3.heads), op.vocab = int(r3.vocab), op.positions = int(r3.positions), op.types = int(r3.types);
+            op.binding2 = r3.binding2, op.binding3 = r3.binding3, op.out2 = r3.out2;
+            op.eps = r3.eps, op.flags = r3.flags;
+        }
         op.name = fixed_str(op.r.name, 64);
         const OpRec& r = op.r;
-        if (r.type > OP_QUANTIZE) return fail(B2_EINVAL, "plan: op %s has unknown type %u", op.name.c_str(), r.type);
-        const bool in_opt = r.type == OP_INPUT_CAST, out_opt = r.type == OP_OUTPUT_CAST;
-        if (!tensor_ok(r.in, in_opt) || !tensor_ok(r.out, out_opt) || !tensor_ok(r.res, true))
+        if (r.type > OP_POOLER) return fail(B2_EINVAL, "plan: op %s has unknown type %u", op.name.c_str(), r.type);
+        const bool transformer_op = r.type >= OP_EMBED_LN;
+        if (transformer_op && (!v3 || h.precision != B2_PREC_FP16))
+            return fail(B2_EINVAL, "plan: op %s: transformer ops need a version-3 fp16 plan", op.name.c_str());
+        const bool in_opt = r.type == OP_INPUT_CAST || r.type == OP_EMBED_LN, out_opt = r.type == OP_OUTPUT_CAST;
+        if (!tensor_ok(r.in, in_opt) || !tensor_ok(r.out, out_opt) || !tensor_ok(r.res, true) || !tensor_ok(op.out2, r.type != OP_EMBED_LN))
             return fail(B2_EINVAL, "plan: op %s references a missing tensor", op.name.c_str());
+        if (r.type != OP_EMBED_LN && (op.out2 != -1 || op.binding2 != -1 || op.binding3 != -1))
+            return fail(B2_EINVAL, "plan: op %s: second output / extra bindings exist for the embedding op only", op.name.c_str());
+        if (r.type == OP_EMBED_LN && r.in != -1) return fail(B2_EINVAL, "plan: embedding %s reads bindings, not a tensor", op.name.c_str());
         if ((r.type == OP_INPUT_CAST || r.type == OP_OUTPUT_CAST) && (r.binding < 0 || r.binding >= int(h.n_bindings)))
             return fail(B2_EINVAL, "plan: cast op %s has a bad binding", op.name.c_str());
         if (r.w_off > h.payload_bytes || r.w_bytes > h.payload_bytes - r.w_off || r.b_off > h.payload_bytes ||
@@ -412,6 +502,11 @@ int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** pa
         if (r.type == OP_CONV) {
             if (r.k == 0 || r.stride == 0 || int(r.taps) != op.kh() * op.kw() || r.taps_phys < r.taps || op.sw() == 0)
                 return fail(B2_EINVAL, "plan: conv %s has bad geometry", op.name.c_str());
+            if ((r.relu & kConvGelu) && (!v3 || (r.relu & (kConvRelu | kConvInt8))))
+                return fail(B2_EINVAL, "plan: conv %s: GELU excludes ReLU and INT8 and needs a version-3 plan", op.name.c_str());
+            if ((r.relu & kConvGelu) && (r.k != 1 || r.kw || r.stride != 1 || r.pad_ || !(r.relu & kConvPacked) ||
+                                         r.cin_phys % 64 || op.groups != 1))
+                return fail(B2_EINVAL, "plan: conv %s: GELU layers are dense 1x1 stride-1 convolutions with packed weights", op.name.c_str());
             const bool i8 = (r.relu & 4) != 0;
             if (op.groups > 1) {  // layouts: plan_format.h (OpRecV2)
                 const uint32_t g = uint32_t(op.groups);
@@ -460,6 +555,9 @@ int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** pa
             if (r.w_bytes != size_t(r.cout) * K * elt || r.b_bytes != size_t(r.cout) * 4)
                 return fail(B2_EINVAL, "plan: fc %s weight size mismatch", op.name.c_str());
             e->flops_per_item += 2.0 * ti.h * ti.w * ti.c * r.cout;
+        } else if (transformer_op) {
+            int rc = validate_transformer_op(e, op);
+            if (rc) return rc;
         }
         e->ops.push_back(op);
     }
@@ -474,7 +572,9 @@ int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** pa
         b.nd = r.nd;
         if (r.nd == 0 || r.nd > 8) return fail(B2_EINVAL, "plan: binding %s has bad rank", b.name.c_str());
         // fp32 is the reference's binding contract; fp16 INPUT bindings are the secondary mode of fp16 engines
-        if (r.dtype != B2_DT_FLOAT && !(r.dtype == B2_DT_HALF && b.is_input && h.precision == B2_PREC_FP16))
+        // (int32 inputs: the token bindings of version-3 plans, checked below)
+        if (r.dtype != B2_DT_FLOAT && !(r.dtype == B2_DT_HALF && b.is_input && h.precision == B2_PREC_FP16) &&
+            !(r.dtype == B2_DT_INT32 && b.is_input && v3))
             return fail(B2_EINVAL, "plan: binding %s: bindings are fp32 (inputs of fp16 engines may be fp16)", b.name.c_str());
         size_t n = 1;
         for (uint32_t d = 0; d < 8; ++d) {
@@ -495,6 +595,34 @@ int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** pa
         const bool s2d = r.type == OP_INPUT_CAST && r.k == 2;  // (its geometry is re-checked when the launch plan is built)
         if (b.is_input != (r.type == OP_INPUT_CAST) || (!s2d && n != size_t(t.c) * t.h * t.w))
             return fail(B2_EINVAL, "plan: cast op %s: binding %s and tensor %s disagree", op.name.c_str(), b.name.c_str(), t.name.c_str());
+        if (b.dtype == B2_DT_INT32)
+            return fail(B2_EINVAL, "plan: cast op %s reads int32 binding %s (int32 bindings feed the embedding op only)", op.name.c_str(),
+                        b.name.c_str());
+    }
+    // int32 bindings: the token inputs of OP_EMBED_LN, [S] per item, and nothing else reads them
+    std::vector<int> int32_readers(e->bindings.size(), 0);
+    for (const Op& op : e->ops) {
+        const OpRec& r = op.r;
+        if (r.type == OP_POOLER && e->tensors[r.out].binding >= 0 && e->bindings[size_t(e->tensors[r.out].binding)].is_input)
+            return fail(B2_EINVAL, "plan: pooler %s writes an input binding", op.name.c_str());
+        if (r.type != OP_EMBED_LN) continue;
+        const uint32_t S = e->tensors[r.out].w;
+        for (int bi : {r.binding, op.binding2, op.binding3}) {
+            if (bi < 0 || bi >= int(h.n_bindings)) return fail(B2_EINVAL, "plan: embedding %s has a bad binding", op.name.c_str());
+            const Binding& b = e->bindings[size_t(bi)];
+            if (b.dtype != B2_DT_INT32 || !b.is_input || b.nd != 1 || b.dims[0] != int32_t(S))
+                return fail(B2_EINVAL, "plan: embedding %s: binding %s must be an int32 input of shape [S = %u]", op.name.c_str(), b.name.c_str(), S);
+            ++int32_readers[size_t(bi)];
+        }
+    }
+    for (size_t i = 0; i < e->bindings.size(); ++i) {
+        if (e->bindings[i].dtype != B2_DT_INT32) continue;
+        if (int32_readers[i] != 1)
+            return fail(B2_EINVAL, "plan: int32 binding %s must feed exactly one embedding op slot", e->bindings[i].name.c_str());
+        for (const Tensor& t : e->tensors)
+            if (t.binding == int(i))
+                return fail(B2_EINVAL, "plan: int32 binding %s is the storage of tensor %s (int32 bindings feed the embedding op only)",
+                            e->bindings[i].name.c_str(), t.name.c_str());
     }
     if (h.n_tactics) {  // tactic table written by an offline tuning run (b2_engine_get_tactics -> builder.attach_tactics)
         if (h.tactics_offset > nbytes || size_t(h.n_tactics) > (nbytes - h.tactics_offset) / sizeof(TacticRec))
@@ -536,7 +664,8 @@ void plan_arena(b2_engine* e) {
     }
     for (size_t i = 0; i < e->ops.size(); ++i) {
         const auto& r = e->ops[i].r;
-        if (r.out >= 0 && e->tensors[r.out].def < 0) e->tensors[r.out].def = int(i);
+        for (int t : {r.out, e->ops[i].out2})
+            if (t >= 0 && e->tensors[t].def < 0) e->tensors[t].def = int(i);
         for (int t : {r.in, r.res})
             if (t >= 0) e->tensors[t].last_use = std::max(e->tensors[t].last_use, int(i));
         // a side op may still be READING its input while the ops before the join run: keep that buffer until the join
@@ -733,6 +862,10 @@ int make_conv_launch(b2_context* c, const Op& op, int batch, const ConvConfig& c
     if (op.groups > 1 && (!span || cfg.ws || cfg.splits > 1 || cfg.cn > 1 || cfg.halo || span % cfg.bn))
         return fail(B2_EINVAL, "conv %s: grouped convolutions run one tile per CTA with an N tile dividing %d (bn=%d ws=%d splits=%d cn=%d halo=%d)",
                     op.name.c_str(), span, cfg.bn, cfg.ws, cfg.splits, cfg.cn, cfg.halo);
+    const bool gelu = (r.relu & b2plan::kConvGelu) != 0;
+    if (gelu && (cfg.ws || cfg.halo || cfg.cn > 1))
+        return fail(B2_EINVAL, "conv %s: GELU layers run on the one-tile-per-CTA kernel (ws=%d halo=%d cn=%d)", op.name.c_str(), cfg.ws, cfg.halo,
+                    cfg.cn);
     b2k::ConvLaunch& cl = *out;
     memset(&cl, 0, sizeof cl);
     cl.kb = conv_kb(c, op);
@@ -771,10 +904,11 @@ int make_conv_launch(b2_context* c, const Op& op, int batch, const ConvConfig& c
     a.stride_w = op.sw();
     a.pad_h = op.ph();
     a.pad_w = op.pw_lo();
-    a.relu = int(r.relu & 1);
+    a.relu = int(r.relu & (b2plan::kConvRelu | b2plan::kConvGelu));  // bit 0 ReLU, bit 3 GELU (epilogues of every tactic)
     a.wpacked = (r.relu & 2) && !c->no_pack ? w : nullptr;
+    // (GELU layers are always read as a plain matrix: their kernel exists for that operand path only)
     const bool tiled = r.k == 1 && op.kw() == 1 && r.stride == 1 && op.sw() == 1 && r.pad_ == 0 && op.pw_lo() == 0 &&
-                       op.pw_hi() == 0 && kb64 && !c->force_im2col;
+                       op.pw_hi() == 0 && kb64 && (!c->force_im2col || gelu);
     a.a_mode = tiled ? b2k::A_TILED : b2k::A_IM2COL;
     if (cfg.halo) {
         const int R = conv_halo_rows(c, op);
@@ -921,11 +1055,11 @@ int autotune_conv(b2_context* c, const Op& op, int batch, int fixed_splits, int 
             if (fixed_splits > 0 && sp != fixed_splits) continue;
             if (span && (ws || sp > 1)) continue;
             if (ws) {  // persistent warp-specialised tactic: 64-wide K, packed weights, no split-K
-                if (c->force_ws < 0 || kbsz != 64 || !(r.relu & 2) || sp != 1) continue;
+                if (c->force_ws < 0 || kbsz != 64 || !(r.relu & 2) || sp != 1 || (r.relu & b2plan::kConvGelu)) continue;
                 if (!b2k::conv_ws_config_exists(bn, st, sps) || b2k::conv_ws_smem(bn, st, sps, r.res >= 0) > 227 * 1024) continue;
                 if (sps == 2 && nkb < 4) continue;
             } else {
-            if (c->force_ws > 0 && kbsz == 64 && (r.relu & 2) && !span) continue;
+            if (c->force_ws > 0 && kbsz == 64 && (r.relu & 2) && !span && !(r.relu & b2plan::kConvGelu)) continue;
             if (!b2k::conv_config_exists(bn, kbsz, st, sps)) continue;
             if (b2k::conv_smem_bytes(bn, st, r.res >= 0, sps) > 227 * 1024) continue;
             }
@@ -942,12 +1076,12 @@ int autotune_conv(b2_context* c, const Op& op, int batch, int fixed_splits, int 
                            (sp - 1) * kpc >= nkb ||
                            size_t(tiles) * sp * 128 * bn * 4 > kSplitWorkspaceBytes))
                 continue;  // split-K only where the plain grid leaves SMs idle
-            const bool cn_forced_here = c->force_cn > 1 && kbsz == 64 && !span && (int(r.cout_phys) / bn) % c->force_cn == 0 &&
+            const bool cn_forced_here = c->force_cn > 1 && kbsz == 64 && !span && !(r.relu & b2plan::kConvGelu) && (int(r.cout_phys) / bn) % c->force_cn == 0 &&
                                         b2k::conv_cluster_config_exists(bn, st, sps, c->force_cn);
             if (!cn_forced_here) candidates.push_back(ConvConfig{bn, st, sp, 0.0, sps, 0, 1});
             // clusters along N that multicast the activation tile: never won a timing (the L2 read is shared but
             // every SM still ingests the whole tile, and the cluster barriers cost latency) -> tried only on request
-            if (kbsz == 64 && c->force_cn > 0 && !span)
+            if (kbsz == 64 && c->force_cn > 0 && !span && !(r.relu & b2plan::kConvGelu))
                 for (int cn = 2; cn <= 4; cn *= 2)
                     if ((int(r.cout_phys) / bn) % cn == 0 && (!c->force_cn || cn == c->force_cn) &&
                         b2k::conv_cluster_config_exists(bn, st, sps, cn))
@@ -1085,7 +1219,9 @@ bool tactic_applies(const b2_context* c, const Op& op, int batch, const ConvConf
     }
     const int kbsz = conv_kb(c, op);
     if (cfg.halo) return conv_halo_rows(c, op) > 0 && b2k::conv_halo_config_exists(cfg.bn);
-    if (cfg.ws) return kbsz == 64 && b2k::conv_ws_config_exists(cfg.bn, cfg.stages, cfg.sps);
+    // the persistent kernel's epilogue has no GELU, and its kernel has no cluster instantiation: a GELU layer takes neither
+    if ((r.relu & b2plan::kConvGelu) && cfg.cn > 1) return false;
+    if (cfg.ws) return kbsz == 64 && !(r.relu & b2plan::kConvGelu) && b2k::conv_ws_config_exists(cfg.bn, cfg.stages, cfg.sps);
     if (!b2k::conv_config_exists(cfg.bn, kbsz, cfg.stages, cfg.sps)) return false;
     if (cfg.splits > 1) {
         const int tiles = ((batch * int(c->e->tensors[r.out].h * c->e->tensors[r.out].w) + 127) / 128) * (int(r.cout_phys) / cfg.bn);
@@ -1463,7 +1599,8 @@ int build_plan(b2_context* c, int batch, Plan** out) {
             }
             case b2plan::OP_OUTPUT_CAST: {
                 const Tensor& t = e->tensors[r.in];
-                L.kind = t.scale > 0.f ? L_OUTPUT_CAST_I8 : L_OUTPUT_CAST;
+                L.kind = t.scale > 0.f ? L_OUTPUT_CAST_I8 : (op.flags & 1) ? L_OUTPUT_ROWS : L_OUTPUT_CAST;
+                if (L.kind == L_OUTPUT_ROWS && !half) return fail(B2_EINVAL, "output cast %s: channels-last outputs need an fp16 engine", op.name.c_str());
                 L.qscale = t.scale;
                 L.in = tptr(r.in);
                 L.out_binding = r.binding;
@@ -1519,21 +1656,23 @@ int build_plan(b2_context* c, int batch, Plan** out) {
                         b2k::conv_smem_bytes(cfg.bn, cfg.stages, r.res >= 0, 2) <= 227 * 1024)
                         cfg.sps = 2;
                     // (the persistent, halo and cluster tactics never take a grouped convolution)
-                    if (c->force_ws > 0 && kbsz == 64 && (r.relu & 2) && cfg.splits == 1 && !span &&
+                    if (c->force_ws > 0 && kbsz == 64 && (r.relu & 2) && cfg.splits == 1 && !span && !(r.relu & b2plan::kConvGelu) &&
                         b2k::conv_ws_config_exists(cfg.bn, cfg.stages, cfg.sps) &&
                         b2k::conv_ws_smem(cfg.bn, cfg.stages, cfg.sps, r.res >= 0) <= 227 * 1024)
                         cfg.ws = std::min(((M + 127) / 128) * (int(r.cout_phys) / cfg.bn), c->force_ws > 1 ? c->force_ws : g_sms);
                     if (c->force_halo > 0 && conv_halo_rows(c, op) && b2k::conv_halo_config_exists(cfg.bn) && cfg.splits == 1 &&
                         int(r.cin_phys) / 64 <= 8 && b2k::conv_halo_smem(cfg.bn, int(to.w), conv_halo_rows(c, op), int(r.cin_phys) / 64) <= 227 * 1024)
                         cfg.halo = 1, cfg.ws = 0, cfg.cn = 1;
-                    if (c->force_cn > 1 && kbsz == 64 && cfg.ws == 0 && !cfg.halo && !span && (int(r.cout_phys) / cfg.bn) % c->force_cn == 0)
+                    if (c->force_cn > 1 && kbsz == 64 && cfg.ws == 0 && !cfg.halo && !span && !(r.relu & b2plan::kConvGelu) &&
+                        (int(r.cout_phys) / cfg.bn) % c->force_cn == 0)
                         cfg.cn = c->force_cn;
                     const bool forced = c->force_bn || c->force_stages || c->force_splits || c->force_sps;
                     const int op_index = int(&op - &e->ops[0]);
                     // member of a persistent-kernel run: 64-channel K blocks, packed weights, 64 | Cout; no tactic to tune.
                     // A grouped layer is never a member: it ends a run
                     const bool net_ok = c->net && !forced && kbsz == 64 && (r.relu & 2) && !c->no_pack && r.cout_phys % 64 == 0 &&
-                                        c->force_ws <= 0 && c->force_cn <= 0 && c->force_halo <= 0 && !c->force_im2col && op.groups == 1;
+                                        c->force_ws <= 0 && c->force_cn <= 0 && c->force_halo <= 0 && !c->force_im2col && op.groups == 1 &&
+                                        !(r.relu & b2plan::kConvGelu);  // (the network kernel's epilogue has no GELU)
                     if (net_ok) {
                         int bn = (r.cout_phys % 128 == 0) ? 128 : 64;
                         if (c->net_bn == 64) bn = 64;
@@ -1565,7 +1704,7 @@ int build_plan(b2_context* c, int batch, Plan** out) {
                     a.Ho = int(to.h), a.Wo = int(to.w), a.Cout = int(r.cout), a.Cout_phys = int(r.cout_phys);
                     a.kh = op.kh(), a.kw = op.kw(), a.taps_phys = int(r.taps_phys);
                     a.stride_h = op.sh(), a.stride_w = op.sw(), a.pad_h = op.ph(), a.pad_w = op.pw_lo();
-                    a.relu = int(r.relu & 1);
+                    a.relu = int(r.relu & (b2plan::kConvRelu | b2plan::kConvGelu));
                     a.w_packed = int((r.relu >> 1) & 1);
                     a.groups = op.groups;
                     a.wk_tap = op.groups == 1 ? int(r.cin_phys) : span ? span : int(r.cin) / op.groups;
@@ -1619,6 +1758,58 @@ int build_plan(b2_context* c, int batch, Plan** out) {
                 L.out_binding = to.binding;
                 L.C = int(ti.c);
                 L.bytes = double(batch) * ti.c * 8.0;
+                break;
+            }
+            case b2plan::OP_EMBED_LN: {
+                const Tensor& to = e->tensors[r.out];
+                L.kind = L_EMBED_LN;
+                L.in_binding = r.binding, L.in_binding2 = op.binding2, L.in_binding3 = op.binding3;
+                b2k::EmbedArgs& a = L.embed;
+                a.tables = reinterpret_cast<const __half*>(e->d_payload + r.w_off);
+                a.gamma = reinterpret_cast<const float*>(e->d_payload + r.b_off);
+                a.beta = a.gamma + to.c;
+                a.out = reinterpret_cast<__half*>(tptr(r.out));
+                a.mask_add = reinterpret_cast<float*>(tptr(op.out2));
+                a.N = batch, a.S = int(to.w), a.C = int(to.c), a.C_phys = int(to.c_phys);
+                a.vocab = op.vocab, a.positions = op.positions, a.types = op.types, a.eps = op.eps;
+                L.bytes = double(batch) * (to.item_bytes + to.w * (12.0 + 3.0 * to.c * 2));
+                break;
+            }
+            case b2plan::OP_LAYERNORM: {
+                const Tensor& ti = e->tensors[r.in];
+                L.kind = L_LAYERNORM;
+                L.in = tptr(r.in), L.out = tptr(r.out);
+                L.bias = reinterpret_cast<const float*>(e->d_payload + r.b_off);
+                L.H = int(ti.h) * int(ti.w), L.C = int(ti.c), L.C_phys = int(ti.c_phys), L.eps = op.eps;
+                L.bytes = 2.0 * batch * ti.item_bytes;
+                break;
+            }
+            case b2plan::OP_ATTENTION: {
+                const Tensor& ti = e->tensors[r.in];
+                const Tensor& to = e->tensors[r.out];
+                L.kind = L_ATTENTION;
+                b2k::AttnLaunch& a = L.attn;
+                a.mask_add = reinterpret_cast<const float*>(tptr(r.res));
+                a.out = reinterpret_cast<__half*>(tptr(r.out));
+                a.N = batch, a.S = int(ti.w), a.heads = op.heads, a.H = int(to.c), a.out_pitch = int(to.c_phys);
+                int rc = make_map_2d(&a.mapQKV, tptr(r.in), ti.c_phys, uint64_t(batch) * ti.w, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B);
+                if (rc) return rc;
+                L.flops = 4.0 * batch * double(ti.w) * ti.w * to.c;
+                L.bytes = double(batch) * (ti.item_bytes + to.item_bytes);
+                break;
+            }
+            case b2plan::OP_POOLER: {
+                const Tensor& ti = e->tensors[r.in];
+                const Tensor& to = e->tensors[r.out];
+                L.kind = L_POOLER;
+                L.in = tptr(r.in);
+                L.out = tptr(r.out);
+                L.out_binding = to.binding;
+                L.w = e->d_payload + r.w_off;
+                L.bias = reinterpret_cast<const float*>(e->d_payload + r.b_off);
+                L.W = int(ti.w), L.C = int(ti.c), L.C_phys = int(ti.c_phys);
+                L.flops = 2.0 * batch * ti.c * ti.c;
+                L.bytes = double(r.w_bytes) + double(batch) * (ti.c * 2.0 + to.item_bytes);
                 break;
             }
             default:
@@ -1686,6 +1877,24 @@ int run_launch(const b2_engine* e, const Launch& L, void* const* bindings, cudaS
             t.out = static_cast<float*>(out);
             return b2k::launch_tail_f16(t, s);
         }
+        case L_EMBED_LN: {
+            b2k::EmbedArgs a = L.embed;
+            a.ids = static_cast<const int*>(in);
+            a.segs = static_cast<const int*>(bindings[L.in_binding2]);
+            a.mask = static_cast<const int*>(bindings[L.in_binding3]);
+            return b2k::launch_embed_ln(a, s);
+        }
+        case L_LAYERNORM:
+            return b2k::launch_layernorm(static_cast<const __half*>(in), static_cast<__half*>(out), L.bias, L.bias + L.C,
+                                         static_cast<long long>(L.N) * L.H, L.C, L.C_phys, L.eps, s);
+        case L_ATTENTION:
+            return b2k::launch_attention(L.attn, s);
+        case L_POOLER:
+            return b2k::launch_pooler(static_cast<const __half*>(in), static_cast<const __half*>(L.w), L.bias, static_cast<float*>(out), L.N,
+                                      L.W, L.C, L.C_phys, s);
+        case L_OUTPUT_ROWS:
+            return b2k::launch_output_cast_rows(static_cast<const __half*>(in), static_cast<float*>(out), static_cast<long long>(L.N) * L.H * L.W,
+                                                L.C, L.C_phys, s);
     }
     return int(cudaErrorInvalidValue);
 }
@@ -1754,8 +1963,8 @@ int instantiate_segment(b2_context* c, Plan* plan, Segment* sg, void* const* bin
     return B2_OK;
 }
 
-// Which argument of a binding-dependent launch carries the binding pointer (positions in the kernels' parameter lists,
-// kernels.cu) and how many arguments the kernel has.
+// Which arguments of a binding-dependent launch carry binding pointers (positions in the kernels' parameter lists,
+// kernels.cu / bert_kernels.cu) and how many arguments the kernel has.
 bool patch_layout(const b2_engine* e, const Launch& L, BindPatch* p) {
     const bool half = e->half();
     switch (L.kind) {
@@ -1763,24 +1972,33 @@ bool patch_layout(const b2_engine* e, const Launch& L, BindPatch* p) {
             if (L.k == 2) p->n_params = 8;                                  // input_cast_s2d_kernel(src, dst, N, C, H, W, pad_l, pad_r)
             else if (half && L.C_phys == 8 && L.C <= 8) p->n_params = 5;    // input_cast_c8_kernel(src, dst, N, C, HW)
             else p->n_params = 6;                                           // input_cast_kernel(src, dst, N, C, HW, C_phys)
-            p->in_index = 0;
+            p->slots = {{0, L.in_binding}};
             return true;
         case L_OUTPUT_CAST:
-            p->n_params = 6, p->out_index = 1;                              // output_cast_kernel(src, dst, N, C, HW, C_phys)
+            p->n_params = 6, p->slots = {{1, L.out_binding}};               // output_cast_kernel(src, dst, N, C, HW, C_phys)
             return true;
         case L_OUTPUT_CAST_I8:
-            p->n_params = 7, p->out_index = 1;                              // output_cast_i8_kernel(src, dst, N, C, HW, C_phys, s)
+            p->n_params = 7, p->slots = {{1, L.out_binding}};               // output_cast_i8_kernel(src, dst, N, C, HW, C_phys, s)
             return true;
         case L_FC:
-            p->n_params = 7, p->out_index = 3;                              // fc kernels (in, w, bias, out, N, K, Cout)
+            p->n_params = 7, p->slots = {{3, L.out_binding}};               // fc kernels (in, w, bias, out, N, K, Cout)
             return L.in_binding < 0;
         case L_SOFTMAX:
             p->n_params = 3;                                                // softmax_kernel(in, out, C)
-            if (L.in_binding >= 0) p->in_index = 0;
-            if (L.out_binding >= 0) p->out_index = 1;
+            if (L.in_binding >= 0) p->slots.push_back({0, L.in_binding});
+            if (L.out_binding >= 0) p->slots.push_back({1, L.out_binding});
             return true;
         case L_TAIL:
             p->n_params = 1, p->is_tail = true, p->tail = L.tail;
+            return true;
+        case L_EMBED_LN:                                                    // embed_ln_kernel(ids, segs, mask, args)
+            p->n_params = 4, p->slots = {{0, L.in_binding}, {1, L.in_binding2}, {2, L.in_binding3}};
+            return true;
+        case L_POOLER:                                                      // pooler_kernel(h, w, b, out, N, S, C, C_phys)
+            p->n_params = 8, p->slots = {{3, L.out_binding}};
+            return true;
+        case L_OUTPUT_ROWS:                                                 // output_cast_rows_kernel(src, dst, rows, C, C_phys)
+            p->n_params = 5, p->slots = {{1, L.out_binding}};
             return true;
         default:
             return false;
@@ -1845,9 +2063,9 @@ int instantiate_plan_graph(b2_context* c, Plan* plan, void* const* bindings, cud
     plan->graph = graph, plan->exec = exec, plan->patches = std::move(patches);
     // the values captured are the ones the graph holds now
     for (BindPatch& p : plan->patches) {
-        const Launch& L = plan->launches[size_t(p.launch)];
-        p.in_value = L.in_binding >= 0 ? bindings[L.in_binding] : nullptr;
-        p.out_value = L.out_binding >= 0 ? bindings[L.out_binding] : nullptr;
+        p.values.clear();
+        for (const auto& sl : p.slots) p.values.push_back(bindings[sl.second]);
+        if (p.is_tail) p.values.push_back(bindings[plan->launches[size_t(p.launch)].out_binding]);
     }
     return B2_OK;
 }
@@ -1855,17 +2073,20 @@ int instantiate_plan_graph(b2_context* c, Plan* plan, void* const* bindings, cud
 // Points the binding-dependent nodes at this request's buffers (no-op for pointers the graph already holds).
 int patch_plan_graph(Plan* plan, void* const* bindings) {
     for (BindPatch& p : plan->patches) {
-        const Launch& L = plan->launches[size_t(p.launch)];
-        void* in = L.in_binding >= 0 ? bindings[L.in_binding] : nullptr;
-        void* out = L.out_binding >= 0 ? bindings[L.out_binding] : nullptr;
-        if (in == p.in_value && out == p.out_value) continue;
-        p.in_value = in, p.out_value = out;
-        if (p.is_tail) {
+        if (p.is_tail) {  // the whole argument struct is replaced: its `out` field is the binding
+            void* out = bindings[plan->launches[size_t(p.launch)].out_binding];
+            if (out == p.values[0]) continue;
+            p.values[0] = out;
             p.tail.out = static_cast<float*>(out);
             p.params[0] = &p.tail;
         } else {
-            if (p.in_index >= 0) p.params[size_t(p.in_index)] = &p.in_value;
-            if (p.out_index >= 0) p.params[size_t(p.out_index)] = &p.out_value;
+            bool same = true;
+            for (size_t k = 0; k < p.slots.size(); ++k) same = same && bindings[p.slots[k].second] == p.values[k];
+            if (same) continue;
+            for (size_t k = 0; k < p.slots.size(); ++k) {
+                p.values[k] = bindings[p.slots[k].second];
+                p.params[size_t(p.slots[k].first)] = &p.values[k];
+            }
         }
         cudaKernelNodeParams np = p.np;
         np.kernelParams = p.params.data();
@@ -1940,6 +2161,7 @@ static int deserialize_impl(b2_runtime* rt, const void* blob, size_t nbytes, boo
         rc = b2k::init_conv_kernels();
         if (!rc) rc = b2k::init_net_kernel();
         if (!rc) rc = b2k::init_conv_i8_kernels();
+        if (!rc) rc = b2k::init_attention_kernels();
         if (rc) return fail(B2_ECUDA, "kernel attribute setup failed: %s", cudaGetErrorString(cudaError_t(rc)));
         const size_t bytes = std::max<size_t>(e->payload_bytes, 256);
         if (rt && rt->alloc) {
@@ -2496,7 +2718,8 @@ const char* b2_context_launch_name(b2_context* c, int batch, int i) {
     const Launch* L = get_launch(c, batch, i);
     if (!L) return nullptr;
     static const char* kinds[] = {"input_cast", "conv_tcgen05", "conv_simt", "maxpool", "avgpool", "fc", "softmax", "output_cast", "net_tcgen05", "tail_pool_fc_softmax",
-                                  "quantize", "conv_i8_tcgen05", "avgpool_i8", "output_cast_i8"};
+                                  "quantize", "conv_i8_tcgen05", "avgpool_i8", "output_cast_i8", "embed_ln", "layernorm", "attention_f16_wgmma",
+                                  "pooler", "output_cast_rows"};
     s = std::string(kinds[L->kind]) + ":" + L->name;
     if (L->kind == L_CONV_TC)
         s += " bn=" + std::to_string(L->conv.bn) + " kb=" + std::to_string(L->conv.kb) +
@@ -2506,7 +2729,8 @@ const char* b2_context_launch_name(b2_context* c, int batch, int i) {
              (L->conv.args.a_mode == b2k::A_TILED ? " tiled" : " im2col") +
              " grid=" + std::to_string(L->conv.grid_n) + "x" + std::to_string(L->conv.grid_m) + "x" +
              std::to_string(L->conv.args.splits) + " kblk=" + std::to_string(L->conv.args.num_kblocks) +
-             (L->conv.args.group_span ? " span=" + std::to_string(L->conv.args.group_span) : std::string());
+             (L->conv.args.group_span ? " span=" + std::to_string(L->conv.args.group_span) : std::string()) +
+             ((L->conv.args.relu & b2plan::kConvGelu) ? " gelu" : "");
     if (L->kind == L_CONV_I8)
         s += " bn=" + std::to_string(L->i8.bn) + " st=" + std::to_string(L->i8.stages) + (L->i8.args.a_mode == b2k::A_TILED ? " tiled" : " im2col") + " grid=" +
              std::to_string(L->i8.grid_n) + "x" + std::to_string(L->i8.grid_m) + " kblk=" + std::to_string(L->i8.args.num_kblocks);

@@ -53,7 +53,10 @@ struct FragPos {
         : row0(64 * (consumer_warp >> 2) + 16 * (consumer_warp & 3) + (lane >> 2)), col0(2 * (lane & 3)) {}
 };
 
-template <int BN, int KB, int STAGES, int SPS, int CN = 1, bool DBG = false, int AV = 0>
+// GELU: the epilogue applies GELU (erf form) after bias and residual instead of the optional ReLU.  Instantiated for the
+// tiled, packed-weight operand path only (AV == 2: the 1x1 layers of transformer encoders); the other instantiations keep
+// the ReLU-only epilogue unchanged.
+template <int BN, int KB, int STAGES, int SPS, int CN = 1, bool DBG = false, int AV = 0, bool GELU = false>
 __global__ void __launch_bounds__(kConvThreads, BN <= 64 ? 2 : 1)
 conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
                  const __grid_constant__ CUtensorMap mapOut, const __grid_constant__ CUtensorMap mapRes,
@@ -393,7 +396,10 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
             v0 += rf.x;
             v1 += rf.y;
         }
-        if (p.relu) {
+        if constexpr (GELU) {
+            v0 = gelu_erf(v0);
+            v1 = gelu_erf(v1);
+        } else if (p.relu) {
             v0 = fmaxf(v0, 0.0f);
             v1 = fmaxf(v1, 0.0f);
         }
@@ -710,7 +716,7 @@ conv_f16_tcgen05_ws(const __grid_constant__ CUtensorMap mapA, const __grid_const
                         v0 += rf.x;
                         v1 += rf.y;
                     }
-                    if (p.relu) {
+                    if (p.relu) {  // (never a GELU layer: the engine refuses this tactic for them)
                         v0 = fmaxf(v0, 0.0f);
                         v1 = fmaxf(v1, 0.0f);
                     }
@@ -886,7 +892,7 @@ conv3x3_halo_tcgen05(const __grid_constant__ CUtensorMap mapIn, const __grid_con
                 const int row = fp.row0 + 8 * h, col = 8 * j + fp.col0;
                 const uint32_t so = static_cast<uint32_t>((col / OW) * (128 * 128)) + swz_off<128>(row, (col % OW) / 8) + (col % 8) * 2;
                 float v0 = acc[4 * j + 2 * h] + s_bias[col], v1 = acc[4 * j + 2 * h + 1] + s_bias[col + 1];
-                if (p.relu) {
+                if (p.relu) {  // (never a GELU layer: the halo tactic is refused for them)
                     v0 = fmaxf(v0, 0.0f);
                     v1 = fmaxf(v1, 0.0f);
                 }
@@ -944,6 +950,14 @@ static int launch_one(const ConvLaunch& L, cudaStream_t stream) {
     dim3 grid(L.grid_n, L.grid_m, L.args.splits);
     const size_t smem = size_t(conv_smem_layout_bytes(BN, STAGES, L.args.residual != nullptr, SPS));
     if (CN > 1 && (KB != 64 || L.grid_n % CN != 0 || L.args.cn != CN)) return static_cast<int>(cudaErrorInvalidValue);
+    if (L.args.relu & 8) {  // GELU: the tiled packed-weight instantiation, one CTA per cluster, no debug stamps
+        if constexpr (CN == 1 && KB == 64) {
+            if (L.args.wpacked != nullptr && L.args.a_mode == A_TILED && L.args.dbg == nullptr && L.args.dbg_mode == 0)
+                return launch_kernel_cluster(conv_f16_tcgen05<BN, KB, STAGES, SPS, 1, false, 2, true>, grid, dim3(kConvThreads), smem, stream,
+                                             true, 1u, L.mapA, L.mapB, L.mapOut, L.mapRes, L.args);
+        }
+        return static_cast<int>(cudaErrorInvalidValue);
+    }
     if (CN == 1 && (L.args.dbg != nullptr || L.args.dbg_mode != 0))
         return launch_kernel_cluster(conv_f16_tcgen05<BN, KB, STAGES, SPS, 1, true>, grid, dim3(kConvThreads), smem, stream, true, 1u, L.mapA,
                                      L.mapB, L.mapOut, L.mapRes, L.args);
@@ -972,6 +986,8 @@ static int init_one() {
             if ((e = static_cast<int>(cudaFuncSetAttribute(conv_f16_tcgen05<BN, KB, STAGES, SPS, 1, false, 1>,
                                                            cudaFuncAttributeMaxDynamicSharedMemorySize, bytes)))) return e;
             if ((e = static_cast<int>(cudaFuncSetAttribute(conv_f16_tcgen05<BN, KB, STAGES, SPS, 1, false, 2>,
+                                                           cudaFuncAttributeMaxDynamicSharedMemorySize, bytes)))) return e;
+            if ((e = static_cast<int>(cudaFuncSetAttribute(conv_f16_tcgen05<BN, KB, STAGES, SPS, 1, false, 2, true>,
                                                            cudaFuncAttributeMaxDynamicSharedMemorySize, bytes)))) return e;
         }
     }
@@ -1188,7 +1204,11 @@ __global__ void conv_simt_kernel(SimtConvArgs a) {
     }
     acc_t v = acc + static_cast<acc_t>(a.bias[co]);
     if (a.residual) v += static_cast<acc_t>(to_f(reinterpret_cast<const T*>(a.residual)[idx]));
-    if (a.relu && v < 0) v = 0;
+    if ((a.relu & 1) && v < 0) v = 0;
+    if (a.relu & 8) {
+        out[idx] = from_f<T>(gelu_erf(static_cast<float>(v)));
+        return;
+    }
     out[idx] = from_f<T>(static_cast<float>(v));
 }
 

@@ -215,4 +215,40 @@ struct TailArgs {
 bool tail_f16_applies(int N, int HW, int C, int Cout);
 int launch_tail_f16(const TailArgs& a, cudaStream_t stream);
 
+// ---------------------------------------------------------------------------------------------
+// transformer encoder operators (bert_kernels.cu); fp16 activations [rows][C_phys], C a multiple of 8
+// ---------------------------------------------------------------------------------------------
+// GELU, erf form, in fp32 (the conv epilogues' ConvArgs::relu bit 3 and the SIMT convolution use it too)
+__device__ __forceinline__ float gelu_erf(float v) { return 0.5f * v * (1.0f + erff(v * 0.70710678118654752f)); }
+
+struct EmbedArgs {
+    const int* ids;        // [N][S] input_ids (clamped into [0, vocab))
+    const int* segs;       // [N][S] segment_ids (clamped into [0, types))
+    const int* mask;       // [N][S] input_mask: non-zero = attend
+    const __half* tables;  // [vocab + positions + types][C] word, position, token-type rows
+    const float* gamma;    // [C]
+    const float* beta;     // [C]
+    __half* out;           // [N][S][C_phys]
+    float* mask_add;       // [N][S]: 0 or -10000
+    int N, S, C, C_phys, vocab, positions, types;
+    float eps;
+};
+int launch_embed_ln(const EmbedArgs& a, cudaStream_t stream);
+// y = (x - mean) / sqrt(var + eps) * gamma + beta over the C channels of each row; fp32 statistics
+int launch_layernorm(const __half* in, __half* out, const float* gamma, const float* beta, long long rows, int C, int C_phys,
+                     float eps, cudaStream_t stream);
+// one CTA per (sequence, head, 64 query rows): S = QK^T * 0.125 + mask, softmax, O = P V (wgmma); S in {64, 128}
+struct AttnLaunch {
+    CUtensorMap mapQKV;    // 2-D tiled [N*S rows, 3H channels], box 64 x 64, 128B swizzle
+    const float* mask_add; // [N][S]
+    __half* out;           // [N*S][out_pitch]
+    int N, S, heads, H, out_pitch;
+};
+int init_attention_kernels();
+int launch_attention(const AttnLaunch& L, cudaStream_t stream);
+// pooled[n][j] = tanh(b[j] + sum_k W[j][k] * h[n][0][k])   (h: [N][S][C_phys] fp16, W: [C][C] fp16, out fp32 [N][C])
+int launch_pooler(const __half* h, const __half* w, const float* b, float* out, int N, int S, int C, int C_phys, cudaStream_t stream);
+// fp16 [rows][C_phys] -> fp32 [rows][C] (channels-last output binding)
+int launch_output_cast_rows(const __half* src, float* dst, long long rows, int C, int C_phys, cudaStream_t stream);
+
 }  // namespace b2k

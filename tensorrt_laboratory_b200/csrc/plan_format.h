@@ -12,6 +12,9 @@ constexpr char kMagic[8] = {'B', '2', 'E', 'N', 'G', 'I', 'N', 'E'};
 // grouped, so every plan without one stays version 1.  The engine reads both.
 constexpr uint32_t kVersion = 1;
 constexpr uint32_t kVersionGrouped = 2;
+// Version 3: OpRecV3 (224 bytes), written only for plans with transformer ops (OP_EMBED_LN ... OP_POOLER), so every CNN
+// plan keeps version 1 / 2.
+constexpr uint32_t kVersionTransformer = 3;
 
 enum OpType : uint32_t {
     OP_INPUT_CAST = 0,   // fp32 NCHW binding -> NHWC activation tensor
@@ -22,6 +25,12 @@ enum OpType : uint32_t {
     OP_SOFTMAX = 5,      // fp32 vector -> fp32 vector
     OP_OUTPUT_CAST = 6,  // NHWC activation tensor -> fp32 NCHW binding (dequantised when the tensor is int8)
     OP_QUANTIZE = 7,     // fp16 NHWC tensor -> int8 NHWC tensor (INT8 engines: in front of the first int8 convolution)
+    // transformer ops (version-3 plans, fp16 engines only; OpRecV3 below)
+    OP_EMBED_LN = 8,     // int32 bindings (ids, segment ids, mask) -> LayerNorm(word + position + type) fp16 [N, 1, S, H]
+                         // and the additive attention mask, fp32 [N, S] (tensor `out2`)
+    OP_LAYERNORM = 9,    // fp16 [.., C] -> fp16 [.., C] over the channels
+    OP_ATTENTION = 10,   // fused QKV tensor [N, 1, S, 3H] + additive mask (tensor `res`) -> context [N, 1, S, H]
+    OP_POOLER = 11,      // tanh(W h[CLS] + b): fp16 [N, 1, S, H] -> fp32 vector [N, H]
 };
 
 enum TensorKind : uint32_t { T_ACT = 0 /* NHWC, engine precision */, T_VEC = 1 /* [N, c] fp32 */ };
@@ -88,6 +97,29 @@ struct OpRecV2 {  // 192 bytes
     uint32_t groups;
     uint8_t reserved[12];
 };
+// Version-3 op record (plans with transformer ops).  OP_CONV: `relu` bit 3 = fused GELU (erf form) after bias and residual;
+// it excludes bit 0 and bit 2 (INT8).
+//   OP_EMBED_LN: binding / binding2 / binding3 = int32 input_ids / segment_ids / input_mask bindings, each [S] per item;
+//     out = fp16 hidden [N, 1, S, H], out2 = fp32 additive mask [N, S] (0 where the mask is non-zero, -10000 where it is 0).
+//     w = fp16 tables [vocab + positions + types][H] (word rows, then position rows, then token-type rows); b = fp32 [gamma H |
+//     beta H].  Ids are clamped into [0, vocab) and segment ids into [0, types), so no table is read out of bounds.
+//   OP_LAYERNORM: in / out fp16 of the same shape; b = fp32 [gamma C | beta C]; eps.
+//   OP_ATTENTION: in = QKV [N, 1, S, 3H] with channel (part * H + head * 64 + d), part 0 = Q, 1 = K, 2 = V; res = the fp32
+//     mask [N, S]; out = [N, 1, S, H], head h at channels 64h ...; heads * 64 == H, S a multiple of 64 and at most 128.
+//   OP_POOLER: in = fp16 [N, 1, S, H]; out = fp32 vector [N, H]; w = fp16 [H][H] (row = output); b = fp32 [H].
+//   OP_OUTPUT_CAST: flags bit 0 = channels-last binding [H * W, C] instead of NCHW.
+struct OpRecV3 {  // 224 bytes
+    OpRec v1;
+    uint32_t groups;
+    uint32_t heads;
+    uint32_t vocab, positions, types;
+    int32_t binding2, binding3;
+    int32_t out2;
+    float eps;
+    uint32_t flags;
+    uint8_t reserved[8];
+};
+enum : uint32_t { kConvRelu = 1, kConvPacked = 2, kConvInt8 = 4, kConvGelu = 8 };
 struct BindingRec {  // 128 bytes
     char name[64];
     uint32_t is_input;
@@ -104,6 +136,7 @@ static_assert(sizeof(TacticRec) == 40, "TacticRec size");
 static_assert(sizeof(TensorRec) == 96, "TensorRec size");
 static_assert(sizeof(OpRec) == 176, "OpRec size");
 static_assert(sizeof(OpRecV2) == 192, "OpRecV2 size");
+static_assert(sizeof(OpRecV3) == 224, "OpRecV3 size");
 static_assert(sizeof(BindingRec) == 128, "BindingRec size");
 
 }  // namespace b2plan

@@ -104,6 +104,32 @@ int trt_manager_infer(trt_manager* m, const char* model_name, int batch, const v
     TRT_CATCH
 }
 
+int trt_manager_infer_bindings(trt_manager* m, const char* model_name, int batch, void* const* host, const size_t* bytes, int n,
+                               double* compute_seconds) {
+    if (!m || !model_name || !host || !bytes) return fail(B2_EINVAL, "bad arguments");
+    TRT_TRY
+    auto model = m->mgr->GetModel(model_name);
+    if (n != int(model->GetBindingsCount())) return fail(B2_EINVAL, "model %s has %u bindings, %d given", model_name, model->GetBindingsCount(), n);
+    if (batch < 1 || batch > model->GetMaxBatchSize()) return fail(B2_EINVAL, "batch %d out of range", batch);
+    for (int i = 0; i < n; ++i)
+        if (!host[i] || bytes[i] != model->GetBinding(uint32_t(i)).bytesPerBatchItem * size_t(batch))
+            return fail(B2_EINVAL, "binding %d (%s): size mismatch", i, model->GetBinding(uint32_t(i)).name.c_str());
+    InferRunner runner(model, m->mgr);
+    auto fut = runner.Infer(
+        [&](Bindings& b) {  // "pre" stage: fill every pinned input binding
+            b.SetBatchSize(uint32_t(batch));
+            for (uint32_t id : model->GetInputBindingIds()) memcpy(b.HostAddress(id), host[id], bytes[id]);
+        },
+        [&](std::shared_ptr<Bindings>& b) {  // "post" stage: read every pinned output binding
+            for (uint32_t id : model->GetOutputBindingIds()) memcpy(host[id], b->HostAddress(id), bytes[id]);
+            return b->ComputeTime();
+        });
+    const double seconds = fut.get();
+    if (compute_seconds) *compute_seconds = seconds;
+    return B2_OK;
+    TRT_CATCH
+}
+
 int trt_manager_infer_batched(trt_manager* m, const char* model_name, int n, const void* inputs, void* outputs, int window_us,
                               int* batches_executed) {
     if (!m || !model_name || n < 1 || !inputs || !outputs) return fail(B2_EINVAL, "bad arguments");

@@ -8,6 +8,7 @@ examples/ONNX/resnet50/build.py:35-67).
   python tools/build_engine.py --prototxt deploy.prototxt --caffemodel weights.caffemodel --precision int8 --batch 32 -o rn.plan
   python tools/build_engine.py --model resnet50 --batch 8 --tune -o rn50_tuned.plan      (on a GPU box: tactics in the file)
   python tools/build_engine.py --model resnext50 --precision fp16 --batch 8 --tune -o rx50.plan  (ResNeXt-50 32x4d)
+  python tools/build_engine.py --model bert-base --seq 128 --batch 16 [--weights bert.npz] --tune -o bert.plan  (fp16)
 Weights: deterministic synthetic weights (the reference's benchmark engines are weightless too, models/README.md:6-7),
 unless --caffemodel names a binary NetParameter (trtexec --model=...); MNIST and --onnx carry their own weights.
 --precision int8: post-training quantization, max-abs calibration on --calib (an .npy [N,C,H,W] fp32) or on synthetic images.
@@ -24,7 +25,9 @@ from tensorrt_laboratory_b200 import builder, graph, weights  # noqa: E402
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--model", choices=["resnet50", "resnet152", "resnext50", "mnist"])
+    ap.add_argument("--model", choices=["resnet50", "resnet152", "resnext50", "mnist", "bert-base"])
+    ap.add_argument("--seq", type=int, default=128, help="bert-base: the sequence length of the plan (64 or 128)")
+    ap.add_argument("--weights", help="bert-base: .npz of Hugging Face BertModel parameters (default: seeded weights)")
     ap.add_argument("--prototxt")
     ap.add_argument("--onnx", help="ONNX CNN classifier (Conv / BatchNormalization / Relu / Add / MaxPool / AveragePool / "
                                    "GlobalAveragePool / Flatten / Reshape / Gemm / MatMul / Softmax), e.g. an ONNX-zoo ResNet")
@@ -45,7 +48,12 @@ def main():
             return caffemodel.load_caffemodel(a.caffemodel, net)
         return weights.random_weights(net, a.seed)
 
-    if a.prototxt:
+    if a.model == "bert-base":  # its own builder: int32 token bindings, fp16 only
+        from tensorrt_laboratory_b200 import bert
+        cfg = bert.BertConfig(seq=a.seq)
+        blob = builder.build_bert_plan(cfg, a.weights, a.batch, seed=a.seed, precision=prec)
+        net = {"name": f"bert-base S={a.seq}"}
+    elif a.prototxt:
         with open(a.prototxt) as f:
             net = graph.parse_prototxt(f.read())
         wts = weights_for(net)
@@ -62,16 +70,17 @@ def main():
     else:
         net = graph.resnet_caffe(int(a.model[6:]))
         wts = weights_for(net)
-    low = graph.lower(net, wts)
-    if prec == builder.PREC_INT8:
-        import numpy as np
-        from tensorrt_laboratory_b200 import quantize
-        if a.calib:
-            calib = np.load(a.calib).astype(np.float32)
-        else:
-            calib = weights.synthetic_input(8, chw=tuple(net["input_dims"][1:]), seed=4321)
-        low = quantize.quantize_lowered(low, calib)
-    blob = builder.build_plan(low, prec, a.batch)
+    if a.model != "bert-base":
+        low = graph.lower(net, wts)
+        if prec == builder.PREC_INT8:
+            import numpy as np
+            from tensorrt_laboratory_b200 import quantize
+            if a.calib:
+                calib = np.load(a.calib).astype(np.float32)
+            else:
+                calib = weights.synthetic_input(8, chw=tuple(net["input_dims"][1:]), seed=4321)
+            low = quantize.quantize_lowered(low, calib)
+        blob = builder.build_plan(low, prec, a.batch)
     if a.tune:
         from tensorrt_laboratory_b200 import capi
         eng = capi.Engine(blob)
