@@ -85,6 +85,7 @@ int load_driver_entry_points() {
 size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 constexpr size_t kSplitWorkspaceBytes = 12u << 20;  // bounds tiles*splits*128*BN*4 (see pick_conv_config)
 constexpr int kMaxSplitTiles = 4096;                 // tile counters per context
+constexpr int kSmemLimit = 227 * 1024;               // dynamic shared memory one CTA may opt in to on sm_90
 
 int env_int(const char* name, int dflt) {
     const char* v = getenv(name);
@@ -302,7 +303,6 @@ struct b2_context {
     int force_cn = 0;   // > 0: this cluster size wherever it divides the N-tile count, -1: never cluster
     int force_ws = 0;   // 1: only the persistent warp-specialised tactic where it applies, -1: never
     int pdl_trigger = 1;
-    int no_pack = 0;    // reserved (packed plans cannot fall back to the tensor-map weight path)
     int no_fold = 0;    // 1: run the stem through the generic 8-channel tap path instead of the row-folded one
     int autotune = 4;  // 0 off (cost model), 1 latency mode, N>=2 throughput mode over N streams
     int fork = 0;      // 1: run side branches (Op::side_join) on a forked stream / a parallel graph branch.  Off by default:
@@ -788,11 +788,11 @@ ConvConfig pick_conv_config(int M, int cout_phys, int kblocks, int kb, bool resi
             if (splits > 1 && (splits - 1) * kpc >= kblocks) continue;  // an empty split
             for (int st : stgs) {
                 if (!b2k::conv_config_exists(bn, kb, st)) continue;
-                if (b2k::conv_smem_bytes(bn, st, residual) > 227 * 1024) continue;
+                if (b2k::conv_smem_bytes(bn, st, residual) > kSmemLimit) continue;
                 if (honor_forced && c->force_stages && st != c->force_stages) continue;
                 if (!(honor_forced && c->force_stages) && !stage_depth_useful(bn, kb, st, kpc)) continue;
                 const double smem = b2k::conv_smem_bytes(bn, st, residual);
-                int per_sm = int(227.0 * 1024 / smem);
+                int per_sm = int(double(kSmemLimit) / smem);
                 per_sm = std::min(per_sm, bn <= 64 ? 2 : 1);  // 384-thread CTAs: the register file holds two only for BN <= 64
                 per_sm = std::max(1, std::min(per_sm, 8));
                 const int ctas = tiles * splits;
@@ -839,11 +839,128 @@ int conv_halo_rows(const b2_context* c, const Op& op) {
     const Tensor& ti = c->e->tensors[r.in];
     const Tensor& to = c->e->tensors[r.out];
     if (op.groups > 1 || r.cin_phys % 64 || r.cout_phys % 64 || op.kh() != 3 || op.kw() != 3 || op.sh() != 1 || op.sw() != 1 || op.ph() != 1 ||
-        op.pw_lo() != 1 || op.pw_hi() != 1 || r.res >= 0 || !(r.relu & 2) || c->no_pack || ti.h != to.h || ti.w != to.w)
+        op.pw_lo() != 1 || op.pw_hi() != 1 || r.res >= 0 || !(r.relu & 2) || ti.h != to.h || ti.w != to.w)
         return 0;
     const int wp = int(to.w) + 2;
     if (wp > 128) return 0;
     return std::min(128 / wp, int(to.h));
+}
+
+// Does `op` run on the wgmma convolution kernels?  fp16 engines, 64-channel K blocks or the 8-channel stem / thin-input
+// path, a multiple of 32 output channels, and for a grouped convolution the packed block-diagonal layout; else SIMT.
+bool conv_on_tensor_cores(const b2_engine* e, const Op& op) {
+    const b2plan::OpRec& r = op.r;
+    const bool kb64 = r.cin_phys % 64 == 0, kb8 = r.cin_phys == 8;
+    return e->half() && (kb64 || kb8) && r.cout_phys % 32 == 0 && (kb64 || r.taps_phys % 2 == 0) && (op.groups == 1 || op.group_span() > 0);
+}
+
+// The persistent kernel needs 64-wide K blocks and packed weights, and has no GELU epilogue; nor does it take a grouped
+// convolution, whose CTAs along N read different channel blocks.
+bool conv_takes_ws(const b2_context* c, const Op& op) {
+    return conv_kb(c, op) == 64 && (op.r.relu & 2) && op.groups == 1 && !(op.r.relu & b2plan::kConvGelu);
+}
+
+// May tactic `cfg` run `op` at `batch`?  The one rule every tactic goes through: the tuners' candidates, the forced
+// options, and tables from the plan, the tune cache or another batch size (which are input, not trusted).
+bool tactic_applies(const b2_context* c, const Op& op, int batch, const ConvConfig& cfg) {
+    const b2plan::OpRec& r = op.r;
+    const Tensor& to = c->e->tensors[r.out];
+    const int span = op.group_span(), kb = conv_kb(c, op);
+    if (cfg.bn <= 0 || int(r.cout_phys) % cfg.bn || cfg.splits < 1 || cfg.sps < 1 || cfg.ws < 0) return false;
+    // grouped: one tile per CTA and N tiles inside one span of input channels; GELU: only the one-tile kernel has it
+    if (op.groups > 1 && (!span || span % cfg.bn || cfg.splits > 1)) return false;
+    if ((op.groups > 1 || (r.relu & b2plan::kConvGelu)) && (cfg.ws || cfg.cn > 1 || cfg.halo)) return false;
+    if (cfg.halo) {
+        const int R = conv_halo_rows(c, op), cblocks = int(r.cin_phys) / 64;
+        return R && cfg.splits == 1 && !cfg.ws && cfg.cn <= 1 && b2k::conv_halo_config_exists(cfg.bn) && cblocks <= 8 &&
+               b2k::conv_halo_smem(cfg.bn, int(to.w), R, cblocks) <= kSmemLimit;
+    }
+    if (cfg.ws)
+        return conv_takes_ws(c, op) && cfg.splits == 1 && cfg.cn <= 1 && b2k::conv_ws_config_exists(cfg.bn, cfg.stages, cfg.sps) &&
+               b2k::conv_ws_smem(cfg.bn, cfg.stages, cfg.sps, r.res >= 0) <= kSmemLimit;
+    if (!b2k::conv_config_exists(cfg.bn, kb, cfg.stages, cfg.sps) || b2k::conv_smem_bytes(cfg.bn, cfg.stages, r.res >= 0, cfg.sps) > kSmemLimit)
+        return false;
+    const int grid_n = int(r.cout_phys) / cfg.bn;
+    if (cfg.cn > 1 && (kb != 64 || grid_n % cfg.cn || !b2k::conv_cluster_config_exists(cfg.bn, cfg.stages, cfg.sps, cfg.cn))) return false;
+    if (cfg.splits > 1) {  // 64-wide K, >= 4 K blocks in every split, and tile counters and fp32 workspace for the whole grid
+        const int nkb = conv_num_kblocks(c, op), kpc = (nkb + cfg.splits - 1) / cfg.splits;
+        const int tiles = (batch * int(to.h * to.w) + 127) / 128 * grid_n;
+        if (kb != 64 || kpc < 4 || (cfg.splits - 1) * kpc >= nkb || tiles > kMaxSplitTiles ||
+            size_t(tiles) * cfg.splits * 128 * cfg.bn * 4 > kSplitWorkspaceBytes)
+            return false;
+    }
+    return true;
+}
+
+// The tactics the per-layer tuner times, in timing order: every tile, persistent and halo tactic the rule admits, less
+// ring depths the K loop cannot use and split-K where the plain grid already fills the GPU.  fixed_splits > 0 admits that
+// split factor only (halo then only at 1).  The forced `ws`, `cn` and `halo` options narrow the list as they do the plan.
+std::vector<ConvConfig> conv_candidates(const b2_context* c, const Op& op, int batch, int fixed_splits) {
+    const b2plan::OpRec& r = op.r;
+    const int kbsz = conv_kb(c, op), nkb = conv_num_kblocks(c, op);
+    const int m_tiles = (batch * int(c->e->tensors[r.out].h * c->e->tensors[r.out].w) + 127) / 128;
+    const bool ws_only = c->force_ws > 0 && conv_takes_ws(c, op);
+    auto ok = [&](const ConvConfig& t) { return tactic_applies(c, op, batch, t); };
+    std::vector<ConvConfig> out;
+    for (int bn : {256, 128, 64, 32}) {
+        if (int(r.cout_phys) % bn) continue;
+        const int tiles = m_tiles * (int(r.cout_phys) / bn);
+        for (int ws = 0; ws <= 1; ++ws)
+        for (int sp : {1, 2, 4, 8})
+        for (int sps = 1; sps <= 2; ++sps)
+        for (int st : {1, 2, 4, 8}) {
+            if ((fixed_splits > 0 && sp != fixed_splits) || (ws ? c->force_ws < 0 : ws_only)) continue;
+            ConvConfig t{bn, st, sp, 0.0, sps, ws ? std::min(tiles, g_sms) : 0, 1};
+            if (!ok(t)) continue;
+            if (ws) {
+                if (sps == 2 && nkb < 4) continue;
+                out.push_back(t);
+                if (tiles > g_sms / 2) t.ws = g_sms / 2, out.push_back(t);  // half the SMs per stream
+                continue;
+            }
+            const int kpc = (nkb + sp - 1) / sp;
+            if (sps == 2 ? (kpc < 4 || st * 2 > kpc + 2) : !stage_depth_useful(bn, kbsz, st, kpc)) continue;  // double-width stages pay on long K loops only
+            if (sp > 1 && (tiles >= 100 || tiles > kMaxSplitTiles / 8 || tiles * sp > 160)) continue;  // split-K only where the plain grid leaves SMs idle
+            // clusters along N that multicast the activation tile: never won a timing (the L2 read is shared but every SM
+            // still ingests the whole tile, and the cluster barriers cost latency) -> tried only on request
+            ConvConfig cl = t;
+            cl.cn = c->force_cn;
+            out.push_back(c->force_cn > 1 && ok(cl) ? cl : t);
+        }
+    }
+    if (c->force_halo >= 0 && fixed_splits <= 1) {
+        std::vector<ConvConfig> halo;
+        for (int bn : {256, 128, 64, 32}) {
+            const ConvConfig h{bn, kHaloStagesTag, 1, 0.0, 1, 0, 1, 1};
+            if (ok(h)) halo.push_back(h);
+        }
+        if (!halo.empty() && c->force_halo > 0) out.clear();
+        out.insert(out.end(), halo.begin(), halo.end());
+    }
+    return out;
+}
+
+// The cost model's tactic under the forced options: `bn`, `stages` and `splits` steer its search (a forced value this
+// layer cannot take is dropped), then `sps`, `ws`, `halo` and `cn` are applied in that order wherever the rule admits
+// them.  bn == 0: the layer has no configuration at all.
+ConvConfig forced_conv_config(const b2_context* c, const Op& op, int batch) {
+    const b2plan::OpRec& r = op.r;
+    const int M = batch * int(c->e->tensors[r.out].h * c->e->tensors[r.out].w);
+    const int kbsz = conv_kb(c, op), nkb = conv_num_kblocks(c, op);
+    ConvConfig cfg = pick_conv_config(M, int(r.cout_phys), nkb, kbsz, r.res >= 0, c, true, op.group_span());
+    if (cfg.bn == 0) cfg = pick_conv_config(M, int(r.cout_phys), nkb, kbsz, r.res >= 0, c, false, op.group_span());
+    if (cfg.bn == 0) return cfg;
+    auto force = [&](auto set) {
+        ConvConfig t = cfg;
+        set(t);
+        if (tactic_applies(c, op, batch, t)) cfg = t;
+    };
+    if (c->force_sps == 2) force([](ConvConfig& t) { t.sps = 2; });
+    if (c->force_ws > 0)
+        force([&](ConvConfig& t) { t.ws = std::min((M + 127) / 128 * (int(r.cout_phys) / t.bn), c->force_ws > 1 ? c->force_ws : g_sms); });
+    if (c->force_halo > 0) force([](ConvConfig& t) { t.halo = 1, t.ws = 0, t.cn = 1; });
+    if (c->force_cn > 1) force([&](ConvConfig& t) { t.cn = c->force_cn; });
+    return cfg;
 }
 
 // Fill a ConvLaunch (kernel arguments + TMA tensor maps) for one conv op under a given configuration.
@@ -858,14 +975,10 @@ int make_conv_launch(b2_context* c, const Op& op, int batch, const ConvConfig& c
     const bool kb64 = r.cin_phys % 64 == 0;
     const bool fold = conv_is_row_folded(c, op);
     const int span = op.group_span();
-    // grouped: the one-tile-per-CTA kernel only, and N tiles that stay inside one span of input channels
-    if (op.groups > 1 && (!span || cfg.ws || cfg.splits > 1 || cfg.cn > 1 || cfg.halo || span % cfg.bn))
-        return fail(B2_EINVAL, "conv %s: grouped convolutions run one tile per CTA with an N tile dividing %d (bn=%d ws=%d splits=%d cn=%d halo=%d)",
-                    op.name.c_str(), span, cfg.bn, cfg.ws, cfg.splits, cfg.cn, cfg.halo);
+    if (!tactic_applies(c, op, batch, cfg))
+        return fail(B2_EINVAL, "conv %s: tactic bn=%d st=%d sps=%d splits=%d ws=%d cn=%d halo=%d does not apply", op.name.c_str(), cfg.bn,
+                    cfg.stages, cfg.sps, cfg.splits, cfg.ws, cfg.cn, cfg.halo);
     const bool gelu = (r.relu & b2plan::kConvGelu) != 0;
-    if (gelu && (cfg.ws || cfg.halo || cfg.cn > 1))
-        return fail(B2_EINVAL, "conv %s: GELU layers run on the one-tile-per-CTA kernel (ws=%d halo=%d cn=%d)", op.name.c_str(), cfg.ws, cfg.halo,
-                    cfg.cn);
     b2k::ConvLaunch& cl = *out;
     memset(&cl, 0, sizeof cl);
     cl.kb = conv_kb(c, op);
@@ -873,11 +986,10 @@ int make_conv_launch(b2_context* c, const Op& op, int batch, const ConvConfig& c
     const int nkb = conv_num_kblocks(c, op);
     cl.bn = cfg.bn;
     cl.stages = cfg.stages;
-    cl.sps = cfg.sps > 0 ? cfg.sps : 1;
+    cl.sps = cfg.sps;
     cl.grid_n = int(r.cout_phys) / cl.bn;
     cl.ws_ctas = cfg.ws;
-    cl.cn = (cfg.cn > 1 && cfg.ws == 0 && cl.kb == 64 && cl.grid_n % cfg.cn == 0 &&
-             b2k::conv_cluster_config_exists(cl.bn, cl.stages, cl.sps, cfg.cn)) ? cfg.cn : 1;
+    cl.cn = std::max(cfg.cn, 1);
     cl.args.cn = cl.cn;
     cl.args.tiles_m = cl.grid_m;
     cl.args.tiles_n = cl.grid_n;
@@ -905,15 +1017,13 @@ int make_conv_launch(b2_context* c, const Op& op, int batch, const ConvConfig& c
     a.pad_h = op.ph();
     a.pad_w = op.pw_lo();
     a.relu = int(r.relu & (b2plan::kConvRelu | b2plan::kConvGelu));  // bit 0 ReLU, bit 3 GELU (epilogues of every tactic)
-    a.wpacked = (r.relu & 2) && !c->no_pack ? w : nullptr;
+    a.wpacked = (r.relu & 2) ? w : nullptr;
     // (GELU layers are always read as a plain matrix: their kernel exists for that operand path only)
     const bool tiled = r.k == 1 && op.kw() == 1 && r.stride == 1 && op.sw() == 1 && r.pad_ == 0 && op.pw_lo() == 0 &&
                        op.pw_hi() == 0 && kb64 && (!c->force_im2col || gelu);
     a.a_mode = tiled ? b2k::A_TILED : b2k::A_IM2COL;
     if (cfg.halo) {
         const int R = conv_halo_rows(c, op);
-        if (!R || !b2k::conv_halo_config_exists(cl.bn) || int(r.cin_phys) / 64 > 8 || b2k::conv_halo_smem(cl.bn, int(to.w), R, int(r.cin_phys) / 64) > 227 * 1024)
-            return fail(B2_EINVAL, "conv %s: the halo tactic does not apply", op.name.c_str());
         cl.halo = 1;
         cl.ws_ctas = 0, cl.cn = 1, a.cn = 1, a.splits = 1, cl.stages = kHaloStagesTag, cl.sps = 1;
         a.halo_rows = R;
@@ -997,185 +1107,110 @@ int make_i8_conv_launch(b2_context* c, const Op& op, int batch, int bn, int stag
     return rc;
 }
 
-// Tactic selection, the role TensorRT's builder plays for the reference's engines: time every instantiated
-// (N tile, pipeline depth) on THIS device with the layer's real shapes and keep the fastest.  Runs once per
-// (engine, layer, batch); results are shared by all contexts of the engine.
-// fixed_halo: -1 free choice, 0 never, 1 only the halo kernel (decided once at max batch: it changes the summation order)
-int autotune_conv(b2_context* c, const Op& op, int batch, int fixed_splits, int fixed_halo, ConvConfig* best_out) {
-    b2_engine* e = c->e;
-    const b2plan::OpRec& r = op.r;
-    const Tensor& to = e->tensors[r.out];
-    const int M = batch * int(to.h) * int(to.w);
-    const int kbsz = conv_kb(c, op);
-    const int nkb = conv_num_kblocks(c, op);
-    // c->autotune == 1: latency mode (one stream).  >= 2: throughput mode -- the candidate is launched on that
-    // many streams at once, which is how the kernels meet each other when several ExecutionContexts overlap
-    // (BASELINE config: 4 contexts); deep pipelines that win alone can lose here because they hog shared memory.
-    const int ns = std::max(1, std::min(c->autotune, 8));
-    std::vector<cudaStream_t> ss(ns, nullptr);
-    std::vector<cudaEvent_t> done(ns, nullptr);
+// Timing harness of the tuners.  c->autotune == 1: latency mode (one stream).  >= 2: throughput mode -- the candidate is
+// launched on that many streams at once, which is how the kernels meet each other when several ExecutionContexts overlap
+// (BASELINE config: 4 contexts); deep pipelines that win alone can lose here because they hog shared memory.
+struct TuneTimer {
+    const int ns;
+    const int iters = std::max(4, env_int("B2_TUNE_ITERS", 12));  // launches per stream and measurement
+    const int reps = std::max(1, env_int("B2_TUNE_REPS", 2));     // measurements per candidate (the quietest counts)
+    std::vector<cudaStream_t> ss;
+    std::vector<cudaEvent_t> done;
     cudaEvent_t e0 = nullptr, e1 = nullptr;
-    bool ok = cudaEventCreate(&e0) == cudaSuccess && cudaEventCreate(&e1) == cudaSuccess;
-    for (int i = 0; i < ns && ok; ++i)
-        ok = cudaStreamCreateWithFlags(&ss[i], cudaStreamNonBlocking) == cudaSuccess &&
-             cudaEventCreateWithFlags(&done[i], cudaEventDisableTiming) == cudaSuccess;
-    auto cleanup = [&] {
-        for (auto s_ : ss)
-            if (s_) cudaStreamDestroy(s_);
+
+    explicit TuneTimer(const b2_context* c) : ns(std::max(1, std::min(c->autotune, 8))), ss(size_t(ns), nullptr), done(size_t(ns), nullptr) {}
+    ~TuneTimer() {
+        for (auto s : ss)
+            if (s) cudaStreamDestroy(s);
         for (auto d : done)
             if (d) cudaEventDestroy(d);
         if (e0) cudaEventDestroy(e0);
         if (e1) cudaEventDestroy(e1);
-    };
-    if (!ok) {
+    }
+    int init() {
+        bool ok = cudaEventCreate(&e0) == cudaSuccess && cudaEventCreate(&e1) == cudaSuccess;
+        for (int i = 0; i < ns && ok; ++i)
+            ok = cudaStreamCreateWithFlags(&ss[size_t(i)], cudaStreamNonBlocking) == cudaSuccess &&
+                 cudaEventCreateWithFlags(&done[size_t(i)], cudaEventDisableTiming) == cudaSuccess;
+        if (ok) return B2_OK;
         cudaGetLastError();
-        cleanup();
         return fail(B2_ECUDA, "autotune: cannot create streams/events");
     }
+    // `launch(k, stream)` issues stream k's copy of the candidate (returns 0 or a cudaError_t).  Two warm-up rounds, then
+    // *ms = the quietest of `reps` windows of `iters` rounds on all streams; returns the first launch or stream error.
+    template <class F>
+    cudaError_t time(F launch, float* ms) {
+        int rc = 0;
+        for (int i = 0; i < 2 && !rc; ++i)
+            for (int k = 0; k < ns && !rc; ++k) rc = launch(k, ss[size_t(k)]);
+        for (auto s : ss) cudaStreamSynchronize(s);
+        *ms = 1e30f;
+        cudaError_t se = cudaSuccess;
+        for (int rep = 0; rep < reps && !rc && se == cudaSuccess; ++rep) {
+            cudaEventRecord(e0, ss[0]);
+            for (int k = 1; k < ns; ++k) cudaStreamWaitEvent(ss[size_t(k)], e0, 0);
+            for (int i = 0; i < iters && !rc; ++i)
+                for (int k = 0; k < ns && !rc; ++k) rc = launch(k, ss[size_t(k)]);
+            for (int k = 1; k < ns; ++k) {
+                cudaEventRecord(done[size_t(k)], ss[size_t(k)]);
+                cudaStreamWaitEvent(ss[0], done[size_t(k)], 0);
+            }
+            cudaEventRecord(e1, ss[0]);
+            se = cudaStreamSynchronize(ss[0]);
+            float t = 0.f;
+            if (se == cudaSuccess && cudaEventElapsedTime(&t, e0, e1) == cudaSuccess) *ms = std::min(*ms, t);
+        }
+        return rc ? cudaError_t(rc) : se;
+    }
+    double us_per_launch(double ms) const { return ms * 1e3 / (iters * ns); }
+};
+
+// Tactic selection, the role TensorRT's builder plays for the reference's engines: time every candidate tactic
+// (conv_candidates) on THIS device with the layer's real shapes and keep the fastest.  Runs once per
+// (engine, layer, batch); results are shared by all contexts of the engine.
+int autotune_conv(b2_context* c, const Op& op, int batch, int fixed_splits, ConvConfig* best_out) {
+    const b2plan::OpRec& r = op.r;
+    const Tensor& to = c->e->tensors[r.out];
+    const int M = batch * int(to.h) * int(to.w);
+    TuneTimer tt(c);
+    int status = tt.init();
+    if (status) return status;
+    const int verbose = env_int("B2_TUNE_VERBOSE", 0);  // 1: the winner per layer, 2: every candidate
     ConvConfig best = *best_out;
     double best_ms = 1e30;
-    const int bns[4] = {256, 128, 64, 32};
-    const int stgs[4] = {1, 2, 4, 8};
-    int status = B2_OK;
-    const int verbose = env_int("B2_TUNE_VERBOSE", 0);             // 1: the winner per layer, 2: every candidate
-    const int iters = std::max(4, env_int("B2_TUNE_ITERS", 12));   // launches per stream and measurement
-    const int reps = std::max(1, env_int("B2_TUNE_REPS", 2));      // measurements per candidate (the quietest counts)
-    const int m_tiles = (M + 127) / 128;
-    const int split_cands[4] = {1, 2, 4, 8};
-    // grouped convolution: the one-tile-per-CTA kernel without split-K or clusters, N tiles dividing the group span
-    const int span = op.group_span();
-    std::vector<ConvConfig> candidates;
-    for (int bn : bns) {
-        if (int(r.cout_phys) % bn || (span && span % bn)) continue;
-        const int tiles = m_tiles * (int(r.cout_phys) / bn);
-        for (int ws = 0; ws <= 1; ++ws)
-        for (int sp : split_cands)
-        for (int sps = 1; sps <= 2; ++sps)
-        for (int st : stgs) {
-            if (fixed_splits > 0 && sp != fixed_splits) continue;
-            if (span && (ws || sp > 1)) continue;
-            if (ws) {  // persistent warp-specialised tactic: 64-wide K, packed weights, no split-K
-                if (c->force_ws < 0 || kbsz != 64 || !(r.relu & 2) || sp != 1 || (r.relu & b2plan::kConvGelu)) continue;
-                if (!b2k::conv_ws_config_exists(bn, st, sps) || b2k::conv_ws_smem(bn, st, sps, r.res >= 0) > 227 * 1024) continue;
-                if (sps == 2 && nkb < 4) continue;
-            } else {
-            if (c->force_ws > 0 && kbsz == 64 && (r.relu & 2) && !span && !(r.relu & b2plan::kConvGelu)) continue;
-            if (!b2k::conv_config_exists(bn, kbsz, st, sps)) continue;
-            if (b2k::conv_smem_bytes(bn, st, r.res >= 0, sps) > 227 * 1024) continue;
-            }
-            const int kpc = (nkb + sp - 1) / sp;
-            if (ws) {
-                candidates.push_back(ConvConfig{bn, st, 1, 0.0, sps, std::min(tiles, g_sms), 1});
-                if (tiles > g_sms / 2) candidates.push_back(ConvConfig{bn, st, 1, 0.0, sps, g_sms / 2, 1});  // half the SMs per stream
+    for (const ConvConfig& cand : conv_candidates(c, op, batch, fixed_splits)) {
+        b2k::ConvLaunch cl0;
+        if ((status = make_conv_launch(c, op, batch, cand, &cl0))) return status;
+        // concurrent split-K launches must not share arrival counters or partial-tile storage
+        std::vector<b2k::ConvLaunch> cls(size_t(tt.ns), cl0);
+        void* tmp_ws = nullptr;
+        if (cand.splits > 1) {
+            const size_t ws_bytes = size_t(cl0.grid_m) * cl0.grid_n * cand.splits * 128 * cand.bn * 4;
+            if (cudaMalloc(&tmp_ws, ws_bytes * tt.ns) != cudaSuccess) {
+                cudaGetLastError();
                 continue;
             }
-            if (sps == 2 && kpc < 4) continue;  // double-width stages only pay on long K loops
-            if (sps == 1 && !stage_depth_useful(bn, kbsz, st, kpc)) continue;
-            if (sps == 2 && st * 2 > kpc + 2) continue;
-            if (sp > 1 && (kbsz != 64 || tiles >= 100 || tiles > kMaxSplitTiles / 8 || kpc < 4 || tiles * sp > 160 ||
-                           (sp - 1) * kpc >= nkb ||
-                           size_t(tiles) * sp * 128 * bn * 4 > kSplitWorkspaceBytes))
-                continue;  // split-K only where the plain grid leaves SMs idle
-            const bool cn_forced_here = c->force_cn > 1 && kbsz == 64 && !span && !(r.relu & b2plan::kConvGelu) && (int(r.cout_phys) / bn) % c->force_cn == 0 &&
-                                        b2k::conv_cluster_config_exists(bn, st, sps, c->force_cn);
-            if (!cn_forced_here) candidates.push_back(ConvConfig{bn, st, sp, 0.0, sps, 0, 1});
-            // clusters along N that multicast the activation tile: never won a timing (the L2 read is shared but
-            // every SM still ingests the whole tile, and the cluster barriers cost latency) -> tried only on request
-            if (kbsz == 64 && c->force_cn > 0 && !span && !(r.relu & b2plan::kConvGelu))
-                for (int cn = 2; cn <= 4; cn *= 2)
-                    if ((int(r.cout_phys) / bn) % cn == 0 && (!c->force_cn || cn == c->force_cn) &&
-                        b2k::conv_cluster_config_exists(bn, st, sps, cn))
-                        candidates.push_back(ConvConfig{bn, st, sp, 0.0, sps, 0, cn});
+            for (int k = 0; k < tt.ns; ++k) {
+                cls[size_t(k)].args.workspace = reinterpret_cast<float*>(static_cast<uint8_t*>(tmp_ws) + ws_bytes * k);
+                cls[size_t(k)].args.tile_counters = c->d_counters + k * (kMaxSplitTiles / 8);
+            }
         }
+        float ms = 0.f;
+        const cudaError_t err = tt.time([&](int k, cudaStream_t s) { return b2k::launch_conv_f16_tcgen05(cls[size_t(k)], s); }, &ms);
+        if (tmp_ws) cudaFree(tmp_ws);
+        if (err != cudaSuccess)
+            return fail(B2_ECUDA, "autotune of %s (bn=%d st=%d) failed: %s", op.name.c_str(), cand.bn, cand.stages, cudaGetErrorString(err));
+        if (verbose > 1)
+            fprintf(stderr, "[b2 tune]   %s b=%d cand bn=%d st=%d sp=%d sps=%d ws=%d cn=%d halo=%d : %.3f us/launch\n", op.name.c_str(),
+                    batch, cand.bn, cand.stages, cand.splits, cand.sps, cand.ws, cand.cn, cand.halo, tt.us_per_launch(ms));
+        if (ms < best_ms) best_ms = ms, best = cand;
     }
-    if (fixed_halo != 0 && c->force_halo >= 0 && (fixed_splits <= 1)) {
-        const int R = conv_halo_rows(c, op);
-        std::vector<ConvConfig> halo_cands;
-        if (R)
-            for (int bn : bns)
-                if (int(r.cout_phys) % bn == 0 && b2k::conv_halo_config_exists(bn) &&
-                    int(r.cin_phys) / 64 <= 8 && b2k::conv_halo_smem(bn, int(to.w), R, int(r.cin_phys) / 64) <= 227 * 1024) {
-                    ConvConfig hc{bn, kHaloStagesTag, 1, 0.0, 1, 0, 1};
-                    hc.halo = 1;
-                    halo_cands.push_back(hc);
-                }
-        if (!halo_cands.empty() && (c->force_halo > 0 || fixed_halo > 0)) candidates.clear();
-        candidates.insert(candidates.end(), halo_cands.begin(), halo_cands.end());
-    }
-    std::vector<std::pair<ConvConfig, double>> timed;
-    for (const ConvConfig& cand : candidates) {
-        {
-            const int bn = cand.bn, st = cand.stages, sp = cand.splits;
-            const int tiles = m_tiles * (int(r.cout_phys) / bn);
-            b2k::ConvLaunch cl0;
-            if ((status = make_conv_launch(c, op, batch, cand, &cl0))) break;
-            // concurrent split-K launches must not share arrival counters or partial-tile storage
-            std::vector<b2k::ConvLaunch> cls(ns, cl0);
-            void* tmp_ws = nullptr;
-            if (sp > 1) {
-                const size_t ws_bytes = size_t(tiles) * sp * 128 * bn * 4;
-                if (cudaMalloc(&tmp_ws, ws_bytes * ns) != cudaSuccess) {
-                    cudaGetLastError();
-                    continue;
-                }
-                for (int k = 0; k < ns; ++k) {
-                    cls[k].args.workspace = reinterpret_cast<float*>(static_cast<uint8_t*>(tmp_ws) + ws_bytes * k);
-                    cls[k].args.tile_counters = c->d_counters + k * (kMaxSplitTiles / 8);
-                }
-            }
-            int rc = 0;
-            for (int i = 0; i < 2 && !rc; ++i)
-                for (int k = 0; k < ns && !rc; ++k) rc = b2k::launch_conv_f16_tcgen05(cls[k], ss[k]);
-            for (int k = 0; k < ns; ++k) cudaStreamSynchronize(ss[k]);
-            float ms = 1e30f;
-            cudaError_t se = cudaSuccess;
-            for (int rep = 0; rep < reps && !rc && se == cudaSuccess; ++rep) {  // keep the quietest measurement
-                cudaEventRecord(e0, ss[0]);
-                for (int k = 1; k < ns; ++k) cudaStreamWaitEvent(ss[k], e0, 0);
-                for (int i = 0; i < iters && !rc; ++i)
-                    for (int k = 0; k < ns && !rc; ++k) rc = b2k::launch_conv_f16_tcgen05(cls[k], ss[k]);
-                for (int k = 1; k < ns; ++k) {
-                    cudaEventRecord(done[k], ss[k]);
-                    cudaStreamWaitEvent(ss[0], done[k], 0);
-                }
-                cudaEventRecord(e1, ss[0]);
-                se = cudaStreamSynchronize(ss[0]);
-                float t = 0.f;
-                if (se == cudaSuccess && cudaEventElapsedTime(&t, e0, e1) == cudaSuccess) ms = std::min(ms, t);
-            }
-            if (tmp_ws) cudaFree(tmp_ws);
-            if (rc || se != cudaSuccess) {
-                status = fail(B2_ECUDA, "autotune of %s (bn=%d st=%d) failed: %s", op.name.c_str(), bn, st,
-                              cudaGetErrorString(rc ? cudaError_t(rc) : se));
-                break;
-            }
-            if (verbose > 1)
-                fprintf(stderr, "[b2 tune]   %s b=%d cand bn=%d st=%d sp=%d sps=%d ws=%d cn=%d halo=%d : %.3f us/launch\n", op.name.c_str(),
-                        batch, cand.bn, cand.stages, cand.splits, cand.sps, cand.ws, cand.cn, cand.halo, ms * 1e3 / (iters * ns));
-            timed.push_back({cand, double(ms)});
-            if (ms < best_ms) best_ms = ms, best = cand;
-        }
-        if (status) break;
-    }
-    cleanup();
-    if (status) return status;
-    // B2_TUNE_TIE_PERMILLE = t > 0: among the one-tile tactics within t/1000 of the fastest, take the WIDEST N tile (fewest
-    // CTAs, least L2->SM traffic per MAC): with several copies of one layer the timing cannot see the SMs a wide tile
-    // leaves to the other contexts' layers.  0 (default) = fastest wins; measured neutral-to-negative, DESIGN.md.
-    const int tie = env_int("B2_TUNE_TIE_PERMILLE", 0);
-    if (tie > 0 && !best.ws && !best.halo && best.splits == 1) {
-        for (const auto& t : timed)
-            if (!t.first.ws && !t.first.halo && t.first.splits == 1 && t.first.cn == best.cn && t.second <= best_ms * (1.0 + tie / 1000.0) &&
-                (t.first.bn > best.bn || (t.first.bn == best.bn && t.second < best_ms)))
-                best = t.first, best_ms = std::min(best_ms, t.second);
-    }
-    best.est_us = best_ms * 1e3 / (iters * ns);
+    best.est_us = tt.us_per_launch(best_ms);
     if (verbose)
         fprintf(stderr, "[b2 tune] %s b=%d M=%d N=%d K=%d best bn=%d st=%d sp=%d sps=%d ws=%d cn=%d halo=%d : %.3f us/launch (%d streams)\n",
-                op.name.c_str(), batch, M, int(r.cout_phys), nkb * kbsz, best.bn, best.stages, best.splits, best.sps, best.ws, best.cn,
-                best.halo, best.est_us, ns);
+                op.name.c_str(), batch, M, int(r.cout_phys), conv_num_kblocks(c, op) * conv_kb(c, op), best.bn, best.stages, best.splits,
+                best.sps, best.ws, best.cn, best.halo, best.est_us, tt.ns);
     *best_out = best;
-    (void)M;
     return B2_OK;
 }
 
@@ -1208,103 +1243,37 @@ void tune_cache_append(const b2_engine* e, int op, int batch, const ConvConfig& 
     fclose(f);
 }
 
-// Can `cfg` (possibly measured at another batch size) run `op` at `batch`?
-bool tactic_applies(const b2_context* c, const Op& op, int batch, const ConvConfig& cfg) {
-    const b2plan::OpRec& r = op.r;
-    if (cfg.bn <= 0 || int(r.cout_phys) % cfg.bn) return false;
-    if (op.groups > 1) {  // grouped: one tile per CTA, no split-K / cluster / halo, N tile inside the group span
-        const int span = op.group_span();
-        return span && span % cfg.bn == 0 && !cfg.halo && !cfg.ws && cfg.splits <= 1 && cfg.cn <= 1 &&
-               b2k::conv_config_exists(cfg.bn, 64, cfg.stages, cfg.sps);
-    }
-    const int kbsz = conv_kb(c, op);
-    if (cfg.halo) return conv_halo_rows(c, op) > 0 && b2k::conv_halo_config_exists(cfg.bn);
-    // the persistent kernel's epilogue has no GELU, and its kernel has no cluster instantiation: a GELU layer takes neither
-    if ((r.relu & b2plan::kConvGelu) && cfg.cn > 1) return false;
-    if (cfg.ws) return kbsz == 64 && !(r.relu & b2plan::kConvGelu) && b2k::conv_ws_config_exists(cfg.bn, cfg.stages, cfg.sps);
-    if (!b2k::conv_config_exists(cfg.bn, kbsz, cfg.stages, cfg.sps)) return false;
-    if (cfg.splits > 1) {
-        const int tiles = ((batch * int(c->e->tensors[r.out].h * c->e->tensors[r.out].w) + 127) / 128) * (int(r.cout_phys) / cfg.bn);
-        if (tiles > kMaxSplitTiles || size_t(tiles) * cfg.splits * 128 * cfg.bn * 4 > kSplitWorkspaceBytes) return false;
-    }
-    return true;
-}
-
 // INT8 twin of autotune_conv: times every (N tile, ring depth) of conv_i8_tcgen05 on `c->autotune` concurrent streams.
 int autotune_i8_conv(b2_context* c, const Op& op, int batch, ConvConfig* best_out) {
     const b2plan::OpRec& r = op.r;
-    const int ns = std::max(1, std::min(c->autotune, 8));
-    std::vector<cudaStream_t> ss(size_t(ns), nullptr);
-    std::vector<cudaEvent_t> done(size_t(ns), nullptr);
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
-    bool ok = cudaEventCreate(&e0) == cudaSuccess && cudaEventCreate(&e1) == cudaSuccess;
-    for (int i = 0; i < ns && ok; ++i)
-        ok = cudaStreamCreateWithFlags(&ss[size_t(i)], cudaStreamNonBlocking) == cudaSuccess &&
-             cudaEventCreateWithFlags(&done[size_t(i)], cudaEventDisableTiming) == cudaSuccess;
-    auto cleanup = [&] {
-        for (auto s_ : ss)
-            if (s_) cudaStreamDestroy(s_);
-        for (auto d : done)
-            if (d) cudaEventDestroy(d);
-        if (e0) cudaEventDestroy(e0);
-        if (e1) cudaEventDestroy(e1);
-    };
-    if (!ok) {
-        cudaGetLastError();
-        cleanup();
-        return fail(B2_ECUDA, "autotune: cannot create streams/events");
-    }
+    TuneTimer tt(c);
+    int status = tt.init();
+    if (status) return status;
     const int verbose = env_int("B2_TUNE_VERBOSE", 0);
-    const int iters = std::max(4, env_int("B2_TUNE_ITERS", 12));
-    const int reps = std::max(1, env_int("B2_TUNE_REPS", 2));
     double best_ms = 1e30;
     ConvConfig best = *best_out;
-    int status = B2_OK;
     for (int bn : {128, 256}) {
         if (int(r.cout_phys) % bn) continue;
-        for (int st = 1; st <= 4 && !status; ++st) {
+        for (int st = 1; st <= 4; ++st) {
             if (!b2k::conv_i8_config_exists(bn, st)) continue;
             b2k::I8ConvLaunch cl;
-            if ((status = make_i8_conv_launch(c, op, batch, bn, st, &cl))) break;
-            int rc = 0;
-            for (int i = 0; i < 2 && !rc; ++i)
-                for (int k = 0; k < ns && !rc; ++k) rc = b2k::launch_conv_i8_tcgen05(cl, ss[size_t(k)]);
-            for (int k = 0; k < ns; ++k) cudaStreamSynchronize(ss[size_t(k)]);
-            float ms = 1e30f;
-            cudaError_t se = cudaSuccess;
-            for (int rep = 0; rep < reps && !rc && se == cudaSuccess; ++rep) {
-                cudaEventRecord(e0, ss[0]);
-                for (int k = 1; k < ns; ++k) cudaStreamWaitEvent(ss[size_t(k)], e0, 0);
-                for (int i = 0; i < iters && !rc; ++i)
-                    for (int k = 0; k < ns && !rc; ++k) rc = b2k::launch_conv_i8_tcgen05(cl, ss[size_t(k)]);
-                for (int k = 1; k < ns; ++k) {
-                    cudaEventRecord(done[size_t(k)], ss[size_t(k)]);
-                    cudaStreamWaitEvent(ss[0], done[size_t(k)], 0);
-                }
-                cudaEventRecord(e1, ss[0]);
-                se = cudaStreamSynchronize(ss[0]);
-                float t = 0.f;
-                if (se == cudaSuccess && cudaEventElapsedTime(&t, e0, e1) == cudaSuccess) ms = std::min(ms, t);
-            }
-            if (rc || se != cudaSuccess) {
-                status = fail(B2_ECUDA, "autotune of %s (int8 bn=%d st=%d) failed: %s", op.name.c_str(), bn, st,
-                              cudaGetErrorString(rc ? cudaError_t(rc) : se));
-                break;
-            }
+            if ((status = make_i8_conv_launch(c, op, batch, bn, st, &cl))) return status;
+            float ms = 0.f;
+            const cudaError_t err = tt.time([&](int, cudaStream_t s) { return b2k::launch_conv_i8_tcgen05(cl, s); }, &ms);
+            if (err != cudaSuccess)
+                return fail(B2_ECUDA, "autotune of %s (int8 bn=%d st=%d) failed: %s", op.name.c_str(), bn, st, cudaGetErrorString(err));
             if (verbose > 1)
                 fprintf(stderr, "[b2 tune]   %s b=%d cand int8 bn=%d st=%d : %.3f us/launch\n", op.name.c_str(), batch, bn, st,
-                        ms * 1e3 / (iters * ns));
+                        tt.us_per_launch(ms));
             if (ms < best_ms) best_ms = ms, best = ConvConfig{bn, st, 1, 0.0, 1, 0, 1};
         }
     }
-    cleanup();
-    if (status) return status;
-    best.est_us = best_ms * 1e3 / (iters * ns);
+    best.est_us = tt.us_per_launch(best_ms);
     if (verbose) {
         const Tensor& to = c->e->tensors[r.out];
         const long long M = (long long)batch * to.h * to.w, K = (long long)r.k * r.k * r.cin_phys;
         fprintf(stderr, "[b2 tune] %s b=%d M=%lld N=%d K=%lld best int8 bn=%d st=%d : %.3f us/launch (%d streams) %.0f TOP/s\n",
-                op.name.c_str(), batch, M, int(r.cout_phys), K, best.bn, best.stages, best.est_us, ns,
+                op.name.c_str(), batch, M, int(r.cout_phys), K, best.bn, best.stages, best.est_us, tt.ns,
                 2.0 * M * r.cout_phys * K / best.est_us * 1e-6);
     }
     *best_out = best;
@@ -1332,9 +1301,7 @@ int tune_engine_batch(b2_context* c, int batch) {
             tune_cache_append(e, int(i), batch, cfg);
             continue;
         }
-        const bool kb64 = r.cin_phys % 64 == 0, kb8 = r.cin_phys == 8;
-        if (!((kb64 || kb8) && r.cout_phys % 32 == 0 && (kb64 || r.taps_phys % 2 == 0))) continue;
-        if (op.groups > 1 && !op.group_span()) continue;  // grouped on the SIMT convolution: nothing to tune
+        if (!conv_on_tensor_cores(e, op)) continue;
         {
             std::lock_guard<std::mutex> lock(e->tune_mutex);
             if (e->tuned.count({int(i), batch})) continue;
@@ -1358,7 +1325,7 @@ int tune_engine_batch(b2_context* c, int batch) {
         }
         ConvConfig cfg = pick_conv_config(batch * int(to.h) * int(to.w), int(r.cout_phys), nkb, kbsz, r.res >= 0, c, false,
                                           op.group_span());
-        int rc = autotune_conv(c, op, batch, splits, -1, &cfg);
+        int rc = autotune_conv(c, op, batch, splits, &cfg);
         if (rc) return rc;
         std::lock_guard<std::mutex> lock(e->tune_mutex);
         e->tuned[{int(i), batch}] = cfg;
@@ -1616,12 +1583,6 @@ int build_plan(b2_context* c, int batch, Plan** out) {
                 const int M = batch * int(to.h) * int(to.w);
                 L.flops = 2.0 * M * r.cout * op.algo_k();
                 L.bytes = double(batch) * (ti.item_bytes + to.item_bytes * (r.res >= 0 ? 2 : 1)) + double(r.w_bytes);
-                const bool kb64 = r.cin_phys % 64 == 0;
-                const bool kb8 = r.cin_phys == 8;
-                // grouped: the tensor cores take the packed block-diagonal layout; any other grouped geometry is SIMT
-                const int span = op.group_span();
-                const bool tc_ok = half && !c->force_simt && (kb64 || kb8) && r.cout_phys % 32 == 0 &&
-                                   (kb64 || r.taps_phys % 2 == 0) && (op.groups == 1 || span > 0);
                 if (r.relu & 4) {  // INT8 tensor path
                     L.kind = L_CONV_I8;
                     // one tactic, by rule: the 128-wide N tile with a ring no deeper than the K loop, shallow enough (2-3
@@ -1644,33 +1605,15 @@ int build_plan(b2_context* c, int batch, Plan** out) {
                     if (!b2k::conv_i8_config_exists(bn, st)) bn = 128, st = 2;
                     int rc = make_i8_conv_launch(c, op, batch, bn, st, &L.i8);
                     if (rc) return rc;
-                } else if (tc_ok) {
+                } else if (!c->force_simt && conv_on_tensor_cores(e, op)) {
                     L.kind = L_CONV_TC;
-                    const int kbsz = conv_kb(c, op);
-                    const int nkb = conv_num_kblocks(c, op);
-                    ConvConfig cfg = pick_conv_config(M, int(r.cout_phys), nkb, kbsz, r.res >= 0, c, true, span);
-                    if (cfg.bn == 0)  // a forced tile that does not divide this layer: fall back to the model
-                        cfg = pick_conv_config(M, int(r.cout_phys), nkb, kbsz, r.res >= 0, c, false, span);
+                    ConvConfig cfg = forced_conv_config(c, op, batch);
                     if (cfg.bn == 0) return fail(B2_EINVAL, "conv %s: no kernel configuration", op.name.c_str());
-                    if (c->force_sps == 2 && b2k::conv_config_exists(cfg.bn, kbsz, cfg.stages, 2) &&
-                        b2k::conv_smem_bytes(cfg.bn, cfg.stages, r.res >= 0, 2) <= 227 * 1024)
-                        cfg.sps = 2;
-                    // (the persistent, halo and cluster tactics never take a grouped convolution)
-                    if (c->force_ws > 0 && kbsz == 64 && (r.relu & 2) && cfg.splits == 1 && !span && !(r.relu & b2plan::kConvGelu) &&
-                        b2k::conv_ws_config_exists(cfg.bn, cfg.stages, cfg.sps) &&
-                        b2k::conv_ws_smem(cfg.bn, cfg.stages, cfg.sps, r.res >= 0) <= 227 * 1024)
-                        cfg.ws = std::min(((M + 127) / 128) * (int(r.cout_phys) / cfg.bn), c->force_ws > 1 ? c->force_ws : g_sms);
-                    if (c->force_halo > 0 && conv_halo_rows(c, op) && b2k::conv_halo_config_exists(cfg.bn) && cfg.splits == 1 &&
-                        int(r.cin_phys) / 64 <= 8 && b2k::conv_halo_smem(cfg.bn, int(to.w), conv_halo_rows(c, op), int(r.cin_phys) / 64) <= 227 * 1024)
-                        cfg.halo = 1, cfg.ws = 0, cfg.cn = 1;
-                    if (c->force_cn > 1 && kbsz == 64 && cfg.ws == 0 && !cfg.halo && !span && !(r.relu & b2plan::kConvGelu) &&
-                        (int(r.cout_phys) / cfg.bn) % c->force_cn == 0)
-                        cfg.cn = c->force_cn;
                     const bool forced = c->force_bn || c->force_stages || c->force_splits || c->force_sps;
                     const int op_index = int(&op - &e->ops[0]);
                     // member of a persistent-kernel run: 64-channel K blocks, packed weights, 64 | Cout; no tactic to tune.
                     // A grouped layer is never a member: it ends a run
-                    const bool net_ok = c->net && !forced && kbsz == 64 && (r.relu & 2) && !c->no_pack && r.cout_phys % 64 == 0 &&
+                    const bool net_ok = c->net && !forced && conv_kb(c, op) == 64 && (r.relu & 2) && r.cout_phys % 64 == 0 &&
                                         c->force_ws <= 0 && c->force_cn <= 0 && c->force_halo <= 0 && !c->force_im2col && op.groups == 1 &&
                                         !(r.relu & b2plan::kConvGelu);  // (the network kernel's epilogue has no GELU)
                     if (net_ok) {
@@ -1707,7 +1650,7 @@ int build_plan(b2_context* c, int batch, Plan** out) {
                     a.relu = int(r.relu & (b2plan::kConvRelu | b2plan::kConvGelu));
                     a.w_packed = int((r.relu >> 1) & 1);
                     a.groups = op.groups;
-                    a.wk_tap = op.groups == 1 ? int(r.cin_phys) : span ? span : int(r.cin) / op.groups;
+                    a.wk_tap = op.groups == 1 ? int(r.cin_phys) : op.group_span() ? op.group_span() : int(r.cin) / op.groups;
                 }
                 break;
             }
@@ -2490,35 +2433,18 @@ int b2_engine_refine_tactics(b2_engine* e, int streams, int passes, double* gain
                 const int m_tiles = (batch * int(e->tensors[r.out].h * e->tensors[r.out].w) + 127) / 128;
                 for (int sp : {2, 4}) {
                     const int tiles = m_tiles * (int(r.cout_phys) / cur.bn);
-                    const int kpc = (nkb + sp - 1) / sp;
-                    if (nkb < 16 || tiles >= 100 || tiles * sp > 160 || kpc < 4 || (sp - 1) * kpc >= nkb || tiles > kMaxSplitTiles / 8 ||
-                        size_t(tiles) * sp * 128 * cur.bn * 4 > kSplitWorkspaceBytes)
-                        continue;
-                    for (int st : {2, 4}) {
-                        if (!b2k::conv_config_exists(cur.bn, kbsz, st, 1) || b2k::conv_smem_bytes(cur.bn, st, r.res >= 0, 1) > 227 * 1024) continue;
-                        cands.push_back(ConvConfig{cur.bn, st, sp, 0.0, 1, 0, 1});
-                    }
+                    if (nkb < 16 || tiles >= 100 || tiles * sp > 160 || tiles > kMaxSplitTiles / 8) continue;
+                    for (int st : {2, 4})
+                        if (tactic_applies(ctx[0].c, op, batch, ConvConfig{cur.bn, st, sp, 0.0, 1, 0, 1}))
+                            cands.push_back(ConvConfig{cur.bn, st, sp, 0.0, 1, 0, 1});
                 }
             }
             if (cur.splits > 1) continue;  // already split: leave it
-            for (int bn : {64, 128, 256}) {
-                if (int(r.cout_phys) % bn) continue;
-                for (int sps = 1; sps <= 2; ++sps)
-                    for (int st : {1, 2, 4, 8}) {
-                        if (!b2k::conv_config_exists(bn, kbsz, st, sps) || b2k::conv_smem_bytes(bn, st, r.res >= 0, sps) > 227 * 1024) continue;
-                        if (st * sps > nkb + 1 && st > 1) continue;  // a ring deeper than the K loop only costs shared memory
-                        if (sps == 2 && nkb < 4) continue;
-                        if (bn == cur.bn && st == cur.stages && sps == cur.sps && !cur.halo) continue;
-                        if (op.groups > 1 && !tactic_applies(ctx[0].c, op, batch, ConvConfig{bn, st, 1, 0.0, sps, 0, 1})) continue;
-                        cands.push_back(ConvConfig{bn, st, 1, 0.0, sps, 0, 1});
-                    }
-                if (conv_halo_rows(ctx[0].c, op) && b2k::conv_halo_config_exists(bn) && int(r.cin_phys) / 64 <= 8 && !(cur.halo && cur.bn == bn) &&
-                    b2k::conv_halo_smem(bn, int(e->tensors[r.out].w), conv_halo_rows(ctx[0].c, op), int(r.cin_phys) / 64) <= 227 * 1024) {
-                    ConvConfig hc{bn, kHaloStagesTag, 1, 0.0, 1, 0, 1};
-                    hc.halo = 1;
-                    cands.push_back(hc);
-                }
-            }
+            // the per-layer tuner's candidates, less the persistent, cluster and split-K tactics and the current one
+            for (const ConvConfig& t : conv_candidates(ctx[0].c, op, batch, 1))
+                if (!t.ws && t.cn <= 1 && t.splits == 1 &&
+                    !(t.bn == cur.bn && t.stages == cur.stages && t.sps == cur.sps && t.halo == cur.halo))
+                    cands.push_back(t);
             ConvConfig best = cur;
             for (const ConvConfig& cand : cands) {
                 {

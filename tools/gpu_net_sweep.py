@@ -23,10 +23,8 @@ for st in settings:
         os.environ["B2_NET_CTAS"] = kv["ctas"]
     if "bn" in kv:
         os.environ["B2_NET_BN"] = kv["bn"]
-    for k in ("B2_TUNE_TIE_PERMILLE", "B2_FUSE_TAIL", "B2_GRAPH", "B2_AUTOTUNE", "B2_ARENA_SLACK", "B2_TAIL_CTAS", "B2_TAIL_PDL", "B2_I8_BN", "B2_I8_STAGES"):
+    for k in ("B2_FUSE_TAIL", "B2_GRAPH", "B2_AUTOTUNE", "B2_ARENA_SLACK", "B2_TAIL_CTAS", "B2_TAIL_PDL", "B2_I8_BN", "B2_I8_STAGES"):
         os.environ.pop(k, None)
-    if "tie" in kv:
-        os.environ["B2_TUNE_TIE_PERMILLE"] = kv["tie"]
     if "tail" in kv:
         os.environ["B2_FUSE_TAIL"] = kv["tail"]
     if "graph" in kv:
