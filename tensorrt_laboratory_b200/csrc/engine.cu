@@ -780,7 +780,8 @@ ConvConfig pick_conv_config(int M, int cout_phys, int kblocks, int kb, bool resi
         if (honor_forced && c->force_bn && bn != c->force_bn) continue;
         const int tiles = m_tiles * (cout_phys / bn);
         for (int splits = 1; splits <= 8; ++splits) {
-            if (c->force_splits && !group_span ? splits != c->force_splits : splits != 1) continue;  // split-K is opt-in (measured slower)
+            // split-K is opt-in (measured slower); a forced split count this layer cannot take is dropped like bn and stages
+            if (honor_forced && c->force_splits && !group_span ? splits != c->force_splits : splits != 1) continue;
             if (splits > 1 && (kb != 64 || kblocks / splits < 4 || tiles * splits > 160 || tiles > kMaxSplitTiles ||
                                size_t(tiles) * splits * 128 * bn * 4 > kSplitWorkspaceBytes))
                 continue;
