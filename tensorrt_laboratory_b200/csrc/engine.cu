@@ -855,10 +855,18 @@ bool conv_on_tensor_cores(const b2_engine* e, const Op& op) {
     return e->half() && (kb64 || kb8) && r.cout_phys % 32 == 0 && (kb64 || r.taps_phys % 2 == 0) && (op.groups == 1 || op.group_span() > 0);
 }
 
+// The persistent stem kernel (conv_stem_ws_tcgen05): the row-folded 7x7 / stride-2 stem with 64 output channels, ReLU and
+// no residual, weights as a [Cout][K] matrix, and at most 128 output pixels per row (its M tile is one output row).
+bool conv_takes_stem_ws(const b2_context* c, const Op& op) {
+    const b2plan::OpRec& r = op.r;
+    return conv_is_row_folded(c, op) && op.kh() == 7 && op.sh() == 2 && r.cout_phys == 64 && c->e->tensors[r.out].w <= 128 &&
+           (r.relu & b2plan::kConvRelu) && !(r.relu & 2) && !(r.relu & b2plan::kConvGelu) && r.res < 0 && op.groups == 1;
+}
+
 // The persistent kernel needs 64-wide K blocks and packed weights, and has no GELU epilogue; nor does it take a grouped
-// convolution, whose CTAs along N read different channel blocks.
+// convolution, whose CTAs along N read different channel blocks.  The stem has a persistent kernel of its own.
 bool conv_takes_ws(const b2_context* c, const Op& op) {
-    return conv_kb(c, op) == 64 && (op.r.relu & 2) && op.groups == 1 && !(op.r.relu & b2plan::kConvGelu);
+    return conv_takes_stem_ws(c, op) || (conv_kb(c, op) == 64 && (op.r.relu & 2) && op.groups == 1 && !(op.r.relu & b2plan::kConvGelu));
 }
 
 // May tactic `cfg` run `op` at `batch`?  The one rule every tactic goes through: the tuners' candidates, the forced
@@ -876,6 +884,9 @@ bool tactic_applies(const b2_context* c, const Op& op, int batch, const ConvConf
         return R && cfg.splits == 1 && !cfg.ws && cfg.cn <= 1 && b2k::conv_halo_config_exists(cfg.bn) && cblocks <= 8 &&
                b2k::conv_halo_smem(cfg.bn, int(to.w), R, cblocks) <= kSmemLimit;
     }
+    if (cfg.ws && conv_is_row_folded(c, op))  // one encoding: N tile 64, the ring depth as the stage count
+        return conv_takes_stem_ws(c, op) && cfg.bn == 64 && cfg.stages == b2k::kStemWsRing && cfg.sps == 1 && cfg.splits == 1 &&
+               cfg.cn <= 1 && b2k::conv_stem_ws_smem() <= kSmemLimit;
     if (cfg.ws)
         return conv_takes_ws(c, op) && cfg.splits == 1 && cfg.cn <= 1 && b2k::conv_ws_config_exists(cfg.bn, cfg.stages, cfg.sps) &&
                b2k::conv_ws_smem(cfg.bn, cfg.stages, cfg.sps, r.res >= 0) <= kSmemLimit;
@@ -929,6 +940,14 @@ std::vector<ConvConfig> conv_candidates(const b2_context* c, const Op& op, int b
             out.push_back(c->force_cn > 1 && ok(cl) ? cl : t);
         }
     }
+    if (conv_takes_stem_ws(c, op) && c->force_ws >= 0 && fixed_splits <= 1) {  // the persistent stem: one CTA per SM, or half the SMs
+        const int rows = batch * int(c->e->tensors[r.out].h);
+        ConvConfig t{64, b2k::kStemWsRing, 1, 0.0, 1, std::min(rows, g_sms), 1};
+        if (ok(t)) {
+            out.push_back(t);
+            if (rows > g_sms / 2) t.ws = g_sms / 2, out.push_back(t);
+        }
+    }
     if (c->force_halo >= 0 && fixed_splits <= 1) {
         std::vector<ConvConfig> halo;
         for (int bn : {256, 128, 64, 32}) {
@@ -958,7 +977,14 @@ ConvConfig forced_conv_config(const b2_context* c, const Op& op, int batch) {
     };
     if (c->force_sps == 2) force([](ConvConfig& t) { t.sps = 2; });
     if (c->force_ws > 0)
-        force([&](ConvConfig& t) { t.ws = std::min((M + 127) / 128 * (int(r.cout_phys) / t.bn), c->force_ws > 1 ? c->force_ws : g_sms); });
+        force([&](ConvConfig& t) {
+            if (conv_takes_stem_ws(c, op)) {  // one work item per band of output rows; its own tactic encoding
+                t = ConvConfig{64, b2k::kStemWsRing, 1, t.est_us, 1, 0, 1};
+                t.ws = std::min(batch * int(c->e->tensors[r.out].h), c->force_ws > 1 ? c->force_ws : g_sms);
+                return;
+            }
+            t.ws = std::min((M + 127) / 128 * (int(r.cout_phys) / t.bn), c->force_ws > 1 ? c->force_ws : g_sms);
+        });
     if (c->force_halo > 0) force([](ConvConfig& t) { t.halo = 1, t.ws = 0, t.cn = 1; });
     if (c->force_cn > 1) force([&](ConvConfig& t) { t.cn = c->force_cn; });
     return cfg;
@@ -1052,6 +1078,11 @@ int make_conv_launch(b2_context* c, const Op& op, int batch, const ConvConfig& c
     else
         rc = make_map_2d(&cl.mapB, w, uint64_t(r.taps_phys) * r.cin_phys, r.cout_phys, uint32_t(cl.kb), uint32_t(cl.bn), swz);
     if (rc) return rc;
+    if (cfg.ws && fold) {  // persistent stem: one output row per M tile, a {C, W, H, N} map clips the pixels past Wo
+        rc = make_map_nhwc(&cl.mapOut, tptr(r.out), int(r.cout_phys), int(to.w), int(to.h), batch, 128, 1);
+        cl.mapRes = cl.mapOut;
+        return rc;
+    }
     // epilogue maps: 128-row x min(64, BN)-column boxes, 128B (or 64B for BN=32) swizzle = conflict-free staging
     const uint32_t ow = cl.bn >= 64 ? 64 : 32;
     const CUtensorMapSwizzle oswz = cl.bn >= 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;

@@ -746,6 +746,169 @@ conv_f16_tcgen05_ws(const __grid_constant__ CUtensorMap mapA, const __grid_const
 }
 
 // =================================================================================================
+// conv_stem_ws_tcgen05 -- persistent tactic for the row-folded 7x7 / stride-2 stem (KB = 32, 64 output channels, Wo <= 128).
+//   A work item is a band of consecutive output rows of one image; gridDim.x CTAs walk the item list with a static
+//   stride, and the band length ceil(N*Ho / gridDim.x) gives every CTA about the same number of rows.  The M tile is
+//   one output row: 128 pixels from the row's first one on; pixels >= Wo are computed and clipped by the 4-D output map.
+//   - The weights (7 filter rows x 64 channels x 32 K = 28 KiB) are loaded once per CTA and stay resident.
+//   - Output row p, filter row r reads input row 2p - 3 + r: the same im2col sub-tile as row p + 1, filter row r - 2.
+//     So a band is a linear sequence of input-row sub-tiles (128 pixels x 32 K, 8 KiB) in a ring of kStemWsRing slots:
+//     row i of the band reads sub-tiles 2i ... 2i + 6, its first row loads 7 and every later row 2 new ones.
+//   - warp 0 = producer (weights once, then the ring, running ahead across rows and bands); warps 4-7 / 8-11 = consumer
+//     warpgroups (pixels 0-63 / 64-127): 14 wgmma of K = 16 per row in the tile kernel's order (filter rows 0..6, two
+//     steps each, scale-d = 0 on the first), then bias + ReLU -> fp16 into one of two staging buffers, so the TMA store
+//     of row p overlaps the MMAs of row p + 1.  Same products, same fp32 summation order: the tile kernel's bits.
+// =================================================================================================
+constexpr int kStemRows = 7;     // filter rows (kh)
+constexpr int kStemStride = 2;   // new sub-tiles per output row (stride_h)
+constexpr int kStemASub = 128 * 32 * 2;
+constexpr int kStemBSub = 64 * 32 * 2;
+constexpr int kStemTile = 128 * 64 * 2;
+__host__ __device__ constexpr int conv_stem_ws_smem_bytes() {
+    return kStemWsRing * kStemASub + kStemRows * kStemBSub + 2 * kStemTile + 512 + 1024;
+}
+
+__global__ void __launch_bounds__(kConvThreads, 1)
+conv_stem_ws_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
+                     const __grid_constant__ CUtensorMap mapOut, const ConvArgs p) {
+    const int Ho = p.HoWo / p.Wo;
+    const int images = p.M / p.HoWo;
+    const int band = min(Ho, (images * Ho + static_cast<int>(gridDim.x) - 1) / static_cast<int>(gridDim.x));
+    const int bands_per_image = (Ho + band - 1) / band;
+    const int num_items = images * bands_per_image;
+    if (static_cast<int>(blockIdx.x) >= num_items) return;  // nothing to do: leave before any barrier or copy exists
+    auto item_rows = [&](int item, int& img, int& p0) -> int {
+        img = item / bands_per_image;
+        p0 = (item - img * bands_per_image) * band;
+        return min(band, Ho - p0);
+    };
+
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+    uint8_t* sA = smem;
+    uint8_t* sB = sA + kStemWsRing * kStemASub;
+    uint8_t* sOut = sB + kStemRows * kStemBSub;  // [2][kStemTile]
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(sOut + 2 * kStemTile);
+    uint64_t* empty_bar = full_bar + kStemWsRing;
+    uint64_t* w_bar = empty_bar + kStemWsRing;
+
+    const int warp = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
+    if (threadIdx.x == 0) {
+        tma_prefetch_desc(&mapA);
+        tma_prefetch_desc(&mapB);
+        tma_prefetch_desc(&mapOut);
+        for (int s = 0; s < kStemWsRing; ++s) {
+            mbar_init(&full_bar[s], 1);
+            mbar_init(&empty_bar[s], kConsumerWarps);
+        }
+        mbar_init(w_bar, 1);
+        fence_barrier_init();
+        fence_proxy_async();
+    }
+    __syncthreads();
+    if (p.pdl_trigger == 0) pdl_launch_dependents();
+
+    if (warp == 0) {
+        // ================= producer: weights once (constants, before the dependency wait), then the A ring =================
+        if (elect_one_sync()) {
+            mbar_expect_tx(w_bar, kStemRows * kStemBSub);
+            for (int r = 0; r < kStemRows; ++r) tma_load_2d(&mapB, w_bar, sB + r * kStemBSub, r * 32, 0);
+        }
+        __syncwarp();
+        pdl_wait();
+        int g = 0;  // sub-tiles loaded by this CTA so far (across bands)
+        for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
+            int img, p0;
+            const int rows = item_rows(item, img, p0);
+            for (int i = 0; i < rows; ++i) {
+                const int base_h = (p0 + i) * p.stride_h - p.pad_h;
+                for (int r = i == 0 ? 0 : kStemRows - kStemStride; r < kStemRows; ++r, ++g) {
+                    const int s = g % kStemWsRing;
+                    mbar_wait(&empty_bar[s], ((g / kStemWsRing) & 1) ^ 1);
+                    if (elect_one_sync()) {
+                        mbar_expect_tx(&full_bar[s], kStemASub);
+                        tma_load_im2col_4d(&mapA, &full_bar[s], sA + s * kStemASub, 0, -p.pad_w, base_h, img, 0,
+                                           static_cast<uint16_t>(r));
+                    }
+                    __syncwarp();
+                }
+            }
+        }
+    } else if (warp >= 4) {
+        // ================= consumers: 14 wgmma per output row, then the epilogue straight from the registers =================
+        pdl_wait();
+        const int cw = warp - 4;
+        const uint32_t wg_off = static_cast<uint32_t>(cw >> 2) * 4096u;  // 64 rows of 64 bytes
+        const FragPos fp(cw, lane);
+        const bool e0 = threadIdx.x == 128;
+        const uint32_t a_base = smem_u32(sA) + wg_off;
+        const uint32_t b_base = smem_u32(sB);
+        float2 bias[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) bias[j] = __ldg(reinterpret_cast<const float2*>(p.bias + 8 * j + fp.col0));
+        mbar_wait(w_bar, 0);
+        float acc[32];
+        int g = 0, lt = 0;
+        for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
+            int img, p0;
+            const int rows = item_rows(item, img, p0);
+            for (int i = 0; i < rows; ++i, ++lt) {
+                const int g0 = g + kStemStride * i;  // sub-tile of filter row 0
+                for (int r = i == 0 ? 0 : kStemRows - kStemStride; r < kStemRows; ++r)
+                    mbar_wait(&full_bar[(g0 + r) % kStemWsRing], ((g0 + r) / kStemWsRing) & 1);
+                auto mma = [&](int t) {  // filter row t / 2, then 2 x (K = 16) inside its 64-byte swizzle row
+                    const int r = t >> 1, j = t & 1;
+                    const uint32_t slot = static_cast<uint32_t>((g0 + r) % kStemWsRing);
+                    const uint64_t ad = make_wgmma_desc(a_base + slot * kStemASub + j * 32, 16, 512, WG_SW64);
+                    const uint64_t bd = make_wgmma_desc(b_base + r * kStemBSub + j * 32, 16, 512, WG_SW64);
+                    wgmma_f16<64>(acc, ad, bd, t > 0 ? 1u : 0u);
+                };
+                wgmma_group<2 * kStemRows>(mma);
+                wgmma_wait<0>();
+                // the sub-tiles the next row of the band does not read go back to the producer (all of them after the last row)
+                __syncwarp();
+                if (lane == 0) {
+                    const int done = i + 1 < rows ? kStemStride : kStemRows;
+                    for (int q = 0; q < done; ++q) mbar_arrive(&empty_bar[(g0 + q) % kStemWsRing]);
+                }
+                const int buf = lt & 1;
+                // (A) the store issued from this staging buffer two rows ago has finished READING it
+                if (e0) tma_store_wait_read1();
+                named_bar_sync(1, 256);
+                uint8_t* const my_out = sOut + buf * kStemTile;
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    const int col = 8 * j + fp.col0;
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const int row = fp.row0 + 8 * h;
+                        const uint32_t so = swz_off<128>(row, col / 8) + (col % 8) * 2;
+                        float v0 = acc[4 * j + 2 * h] + bias[j].x, v1 = acc[4 * j + 2 * h + 1] + bias[j].y;
+                        if (p.relu) {
+                            v0 = fmaxf(v0, 0.0f);
+                            v1 = fmaxf(v1, 0.0f);
+                        }
+                        *reinterpret_cast<__half2*>(my_out + so) = __floats2half2_rn(v0, v1);
+                    }
+                }
+                fence_proxy_async();
+                // (B) every consumer has staged its output rows
+                named_bar_sync(2, 256);
+                if (e0) {
+                    tma_store_4d(&mapOut, my_out, 0, 0, p0 + i, img);  // pixels >= Wo are clipped by the map
+                    tma_store_commit();
+                }
+            }
+            g += kStemRows + kStemStride * (rows - 1);
+        }
+        if (p.pdl_trigger == 1) pdl_launch_dependents();
+        if (e0) tma_store_wait_read0();  // shared memory must outlive the last bulk store's read
+    }
+    __syncthreads();
+}
+
+// =================================================================================================
 // conv3x3_halo_tcgen05 -- 3x3 / stride 1 / pad 1 convolution that brings every input pixel into shared memory ONCE per
 //   (tile, 64-channel block) instead of once per filter tap.
 //
@@ -1035,9 +1198,21 @@ static int launch_conv_halo(const ConvLaunch& L, cudaStream_t stream) {
 int init_conv_ws_kernels();
 int launch_conv_f16_tcgen05_ws(const ConvLaunch& L, cudaStream_t stream);
 
+int conv_stem_ws_smem() { return conv_stem_ws_smem_bytes(); }
+static int launch_conv_stem_ws(const ConvLaunch& L, cudaStream_t stream) {
+    const ConvArgs& a = L.args;
+    if (L.bn != 64 || a.Cout != 64 || a.Wo > 128 || a.taps != kStemRows || a.stride_h != kStemStride || a.residual != nullptr)
+        return static_cast<int>(cudaErrorInvalidValue);
+    return launch_kernel(conv_stem_ws_tcgen05, dim3(L.ws_ctas), dim3(kConvThreads), size_t(conv_stem_ws_smem_bytes()), stream, true,
+                         L.mapA, L.mapB, L.mapOut, L.args);
+}
+
 int init_conv_kernels() {
     int e = init_conv_ws_kernels();
     if (e) return e;
+    if ((e = static_cast<int>(cudaFuncSetAttribute(conv_stem_ws_tcgen05, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                   conv_stem_ws_smem_bytes()))))
+        return e;
     if ((e = init_conv_halo_kernels())) return e;
 #define B2_INIT(BN_, KB_, ST_, SPS_) \
     if ((e = init_one<BN_, KB_, ST_, SPS_>())) return e;
@@ -1052,7 +1227,7 @@ int init_conv_kernels() {
 
 int launch_conv_f16_tcgen05(const ConvLaunch& L, cudaStream_t stream) {
     if (L.halo) return launch_conv_halo(L, stream);
-    if (L.ws_ctas > 0) return launch_conv_f16_tcgen05_ws(L, stream);
+    if (L.ws_ctas > 0) return L.kb == 32 ? launch_conv_stem_ws(L, stream) : launch_conv_f16_tcgen05_ws(L, stream);
     if (L.cn > 1) {
 #define B2_CASE_CL(BN_, ST_, SPS_, CN_) \
     if (L.bn == BN_ && L.kb == 64 && L.stages == ST_ && L.sps == SPS_ && L.cn == CN_) return launch_one<BN_, 64, ST_, SPS_, CN_>(L, stream);

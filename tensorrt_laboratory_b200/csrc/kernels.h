@@ -75,6 +75,10 @@ bool conv_halo_config_exists(int bn);                                // 3x3 halo
 int conv_halo_smem(int bn, int w, int r, int cblocks);
 bool conv_ws_config_exists(int bn, int stages, int sps);             // persistent warp-specialised variant
 int conv_ws_smem(int bn, int stages, int sps, bool residual);
+// persistent row-folded stem (KB == 32 with ws_ctas > 0): a ring of kStemWsRing filter-row sub-tiles, reported as its
+// pipeline depth; 7x7 / stride-2 filters, 64 output channels, Wo <= 128, BN = 64, no residual
+constexpr int kStemWsRing = 16;
+int conv_stem_ws_smem();
 // programmatic dependent launch on/off for every kernel of this library (default on)
 void set_pdl(bool on);
 bool get_pdl();
