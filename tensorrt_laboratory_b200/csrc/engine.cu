@@ -792,10 +792,8 @@ ConvConfig pick_conv_config(int M, int cout_phys, int kblocks, int kb, bool resi
                 if (b2k::conv_smem_bytes(bn, st, residual) > kSmemLimit) continue;
                 if (honor_forced && c->force_stages && st != c->force_stages) continue;
                 if (!(honor_forced && c->force_stages) && !stage_depth_useful(bn, kb, st, kpc)) continue;
-                const double smem = b2k::conv_smem_bytes(bn, st, residual);
-                int per_sm = int(double(kSmemLimit) / smem);
-                per_sm = std::min(per_sm, bn <= 64 ? 2 : 1);  // 384-thread CTAs: the register file holds two only for BN <= 64
-                per_sm = std::max(1, std::min(per_sm, 8));
+                // CTAs sharing an SM: registers, threads and shared memory of the real instantiation
+                const int per_sm = std::max(1, b2k::conv_residency(bn, kb, st, 1, residual));
                 const int ctas = tiles * splits;
                 const int waves = (ctas + g_sms * per_sm - 1) / (g_sms * per_sm);
                 const int sharing = std::max(1, std::min(per_sm, (ctas + g_sms - 1) / g_sms));
@@ -1145,7 +1143,7 @@ int make_i8_conv_launch(b2_context* c, const Op& op, int batch, int bn, int stag
 struct TuneTimer {
     const int ns;
     const int iters = std::max(4, env_int("B2_TUNE_ITERS", 12));  // launches per stream and measurement
-    const int reps = std::max(1, env_int("B2_TUNE_REPS", 2));     // measurements per candidate (the quietest counts)
+    const int reps = std::max(1, env_int("B2_TUNE_REPS", 3));     // measurements per candidate (the quietest counts)
     std::vector<cudaStream_t> ss;
     std::vector<cudaEvent_t> done;
     cudaEvent_t e0 = nullptr, e1 = nullptr;
@@ -1169,7 +1167,11 @@ struct TuneTimer {
         return fail(B2_ECUDA, "autotune: cannot create streams/events");
     }
     // `launch(k, stream)` issues stream k's copy of the candidate (returns 0 or a cudaError_t).  Two warm-up rounds, then
-    // *ms = the quietest of `reps` windows of `iters` rounds on all streams; returns the first launch or stream error.
+    // one window of `iters` rounds on all streams is captured into a CUDA graph (stream k forks from and joins stream 0),
+    // and *ms = the quietest of `reps` launches of that graph; returns the first launch, capture or stream error.
+    // A graph, because the forward pass runs as one and because issuing the window launch by launch from the host takes
+    // about as long as the GPU needs to run it: that timing followed the host's enqueue rate (the same tactic measured
+    // 2.6 and 4.7 us per launch in two tunings) and the winner of a layer was close to a random pick.
     template <class F>
     cudaError_t time(F launch, float* ms) {
         int rc = 0;
@@ -1177,21 +1179,34 @@ struct TuneTimer {
             for (int k = 0; k < ns && !rc; ++k) rc = launch(k, ss[size_t(k)]);
         for (auto s : ss) cudaStreamSynchronize(s);
         *ms = 1e30f;
-        cudaError_t se = cudaSuccess;
+        if (rc) return cudaError_t(rc);
+        cudaGraph_t g = nullptr;
+        cudaGraphExec_t ge = nullptr;
+        cudaError_t se = cudaStreamBeginCapture(ss[0], cudaStreamCaptureModeThreadLocal);
+        if (se != cudaSuccess) return se;
+        cudaEventRecord(done[0], ss[0]);  // fork
+        for (int k = 1; k < ns; ++k) cudaStreamWaitEvent(ss[size_t(k)], done[0], 0);
+        for (int i = 0; i < iters && !rc; ++i)
+            for (int k = 0; k < ns && !rc; ++k) rc = launch(k, ss[size_t(k)]);
+        for (int k = 1; k < ns; ++k) {  // join
+            cudaEventRecord(done[size_t(k)], ss[size_t(k)]);
+            cudaStreamWaitEvent(ss[0], done[size_t(k)], 0);
+        }
+        se = cudaStreamEndCapture(ss[0], &g);
+        if (!rc && se == cudaSuccess) se = cudaGraphInstantiate(&ge, g, 0);
+        if (!rc && se == cudaSuccess) se = cudaGraphLaunch(ge, ss[0]);  // first launch of the graph: uploads it
+        if (!rc && se == cudaSuccess) se = cudaStreamSynchronize(ss[0]);
         for (int rep = 0; rep < reps && !rc && se == cudaSuccess; ++rep) {
             cudaEventRecord(e0, ss[0]);
-            for (int k = 1; k < ns; ++k) cudaStreamWaitEvent(ss[size_t(k)], e0, 0);
-            for (int i = 0; i < iters && !rc; ++i)
-                for (int k = 0; k < ns && !rc; ++k) rc = launch(k, ss[size_t(k)]);
-            for (int k = 1; k < ns; ++k) {
-                cudaEventRecord(done[size_t(k)], ss[size_t(k)]);
-                cudaStreamWaitEvent(ss[0], done[size_t(k)], 0);
-            }
+            se = cudaGraphLaunch(ge, ss[0]);
             cudaEventRecord(e1, ss[0]);
-            se = cudaStreamSynchronize(ss[0]);
+            if (se == cudaSuccess) se = cudaStreamSynchronize(ss[0]);
             float t = 0.f;
             if (se == cudaSuccess && cudaEventElapsedTime(&t, e0, e1) == cudaSuccess) *ms = std::min(*ms, t);
         }
+        if (ge) cudaGraphExecDestroy(ge);
+        if (g) cudaGraphDestroy(g);
+        if (rc || se != cudaSuccess) cudaGetLastError();
         return rc ? cudaError_t(rc) : se;
     }
     double us_per_launch(double ms) const { return ms * 1e3 / (iters * ns); }
@@ -2668,6 +2683,20 @@ int b2_context_debug_net_timing(b2_context* c, int batch, void* const* bindings,
     cudaFree(d);
     if (rc) return rc;
     if (se != cudaSuccess) return fail(B2_ECUDA, "debug launch failed: %s", cudaGetErrorString(se));
+    return B2_OK;
+}
+
+// Debug aid (not part of the drop-in surface): CTAs of one convolution instantiation that fit on an SM of the current
+// device -- the tile kernel at (bn, kb, stages, sps, residual), or with halo_w > 0 the halo kernel at N tile bn for an
+// output width halo_w, halo_rows rows per tile and cblocks channel blocks.  The number the cost model uses.
+int b2_debug_conv_residency(int bn, int kb, int stages, int sps, int residual, int halo_w, int halo_rows, int cblocks,
+                            int* ctas_per_sm) {
+    if (!ctas_per_sm) return fail(B2_EINVAL, "null output");
+    const int rc = b2k::init_conv_kernels();
+    if (rc) return fail(B2_ECUDA, "kernel attribute setup failed: %s", cudaGetErrorString(cudaError_t(rc)));
+    *ctas_per_sm = b2k::conv_residency(bn, kb, stages, sps, residual != 0, halo_w, halo_rows, cblocks);
+    if (*ctas_per_sm <= 0)
+        return fail(B2_EINVAL, "no residency for bn=%d kb=%d st=%dx%d res=%d halo_w=%d", bn, kb, stages, sps, residual, halo_w);
     return B2_OK;
 }
 

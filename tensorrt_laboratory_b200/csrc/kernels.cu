@@ -2,9 +2,9 @@
 //
 //  * conv_f16_tcgen05 -- implicit-GEMM convolution: TMA (tiled or im2col mode) -> 128B-swizzled smem ->
 //    wgmma (64xBNx16 per warpgroup, fp16 x fp16 -> fp32 in registers) -> epilogue with bias / residual / ReLU
-//    fused -> swizzled smem tile -> TMA store.  One 128xBN output tile per CTA of 12 warps: warp 0 = activation
-//    producer, warp 3 = weight producer (64-wide K-blocks), warps 4-7 and 8-11 = the two consumer warpgroups
-//    (output rows 0-63 and 64-127: wgmma + epilogue).
+//    fused -> swizzled smem tile -> TMA store.  One 128xBN output tile per CTA of 10 warps: warps 0-3 and 4-7 = the
+//    two consumer warpgroups (output rows 0-63 and 64-127: wgmma + epilogue), warp 8 = activation (and residual)
+//    producer, warp 9 = weight producer (64-wide K-blocks).
 //  * SIMT kernels -- fp32-engine reference path (fp64 accumulate) and the non-GEMM operators
 //    (layout casts, max/avg pool, FC, softmax).
 //
@@ -15,6 +15,10 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+
+#include <array>
+#include <map>
+#include <mutex>
 
 #include "ptx_sm90.cuh"
 #include "wgmma_sm90.cuh"
@@ -42,8 +46,20 @@ __host__ __device__ constexpr int conv_smem_layout_bytes(int bn, int stages, boo
 // AV resolves the operand paths at compile time for the production instantiations: 1 = im2col-mode activations + packed
 // weights, 2 = tiled activations + packed weights, 0 = decided at run time from ConvArgs (thin-K paths, unpacked plans,
 // clusters, debug).
-constexpr int kConvThreads = 384;
-constexpr int kConsumerWarps = 8;  // warps 4..11: two warpgroups of 64 output rows each
+//
+// Tile and halo kernels: 10 warps.  Warps 0-7 are the two consumer warpgroups (wgmma needs a warpgroup to start on a warp
+// index divisible by 4), warp 8 loads the activations (and the residual tile), warp 9 the weights (and the bias).  No
+// warp idles, so at <= 96 registers per thread two 128-wide CTAs share an SM's register file (three 64-wide ones at
+// <= 64): one CTA's prologue, first TMA round trip and epilogue then overlap the other's MMAs.
+constexpr int kConvThreads = 320;
+constexpr int kConsumerWarps = 8;  // two warpgroups of 64 output rows each
+constexpr int kActWarp = 8;        // tile / halo kernels: activation producer
+constexpr int kWgtWarp = 9;        // tile / halo kernels: weight producer
+// CTAs per SM the tile and halo kernels are compiled for (their register budget); __graft_entry__.py checks the
+// ptxas report against the same rule
+__host__ __device__ constexpr int conv_min_ctas(int bn) { return bn <= 64 ? 3 : bn <= 128 ? 2 : 1; }
+// Persistent and stem kernels: 12 warps, warps 4-7 / 8-11 the consumer warpgroups, warps 0-3 producers (some idle).
+constexpr int kConvWsThreads = 384;
 
 // Thread (warp w of its warpgroup, lane l) of consumer warpgroup `wg` owns rows 64 wg + 16 w + l/4 (+8) and columns
 // 8j + 2(l%4) (+1) of the 128 x BN tile (wgmma fragment layout, wgmma_sm90.cuh).
@@ -57,7 +73,7 @@ struct FragPos {
 // tiled, packed-weight operand path only (AV == 2: the 1x1 layers of transformer encoders); the other instantiations keep
 // the ReLU-only epilogue unchanged.
 template <int BN, int KB, int STAGES, int SPS, int CN = 1, bool DBG = false, int AV = 0, bool GELU = false>
-__global__ void __launch_bounds__(kConvThreads, BN <= 64 ? 2 : 1)
+__global__ void __launch_bounds__(kConvThreads, conv_min_ctas(BN))
 conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
                  const __grid_constant__ CUtensorMap mapOut, const __grid_constant__ CUtensorMap mapRes,
                  const ConvArgs p) {
@@ -140,7 +156,7 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
     }
     __syncthreads();
     if (cn > 1) cluster_sync_all();  // peers' barriers exist before anything is multicast at them
-    if (warp == 3) {  // bias -> smem while the pipeline spins up; published by the pre-epilogue barrier
+    if (warp == kWgtWarp) {  // bias -> smem while the pipeline spins up; published by the pre-epilogue barrier
 #pragma unroll
         for (int i = 0; i < BN / 32; ++i) s_bias[lane + 32 * i] = __ldg(p.bias + n0 + lane + 32 * i);
     }
@@ -185,7 +201,7 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
         for (int b = 0; b < NBOX; ++b) tma_load_2d(&mapRes, res_bar, sRes + b * (128 * OROWB), n0 + b * OW, m0);
     };
 
-    if (warp == 0) {
+    if (warp == kActWarp) {
         {
             // ================= TMA producer (whole warp converged, one elected lane issues) =================
             int img0 = 0, p0 = 0, q0 = 0;
@@ -254,7 +270,7 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
                     }
                 }
             };
-            // For 64-wide K-blocks the weights have their own issuing thread (warp 3): one thread needs ~200 cycles
+            // For 64-wide K-blocks the weights have their own issuing thread (warp 9): one thread needs ~200 cycles
             // per TMA instruction, which is what paces the main loop.
             constexpr bool kSplitProducers = KB == 64;
             const int npre = nk < STAGES ? nk : STAGES;
@@ -297,9 +313,10 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
     }
 
     // ================= consumers: wgmma over the ring, accumulators in registers =================
-    const int cw = warp - 4;  // consumer warp 0..7 (warpgroup cw / 4)
+    const int cw = warp;  // consumer warp 0..7 (warpgroup cw / 4); warps 8 and 9 are the producers
+    const bool consumer = warp < kConsumerWarps;
     float acc[BN / 2];
-    if (warp >= 4) {
+    if (consumer) {
         const uint32_t wg = static_cast<uint32_t>(cw >> 2);
         // one arrival per consumer warp (on every CTA of the cluster: a peer refills its slice of our stage)
         auto release_stage = [&](int st) {
@@ -367,7 +384,7 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
         if (dbg && cw == 0 && lane == 0) dbg[4] = clock64(), dbg[14] = mw, dbg[15] = mi;
     }
 
-    if (warp == 3 && KB == 64) {
+    if (warp == kWgtWarp && KB == 64) {
         // ================= weight producer: constants, so no dependency wait; only the ring's empty barriers ====
         for (int i = 0; i < nk; ++i) {
             const int s = i % STAGES;
@@ -380,7 +397,7 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
     // ====== epilogue (consumer warpgroups): registers -> bias/residual/ReLU -> fp16 -> swizzled smem tile -> TMA store ======
     pdl_wait();  // every global access below depends on the previous kernel
     __syncthreads();  // every role has left its loop: the pipeline buffers are free to become the output staging tile; s_bias visible
-    if (dbg && threadIdx.x == 128) dbg[5] = clock64();
+    if (dbg && threadIdx.x == 0) dbg[5] = clock64();  // (thread 0: consumer warp 0, lane 0)
     if (p.pdl_trigger == 1) pdl_launch_dependents();
     const FragPos fp(cw, lane);
 
@@ -408,7 +425,7 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
 
     bool do_store = true;
     if (!split) {
-        if (warp >= 4) {
+        if (consumer) {
             if (has_res) mbar_wait(res_bar, 0);
 #pragma unroll
             for (int j = 0; j < BN / 8; ++j)
@@ -419,7 +436,7 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
         // ---- split-K: publish the fp32 partial tile, the last CTA of the tile reduces IN FIXED ORDER ----
         const int tile = blockIdx.y * gridDim.x + blockIdx.x;
         float* ws_tile = p.workspace + static_cast<size_t>(tile) * p.splits * (128 * BN);
-        if (warp >= 4) {
+        if (consumer) {
             float* mine = ws_tile + static_cast<size_t>(blockIdx.z) * (128 * BN);
 #pragma unroll
             for (int j = 0; j < BN / 8; ++j)
@@ -429,7 +446,7 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
                            make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]));
         }
         __syncthreads();
-        if (threadIdx.x == 0) {
+        if (threadIdx.x == kActWarp * 32) {
             __threadfence();  // cumulative: orders the whole CTA's partial-tile stores before the arrival
             const int prev = atomicAdd(p.tile_counters + tile, 1);
             const uint32_t last = (prev == p.splits - 1) ? 1u : 0u;
@@ -441,7 +458,7 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
         }
         __syncthreads();
         do_store = *last_flag != 0;
-        if (do_store && warp >= 4) {
+        if (do_store && consumer) {
             __threadfence();
             if (has_res) mbar_wait(res_bar, 0);
 #pragma unroll 4
@@ -460,11 +477,11 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
             }
         }
     }
-    if (dbg && threadIdx.x == 128) dbg[6] = clock64();
+    if (dbg && threadIdx.x == 0) dbg[6] = clock64();
     if (p.pdl_trigger == 2) pdl_launch_dependents();  // latest useful point: only the output store is left
     fence_proxy_async();  // generic-proxy smem writes -> visible to the TMA (async proxy)
     __syncthreads();
-    if (threadIdx.x == 0 && do_store) {
+    if (threadIdx.x == kActWarp * 32 && do_store) {  // the activation producer: consumer warps may retire
         // rows >= M and nothing else are clipped by the tensor map; one bulk store per 64-column box
 #pragma unroll
         for (int b = 0; b < NBOX; ++b) tma_store_2d(&mapOut, sOut + b * (128 * OROWB), n0 + b * OW, m0);
@@ -473,14 +490,14 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
     if (cn > 1) {
         // peers arrive on THIS CTA's empty barriers when their MMAs retire: hear the last release of every stage before
         // the shared memory can go to another CTA, then leave together
-        if (warp == 1) {
+        if (warp == kWgtWarp) {
             const int first = nk > STAGES ? nk - STAGES : 0;
             for (int i = first; i < nk; ++i) mbar_wait(&empty_bar[i % STAGES], (i / STAGES) & 1);
         }
         __syncthreads();
         cluster_sync_all();
     }
-    if (dbg && threadIdx.x == 128) {
+    if (dbg && threadIdx.x == 0) {
         dbg[7] = clock64();
         unsigned long long gt;
         asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt));
@@ -506,7 +523,7 @@ __host__ __device__ constexpr int conv_ws_smem_bytes(int bn, int stages, int sps
 }
 
 template <int BN, int STAGES, int SPS>
-__global__ void __launch_bounds__(kConvThreads, 1)
+__global__ void __launch_bounds__(kConvWsThreads, 1)
 conv_f16_tcgen05_ws(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapOut,
                     const __grid_constant__ CUtensorMap mapRes, const ConvArgs p) {
     constexpr int A_SUBBLK = 128 * 64 * 2;
@@ -768,7 +785,7 @@ __host__ __device__ constexpr int conv_stem_ws_smem_bytes() {
     return kStemWsRing * kStemASub + kStemRows * kStemBSub + 2 * kStemTile + 512 + 1024;
 }
 
-__global__ void __launch_bounds__(kConvThreads, 1)
+__global__ void __launch_bounds__(kConvWsThreads, 1)
 conv_stem_ws_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
                      const __grid_constant__ CUtensorMap mapOut, const ConvArgs p) {
     const int Ho = p.HoWo / p.Wo;
@@ -920,7 +937,7 @@ conv_stem_ws_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_cons
 //   Columns ww = W, W+1 of every row compute garbage that the output TMA store (box {BN, W+2, R, 1} at w = 0) clips.
 //   A traffic per tile and channel block: (R+2)(W+2) pixel rows instead of 9 x 128.
 //
-//   warp 0 = halo producer, warp 3 = weight producer, warps 4-11 = two consumer warpgroups (wgmma + epilogue).
+//   warps 0-7 = two consumer warpgroups (wgmma + epilogue), warp 8 = halo producer, warp 9 = weight producer.
 //   The halo blocks of ALL channel blocks stay resident, so the K loop runs tap outer / channel block inner exactly
 //   like the im2col kernel: same products in the same fp32 summation order -> bit-identical results, whichever of the
 //   two tactics the tuner picks.
@@ -939,7 +956,7 @@ __host__ __device__ constexpr int halo_smem_bytes(int bn, int w, int r, int cblo
 }
 
 template <int BN>
-__global__ void __launch_bounds__(kConvThreads, 1)
+__global__ void __launch_bounds__(kConvThreads, conv_min_ctas(BN))
 conv3x3_halo_tcgen05(const __grid_constant__ CUtensorMap mapIn, const __grid_constant__ CUtensorMap mapOut, const ConvArgs p) {
     constexpr int NB = halo_b_stages(BN);
     constexpr int B_BLK = BN * 128;  // one tap of one 64-channel block: BN rows of 128 B (pre-swizzled)
@@ -984,7 +1001,7 @@ conv3x3_halo_tcgen05(const __grid_constant__ CUtensorMap mapIn, const __grid_con
     if (p.pdl_trigger == 0) pdl_launch_dependents();
 
     float acc[BN / 2];
-    if (warp == 0) {
+    if (warp == kActWarp) {
         // ================= halo producer =================
         const uint32_t halo_bytes = static_cast<uint32_t>((R + 2) * Wp * 128);
         pdl_wait();
@@ -995,9 +1012,9 @@ conv3x3_halo_tcgen05(const __grid_constant__ CUtensorMap mapIn, const __grid_con
             }
         }
         __syncwarp();
-    } else if (warp >= 4) {
+    } else if (warp < kConsumerWarps) {
         // ================= consumers: wgmma, accumulators in registers =================
-        const uint32_t wg_off = static_cast<uint32_t>((warp - 4) >> 2) * 8192u;  // 64 pixel rows of 128 B
+        const uint32_t wg_off = static_cast<uint32_t>(warp >> 2) * 8192u;  // 64 pixel rows of 128 B
         int i = 0;
 #pragma unroll 1
         for (int tap = 0; tap < 9; ++tap) {
@@ -1027,7 +1044,7 @@ conv3x3_halo_tcgen05(const __grid_constant__ CUtensorMap mapIn, const __grid_con
         wgmma_wait<0>();
         __syncwarp();
         if (lane == 0) mbar_arrive(&b_empty[(nsteps - 1) % NB]);
-    } else if (warp == 3) {
+    } else if (warp == kWgtWarp) {
         // ================= weight producer (constants: no dependency wait) =================
         for (int i = lane; i < BN; i += 32) s_bias[i] = __ldg(p.bias + n0 + i);
         for (int i = 0; i < nsteps; ++i) {
@@ -1046,8 +1063,8 @@ conv3x3_halo_tcgen05(const __grid_constant__ CUtensorMap mapIn, const __grid_con
     pdl_wait();
     __syncthreads();
     if (p.pdl_trigger == 1) pdl_launch_dependents();
-    if (warp >= 4) {
-        const FragPos fp(warp - 4, lane);
+    if (warp < kConsumerWarps) {
+        const FragPos fp(warp, lane);
 #pragma unroll
         for (int j = 0; j < BN / 8; ++j) {
 #pragma unroll
@@ -1065,7 +1082,7 @@ conv3x3_halo_tcgen05(const __grid_constant__ CUtensorMap mapIn, const __grid_con
     }
     fence_proxy_async();
     __syncthreads();
-    if (threadIdx.x == 0) {
+    if (threadIdx.x == kActWarp * 32) {
         // box {64 ch, W+2, R, 1} at w = 0: the two garbage columns of every row and rows past H are clipped
 #pragma unroll
         for (int b = 0; b < NBOX; ++b) tma_store_4d(&mapOut, sOut + b * (128 * 128), n0 + b * OW, 0, h0, img);
@@ -1137,24 +1154,30 @@ static int launch_one(const ConvLaunch& L, cudaStream_t stream) {
                                  static_cast<unsigned>(CN), L.mapA, L.mapB, L.mapOut, L.mapRes, L.args);
 }
 
+// Opt a tile or halo instantiation in to `bytes` of dynamic shared memory, and ask for the largest shared-memory carveout:
+// a CTA needs less than half of an SM's 228 KiB in the shallow-ring configurations, and an L1 split picked for one CTA
+// would quietly cap the SM at one.
+template <typename Kern>
+static int set_conv_smem(Kern kern, int bytes) {
+    int e = static_cast<int>(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    if (!e) e = static_cast<int>(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    return e;
+}
+
 template <int BN, int KB, int STAGES, int SPS, int CN = 1>
 static int init_one() {
     const int want = conv_smem_layout_bytes(BN, STAGES, true, SPS);
     const int bytes = want > 227 * 1024 ? conv_smem_layout_bytes(BN, STAGES, false, SPS) : want;
     if (CN == 1) {
-        int e = static_cast<int>(cudaFuncSetAttribute(conv_f16_tcgen05<BN, KB, STAGES, SPS, 1, true>,
-                                                      cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+        int e = set_conv_smem(conv_f16_tcgen05<BN, KB, STAGES, SPS, 1, true>, bytes);
         if (e) return e;
         if constexpr (KB == 64) {
-            if ((e = static_cast<int>(cudaFuncSetAttribute(conv_f16_tcgen05<BN, KB, STAGES, SPS, 1, false, 1>,
-                                                           cudaFuncAttributeMaxDynamicSharedMemorySize, bytes)))) return e;
-            if ((e = static_cast<int>(cudaFuncSetAttribute(conv_f16_tcgen05<BN, KB, STAGES, SPS, 1, false, 2>,
-                                                           cudaFuncAttributeMaxDynamicSharedMemorySize, bytes)))) return e;
-            if ((e = static_cast<int>(cudaFuncSetAttribute(conv_f16_tcgen05<BN, KB, STAGES, SPS, 1, false, 2, true>,
-                                                           cudaFuncAttributeMaxDynamicSharedMemorySize, bytes)))) return e;
+            if ((e = set_conv_smem(conv_f16_tcgen05<BN, KB, STAGES, SPS, 1, false, 1>, bytes))) return e;
+            if ((e = set_conv_smem(conv_f16_tcgen05<BN, KB, STAGES, SPS, 1, false, 2>, bytes))) return e;
+            if ((e = set_conv_smem(conv_f16_tcgen05<BN, KB, STAGES, SPS, 1, false, 2, true>, bytes))) return e;
         }
     }
-    return static_cast<int>(cudaFuncSetAttribute(conv_f16_tcgen05<BN, KB, STAGES, SPS, CN>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    return set_conv_smem(conv_f16_tcgen05<BN, KB, STAGES, SPS, CN>, bytes);
 }
 
 int conv_smem_bytes(int bn, int stages, bool residual, int sps) { return conv_smem_layout_bytes(bn, stages, residual, sps); }
@@ -1172,10 +1195,9 @@ int conv_halo_smem(int bn, int w, int r, int cblocks) { return halo_smem_bytes(b
 bool conv_halo_config_exists(int bn) { return bn == 64 || bn == 128 || bn == 256; }
 static int init_conv_halo_kernels() {
     int e;
-    if ((e = static_cast<int>(cudaFuncSetAttribute(conv3x3_halo_tcgen05<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)))) return e;
-    if ((e = static_cast<int>(cudaFuncSetAttribute(conv3x3_halo_tcgen05<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)))) return e;
-    if ((e = static_cast<int>(cudaFuncSetAttribute(conv3x3_halo_tcgen05<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)))) return e;
-    return 0;
+    if ((e = set_conv_smem(conv3x3_halo_tcgen05<64>, 227 * 1024))) return e;
+    if ((e = set_conv_smem(conv3x3_halo_tcgen05<128>, 227 * 1024))) return e;
+    return set_conv_smem(conv3x3_halo_tcgen05<256>, 227 * 1024);
 }
 static int launch_conv_halo(const ConvLaunch& L, cudaStream_t stream) {
     const int R = L.args.halo_rows;
@@ -1203,7 +1225,7 @@ static int launch_conv_stem_ws(const ConvLaunch& L, cudaStream_t stream) {
     const ConvArgs& a = L.args;
     if (L.bn != 64 || a.Cout != 64 || a.Wo > 128 || a.taps != kStemRows || a.stride_h != kStemStride || a.residual != nullptr)
         return static_cast<int>(cudaErrorInvalidValue);
-    return launch_kernel(conv_stem_ws_tcgen05, dim3(L.ws_ctas), dim3(kConvThreads), size_t(conv_stem_ws_smem_bytes()), stream, true,
+    return launch_kernel(conv_stem_ws_tcgen05, dim3(L.ws_ctas), dim3(kConvWsThreads), size_t(conv_stem_ws_smem_bytes()), stream, true,
                          L.mapA, L.mapB, L.mapOut, L.args);
 }
 
@@ -1250,7 +1272,7 @@ int launch_conv_f16_tcgen05(const ConvLaunch& L, cudaStream_t stream) {
 template <int BN, int STAGES, int SPS>
 static int launch_one_ws(const ConvLaunch& L, cudaStream_t stream) {
     const size_t smem = size_t(conv_ws_smem_bytes(BN, STAGES, SPS, L.args.residual != nullptr));
-    return launch_kernel(conv_f16_tcgen05_ws<BN, STAGES, SPS>, dim3(L.ws_ctas), dim3(kConvThreads), smem, stream, true, L.mapA, L.mapOut,
+    return launch_kernel(conv_f16_tcgen05_ws<BN, STAGES, SPS>, dim3(L.ws_ctas), dim3(kConvWsThreads), smem, stream, true, L.mapA, L.mapOut,
                          L.mapRes, L.args);
 }
 
@@ -1301,6 +1323,47 @@ bool conv_config_exists(int bn, int kb, int stages, int sps) {
     B2_FOR_EACH_CONV(B2_HAS)
 #undef B2_HAS
     return false;
+}
+
+// CTAs per SM of the tile kernel at (bn, kb, stages, sps, residual), or of the halo kernel (halo_w > 0) at that output
+// width, rows per tile and channel-block count: the occupancy calculator at the real dynamic shared memory, so registers,
+// threads, shared memory and the carveout set by init_conv_kernels() all count.  The generic (AV = 0) instantiation
+// stands for its operand-path variants: they share its launch bounds, and the build refuses a variant whose registers
+// break them.  Cached per configuration; 0 when the configuration does not exist or the query fails.
+int conv_residency(int bn, int kb, int stages, int sps, bool residual, int halo_w, int halo_rows, int cblocks) {
+    static std::mutex mu;
+    static std::map<std::array<int, 8>, int> cache;
+    const std::array<int, 8> key{bn, kb, stages, sps, residual ? 1 : 0, halo_w, halo_rows, cblocks};
+    {
+        std::lock_guard<std::mutex> lock(mu);
+        const auto it = cache.find(key);
+        if (it != cache.end()) return it->second;
+    }
+    const void* fn = nullptr;
+    int smem = 0;
+    if (halo_w > 0) {
+        smem = halo_smem_bytes(bn, halo_w, halo_rows, cblocks);
+        if (bn == 64) fn = reinterpret_cast<const void*>(conv3x3_halo_tcgen05<64>);
+        if (bn == 128) fn = reinterpret_cast<const void*>(conv3x3_halo_tcgen05<128>);
+        if (bn == 256) fn = reinterpret_cast<const void*>(conv3x3_halo_tcgen05<256>);
+    } else {
+        smem = conv_smem_layout_bytes(bn, stages, residual, sps);
+#define B2_FN(BN_, KB_, ST_, SPS_) \
+    if (bn == BN_ && kb == KB_ && stages == ST_ && sps == SPS_) fn = reinterpret_cast<const void*>(conv_f16_tcgen05<BN_, KB_, ST_, SPS_>);
+        B2_FOR_EACH_CONV(B2_FN)
+#undef B2_FN
+    }
+    if (!fn || smem > 227 * 1024) return 0;
+    int n = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, fn, kConvThreads, static_cast<size_t>(smem)) != cudaSuccess) {
+        cudaGetLastError();
+        return 0;
+    }
+    if (n > 0) {  // (0 before the attributes are set is not cached)
+        std::lock_guard<std::mutex> lock(mu);
+        cache[key] = n;
+    }
+    return n;
 }
 
 // =================================================================================================

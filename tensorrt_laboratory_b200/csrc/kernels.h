@@ -73,6 +73,9 @@ int conv_smem_bytes(int bn, int stages, bool residual, int sps = 1);  // dynamic
 bool conv_cluster_config_exists(int bn, int stages, int sps, int cn);  // cluster-multicast instantiations
 bool conv_halo_config_exists(int bn);                                // 3x3 halo variant
 int conv_halo_smem(int bn, int w, int r, int cblocks);
+// CTAs of the tile kernel (halo_w == 0) or of the halo kernel (output width halo_w, halo_rows rows per tile, cblocks
+// channel blocks) that fit on one SM; needs init_conv_kernels() and a current device, 0 if unknown.  Cached.
+int conv_residency(int bn, int kb, int stages, int sps, bool residual, int halo_w = 0, int halo_rows = 0, int cblocks = 0);
 bool conv_ws_config_exists(int bn, int stages, int sps);             // persistent warp-specialised variant
 int conv_ws_smem(int bn, int stages, int sps, bool residual);
 // persistent row-folded stem (KB == 32 with ws_ctas > 0): a ring of kStemWsRing filter-row sub-tiles, reported as its
