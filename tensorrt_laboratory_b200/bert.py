@@ -22,7 +22,7 @@ class BertConfig:
     vocab: int = 30522
     positions: int = 512
     types: int = 2
-    seq: int = 128          # the sequence length S a plan is built for (a multiple of 64, at most 128)
+    seq: int = 128          # the sequence length S a plan is built for (64, 128, 256, 384 or 512; at most positions)
     eps: float = 1e-12      # LayerNorm epsilon
 
 

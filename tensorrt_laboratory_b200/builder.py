@@ -365,7 +365,8 @@ def _serialize(tensors: List[dict], ops: List[dict], bindings: List[dict], paylo
 
 def build_bert_plan(cfg=None, weights=None, max_batch: int = 16, seed: int = 0, precision: int = PREC_FP16,
                     name: Optional[str] = None, taps: Sequence[str] = ()) -> bytes:
-    """BERT encoder + pooler (``bert.BertConfig``; default BERT-base at S = 128) -> fp16 plan (version 3).
+    """BERT encoder + pooler (``bert.BertConfig``; default BERT-base at S = 128; S = 64, 128, 256, 384 or 512) -> fp16
+    plan (version 3).
 
     ``weights``: a dict or ``.npz`` path in Hugging Face ``BertModel`` names (``bert.load_weights``); default: seeded
     ``bert.random_weights(cfg, seed)``.  Activations are ``T_ACT`` tensors [N, 1, S, C], so every GEMM is a 1x1
@@ -385,9 +386,8 @@ def build_bert_plan(cfg=None, weights=None, max_batch: int = 16, seed: int = 0, 
     if precision != PREC_FP16:
         raise ValueError("precision must be PREC_FP16")
     S, H, F = cfg.seq, cfg.hidden, cfg.ffn
-    if S % 64 or not 0 < S <= 128:
-        raise ValueError(f"sequence length {S}: a plan is built for S a multiple of 64 and at most 128 "
-                         "(longer sequences need an online softmax)")
+    if S not in (64, 128, 256, 384, 512):
+        raise ValueError(f"sequence length {S}: a plan is built for S a multiple of 64 up to 128, or a multiple of 128 up to 512")
     if cfg.heads * 64 != H:
         raise ValueError(f"heads * 64 must equal the hidden size ({cfg.heads} * 64 != {H})")
     if F % 64 or H > 1024 or S > cfg.positions:

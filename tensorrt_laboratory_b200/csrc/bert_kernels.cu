@@ -6,6 +6,8 @@
 //  * attention_f16_wgmma  -- one CTA (one warpgroup) per (sequence, head, 64 query rows): Q, K, V by TMA, S = Q K^T with
 //                            wgmma into registers, scale + mask + softmax in registers, P fed to P V as the register A
 //                            operand of wgmma, O written at channel 64 * head
+//  * attention_f16_wgmma_ks -- S = 256, 384, 512: the same per 128-key block, S / 128 warpgroups splitting the keys; row
+//                            maxima, row sums and partial O's combined across warpgroups through shared memory
 //  * pooler_kernel        -- tanh(W h[CLS] + b), fp32 out
 //
 // Numerics (DESIGN.md, "BERT numerics"): every sum below runs in a fixed order -- a lane adds its own elements in index
@@ -302,6 +304,172 @@ attention_f16_wgmma(const __grid_constant__ CUtensorMap mapQKV, const float* __r
     }
 }
 
+// S in {256, 384, 512}: the S = 128 computation run by S / 128 warpgroups that split the keys; warpgroup w owns keys
+// 128w ... 128w + 127.  Q, K, V and V^T as in AttnSmem; once V^T is built the untransposed V is dead, and the partial O's
+// of warpgroups 1 ... WG - 1 (16 KiB each) are written over it.
+template <int S>
+struct AttnKsSmem {
+    static constexpr int WG = S / 128;
+    static constexpr int Q = 0;
+    static constexpr int K = 64 * 128;
+    static constexpr int V = K + S * 128;
+    static constexpr int VT = V + S * 128;
+    static constexpr int MASK = VT + S * 128;     // the sequence's S additive mask values (fp32)
+    static constexpr int RMAX = MASK + S * 4;     // [WG][64 rows] row maximum over each warpgroup's keys
+    static constexpr int RSUM = RMAX + WG * 256;  // [WG][64 rows] row sum over each warpgroup's keys
+    static constexpr int BAR = RSUM + WG * 256;
+    static constexpr int BYTES = BAR + 64 + 1024;
+    static_assert((WG - 1) * 32 * 128 * 4 <= S * 128, "partial O's fit over V");
+};
+
+// Same arithmetic as attention_f16_wgmma<128> per 128-key block; across blocks the row maximum is the maximum of the
+// blocks' maxima, the row sum and O add the blocks' partial sums and partial P V in warpgroup order (w = 0, 1, ...), in
+// fp32, and O is rounded to fp16 once.  The order depends on S alone.
+template <int S>
+__global__ void __launch_bounds__(S, 1)
+attention_f16_wgmma_ks(const __grid_constant__ CUtensorMap mapQKV, const float* __restrict__ mask_add, __half* __restrict__ out, int heads,
+                       int H, int out_pitch) {
+    static_assert(S == 256 || S == 384 || S == 512, "sequence lengths 256, 384 and 512");
+    using L = AttnKsSmem<S>;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+    uint64_t* bar = reinterpret_cast<uint64_t*>(smem + L::BAR);
+    float* mask_s = reinterpret_cast<float*>(smem + L::MASK);
+    float* rmax = reinterpret_cast<float*>(smem + L::RMAX);
+    float* rsum = reinterpret_cast<float*>(smem + L::RSUM);
+    const int n = blockIdx.x / heads, head = blockIdx.x - n * heads;
+    const int q0 = blockIdx.y * 64;
+    const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;  // S threads: one per key
+    if (tid == 0) {
+        tma_prefetch_desc(&mapQKV);
+        mbar_init(bar, 1);
+        fence_barrier_init();
+    }
+    __syncthreads();
+    pdl_launch_dependents();
+    pdl_wait();  // Q, K, V and the mask are the previous kernels' output
+    if (tid == 0) {
+        mbar_expect_tx(bar, static_cast<uint32_t>((64 + 2 * S) * 128));
+        const int row0 = n * S;
+        tma_load_2d(&mapQKV, bar, smem + L::Q, head * 64, row0 + q0);
+#pragma unroll
+        for (int b = 0; b < S / 64; ++b) {
+            tma_load_2d(&mapQKV, bar, smem + L::K + b * 8192, H + head * 64, row0 + 64 * b);
+            tma_load_2d(&mapQKV, bar, smem + L::V + b * 8192, 2 * H + head * 64, row0 + 64 * b);
+        }
+    }
+    mask_s[tid] = __ldg(mask_add + static_cast<size_t>(n) * S + tid);
+    mbar_wait(bar, 0);
+    for (int e = tid; e < S * 32; e += S) {
+        const int d = e & 63, key = (e >> 6) * 2;
+        const __half v0 = *reinterpret_cast<const __half*>(smem + L::V + sw128(key, d));
+        const __half v1 = *reinterpret_cast<const __half*>(smem + L::V + sw128(key + 1, d));
+        *reinterpret_cast<__half2*>(smem + L::VT + (key >> 6) * 8192 + sw128(d, key & 63)) = __halves2half2(v0, v1);
+    }
+    fence_proxy_async();
+    __syncthreads();
+
+    // this warpgroup's block of scores: 64 x 128, K = 64
+    float sacc[64];
+    const uint32_t q_addr = smem_u32(smem + L::Q), k_addr = smem_u32(smem + L::K + wg * 128 * 128);
+    wgmma_group<4>([&](int j) {
+        wgmma_f16<128>(sacc, make_wgmma_desc(q_addr + j * 32, 16, 1024, WG_SW128), make_wgmma_desc(k_addr + j * 32, 16, 1024, WG_SW128),
+                       j > 0 ? 1u : 0u);
+    });
+    wgmma_wait<0>();
+
+    const int r0 = 16 * warp + (lane >> 2);  // this thread's rows r0 and r0 + 8; key columns 128 wg + 8j + 2(l%4) + e
+    const float* mk = mask_s + 128 * wg + 2 * (lane & 3);
+    float mx[2] = {-3.0e38f, -3.0e38f};
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+        const float2 m2 = *reinterpret_cast<const float2*>(mk + 8 * j);
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                float& v = sacc[4 * j + 2 * h + e];
+                v = __fadd_rn(__fmul_rn(v, 0.125f), e ? m2.y : m2.x);
+                mx[h] = fmaxf(mx[h], v);
+            }
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+        mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+        if ((lane & 3) == 0) rmax[wg * 64 + r0 + 8 * h] = mx[h];
+    }
+    __syncthreads();
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        mx[h] = rmax[r0 + 8 * h];
+#pragma unroll
+        for (int w = 1; w < L::WG; ++w) mx[h] = fmaxf(mx[h], rmax[w * 64 + r0 + 8 * h]);
+    }
+    float sum[2] = {0.f, 0.f};
+#pragma unroll
+    for (int j = 0; j < 16; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                float& v = sacc[4 * j + 2 * h + e];
+                v = expf(__fsub_rn(v, mx[h]));
+                sum[h] = __fadd_rn(sum[h], v);
+            }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        sum[h] = __fadd_rn(sum[h], __shfl_xor_sync(0xffffffffu, sum[h], 1));
+        sum[h] = __fadd_rn(sum[h], __shfl_xor_sync(0xffffffffu, sum[h], 2));
+        if ((lane & 3) == 0) rsum[wg * 64 + r0 + 8 * h] = sum[h];
+    }
+    __syncthreads();
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        sum[h] = rsum[r0 + 8 * h];
+#pragma unroll
+        for (int w = 1; w < L::WG; ++w) sum[h] = __fadd_rn(sum[h], rsum[w * 64 + r0 + 8 * h]);
+    }
+    uint32_t pa[8][4];
+#pragma unroll
+    for (int t = 0; t < 8; ++t)
+#pragma unroll
+        for (int half = 0; half < 2; ++half) {
+            const int j = 2 * t + half;
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+                pa[t][2 * half + h] = pack_h2(__fdiv_rn(sacc[4 * j + 2 * h], sum[h]), __fdiv_rn(sacc[4 * j + 2 * h + 1], sum[h]));
+        }
+
+    // partial O = P V over this warpgroup's keys: V^T blocks 2 wg and 2 wg + 1
+    float oacc[32];
+    const uint32_t vt_addr = smem_u32(smem + L::VT + wg * 2 * 8192);
+    wgmma_group<8>([&](int t) {
+        wgmma_f16_rs_n64(oacc, pa[t], make_wgmma_desc(vt_addr + (t >> 2) * 8192 + (t & 3) * 32, 16, 1024, WG_SW128), t > 0 ? 1u : 0u);
+    });
+    wgmma_wait<0>();
+
+    // warpgroups 1 ... WG - 1 hand their partial O to warpgroup 0 through the dead V region, [slot][register][thread]
+    float* part = reinterpret_cast<float*>(smem + L::V);
+    const int wt = tid & 127;
+    if (wg > 0)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) part[((wg - 1) * 32 + i) * 128 + wt] = oacc[i];
+    __syncthreads();
+    if (wg > 0) return;
+#pragma unroll
+    for (int w = 1; w < L::WG; ++w)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) oacc[i] = __fadd_rn(oacc[i], part[((w - 1) * 32 + i) * 128 + wt]);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        __half* orow = out + static_cast<size_t>(n * S + q0 + r0 + 8 * h) * out_pitch + head * 64 + 2 * (lane & 3);
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+            *reinterpret_cast<__half2*>(orow + 8 * j) = __floats2half2_rn(oacc[4 * j + 2 * h], oacc[4 * j + 2 * h + 1]);
+    }
+}
+
 // pooled[n][j] = tanh(b[j] + W[j] . h[n][0]): one warp per output channel j, its weight row held in registers (loaded
 // before the dependency wait: weights are constants)
 __global__ void __launch_bounds__(256) pooler_kernel(const __half* __restrict__ h, const __half* __restrict__ w, const float* __restrict__ b,
@@ -365,6 +533,12 @@ int init_attention_kernels() {
     cudaError_t e = cudaFuncSetAttribute(attention_f16_wgmma<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnSmem<64>::BYTES);
     if (e == cudaSuccess)
         e = cudaFuncSetAttribute(attention_f16_wgmma<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnSmem<128>::BYTES);
+    if (e == cudaSuccess)
+        e = cudaFuncSetAttribute(attention_f16_wgmma_ks<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnKsSmem<256>::BYTES);
+    if (e == cudaSuccess)
+        e = cudaFuncSetAttribute(attention_f16_wgmma_ks<384>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnKsSmem<384>::BYTES);
+    if (e == cudaSuccess)
+        e = cudaFuncSetAttribute(attention_f16_wgmma_ks<512>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnKsSmem<512>::BYTES);
     return static_cast<int>(e);
 }
 
@@ -376,6 +550,15 @@ int launch_attention(const AttnLaunch& L, cudaStream_t stream) {
     if (L.S == 128)
         return launch_pdl(attention_f16_wgmma<128>, grid, dim3(128), AttnSmem<128>::BYTES, stream, L.mapQKV, L.mask_add, L.out, L.heads, L.H,
                           L.out_pitch);
+    if (L.S == 256)
+        return launch_pdl(attention_f16_wgmma_ks<256>, grid, dim3(256), AttnKsSmem<256>::BYTES, stream, L.mapQKV, L.mask_add, L.out, L.heads,
+                          L.H, L.out_pitch);
+    if (L.S == 384)
+        return launch_pdl(attention_f16_wgmma_ks<384>, grid, dim3(384), AttnKsSmem<384>::BYTES, stream, L.mapQKV, L.mask_add, L.out, L.heads,
+                          L.H, L.out_pitch);
+    if (L.S == 512)
+        return launch_pdl(attention_f16_wgmma_ks<512>, grid, dim3(512), AttnKsSmem<512>::BYTES, stream, L.mapQKV, L.mask_add, L.out, L.heads,
+                          L.H, L.out_pitch);
     return static_cast<int>(cudaErrorInvalidValue);
 }
 

@@ -372,7 +372,8 @@ int validate_transformer_op(b2_engine* e, const Op& op) {
                 return fail(B2_EINVAL, "plan: attention %s: needs a fused fp16 QKV input of 3 x %u channels", nm, to.c);
             if (ti.h != 1 || to.h != 1 || ti.w != to.w || tm.kind != T_VEC || tm.c != ti.w)
                 return fail(B2_EINVAL, "plan: attention %s: S does not match between QKV, output and mask", nm);
-            if (ti.w % 64 || ti.w > 128) return fail(B2_EINVAL, "plan: attention %s: S = %u (a multiple of 64, at most 128)", nm, ti.w);
+            if (ti.w != 64 && (ti.w == 0 || ti.w % 128 || ti.w > 512))
+                return fail(B2_EINVAL, "plan: attention %s: S = %u (64, or a multiple of 128 up to 512)", nm, ti.w);
             if (r.w_bytes || r.b_bytes) return fail(B2_EINVAL, "plan: attention %s carries no weights", nm);
             e->flops_per_item += 4.0 * double(ti.w) * ti.w * to.c;  // Q K^T and P V
             break;
@@ -2707,7 +2708,7 @@ const char* b2_context_launch_name(b2_context* c, int batch, int i) {
     static const char* kinds[] = {"input_cast", "conv_tcgen05", "conv_simt", "maxpool", "avgpool", "fc", "softmax", "output_cast", "net_tcgen05", "tail_pool_fc_softmax",
                                   "quantize", "conv_i8_tcgen05", "avgpool_i8", "output_cast_i8", "embed_ln", "layernorm", "attention_f16_wgmma",
                                   "pooler", "output_cast_rows"};
-    s = std::string(kinds[L->kind]) + ":" + L->name;
+    s = std::string(kinds[L->kind]) + (L->kind == L_ATTENTION && L->attn.S > 128 ? "_ks" : "") + ":" + L->name;  // key-split kernel
     if (L->kind == L_CONV_TC)
         s += " bn=" + std::to_string(L->conv.bn) + " kb=" + std::to_string(L->conv.kb) +
              " st=" + std::to_string(L->conv.stages) + "x" + std::to_string(L->conv.sps) +

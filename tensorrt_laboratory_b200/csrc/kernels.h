@@ -244,7 +244,8 @@ int launch_embed_ln(const EmbedArgs& a, cudaStream_t stream);
 // y = (x - mean) / sqrt(var + eps) * gamma + beta over the C channels of each row; fp32 statistics
 int launch_layernorm(const __half* in, __half* out, const float* gamma, const float* beta, long long rows, int C, int C_phys,
                      float eps, cudaStream_t stream);
-// one CTA per (sequence, head, 64 query rows): S = QK^T * 0.125 + mask, softmax, O = P V (wgmma); S in {64, 128}
+// one CTA per (sequence, head, 64 query rows): S = QK^T * 0.125 + mask, softmax, O = P V (wgmma); S in {64, 128} on one
+// warpgroup, S in {256, 384, 512} on S / 128 warpgroups that split the keys (attention_f16_wgmma_ks)
 struct AttnLaunch {
     CUtensorMap mapQKV;    // 2-D tiled [N*S rows, 3H channels], box 64 x 64, 128B swizzle
     const float* mask_add; // [N][S]

@@ -105,7 +105,8 @@ struct OpRecV2 {  // 192 bytes
 //     beta H].  Ids are clamped into [0, vocab) and segment ids into [0, types), so no table is read out of bounds.
 //   OP_LAYERNORM: in / out fp16 of the same shape; b = fp32 [gamma C | beta C]; eps.
 //   OP_ATTENTION: in = QKV [N, 1, S, 3H] with channel (part * H + head * 64 + d), part 0 = Q, 1 = K, 2 = V; res = the fp32
-//     mask [N, S]; out = [N, 1, S, H], head h at channels 64h ...; heads * 64 == H, S a multiple of 64 and at most 128.
+//     mask [N, S]; out = [N, 1, S, H], head h at channels 64h ...; heads * 64 == H, S = 64 or a multiple of 128 up to
+//     512 (S > 128 runs the key-split kernel).
 //   OP_POOLER: in = fp16 [N, 1, S, H]; out = fp32 vector [N, H]; w = fp16 [H][H] (row = output); b = fp32 [H].
 //   OP_OUTPUT_CAST: flags bit 0 = channels-last binding [H * W, C] instead of NCHW.
 struct OpRecV3 {  // 224 bytes

@@ -1,10 +1,11 @@
 #!/usr/bin/env python
-"""BERT-base fp16, batch 16, S = 128 (seeded weights, random tokens with ragged padding): device-resident sequences/s of
-4 concurrent contexts with tactics tuned at load, end-to-end requests through the C++ InferenceManager (p50 / p99), and
-the whole-program FLOP rate from the algorithmic FLOPs of the shapes, as one JSON line.  The SM clock and the power limit
-are read in the same run.
+"""BERT-base fp16, batch 16, S = 128 by default (seeded weights, random tokens with ragged padding): device-resident
+sequences/s of 4 concurrent contexts with tactics tuned at load, end-to-end requests through the C++ InferenceManager
+(p50 / p99), the whole-program FLOP rate from the algorithmic FLOPs of the shapes, and the attention launches' share of
+one serialised forward pass (per-launch CUDA events), as one JSON line.  The SM clock and the power limit are read in the
+same run.
 
-  python tools/bench_bert.py --steps 500 --warmup 20 [--dump-outputs DIR]
+  python tools/bench_bert.py --steps 500 --warmup 20 [--seq 128] [--batch 16] [--dump-outputs DIR]
 """
 import argparse
 import json
@@ -20,7 +21,7 @@ sys.path.insert(0, ROOT)
 from bench import ClockSampler  # noqa: E402
 from tensorrt_laboratory_b200 import bert, builder, capi  # noqa: E402
 
-BATCH, CONTEXTS = 16, 4
+CONTEXTS = 4
 
 
 def algorithmic_flops_per_sequence(cfg: bert.BertConfig) -> dict:
@@ -42,6 +43,8 @@ def inputs(cfg: bert.BertConfig, n: int, seed: int = 1) -> dict:
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--seq", type=int, default=128, help="sequence length S (64, 128, 256, 384 or 512)")
+    ap.add_argument("--batch", type=int, default=16, help="sequences per step and per request")
     ap.add_argument("--steps", type=int, default=500)
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--requests", type=int, default=200, help="end-to-end InferenceManager requests")
@@ -52,38 +55,43 @@ def main():
         raise SystemExit("bench_bert.py: no CUDA device visible and there is no CPU fallback")
     lib = capi.load()
     capi.check(lib.b2_device_set(a.device))
-    cfg = bert.BERT_BASE
-    blob = builder.build_bert_plan(cfg, max_batch=BATCH, seed=0)
+    cfg = bert.BertConfig(seq=a.seq)
+    batch = a.batch
+    blob = builder.build_bert_plan(cfg, max_batch=batch, seed=0)
     eng = capi.Engine(blob)
     eng.tune(CONTEXTS)  # tactics timed in the regime of the run, ahead of the timed window
     tuned = builder.attach_tactics(blob, eng.tactics())
-    x = inputs(cfg, BATCH)
+    x = inputs(cfg, batch)
     sessions = [capi.Session(eng) for _ in range(CONTEXTS)]
     for s in sessions:
         for i, b in enumerate(eng.bindings):
             if b["is_input"]:
-                s.host_array(i, BATCH)[...] = x[b["name"]]
-        s.h2d(BATCH)
-        s.prepare(BATCH)
+                s.host_array(i, batch)[...] = x[b["name"]]
+        s.h2d(batch)
+        s.prepare(batch)
     sampler = ClockSampler(a.device)
     for i in range(max(a.warmup, CONTEXTS)):
-        sessions[i % CONTEXTS].enqueue(BATCH)
+        sessions[i % CONTEXTS].enqueue(batch)
     capi.check(lib.b2_device_sync())
     sampler.start()
     t0 = time.perf_counter()
     for i in range(a.steps):
-        sessions[i % CONTEXTS].enqueue(BATCH)
+        sessions[i % CONTEXTS].enqueue(batch)
     capi.check(lib.b2_device_sync())
     dt = time.perf_counter() - t0
     clocks = sampler.stop()
     if a.dump_outputs:
         last = sessions[(a.steps - 1) % CONTEXTS]
-        last.d2h(BATCH)
+        last.d2h(batch)
         last.stream.sync()
         os.makedirs(a.dump_outputs, exist_ok=True)
         for i, b in enumerate(eng.bindings):
             if not b["is_input"]:
-                np.save(os.path.join(a.dump_outputs, f"bert_{b['name']}.npy"), last.host_array(i, BATCH).copy())
+                np.save(os.path.join(a.dump_outputs, f"bert_{b['name']}.npy"), last.host_array(i, batch).copy())
+    for _ in range(3):  # the last of three serialised passes
+        prof = sessions[0].profile(batch)
+    attn = [p for p in prof if p["name"].startswith("attention_f16_wgmma")]
+    attn_ms, pass_ms = sum(p["ms"] for p in attn), sum(p["ms"] for p in prof)
     for s in sessions:
         s.close()
     eng.destroy()
@@ -107,15 +115,19 @@ def main():
     except Exception:
         power_limit = None
     fl = algorithmic_flops_per_sequence(cfg)
-    seq_s = a.steps * BATCH / dt
+    seq_s = a.steps * batch / dt
     print(json.dumps({
-        "metric": "BERT-base fp16 b=16 S=128 sequences/sec", "value": seq_s, "unit": "sequences/s",
-        "workload": f"BERT-base (12 layers, hidden 768) fp16, batch={BATCH}, S={cfg.seq}, {CONTEXTS} concurrent contexts, "
+        "metric": f"BERT-base fp16 b={batch} S={cfg.seq} sequences/sec", "value": seq_s, "unit": "sequences/s",
+        "workload": f"BERT-base (12 layers, hidden 768) fp16, batch={batch}, S={cfg.seq}, {CONTEXTS} concurrent contexts, "
                     "tuned tactics, token bindings resident in HBM",
         "ms_per_step": dt * 1e3 / a.steps, "steps": a.steps,
         "algorithmic_gflop_per_sequence": {k: v / 1e9 for k, v in fl.items()},
         "whole_program_tflops": fl["total"] * seq_s / 1e12,
-        "e2e_inference_manager": {"requests": a.requests, "batch": BATCH, "sequences_per_s": a.requests * BATCH / e2e,
+        "attention_profile": {"kernel": attn[0]["name"].split(":")[0], "launches": len(attn), "ms": attn_ms,
+                              "share_of_forward_pass": attn_ms / pass_ms, "forward_pass_ms": pass_ms,
+                              "tflops": sum(p["flops"] for p in attn) / (attn_ms * 1e-3) / 1e12,
+                              "note": "one serialised forward pass, per-launch CUDA events"},
+        "e2e_inference_manager": {"requests": a.requests, "batch": batch, "sequences_per_s": a.requests * batch / e2e,
                                   "p50_ms": float(np.percentile(lat, 50) * 1e3), "p99_ms": float(np.percentile(lat, 99) * 1e3),
                                   "note": "one request in flight at a time"},
         "device": capi.device_info(a.device), "power_limit": power_limit, "clocks": clocks,

@@ -26,7 +26,7 @@ from tensorrt_laboratory_b200 import builder, graph, weights  # noqa: E402
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--model", choices=["resnet50", "resnet152", "resnext50", "mnist", "bert-base"])
-    ap.add_argument("--seq", type=int, default=128, help="bert-base: the sequence length of the plan (64 or 128)")
+    ap.add_argument("--seq", type=int, default=128, help="bert-base: the sequence length of the plan (64, 128, 256, 384 or 512)")
     ap.add_argument("--weights", help="bert-base: .npz of Hugging Face BertModel parameters (default: seeded weights)")
     ap.add_argument("--prototxt")
     ap.add_argument("--onnx", help="ONNX CNN classifier (Conv / BatchNormalization / Relu / Add / MaxPool / AveragePool / "
