@@ -228,7 +228,8 @@ struct ConvConfig {
     int sps = 1;  // 64-wide K sub-blocks per pipeline stage
     int ws = 0;   // > 0: persistent warp-specialised kernel with this many CTAs
     int cn = 1;   // CTAs per cluster along N sharing the activation tile by TMA multicast (1 = no cluster)
-    int halo = 0; // 1: 3x3 halo kernel (input block resident in smem, taps = shifted views)
+    int halo = 0; // 1: 3x3 halo kernel (input block resident in smem, taps = shifted views); 2: the halo kernel with the
+                  // next op (fuse_partner) run on its output in the same launch -- that op then has no launch of its own
 };
 // A pipeline deeper than the K loop is pure shared-memory cost: admit depths up to the smallest instantiated one
 // that covers the loop (or the deepest available when none does).
@@ -300,6 +301,7 @@ struct b2_context {
     int force_splits = 0;
     int force_sps = 0;
     int force_halo = 0; // 1: the 3x3 halo kernel wherever it applies, -1: never
+    int force_fuse = 0; // 1: every 3x3 -> 1x1 pair fuse_partner admits runs as one launch, -1: never (tables included)
     int force_cn = 0;   // > 0: this cluster size wherever it divides the N-tile count, -1: never cluster
     int force_ws = 0;   // 1: only the persistent warp-specialised tactic where it applies, -1: never
     int pdl_trigger = 1;
@@ -642,6 +644,8 @@ int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** pa
     return B2_OK;
 }
 
+int fuse_partner(const b2_engine* e, int i);
+
 // ---- activation arena: first-fit over live intervals ------------------------------------------
 void plan_arena(b2_engine* e) {
     // side branches: a conv whose output is consumed exactly once, as the residual of a later op, with at least one
@@ -671,6 +675,9 @@ void plan_arena(b2_engine* e) {
             if (t >= 0) e->tensors[t].last_use = std::max(e->tensors[t].last_use, int(i));
         // a side op may still be READING its input while the ops before the join run: keep that buffer until the join
         if (e->ops[i].side_join >= 0 && r.in >= 0) e->tensors[r.in].last_use = std::max(e->tensors[r.in].last_use, e->ops[i].side_join);
+        // a 3x3 that may run fused with the next op reads its input while that op's output is written
+        const int j = fuse_partner(e, int(i));
+        if (j >= 0) e->tensors[r.in].last_use = std::max(e->tensors[r.in].last_use, j);
     }
     struct Live {
         size_t off, size;
@@ -834,16 +841,41 @@ int conv_num_kblocks(const b2_context* c, const Op& op) {
 // 3x3 / stride 1 / pad 1 on 64-channel blocks with packed weights and no fused residual: the halo kernel applies.
 // Returns the rows per tile R (0 = not applicable).  Never for a grouped convolution (its tiles read channel blocks
 // that depend on the N tile).
-int conv_halo_rows(const b2_context* c, const Op& op) {
+int conv_halo_rows(const b2_engine* e, const Op& op) {
     const b2plan::OpRec& r = op.r;
-    const Tensor& ti = c->e->tensors[r.in];
-    const Tensor& to = c->e->tensors[r.out];
+    const Tensor& ti = e->tensors[r.in];
+    const Tensor& to = e->tensors[r.out];
     if (op.groups > 1 || r.cin_phys % 64 || r.cout_phys % 64 || op.kh() != 3 || op.kw() != 3 || op.sh() != 1 || op.sw() != 1 || op.ph() != 1 ||
         op.pw_lo() != 1 || op.pw_hi() != 1 || r.res >= 0 || !(r.relu & 2) || ti.h != to.h || ti.w != to.w)
         return 0;
     const int wp = int(to.w) + 2;
     if (wp > 128) return 0;
     return std::min(128 / wp, int(to.h));
+}
+int conv_halo_rows(const b2_context* c, const Op& op) { return conv_halo_rows(c->e, op); }
+bool conv_on_tensor_cores(const b2_engine* e, const Op& op);
+
+// The 1x1 convolution that the 3x3 op `i` can run inside its own launch (conv3x3_halo_1x1_tcgen05), or -1.  Op i takes
+// the halo kernel over all of its output channels (64, 128 or 256); op j = i + 1 is a 1x1 / stride-1 packed-weight
+// convolution with a residual, no GELU and no groups, whose input is i's output; that tensor is read by nothing else and
+// is not a binding.  Shapes only: whether the fused launch runs is a tactic (ConvConfig::halo == 2 on op i).
+int fuse_partner(const b2_engine* e, int i) {
+    if (!e->half() || e->int8() || i < 0 || size_t(i) + 1 >= e->ops.size()) return -1;
+    const Op &oi = e->ops[size_t(i)], &oj = e->ops[size_t(i) + 1];
+    const b2plan::OpRec &ri = oi.r, &rj = oj.r;
+    if (ri.type != b2plan::OP_CONV || rj.type != b2plan::OP_CONV || (ri.relu & (4 | b2plan::kConvGelu)) || conv_halo_rows(e, oi) == 0 ||
+        !b2k::conv_halo_config_exists(int(ri.cout_phys)) || ri.cin_phys / 64 > 8)
+        return -1;
+    if (rj.in != ri.out || rj.res < 0 || rj.res == ri.out || oj.kh() != 1 || oj.kw() != 1 || oj.sh() != 1 || oj.sw() != 1 || oj.ph() != 0 ||
+        oj.pw_lo() != 0 || oj.pw_hi() != 0 || oj.groups != 1 || !(rj.relu & 2) || (rj.relu & (4 | b2plan::kConvGelu)) ||
+        rj.cin_phys != ri.cout_phys || rj.cout_phys % 64 || !conv_on_tensor_cores(e, oj) || e->tensors[ri.out].binding >= 0)
+        return -1;
+    for (size_t k = 0; k < e->ops.size(); ++k) {
+        const b2plan::OpRec& rk = e->ops[k].r;
+        if (k != size_t(i) + 1 && (rk.in == ri.out || rk.res == ri.out || e->ops[k].out2 == ri.out)) return -1;
+        if (k == size_t(i) + 1 && rk.res == ri.out) return -1;
+    }
+    return i + 1;
 }
 
 // Does `op` run on the wgmma convolution kernels?  fp16 engines, 64-channel K blocks or the 8-channel stem / thin-input
@@ -878,9 +910,15 @@ bool tactic_applies(const b2_context* c, const Op& op, int batch, const ConvConf
     // grouped: one tile per CTA and N tiles inside one span of input channels; GELU: only the one-tile kernel has it
     if (op.groups > 1 && (!span || span % cfg.bn || cfg.splits > 1)) return false;
     if ((op.groups > 1 || (r.relu & b2plan::kConvGelu)) && (cfg.ws || cfg.cn > 1 || cfg.halo)) return false;
+    if (cfg.halo == 2) {  // one CTA owns all of the 3x3's output channels, i.e. the whole K of the 1x1
+        const int j = fuse_partner(c->e, int(&op - &c->e->ops[0]));
+        const int R = conv_halo_rows(c, op), cblocks = int(r.cin_phys) / 64;
+        return j >= 0 && c->force_fuse >= 0 && cfg.bn == int(r.cout_phys) && cfg.splits == 1 && !cfg.ws && cfg.cn <= 1 &&
+               b2k::conv_halo_fused_smem(cfg.bn, int(to.w), R, cblocks, int(c->e->ops[size_t(j)].r.cout_phys)) <= kSmemLimit;
+    }
     if (cfg.halo) {
         const int R = conv_halo_rows(c, op), cblocks = int(r.cin_phys) / 64;
-        return R && cfg.splits == 1 && !cfg.ws && cfg.cn <= 1 && b2k::conv_halo_config_exists(cfg.bn) && cblocks <= 8 &&
+        return cfg.halo == 1 && R && cfg.splits == 1 && !cfg.ws && cfg.cn <= 1 && b2k::conv_halo_config_exists(cfg.bn) && cblocks <= 8 &&
                b2k::conv_halo_smem(cfg.bn, int(to.w), R, cblocks) <= kSmemLimit;
     }
     if (cfg.ws && conv_is_row_folded(c, op))  // one encoding: N tile 64, the ring depth as the stage count
@@ -901,6 +939,16 @@ bool tactic_applies(const b2_context* c, const Op& op, int batch, const ConvConf
             return false;
     }
     return true;
+}
+
+// Fewest concurrent streams of a tuning regime (b2_engine_tune / refine) in which the fused tactic is timed at all
+constexpr int kFuseMinStreams = 4;
+
+// The fused 3x3 -> 1x1 tactic of op `op` (tactic_applies decides whether it may run)
+ConvConfig fused_conv_config(const Op& op) {
+    ConvConfig f{int(op.r.cout_phys), kHaloStagesTag, 1, 0.0, 1, 0, 1};
+    f.halo = 2;
+    return f;
 }
 
 // The tactics the per-layer tuner times, in timing order: every tile, persistent and halo tactic the rule admits, less
@@ -1056,8 +1104,21 @@ int make_conv_launch(b2_context* c, const Op& op, int batch, const ConvConfig& c
         cl.grid_m = batch * ((int(to.h) + R - 1) / R);
         int rc = make_map_nhwc(&cl.mapA, tptr(r.in), int(r.cin_phys), int(ti.w), int(ti.h), batch, uint32_t(ti.w) + 2, uint32_t(R) + 2);
         if (rc) return rc;
+        cl.mapB = cl.mapA;
+        if (cfg.halo == 2) {  // the 1x1's output and residual through the halo store's box geometry
+            const Op& oj = e->ops[size_t(fuse_partner(e, int(&op - &e->ops[0])))];
+            const b2plan::OpRec& rj = oj.r;
+            cl.halo = 2;
+            cl.c2.wpacked = e->d_payload + rj.w_off;
+            cl.c2.bias = reinterpret_cast<const float*>(e->d_payload + rj.b_off);
+            cl.c2.Cout = int(rj.cout_phys);
+            cl.c2.relu = int(rj.relu & b2plan::kConvRelu);
+            rc = make_map_nhwc(&cl.mapOut, tptr(rj.out), int(rj.cout_phys), int(to.w), int(to.h), batch, uint32_t(to.w) + 2, uint32_t(R));
+            if (!rc) rc = make_map_nhwc(&cl.mapRes, tptr(rj.res), int(rj.cout_phys), int(to.w), int(to.h), batch, uint32_t(to.w) + 2, uint32_t(R));
+            return rc;
+        }
         rc = make_map_nhwc(&cl.mapOut, tptr(r.out), int(r.cout_phys), int(to.w), int(to.h), batch, uint32_t(to.w) + 2, uint32_t(R));
-        cl.mapB = cl.mapA, cl.mapRes = cl.mapOut;
+        cl.mapRes = cl.mapOut;
         return rc;
     }
     const CUtensorMapSwizzle swz = kb64 ? CU_TENSOR_MAP_SWIZZLE_128B : (fold ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_NONE);
@@ -1263,7 +1324,7 @@ int autotune_conv(b2_context* c, const Op& op, int batch, int fixed_splits, Conv
 }
 
 // ---- tactic cache file (B2_TUNE_CACHE=<path>): the analogue of a TensorRT timing cache.  One line per tuned conv:
-//      <engine name> <op index> <batch> <bn> <stages> <splits> <sps> <persistent CTAs or 0> <cluster size> <halo 0/1>
+//      <engine name> <op index> <batch> <bn> <stages> <splits> <sps> <persistent CTAs or 0> <cluster size> <halo 0/1/2>
 void tune_cache_load(b2_engine* e) {
     if (e->tune_cache_loaded) return;
     e->tune_cache_loaded = true;
@@ -1378,6 +1439,42 @@ int tune_engine_batch(b2_context* c, int batch) {
         std::lock_guard<std::mutex> lock(e->tune_mutex);
         e->tuned[{int(i), batch}] = cfg;
         tune_cache_append(e, int(i), batch, cfg);
+    }
+    // A 3x3 and the 1x1 after it as one launch: timed in the same regime, kept only where it beats the two best
+    // unfused launches together (bit-identical either way).  Pairs whose times this tuning did not measure stay as they are.
+    // A throughput tactic: the fused CTA trades parallelism (one CTA owns the 3x3's channels and all of the 1x1's) for
+    // bytes and a launch, so it is only considered when the tuning regime is kFuseMinStreams or more concurrent streams;
+    // fewer keep the two launches.
+    for (size_t i = 0; i < e->ops.size() && c->force_fuse >= 0 && c->autotune >= kFuseMinStreams; ++i) {
+        const Op& op = e->ops[i];
+        const int j = fuse_partner(e, int(i));
+        if (j < 0) continue;
+        double unfused_us = 0;
+        {
+            std::lock_guard<std::mutex> lock(e->tune_mutex);
+            const auto a = e->tuned.find({int(i), batch}), b = e->tuned.find({j, batch});
+            if (a == e->tuned.end() || b == e->tuned.end() || a->second.halo == 2 || !(a->second.est_us > 0) || !(b->second.est_us > 0)) continue;
+            unfused_us = a->second.est_us + b->second.est_us;
+        }
+        ConvConfig f = fused_conv_config(op);
+        if (!tactic_applies(c, op, batch, f)) continue;
+        b2k::ConvLaunch cl;
+        int rc = make_conv_launch(c, op, batch, f, &cl);
+        if (rc) return rc;
+        TuneTimer tt(c);
+        if ((rc = tt.init())) return rc;
+        float ms = 0.f;
+        const cudaError_t err = tt.time([&](int, cudaStream_t s) { return b2k::launch_conv_f16_tcgen05(cl, s); }, &ms);
+        if (err != cudaSuccess) return fail(B2_ECUDA, "autotune of %s fused with %s failed: %s", op.name.c_str(), e->ops[size_t(j)].name.c_str(), cudaGetErrorString(err));
+        f.est_us = tt.us_per_launch(ms);
+        if (env_int("B2_TUNE_VERBOSE", 0))
+            fprintf(stderr, "[b2 tune] %s+%s b=%d fused : %.3f us/launch against %.3f unfused (%d streams) -> %s\n", op.name.c_str(),
+                    e->ops[size_t(j)].name.c_str(), batch, f.est_us, unfused_us, tt.ns, f.est_us < unfused_us ? "fused" : "unfused");
+        if (f.est_us < unfused_us) {
+            std::lock_guard<std::mutex> lock(e->tune_mutex);
+            e->tuned[{int(i), batch}] = f;
+            tune_cache_append(e, int(i), batch, f);
+        }
     }
     return B2_OK;
 }
@@ -1526,6 +1623,35 @@ int fuse_net_runs(b2_context* c, Plan* plan, int batch) {
     ls = std::move(fused);
     plan->has_net = true;
     return B2_OK;
+}
+
+// Every 3x3 launch whose tactic is the fused one (halo == 2) absorbs the launch of the next op, the 1x1 its kernel runs
+// (launch index == op index on entry).  The fused launch does both ops' work less the tensor between them; a side branch
+// that joined at the 1x1 joins at the fused launch.
+void fuse_bottlenecks(b2_context* c, Plan* plan, int batch) {
+    std::vector<Launch>& ls = plan->launches;
+    if (std::none_of(ls.begin(), ls.end(), [](const Launch& L) { return L.kind == L_CONV_TC && L.conv.halo == 2; })) return;
+    std::vector<int> new_index(ls.size());
+    std::vector<Launch> out;
+    for (size_t k = 0; k < ls.size(); ++k) {
+        new_index[k] = int(out.size());
+        if (ls[k].kind == L_CONV_TC && ls[k].conv.halo == 2 && k + 1 < ls.size()) {
+            Launch& J = ls[k + 1];
+            Launch L = std::move(ls[k]);
+            const Tensor& mid = c->e->tensors[c->e->ops[k].r.out];
+            L.name += "+" + J.name;
+            L.flops += J.flops;
+            L.bytes += J.bytes - 2.0 * batch * double(mid.item_bytes);
+            new_index[k + 1] = new_index[k];
+            ++k;
+            out.push_back(std::move(L));
+            continue;
+        }
+        out.push_back(std::move(ls[k]));
+    }
+    for (Launch& L : out)
+        if (L.side_join >= 0) L.side_join = new_index[size_t(L.side_join)];
+    ls = std::move(out);
 }
 
 // global average pool -> FC -> softmax (the classifier tail) as one launch; the pooled tensor and the logits vector of
@@ -1681,6 +1807,10 @@ int build_plan(b2_context* c, int batch, Plan** out) {
                         if (it == e->tuned.end()) it = e->tuned.find({op_index, e->max_batch});
                         if (it != e->tuned.end() && tactic_applies(c, op, batch, it->second)) cfg = it->second;
                     }
+                    if (!net_ok && c->force_fuse > 0) {
+                        const ConvConfig f = fused_conv_config(op);
+                        if (tactic_applies(c, op, batch, f)) cfg = f;
+                    }
                     if (op.side_join >= 0 && cfg.splits > 1) cfg.splits = 1;  // forced / cached tactic on a side-branch op
                     int rc = make_conv_launch(c, op, batch, cfg, &L.conv);
                     if (rc) return rc;
@@ -1808,6 +1938,7 @@ int build_plan(b2_context* c, int batch, Plan** out) {
         }
         plan->launches.push_back(std::move(L));
     }
+    fuse_bottlenecks(c, plan.get(), batch);
     int rc = fuse_net_runs(c, plan.get(), batch);
     if (rc) return rc;
     fuse_tail(c, plan.get(), batch);
@@ -2238,6 +2369,7 @@ int b2_context_create(b2_engine* e, b2_context** out) {
     c->force_ws = env_int("B2_FORCE_WS", 0);
     c->force_cn = env_int("B2_FORCE_CN", 0);
     c->force_halo = env_int("B2_FORCE_HALO", 0);
+    c->force_fuse = env_int("B2_FORCE_FUSE", 0);
     c->pdl_trigger = env_int("B2_PDL_TRIGGER", 1);
     c->autotune = env_int("B2_AUTOTUNE", 4);
     c->fork = env_int("B2_FORK", 0);
@@ -2305,6 +2437,7 @@ int b2_context_set_option(b2_context* c, const char* key, int value) {
     else if (k == "ws") c->force_ws = value;
     else if (k == "cn") c->force_cn = value;
     else if (k == "halo") c->force_halo = value;
+    else if (k == "fuse") c->force_fuse = value;
     else if (k == "fork") c->fork = value;
     else if (k == "net") c->net = value;
     else if (k == "net_ctas") c->net_ctas = value;
@@ -2493,6 +2626,8 @@ int b2_engine_refine_tactics(b2_engine* e, int streams, int passes, double* gain
                 if (!t.ws && t.cn <= 1 && t.splits == 1 &&
                     !(t.bn == cur.bn && t.stages == cur.stages && t.sps == cur.sps && t.halo == cur.halo))
                     cands.push_back(t);
+            if (streams >= kFuseMinStreams && cur.halo != 2 && tactic_applies(ctx[0].c, op, batch, fused_conv_config(op)))
+                cands.push_back(fused_conv_config(op));
             ConvConfig best = cur;
             for (const ConvConfig& cand : cands) {
                 {
@@ -2713,7 +2848,8 @@ const char* b2_context_launch_name(b2_context* c, int batch, int i) {
         s += " bn=" + std::to_string(L->conv.bn) + " kb=" + std::to_string(L->conv.kb) +
              " st=" + std::to_string(L->conv.stages) + "x" + std::to_string(L->conv.sps) +
              (L->conv.ws_ctas ? " ws=" + std::to_string(L->conv.ws_ctas) : std::string()) +
-             (L->conv.cn > 1 ? " cn=" + std::to_string(L->conv.cn) : std::string()) + (L->conv.halo ? " halo" : "") +
+             (L->conv.cn > 1 ? " cn=" + std::to_string(L->conv.cn) : std::string()) +
+             (L->conv.halo == 2 ? " halo fused" : L->conv.halo ? " halo" : "") +
              (L->conv.args.a_mode == b2k::A_TILED ? " tiled" : " im2col") +
              " grid=" + std::to_string(L->conv.grid_n) + "x" + std::to_string(L->conv.grid_m) + "x" +
              std::to_string(L->conv.args.splits) + " kblk=" + std::to_string(L->conv.args.num_kblocks) +

@@ -1090,6 +1090,238 @@ conv3x3_halo_tcgen05(const __grid_constant__ CUtensorMap mapIn, const __grid_con
     }
 }
 
+// =================================================================================================
+// conv3x3_halo_1x1_tcgen05 -- a bottleneck's 3x3 (exactly as conv3x3_halo_tcgen05, over ALL of its BN output channels)
+//   followed by the 1x1 that reads it, with that 1x1's bias + residual + ReLU: the 3x3 output never leaves the SM.
+//
+//   Phase 1 is the halo kernel's K loop.  Its epilogue rounds bias + ReLU to fp16 into the drained halo buffers as BN/64
+//   128-row x 64-channel SWIZZLE_128B boxes: the layout of the tile kernel's A stages, so that tile is the 1x1's A
+//   operand with the whole of its K.  Phase 2 walks the 1x1's output channels in 64-wide chunks: the packed weight
+//   blocks [K/64][Cout/32][32][128 B] stream through the same B ring (the weight producer just keeps going), each chunk
+//   accumulates its K-blocks and k16 steps in ascending order, and its epilogue adds bias, then the residual, then ReLU in
+//   fp32 exactly like the tile kernel's -- the same bits as the unfused pair.  Rows of the tile are the halo kernel's
+//   padded coordinates: residual loads and output stores are 4-D boxes {64, W+2, R, 1} at w = 0, so the two garbage
+//   columns and the rows past H are zero-filled on load and clipped on store.  Two residual buffers: the chunk after next
+//   is loaded as soon as a chunk's output (staged in place over its residual) has been read by its store.
+//   warps 0-7 consumers, warp 8 halo / residual loads and output stores, warp 9 weights and biases.
+// =================================================================================================
+constexpr int kFuseChunk = 64;                          // 1x1 output channels per phase-2 chunk: one TMA box
+constexpr int kFuseTile = 128 * kFuseChunk * 2;         // one residual / output staging buffer
+__host__ __device__ constexpr int halo_fused_smem_bytes(int bn, int w, int r, int cblocks, int cout2) {
+    const int halo = cblocks * halo_a_stage_bytes(w, r), a2 = bn * 256;  // the 3x3 output tile reuses the halo buffers
+    return (halo > a2 ? halo : a2) + 2 * kFuseTile + halo_b_stages(bn) * bn * 128 + 256 + (bn + cout2) * 4 + 1024;
+}
+
+template <int BN>
+__global__ void __launch_bounds__(kConvThreads, conv_min_ctas(BN))
+conv3x3_halo_1x1_tcgen05(const __grid_constant__ CUtensorMap mapIn, const __grid_constant__ CUtensorMap mapRes,
+                         const __grid_constant__ CUtensorMap mapOut, const ConvArgs p, const Conv1x1Args q) {
+    constexpr int NB = halo_b_stages(BN);
+    constexpr int B_BLK = BN * 128;
+    constexpr int C_BLK = kFuseChunk * 128;  // one K-block of one chunk's 1x1 weights
+    constexpr int KB2 = BN / 64;             // K-blocks of the 1x1
+
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+    const int W = p.Wo, Wp = p.Wo + 2, R = p.halo_rows;
+    const int a_stage = halo_a_stage_bytes(W, R);
+    const int cblocks = p.cblocks;
+    const int region0 = max(cblocks * a_stage, BN * 256);
+    uint8_t* sA = smem;              // phase 1: halo blocks; phase 2: the 3x3 output tile
+    uint8_t* sR = smem + region0;    // two residual buffers (the output is staged in place)
+    uint8_t* sB = sR + 2 * kFuseTile;
+    uint8_t* tail = sB + NB * B_BLK;
+    uint64_t* a_full = reinterpret_cast<uint64_t*>(tail);
+    uint64_t* b_full = a_full + kHaloMaxCBlocks;
+    uint64_t* b_empty = b_full + NB;
+    uint64_t* r_full = b_empty + NB;   // residual of chunk c landed in buffer c % 2
+    uint64_t* e_done = r_full + 2;     // output of chunk c staged in buffer c % 2
+    uint64_t* bias_bar = e_done + 2;   // both bias vectors in smem
+    float* s_bias = reinterpret_cast<float*>(tail + 256);
+    float* s_bias2 = s_bias + BN;
+
+    const int warp = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
+    const int Ho = p.HoWo / p.Wo;
+    const int tiles_per_img = (Ho + R - 1) / R;
+    const int img = blockIdx.y / tiles_per_img;
+    const int h0 = (blockIdx.y - img * tiles_per_img) * R;
+    const int nsteps = cblocks * 9;
+    const int nchunks = q.Cout / kFuseChunk;
+    const int nsteps_all = nsteps + nchunks * KB2;
+
+    if (threadIdx.x == 0) {
+        tma_prefetch_desc(&mapIn);
+        tma_prefetch_desc(&mapRes);
+        tma_prefetch_desc(&mapOut);
+        for (int s = 0; s < cblocks; ++s) mbar_init(&a_full[s], 1);
+        for (int s = 0; s < NB; ++s) {
+            mbar_init(&b_full[s], 1);
+            mbar_init(&b_empty[s], kConsumerWarps);
+        }
+        for (int s = 0; s < 2; ++s) {
+            mbar_init(&r_full[s], 1);
+            mbar_init(&e_done[s], kConsumerWarps);
+        }
+        mbar_init(bias_bar, 32);
+        fence_barrier_init();
+        fence_proxy_async();
+    }
+    __syncthreads();
+    if (p.pdl_trigger == 0) pdl_launch_dependents();
+
+    if (warp == kActWarp) {
+        // ================= halo + residual loads, output stores =================
+        const uint32_t box_bytes = static_cast<uint32_t>(R * Wp * 128);
+        auto load_res = [&](int c) {
+            mbar_expect_tx(&r_full[c & 1], box_bytes);
+            tma_load_4d(&mapRes, &r_full[c & 1], sR + (c & 1) * kFuseTile, c * kFuseChunk, 0, h0, img);
+        };
+        pdl_wait();
+        if (elect_one_sync()) {
+            for (int cb = 0; cb < cblocks; ++cb) {
+                mbar_expect_tx(&a_full[cb], static_cast<uint32_t>((R + 2) * Wp * 128));
+                tma_load_4d(&mapIn, &a_full[cb], sA + cb * a_stage, cb * 64, -1, h0 - 1, img);
+            }
+            for (int c = 0; c < 2 && c < nchunks; ++c) load_res(c);
+            for (int c = 0; c < nchunks; ++c) {
+                mbar_wait(&e_done[c & 1], (c >> 1) & 1);
+                tma_store_4d(&mapOut, sR + (c & 1) * kFuseTile, c * kFuseChunk, 0, h0, img);
+                tma_store_commit_and_wait_read();  // the buffer may be refilled
+                if (c + 2 < nchunks) load_res(c + 2);
+            }
+        }
+        __syncwarp();
+    } else if (warp < kConsumerWarps) {
+        const uint32_t wg = static_cast<uint32_t>(warp >> 2);
+        const uint32_t wg_off = wg * 8192u;  // 64 pixel rows of 128 B
+        // ================= phase 1: the 3x3, as conv3x3_halo_tcgen05 =================
+        float acc[BN / 2];
+        int i = 0;
+#pragma unroll 1
+        for (int tap = 0; tap < 9; ++tap) {
+            const int r = tap / 3, sx = tap - r * 3;
+            const uint32_t tap_off = static_cast<uint32_t>((r * Wp + sx) * 128);
+#pragma unroll 1
+            for (int cb = 0; cb < cblocks; ++cb, ++i) {
+                const int sb = i % NB;
+                if (tap == 0) mbar_wait(&a_full[cb], 0);
+                mbar_wait(&b_full[sb], (i / NB) & 1);
+                const uint32_t a_addr = smem_u32(sA + cb * a_stage) + tap_off + wg_off;
+                const uint32_t b_addr = smem_u32(sB + sb * B_BLK);
+                wgmma_fence();
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const uint64_t ad = make_wgmma_desc(a_addr + j * 32, 16, 1024, WG_SW128);
+                    const uint64_t bd = make_wgmma_desc(b_addr + j * 32, 16, 1024, WG_SW128);
+                    wgmma_f16<BN>(acc, ad, bd, (i > 0 || j > 0) ? 1u : 0u);
+                }
+                wgmma_commit();
+                wgmma_wait<1>();
+                __syncwarp();
+                if (i > 0 && lane == 0) mbar_arrive(&b_empty[(i - 1) % NB]);
+            }
+        }
+        wgmma_wait<0>();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&b_empty[(nsteps - 1) % NB]);
+
+        // ---- the 3x3's epilogue: bias + ReLU -> fp16 -> the 1x1's A tile (over the halo blocks both warpgroups read) ----
+        named_bar_sync(1, kConsumerWarps * 32);
+        mbar_wait(bias_bar, 0);
+        const FragPos fp(warp, lane);
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int row = fp.row0 + 8 * h, col = 8 * j + fp.col0;
+                const uint32_t so = static_cast<uint32_t>((col / 64) * (128 * 128)) + swz_off<128>(row, (col % 64) / 8) + (col % 8) * 2;
+                float v0 = acc[4 * j + 2 * h] + s_bias[col], v1 = acc[4 * j + 2 * h + 1] + s_bias[col + 1];
+                if (p.relu) {
+                    v0 = fmaxf(v0, 0.0f);
+                    v1 = fmaxf(v1, 0.0f);
+                }
+                *reinterpret_cast<__half2*>(sA + so) = __floats2half2_rn(v0, v1);
+            }
+        }
+        fence_proxy_async();                       // generic stores -> the wgmma (async proxy) reads below
+        named_bar_sync(2 + wg, 128);               // a warpgroup reads back exactly the 64 rows it wrote
+
+        // ================= phase 2: the 1x1 in 64-channel chunks =================
+#pragma unroll 1
+        for (int c = 0; c < nchunks; ++c) {
+            float acc2[kFuseChunk / 2];
+#pragma unroll
+            for (int kb = 0; kb < KB2; ++kb, ++i) {
+                const int sb = i % NB;
+                mbar_wait(&b_full[sb], (i / NB) & 1);
+                const uint32_t a_addr = smem_u32(sA + kb * (128 * 128)) + wg_off;
+                const uint32_t b_addr = smem_u32(sB + sb * B_BLK);
+                wgmma_fence();
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const uint64_t ad = make_wgmma_desc(a_addr + j * 32, 16, 1024, WG_SW128);
+                    const uint64_t bd = make_wgmma_desc(b_addr + j * 32, 16, 1024, WG_SW128);
+                    wgmma_f16<kFuseChunk>(acc2, ad, bd, (kb > 0 || j > 0) ? 1u : 0u);
+                }
+                wgmma_commit();
+                wgmma_wait<1>();
+                __syncwarp();
+                if (kb > 0 && lane == 0) mbar_arrive(&b_empty[(i - 1) % NB]);
+            }
+            wgmma_wait<0>();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&b_empty[(i - 1) % NB]);
+            if (c == nchunks - 1 && p.pdl_trigger == 1) pdl_launch_dependents();
+            // bias, then residual, then ReLU: the tile kernel's order
+            uint8_t* buf = sR + (c & 1) * kFuseTile;
+            mbar_wait(&r_full[c & 1], (c >> 1) & 1);
+#pragma unroll
+            for (int j = 0; j < kFuseChunk / 8; ++j) {
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int row = fp.row0 + 8 * h, col = 8 * j + fp.col0;
+                    const uint32_t so = swz_off<128>(row, col / 8) + (col % 8) * 2;
+                    float v0 = acc2[4 * j + 2 * h] + s_bias2[c * kFuseChunk + col];
+                    float v1 = acc2[4 * j + 2 * h + 1] + s_bias2[c * kFuseChunk + col + 1];
+                    const float2 rf = __half22float2(*reinterpret_cast<const __half2*>(buf + so));
+                    v0 += rf.x;
+                    v1 += rf.y;
+                    if (q.relu) {
+                        v0 = fmaxf(v0, 0.0f);
+                        v1 = fmaxf(v1, 0.0f);
+                    }
+                    *reinterpret_cast<__half2*>(buf + so) = __floats2half2_rn(v0, v1);
+                }
+            }
+            fence_proxy_async();  // -> the TMA store
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&e_done[c & 1]);
+        }
+    } else if (warp == kWgtWarp) {
+        // ================= weights of both convolutions through one ring (constants: no dependency wait) =================
+        for (int i = lane; i < BN; i += 32) s_bias[i] = __ldg(p.bias + i);
+        for (int i = lane; i < q.Cout; i += 32) s_bias2[i] = __ldg(q.bias + i);
+        mbar_arrive(bias_bar);
+        for (int i = 0; i < nsteps_all; ++i) {
+            const int sb = i % NB;
+            if (i >= NB) mbar_wait(&b_empty[sb], ((i / NB) & 1) ^ 1);
+            if (elect_one_sync()) {
+                if (i < nsteps) {
+                    mbar_expect_tx(&b_full[sb], B_BLK);
+                    bulk_load_1d(&b_full[sb], sB + sb * B_BLK, p.wpacked + static_cast<size_t>(i) * (BN >> 5) * 4096, B_BLK);
+                } else {
+                    const int t = i - nsteps, c = t / KB2, kb = t - c * KB2;
+                    mbar_expect_tx(&b_full[sb], C_BLK);
+                    bulk_load_1d(&b_full[sb], sB + sb * B_BLK,
+                                 q.wpacked + (static_cast<size_t>(kb) * (q.Cout >> 5) + c * (kFuseChunk >> 5)) * 4096, C_BLK);
+                }
+            }
+            __syncwarp();
+        }
+    }
+}
+
 static bool g_use_pdl = true;
 void set_pdl(bool on) { g_use_pdl = on; }
 bool get_pdl() { return g_use_pdl; }
@@ -1197,9 +1429,28 @@ static int init_conv_halo_kernels() {
     int e;
     if ((e = set_conv_smem(conv3x3_halo_tcgen05<64>, 227 * 1024))) return e;
     if ((e = set_conv_smem(conv3x3_halo_tcgen05<128>, 227 * 1024))) return e;
-    return set_conv_smem(conv3x3_halo_tcgen05<256>, 227 * 1024);
+    if ((e = set_conv_smem(conv3x3_halo_tcgen05<256>, 227 * 1024))) return e;
+    if ((e = set_conv_smem(conv3x3_halo_1x1_tcgen05<64>, 227 * 1024))) return e;
+    if ((e = set_conv_smem(conv3x3_halo_1x1_tcgen05<128>, 227 * 1024))) return e;
+    return set_conv_smem(conv3x3_halo_1x1_tcgen05<256>, 227 * 1024);
+}
+int conv_halo_fused_smem(int bn, int w, int r, int cblocks, int cout2) { return halo_fused_smem_bytes(bn, w, r, cblocks, cout2); }
+static int launch_conv_halo_fused(const ConvLaunch& L, cudaStream_t stream) {
+    const int R = L.args.halo_rows;
+    const size_t smem = size_t(halo_fused_smem_bytes(L.bn, L.args.Wo, R, L.args.cblocks, L.c2.Cout));
+    if (smem > 227 * 1024 || R < 1 || R * (L.args.Wo + 2) > 128 || L.args.cblocks > kHaloMaxCBlocks || L.grid_n != 1 ||
+        L.bn != L.args.Cout || L.c2.Cout < kFuseChunk || L.c2.Cout % kFuseChunk)
+        return static_cast<int>(cudaErrorInvalidValue);
+    dim3 grid(1, L.grid_m, 1);
+    switch (L.bn) {
+        case 64: return launch_kernel(conv3x3_halo_1x1_tcgen05<64>, grid, dim3(kConvThreads), smem, stream, true, L.mapA, L.mapRes, L.mapOut, L.args, L.c2);
+        case 128: return launch_kernel(conv3x3_halo_1x1_tcgen05<128>, grid, dim3(kConvThreads), smem, stream, true, L.mapA, L.mapRes, L.mapOut, L.args, L.c2);
+        case 256: return launch_kernel(conv3x3_halo_1x1_tcgen05<256>, grid, dim3(kConvThreads), smem, stream, true, L.mapA, L.mapRes, L.mapOut, L.args, L.c2);
+    }
+    return static_cast<int>(cudaErrorInvalidValue);
 }
 static int launch_conv_halo(const ConvLaunch& L, cudaStream_t stream) {
+    if (L.halo == 2) return launch_conv_halo_fused(L, stream);
     const int R = L.args.halo_rows;
     const size_t smem = size_t(halo_smem_bytes(L.bn, L.args.Wo, R, L.args.cblocks));
     if (smem > 227 * 1024 || R < 1 || R * (L.args.Wo + 2) > 128 || L.args.cblocks > kHaloMaxCBlocks) return static_cast<int>(cudaErrorInvalidValue);

@@ -47,6 +47,14 @@ struct ConvArgs {
                              // starting at channel (n0 / group_span) * group_span; cblocks = group_span / 64.  0 = dense
 };
 
+// The 1x1 / stride-1 convolution a fused bottleneck launch (ConvLaunch::halo == 2) runs on the 3x3's output, with residual
+struct Conv1x1Args {
+    const uint8_t* wpacked;  // [Cin/64][Cout/32][32][128 B] pre-swizzled blocks, Cin = the 3x3's output channels
+    const float* bias;       // [Cout]
+    int Cout;                // multiple of 64
+    int relu;
+};
+
 struct ConvLaunch {
     CUtensorMap mapA;  // activations: 2-D tiled [M, Cin] or 4-D im2col (C, W, H, N)
     CUtensorMap mapB;  // weights: 2-D tiled [Cout_phys, Ktot]
@@ -61,7 +69,10 @@ struct ConvLaunch {
     int grid_m, grid_n;
     int cn;            // cluster size along N (1, 2 or 4; KB == 64 only): mapA's box is then 128/cn rows
     int halo;          // 1: conv3x3_halo_tcgen05 (3x3 s1 p1; mapA / mapOut are 4-D tiled {C, W, H, N} maps; grid_m = N * ceil(H/R))
+                       // 2: conv3x3_halo_1x1_tcgen05, the 3x3 then the 1x1 `c2` on its output (grid_n = 1; mapOut / mapRes
+                       //    are the 1x1's output and residual as 4-D {64, W+2, R, 1} boxes)
     int ws_ctas;       // > 0: persistent warp-specialised variant with this many CTAs (0: one tile per CTA)
+    Conv1x1Args c2;    // halo == 2
 };
 
 // returns 0 or a cudaError_t
@@ -73,6 +84,7 @@ int conv_smem_bytes(int bn, int stages, bool residual, int sps = 1);  // dynamic
 bool conv_cluster_config_exists(int bn, int stages, int sps, int cn);  // cluster-multicast instantiations
 bool conv_halo_config_exists(int bn);                                // 3x3 halo variant
 int conv_halo_smem(int bn, int w, int r, int cblocks);
+int conv_halo_fused_smem(int bn, int w, int r, int cblocks, int cout2);  // the 3x3 + 1x1 variant (halo == 2)
 // CTAs of the tile kernel (halo_w == 0) or of the halo kernel (output width halo_w, halo_rows rows per tile, cblocks
 // channel blocks) that fit on one SM; needs init_conv_kernels() and a current device, 0 if unknown.  Cached.
 int conv_residency(int bn, int kb, int stages, int sps, bool residual, int halo_w = 0, int halo_rows = 0, int cblocks = 0);
