@@ -18,6 +18,7 @@ PREC_FP32, PREC_FP16, PREC_INT8 = 0, 1, 2
 OP_INPUT_CAST, OP_CONV, OP_MAXPOOL, OP_AVGPOOL, OP_FC, OP_SOFTMAX, OP_OUTPUT_CAST, OP_QUANTIZE = range(8)
 OP_EMBED_LN, OP_LAYERNORM, OP_ATTENTION, OP_POOLER = range(8, 12)   # transformer ops (version-3 plans)
 CONV_RELU, CONV_PACKED, CONV_INT8, CONV_GELU = 1, 2, 4, 8            # OpRec.relu bits of a convolution
+FLAG_ROWS_OUT, FLAG_PACKED = 1, 2  # OpRecV3.flags: channels-last output cast; op on packed (padding-free) rows
 T_ACT, T_VEC = 0, 1
 MAGIC = b"B2ENGINE"
 VERSION = 1           # plans without grouped convolutions: 176-byte op records
@@ -364,7 +365,7 @@ def _serialize(tensors: List[dict], ops: List[dict], bindings: List[dict], paylo
 
 
 def build_bert_plan(cfg=None, weights=None, max_batch: int = 16, seed: int = 0, precision: int = PREC_FP16,
-                    name: Optional[str] = None, taps: Sequence[str] = ()) -> bytes:
+                    name: Optional[str] = None, taps: Sequence[str] = (), remove_padding: bool = False) -> bytes:
     """BERT encoder + pooler (``bert.BertConfig``; default BERT-base at S = 128; S = 64, 128, 256, 384 or 512) -> fp16
     plan (version 3).
 
@@ -376,7 +377,14 @@ def build_bert_plan(cfg=None, weights=None, max_batch: int = 16, seed: int = 0, 
     ``segment_ids``, ``input_mask`` ([S] per item, mask 1 = attend); fp32 ``last_hidden_state`` ([S, H], token-major) and
     ``pooled_output`` ([H]).  ``taps``: names of intermediate activation tensors (``embeddings``, ``l{i}.qkv``,
     ``l{i}.context``, ``l{i}.attn_sum``, ``l{i}.attn_ln``, ``l{i}.ffn``, ``l{i}.ffn_sum``, ``l{i}.out``) to expose as
-    extra fp32 [S, C] output bindings of the same names."""
+    extra fp32 [S, C] output bindings of the same names.
+
+    ``remove_padding``: a packed plan.  Same bindings, but only the tokens with ``input_mask != 0`` are computed: the
+    embedding packs each batch's valid tokens into consecutive rows (in item and position order, each with its original
+    position embedding), every GEMM and LayerNorm stops at the live row count, and attention runs per item over its own
+    tokens.  ``last_hidden_state`` and the taps hold the encoder output at valid positions and exactly 0 at masked ones;
+    ``pooled_output`` pools position 0, which is a zero row -- giving tanh(bias) -- when position 0 is masked.  For
+    right-padded masks the valid rows are bit-identical to the padded plan's; any mask pattern is accepted."""
     from . import bert as Bm
     cfg = cfg or Bm.BERT_BASE
     if precision == PREC_FP32:
@@ -420,21 +428,23 @@ def build_bert_plan(cfg=None, weights=None, max_batch: int = 16, seed: int = 0, 
         b_off, b_bytes = add_payload(b.astype(np.float32))
         return dict(name=oname, type=OP_CONV, inp=ti, res=res, out=to, binding=-1, k=1, stride=1, pad=0,
                     relu=CONV_PACKED | (CONV_GELU if gelu else 0), cin=cin, cout=cout, cin_phys=cin, cout_phys=cout, taps=1,
-                    taps_phys=1, w_off=w_off, w_bytes=w_bytes, b_off=b_off, b_bytes=b_bytes)
+                    taps_phys=1, w_off=w_off, w_bytes=w_bytes, b_off=b_off, b_bytes=b_bytes, flags=pk)
 
     def gamma_beta(prefix: str):
         return add_payload(np.concatenate([W[prefix + ".weight"], W[prefix + ".bias"]]).astype(np.float32))
 
     # bindings 0..2: int32 inputs, 3: last_hidden_state, 4: pooled_output
+    pk = FLAG_PACKED if remove_padding else 0
     x = act("embeddings", H)
-    mask = vec("attention_mask_add", S)
+    # padded: the additive attention mask [S]; packed: the packing index (pos_map and seq_off, S + 2 int32 words per item)
+    mask = vec("packing_index", S + 2) if remove_padding else vec("attention_mask_add", S)
     tables = np.concatenate([W["embeddings.word_embeddings.weight"], W["embeddings.position_embeddings.weight"],
                              W["embeddings.token_type_embeddings.weight"]]).astype(np.float16)
     w_off, w_bytes = add_payload(tables)
     b_off, b_bytes = gamma_beta("embeddings.LayerNorm")
     ops.append(dict(name="embeddings", type=OP_EMBED_LN, inp=-1, res=-1, out=x, binding=0, binding2=1, binding3=2, out2=mask,
                     cin=H, cout=H, cin_phys=H, cout_phys=H, vocab=cfg.vocab, positions=cfg.positions, types=cfg.types,
-                    eps=cfg.eps, w_off=w_off, w_bytes=w_bytes, b_off=b_off, b_bytes=b_bytes))
+                    eps=cfg.eps, w_off=w_off, w_bytes=w_bytes, b_off=b_off, b_bytes=b_bytes, flags=pk))
     for i in range(cfg.layers):
         p = f"encoder.layer.{i}."
         qkv, ctx, att, h1 = act(f"l{i}.qkv", 3 * H), act(f"l{i}.context", H), act(f"l{i}.attn_sum", H), act(f"l{i}.attn_ln", H)
@@ -442,21 +452,23 @@ def build_bert_plan(cfg=None, weights=None, max_batch: int = 16, seed: int = 0, 
         Wqkv = np.concatenate([W[p + f"attention.self.{m}.weight"] for m in ("query", "key", "value")])
         bqkv = np.concatenate([W[p + f"attention.self.{m}.bias"] for m in ("query", "key", "value")])
         ops.append(gemm(f"l{i}.qkv", x, qkv, Wqkv, bqkv))
-        ops.append(dict(name=f"l{i}.attention", type=OP_ATTENTION, inp=qkv, res=mask, out=ctx, binding=-1, heads=cfg.heads))
+        ops.append(dict(name=f"l{i}.attention", type=OP_ATTENTION, inp=qkv, res=mask, out=ctx, binding=-1, heads=cfg.heads, flags=pk))
         ops.append(gemm(f"l{i}.attn_out", ctx, att, W[p + "attention.output.dense.weight"], W[p + "attention.output.dense.bias"], res=x))
         b_off, b_bytes = gamma_beta(p + "attention.output.LayerNorm")
-        ops.append(dict(name=f"l{i}.attn_ln", type=OP_LAYERNORM, inp=att, res=-1, out=h1, binding=-1, eps=cfg.eps, b_off=b_off, b_bytes=b_bytes))
+        ops.append(dict(name=f"l{i}.attn_ln", type=OP_LAYERNORM, inp=att, res=-1, out=h1, binding=-1, eps=cfg.eps, b_off=b_off, b_bytes=b_bytes,
+                        flags=pk))
         ops.append(gemm(f"l{i}.ffn1", h1, ffn, W[p + "intermediate.dense.weight"], W[p + "intermediate.dense.bias"], gelu=True))
         ops.append(gemm(f"l{i}.ffn2", ffn, fsum, W[p + "output.dense.weight"], W[p + "output.dense.bias"], res=h1))
         b_off, b_bytes = gamma_beta(p + "output.LayerNorm")
-        ops.append(dict(name=f"l{i}.out_ln", type=OP_LAYERNORM, inp=fsum, res=-1, out=h2, binding=-1, eps=cfg.eps, b_off=b_off, b_bytes=b_bytes))
+        ops.append(dict(name=f"l{i}.out_ln", type=OP_LAYERNORM, inp=fsum, res=-1, out=h2, binding=-1, eps=cfg.eps, b_off=b_off, b_bytes=b_bytes,
+                        flags=pk))
         x = h2
     pooled = vec("pooled_output", H, binding=4)
     w_off, w_bytes = add_payload(W["pooler.dense.weight"].astype(np.float16))
     b_off, b_bytes = add_payload(W["pooler.dense.bias"].astype(np.float32))
     ops.append(dict(name="pooler", type=OP_POOLER, inp=x, res=-1, out=pooled, binding=-1, cin=H, cout=H, cin_phys=H, cout_phys=H,
-                    w_off=w_off, w_bytes=w_bytes, b_off=b_off, b_bytes=b_bytes))
-    ops.append(dict(name="cast:last_hidden_state", type=OP_OUTPUT_CAST, inp=x, res=-1, out=-1, binding=3, flags=1))
+                    w_off=w_off, w_bytes=w_bytes, b_off=b_off, b_bytes=b_bytes, flags=pk))
+    ops.append(dict(name="cast:last_hidden_state", type=OP_OUTPUT_CAST, inp=x, res=-1, out=-1, binding=3, flags=FLAG_ROWS_OUT | pk))
     bindings = [dict(name=n, is_input=1, dtype=3, tensor=0, dims=[S]) for n in ("input_ids", "segment_ids", "input_mask")]
     bindings.append(dict(name="last_hidden_state", is_input=0, dtype=0, tensor=x, dims=[S, H]))
     bindings.append(dict(name="pooled_output", is_input=0, dtype=0, tensor=pooled, dims=[H]))
@@ -465,8 +477,8 @@ def build_bert_plan(cfg=None, weights=None, max_batch: int = 16, seed: int = 0, 
         if ti is None:
             raise ValueError(f"tap {tap!r}: no such activation tensor")
         bindings.append(dict(name=tap, is_input=0, dtype=0, tensor=ti, dims=[S, tensors[ti]["c"]]))
-        ops.append(dict(name="cast:" + tap, type=OP_OUTPUT_CAST, inp=ti, res=-1, out=-1, binding=len(bindings) - 1, flags=1))
-    default_name = f"bert_l{cfg.layers}_h{H}_s{S}"
+        ops.append(dict(name="cast:" + tap, type=OP_OUTPUT_CAST, inp=ti, res=-1, out=-1, binding=len(bindings) - 1, flags=FLAG_ROWS_OUT | pk))
+    default_name = f"bert_l{cfg.layers}_h{H}_s{S}" + ("_packed" if remove_padding else "")
     return _serialize(tensors, ops, bindings, payload, PREC_FP16, max_batch, name or default_name)
 
 

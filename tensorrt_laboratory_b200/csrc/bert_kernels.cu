@@ -9,6 +9,9 @@
 //  * attention_f16_wgmma_ks -- S = 256, 384, 512: the same per 128-key block, S / 128 warpgroups splitting the keys; row
 //                            maxima, row sums and partial O's combined across warpgroups through shared memory
 //  * pooler_kernel        -- tanh(W h[CLS] + b), fp32 out
+//  Packed (padding-free) plans: embed_ln_packed_kernel writes only the valid tokens, to consecutive rows, and the packing
+//  index; the attention kernels' VARLEN variants run each item over its own rows; output_unpack_rows_kernel and the
+//  pooler read packed rows through the index (DESIGN.md, "Packed BERT").
 //
 // Numerics (DESIGN.md, "BERT numerics"): every sum below runs in a fixed order -- a lane adds its own elements in index
 // order, then the warp combines lanes with an xor butterfly -- so a row's result does not depend on the batch, the grid
@@ -132,14 +135,76 @@ __global__ void __launch_bounds__(32 * kRowWarps) embed_ln_kernel(const int* __r
     ln_row_store(x, nv, lane, a.C, a.eps, a.gamma, a.beta, a.out + row * a.C_phys, a.C_phys);
 }
 
+// Packed embedding: the same rows as embed_ln_kernel, written only for tokens with input_mask != 0, to consecutive packed
+// rows in (item, position) order, plus the packing index (EmbedArgs::pack).  One CTA per 32 consecutive positions of the
+// flattened [N][S] mask (S % 32 == 0): the packed row of flat position p is the number of non-zero mask entries before p,
+// counted by every CTA for its own first position, so the index needs no second launch.
+constexpr int kPackPositions = 32;
+constexpr int kPackWarps = 8;
+__global__ void __launch_bounds__(32 * kPackWarps) embed_ln_packed_kernel(const int* __restrict__ ids, const int* __restrict__ segs,
+                                                                        const int* __restrict__ mask, const EmbedArgs a) {
+    __shared__ int s_count[kPackWarps];
+    pdl_launch_dependents();
+    pdl_wait();
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const long long total = static_cast<long long>(a.N) * a.S;
+    const long long p0 = static_cast<long long>(blockIdx.x) * kPackPositions;
+    int c = 0;
+    for (long long i = threadIdx.x; i < p0; i += 32 * kPackWarps) c += __ldg(mask + i) != 0;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
+    if (lane == 0) s_count[warp] = c;
+    __syncthreads();
+    int base = 0;
+#pragma unroll
+    for (int w = 0; w < kPackWarps; ++w) base += s_count[w];
+    const bool valid = __ldg(mask + p0 + lane) != 0;
+    const unsigned ballot = __ballot_sync(0xffffffffu, valid);
+    int* pos_map = a.pack;
+    int* seq_off = a.pack + total;
+    const int n = static_cast<int>(p0 / a.S), s0 = static_cast<int>(p0 - static_cast<long long>(n) * a.S);
+    if (warp == 0) {
+        pos_map[p0 + lane] = valid ? base + __popc(ballot & ((1u << lane) - 1u)) : -1;
+        if (lane == 0 && s0 == 0) seq_off[n] = base;
+        if (lane == 0 && p0 + kPackPositions == total) seq_off[a.N] = base + __popc(ballot);
+    }
+    const int nvec = a.C / 8;
+    const int nv = (nvec - lane + 31) / 32;
+    for (int k = warp; k < kPackPositions; k += kPackWarps) {
+        if (!((ballot >> k) & 1u)) continue;
+        const long long flat = p0 + k;
+        const long long row = base + __popc(ballot & ((1u << k) - 1u));
+        const int s = s0 + k;
+        const int id = min(max(__ldg(ids + flat), 0), a.vocab - 1);
+        const int seg = min(max(__ldg(segs + flat), 0), a.types - 1);
+        const uint4* w = reinterpret_cast<const uint4*>(a.tables + static_cast<size_t>(id) * a.C);
+        const uint4* p = reinterpret_cast<const uint4*>(a.tables + static_cast<size_t>(a.vocab + s) * a.C);
+        const uint4* t = reinterpret_cast<const uint4*>(a.tables + static_cast<size_t>(a.vocab + a.positions + seg) * a.C);
+        float x[kLnMaxVec][8];
+#pragma unroll
+        for (int q = 0; q < kLnMaxVec; ++q) {
+            if (q >= nv) continue;
+            const int v = lane + 32 * q;
+            float fw[8], fp[8], ft[8];
+            unpack8(__ldg(w + v), fw);
+            unpack8(__ldg(p + v), fp);
+            unpack8(__ldg(t + v), ft);
+#pragma unroll
+            for (int e = 0; e < 8; ++e) x[q][e] = __fadd_rn(__fadd_rn(fw[e], fp[e]), ft[e]);  // (word + position) + type
+        }
+        ln_row_store(x, nv, lane, a.C, a.eps, a.gamma, a.beta, a.out + row * a.C_phys, a.C_phys);
+    }
+}
+
 __global__ void __launch_bounds__(32 * kRowWarps) layernorm_h8_kernel(const __half* __restrict__ in, __half* __restrict__ out,
                                                                    const float* __restrict__ gamma, const float* __restrict__ beta,
-                                                                   long long rows, int C, int C_phys, float eps) {
+                                                                   long long rows, int C, int C_phys, float eps,
+                                                                   const int* __restrict__ live) {
     pdl_launch_dependents();
     pdl_wait();
     const int lane = threadIdx.x & 31;
     const long long row = static_cast<long long>(blockIdx.x) * kRowWarps + (threadIdx.x >> 5);
-    if (row >= rows) return;
+    if (row >= rows || (live && row >= *live)) return;
     const uint4* src = reinterpret_cast<const uint4*>(in + row * C_phys);
     const int nv = (C / 8 - lane + 31) / 32;
     float x[kLnMaxVec][8];
@@ -181,10 +246,16 @@ __device__ __forceinline__ uint32_t sw128(int row, int col) {
     return static_cast<uint32_t>(row * 128 + ((((col >> 3) ^ row) & 7) << 4) + (col & 7) * 2);
 }
 
-template <int S>
+// VARLEN (packed plans): item n is rows seq_off[n] ... seq_off[n + 1] - 1 of the packed QKV tensor, its length len.  A CTA
+// whose query tile starts at or past len exits; key blocks of 64 rows past len are not loaded; a key column >= len gets
+// the score -3e38 (so P = 0 exactly) by selection, and its V row is zeroed in V^T, since the rows past len belong to the
+// next item or hold stale data that may not be finite.  Query rows >= len are not stored.  Every valid key takes the
+// same column and the same place in every sum as in the padded kernel, where a masked key's P is 0 as well: for a
+// right-padded item the valid rows come out bit-identical.
+template <int S, bool VARLEN = false>
 __global__ void __launch_bounds__(128, 1)
 attention_f16_wgmma(const __grid_constant__ CUtensorMap mapQKV, const float* __restrict__ mask_add, __half* __restrict__ out, int heads,
-                    int H, int out_pitch) {
+                    int H, int out_pitch, const int* __restrict__ seq_off) {
     static_assert(S == 64 || S == 128, "sequence lengths 64 and 128");
     using L = AttnSmem<S>;
     extern __shared__ uint8_t smem_raw[];
@@ -201,30 +272,43 @@ attention_f16_wgmma(const __grid_constant__ CUtensorMap mapQKV, const float* __r
     __syncthreads();
     pdl_launch_dependents();
     pdl_wait();  // Q, K, V and the mask are the previous kernels' output
+    int row0 = n * S, len = S;
+    if constexpr (VARLEN) {
+        row0 = seq_off[n];
+        len = seq_off[n + 1] - row0;
+        if (q0 >= len) return;
+    }
+    const int kblocks = VARLEN ? (len + 63) / 64 : S / 64;  // 64-row key / value blocks loaded
     if (tid == 0) {
-        mbar_expect_tx(bar, static_cast<uint32_t>((64 + 2 * S) * 128));
-        const int row0 = n * S;
+        mbar_expect_tx(bar, static_cast<uint32_t>((64 + 2 * 64 * kblocks) * 128));
         tma_load_2d(&mapQKV, bar, smem + L::Q, head * 64, row0 + q0);
 #pragma unroll
         for (int b = 0; b < S / 64; ++b) {
+            if (VARLEN && b >= kblocks) break;
             tma_load_2d(&mapQKV, bar, smem + L::K + b * 8192, H + head * 64, row0 + 64 * b);
             tma_load_2d(&mapQKV, bar, smem + L::V + b * 8192, 2 * H + head * 64, row0 + 64 * b);
         }
     }
     // this thread's key columns: 8j + 2(l%4) + e
     float mk[S / 4];
+    if constexpr (!VARLEN) {
 #pragma unroll
-    for (int j = 0; j < S / 8; ++j) {
-        const float2 m2 = __ldg(reinterpret_cast<const float2*>(mask_add + static_cast<size_t>(n) * S + 8 * j + 2 * (lane & 3)));
-        mk[2 * j] = m2.x;
-        mk[2 * j + 1] = m2.y;
+        for (int j = 0; j < S / 8; ++j) {
+            const float2 m2 = __ldg(reinterpret_cast<const float2*>(mask_add + static_cast<size_t>(n) * S + 8 * j + 2 * (lane & 3)));
+            mk[2 * j] = m2.x;
+            mk[2 * j + 1] = m2.y;
+        }
     }
     mbar_wait(bar, 0);
     // V [key][d] -> V^T [d][key] (K-major B operand of P V), 2 keys x 1 d per step
     for (int e = tid; e < S * 32; e += 128) {
         const int d = e & 63, key = (e >> 6) * 2;
-        const __half v0 = *reinterpret_cast<const __half*>(smem + L::V + sw128(key, d));
-        const __half v1 = *reinterpret_cast<const __half*>(smem + L::V + sw128(key + 1, d));
+        __half v0 = *reinterpret_cast<const __half*>(smem + L::V + sw128(key, d));
+        __half v1 = *reinterpret_cast<const __half*>(smem + L::V + sw128(key + 1, d));
+        if (VARLEN) {
+            if (key >= len) v0 = __float2half_rn(0.f);
+            if (key + 1 >= len) v1 = __float2half_rn(0.f);
+        }
         *reinterpret_cast<__half2*>(smem + L::VT + (key >> 6) * 8192 + sw128(d, key & 63)) = __halves2half2(v0, v1);
     }
     fence_proxy_async();  // generic-proxy stores -> visible to wgmma
@@ -249,7 +333,10 @@ attention_f16_wgmma(const __grid_constant__ CUtensorMap mapQKV, const float* __r
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
                 float& v = sacc[4 * j + 2 * h + e];
-                v = __fadd_rn(__fmul_rn(v, 0.125f), mk[2 * j + e]);
+                if constexpr (VARLEN)
+                    v = 8 * j + 2 * (lane & 3) + e < len ? __fmul_rn(v, 0.125f) : -3.0e38f;
+                else
+                    v = __fadd_rn(__fmul_rn(v, 0.125f), mk[2 * j + e]);
                 mx[h] = fmaxf(mx[h], v);
             }
     float sum[2] = {0.f, 0.f};
@@ -297,7 +384,8 @@ attention_f16_wgmma(const __grid_constant__ CUtensorMap mapQKV, const float* __r
     const int r0 = 16 * warp + (lane >> 2);
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-        __half* orow = out + static_cast<size_t>(n * S + q0 + r0 + 8 * h) * out_pitch + head * 64 + 2 * (lane & 3);
+        if (VARLEN && q0 + r0 + 8 * h >= len) continue;
+        __half* orow = out + static_cast<size_t>(row0 + q0 + r0 + 8 * h) * out_pitch + head * 64 + 2 * (lane & 3);
 #pragma unroll
         for (int j = 0; j < 8; ++j)
             *reinterpret_cast<__half2*>(orow + 8 * j) = __floats2half2_rn(oacc[4 * j + 2 * h], oacc[4 * j + 2 * h + 1]);
@@ -325,10 +413,13 @@ struct AttnKsSmem {
 // Same arithmetic as attention_f16_wgmma<128> per 128-key block; across blocks the row maximum is the maximum of the
 // blocks' maxima, the row sum and O add the blocks' partial sums and partial P V in warpgroup order (w = 0, 1, ...), in
 // fp32, and O is rounded to fp16 once.  The order depends on S alone.
-template <int S>
+// VARLEN: as attention_f16_wgmma<S, true>; a warpgroup whose 128-key block starts at or past the item's length runs no
+// MMA and contributes what the padded kernel's fully masked block does: row maximum -3e38 (never the maximum), row sum 0,
+// partial O 0.
+template <int S, bool VARLEN = false>
 __global__ void __launch_bounds__(S, 1)
 attention_f16_wgmma_ks(const __grid_constant__ CUtensorMap mapQKV, const float* __restrict__ mask_add, __half* __restrict__ out, int heads,
-                       int H, int out_pitch) {
+                       int H, int out_pitch, const int* __restrict__ seq_off) {
     static_assert(S == 256 || S == 384 || S == 512, "sequence lengths 256, 384 and 512");
     using L = AttnKsSmem<S>;
     extern __shared__ uint8_t smem_raw[];
@@ -348,22 +439,35 @@ attention_f16_wgmma_ks(const __grid_constant__ CUtensorMap mapQKV, const float* 
     __syncthreads();
     pdl_launch_dependents();
     pdl_wait();  // Q, K, V and the mask are the previous kernels' output
+    int row0 = n * S, len = S;
+    if constexpr (VARLEN) {
+        row0 = seq_off[n];
+        len = seq_off[n + 1] - row0;
+        if (q0 >= len) return;
+    }
+    const int kblocks = VARLEN ? (len + 63) / 64 : S / 64;
+    const bool active = !VARLEN || 128 * wg < len;  // this warpgroup's key block holds a valid key
     if (tid == 0) {
-        mbar_expect_tx(bar, static_cast<uint32_t>((64 + 2 * S) * 128));
-        const int row0 = n * S;
+        mbar_expect_tx(bar, static_cast<uint32_t>((64 + 2 * 64 * kblocks) * 128));
         tma_load_2d(&mapQKV, bar, smem + L::Q, head * 64, row0 + q0);
 #pragma unroll
         for (int b = 0; b < S / 64; ++b) {
+            if (VARLEN && b >= kblocks) break;
             tma_load_2d(&mapQKV, bar, smem + L::K + b * 8192, H + head * 64, row0 + 64 * b);
             tma_load_2d(&mapQKV, bar, smem + L::V + b * 8192, 2 * H + head * 64, row0 + 64 * b);
         }
     }
-    mask_s[tid] = __ldg(mask_add + static_cast<size_t>(n) * S + tid);
+    if constexpr (!VARLEN) mask_s[tid] = __ldg(mask_add + static_cast<size_t>(n) * S + tid);
     mbar_wait(bar, 0);
     for (int e = tid; e < S * 32; e += S) {
         const int d = e & 63, key = (e >> 6) * 2;
-        const __half v0 = *reinterpret_cast<const __half*>(smem + L::V + sw128(key, d));
-        const __half v1 = *reinterpret_cast<const __half*>(smem + L::V + sw128(key + 1, d));
+        if (VARLEN && key >= 128 * ((len + 127) / 128)) break;  // key blocks of inactive warpgroups: never read
+        __half v0 = *reinterpret_cast<const __half*>(smem + L::V + sw128(key, d));
+        __half v1 = *reinterpret_cast<const __half*>(smem + L::V + sw128(key + 1, d));
+        if (VARLEN) {
+            if (key >= len) v0 = __float2half_rn(0.f);
+            if (key + 1 >= len) v1 = __float2half_rn(0.f);
+        }
         *reinterpret_cast<__half2*>(smem + L::VT + (key >> 6) * 8192 + sw128(d, key & 63)) = __halves2half2(v0, v1);
     }
     fence_proxy_async();
@@ -372,24 +476,33 @@ attention_f16_wgmma_ks(const __grid_constant__ CUtensorMap mapQKV, const float* 
     // this warpgroup's block of scores: 64 x 128, K = 64
     float sacc[64];
     const uint32_t q_addr = smem_u32(smem + L::Q), k_addr = smem_u32(smem + L::K + wg * 128 * 128);
-    wgmma_group<4>([&](int j) {
-        wgmma_f16<128>(sacc, make_wgmma_desc(q_addr + j * 32, 16, 1024, WG_SW128), make_wgmma_desc(k_addr + j * 32, 16, 1024, WG_SW128),
-                       j > 0 ? 1u : 0u);
-    });
-    wgmma_wait<0>();
+    if (active) {
+        wgmma_group<4>([&](int j) {
+            wgmma_f16<128>(sacc, make_wgmma_desc(q_addr + j * 32, 16, 1024, WG_SW128), make_wgmma_desc(k_addr + j * 32, 16, 1024, WG_SW128),
+                           j > 0 ? 1u : 0u);
+        });
+        wgmma_wait<0>();
+    } else {
+#pragma unroll
+        for (int i = 0; i < 64; ++i) sacc[i] = 0.f;
+    }
 
     const int r0 = 16 * warp + (lane >> 2);  // this thread's rows r0 and r0 + 8; key columns 128 wg + 8j + 2(l%4) + e
     const float* mk = mask_s + 128 * wg + 2 * (lane & 3);
     float mx[2] = {-3.0e38f, -3.0e38f};
 #pragma unroll
     for (int j = 0; j < 16; ++j) {
-        const float2 m2 = *reinterpret_cast<const float2*>(mk + 8 * j);
+        float2 m2 = make_float2(0.f, 0.f);
+        if constexpr (!VARLEN) m2 = *reinterpret_cast<const float2*>(mk + 8 * j);
 #pragma unroll
         for (int h = 0; h < 2; ++h)
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
                 float& v = sacc[4 * j + 2 * h + e];
-                v = __fadd_rn(__fmul_rn(v, 0.125f), e ? m2.y : m2.x);
+                if constexpr (VARLEN)
+                    v = 128 * wg + 8 * j + 2 * (lane & 3) + e < len ? __fmul_rn(v, 0.125f) : -3.0e38f;
+                else
+                    v = __fadd_rn(__fmul_rn(v, 0.125f), e ? m2.y : m2.x);
                 mx[h] = fmaxf(mx[h], v);
             }
     }
@@ -444,10 +557,15 @@ attention_f16_wgmma_ks(const __grid_constant__ CUtensorMap mapQKV, const float* 
     // partial O = P V over this warpgroup's keys: V^T blocks 2 wg and 2 wg + 1
     float oacc[32];
     const uint32_t vt_addr = smem_u32(smem + L::VT + wg * 2 * 8192);
-    wgmma_group<8>([&](int t) {
-        wgmma_f16_rs_n64(oacc, pa[t], make_wgmma_desc(vt_addr + (t >> 2) * 8192 + (t & 3) * 32, 16, 1024, WG_SW128), t > 0 ? 1u : 0u);
-    });
-    wgmma_wait<0>();
+    if (active) {
+        wgmma_group<8>([&](int t) {
+            wgmma_f16_rs_n64(oacc, pa[t], make_wgmma_desc(vt_addr + (t >> 2) * 8192 + (t & 3) * 32, 16, 1024, WG_SW128), t > 0 ? 1u : 0u);
+        });
+        wgmma_wait<0>();
+    } else {
+#pragma unroll
+        for (int i = 0; i < 32; ++i) oacc[i] = 0.f;
+    }
 
     // warpgroups 1 ... WG - 1 hand their partial O to warpgroup 0 through the dead V region, [slot][register][thread]
     float* part = reinterpret_cast<float*>(smem + L::V);
@@ -463,7 +581,8 @@ attention_f16_wgmma_ks(const __grid_constant__ CUtensorMap mapQKV, const float* 
         for (int i = 0; i < 32; ++i) oacc[i] = __fadd_rn(oacc[i], part[((w - 1) * 32 + i) * 128 + wt]);
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-        __half* orow = out + static_cast<size_t>(n * S + q0 + r0 + 8 * h) * out_pitch + head * 64 + 2 * (lane & 3);
+        if (VARLEN && q0 + r0 + 8 * h >= len) continue;
+        __half* orow = out + static_cast<size_t>(row0 + q0 + r0 + 8 * h) * out_pitch + head * 64 + 2 * (lane & 3);
 #pragma unroll
         for (int j = 0; j < 8; ++j)
             *reinterpret_cast<__half2*>(orow + 8 * j) = __floats2half2_rn(oacc[4 * j + 2 * h], oacc[4 * j + 2 * h + 1]);
@@ -471,9 +590,11 @@ attention_f16_wgmma_ks(const __grid_constant__ CUtensorMap mapQKV, const float* 
 }
 
 // pooled[n][j] = tanh(b[j] + W[j] . h[n][0]): one warp per output channel j, its weight row held in registers (loaded
-// before the dependency wait: weights are constants)
+// before the dependency wait: weights are constants).  pos_map (packed plans): h[n][0] is packed row pos_map[n * S]; -1
+// (position 0 masked) pools a zero row, tanh(b[j])
 __global__ void __launch_bounds__(256) pooler_kernel(const __half* __restrict__ h, const __half* __restrict__ w, const float* __restrict__ b,
-                                                     float* __restrict__ out, int N, int S, int C, int C_phys) {
+                                                     float* __restrict__ out, int N, int S, int C, int C_phys,
+                                                     const int* __restrict__ pos_map) {
     const int lane = threadIdx.x & 31;
     const int j = blockIdx.x * 8 + (threadIdx.x >> 5);
     const int nv = (C / 8 - lane + 31) / 32;
@@ -489,11 +610,12 @@ __global__ void __launch_bounds__(256) pooler_kernel(const __half* __restrict__ 
     if (j >= C) return;
     const float bj = __ldg(b + j);
     for (int n = 0; n < N; ++n) {
-        const uint4* hrow = reinterpret_cast<const uint4*>(h + static_cast<size_t>(n) * S * C_phys);  // token 0 = [CLS]
+        const long long r = pos_map ? pos_map[static_cast<size_t>(n) * S] : static_cast<long long>(n) * S;  // token 0 = [CLS]
+        const uint4* hrow = reinterpret_cast<const uint4*>(h + r * C_phys);
         float acc = 0.f;
 #pragma unroll
         for (int k = 0; k < kLnMaxVec; ++k) {
-            if (k >= nv) continue;
+            if (k >= nv || r < 0) continue;
             float x[8];
             unpack8(hrow[lane + 32 * k], x);
 #pragma unroll
@@ -513,63 +635,98 @@ __global__ void output_cast_rows_kernel(const __half* __restrict__ src, float* _
     dst[idx] = __half2float(src[r * C_phys + (idx - r * C)]);
 }
 
+__global__ void output_unpack_rows_kernel(const __half* __restrict__ src, float* __restrict__ dst, const int* __restrict__ pos_map,
+                                          long long rows, int C, int C_phys) {
+    pdl_launch_dependents();
+    pdl_wait();
+    const long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
+    if (idx >= rows * C) return;
+    const long long r = idx / C;
+    const int pr = pos_map[r];
+    dst[idx] = pr < 0 ? 0.0f : __half2float(src[static_cast<long long>(pr) * C_phys + (idx - r * C)]);
+}
+
 }  // namespace
 
 int launch_embed_ln(const EmbedArgs& a, cudaStream_t stream) {
     if (a.C % 8 || a.C > 32 * kLnMaxVec * 8) return static_cast<int>(cudaErrorInvalidValue);
     const long long rows = static_cast<long long>(a.N) * a.S;
+    if (a.pack) {
+        if (a.S % kPackPositions) return static_cast<int>(cudaErrorInvalidValue);
+        return launch_pdl(embed_ln_packed_kernel, dim3(static_cast<unsigned>(rows / kPackPositions)), dim3(32 * kPackWarps), 0, stream, a.ids,
+                          a.segs, a.mask, a);
+    }
     return launch_pdl(embed_ln_kernel, dim3(static_cast<unsigned>((rows + kRowWarps - 1) / kRowWarps)), dim3(32 * kRowWarps), 0, stream, a.ids, a.segs,
                       a.mask, a);
 }
 
 int launch_layernorm(const __half* in, __half* out, const float* gamma, const float* beta, long long rows, int C, int C_phys, float eps,
-                     cudaStream_t stream) {
+                     const int* live, cudaStream_t stream) {
     if (C % 8 || C > 32 * kLnMaxVec * 8) return static_cast<int>(cudaErrorInvalidValue);
     return launch_pdl(layernorm_h8_kernel, dim3(static_cast<unsigned>((rows + kRowWarps - 1) / kRowWarps)), dim3(32 * kRowWarps), 0, stream,
-                      in, out, gamma, beta, rows, C, C_phys, eps);
+                      in, out, gamma, beta, rows, C, C_phys, eps, live);
 }
 
 int init_attention_kernels() {
-    cudaError_t e = cudaFuncSetAttribute(attention_f16_wgmma<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnSmem<64>::BYTES);
-    if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(attention_f16_wgmma<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnSmem<128>::BYTES);
-    if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(attention_f16_wgmma_ks<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnKsSmem<256>::BYTES);
-    if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(attention_f16_wgmma_ks<384>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnKsSmem<384>::BYTES);
-    if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(attention_f16_wgmma_ks<512>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnKsSmem<512>::BYTES);
+    cudaError_t e = cudaSuccess;
+    auto set = [&](auto kern, int bytes) {
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    };
+    set(attention_f16_wgmma<64>, AttnSmem<64>::BYTES);
+    set(attention_f16_wgmma<128>, AttnSmem<128>::BYTES);
+    set(attention_f16_wgmma_ks<256>, AttnKsSmem<256>::BYTES);
+    set(attention_f16_wgmma_ks<384>, AttnKsSmem<384>::BYTES);
+    set(attention_f16_wgmma_ks<512>, AttnKsSmem<512>::BYTES);
+    set(attention_f16_wgmma<64, true>, AttnSmem<64>::BYTES);
+    set(attention_f16_wgmma<128, true>, AttnSmem<128>::BYTES);
+    set(attention_f16_wgmma_ks<256, true>, AttnKsSmem<256>::BYTES);
+    set(attention_f16_wgmma_ks<384, true>, AttnKsSmem<384>::BYTES);
+    set(attention_f16_wgmma_ks<512, true>, AttnKsSmem<512>::BYTES);
     return static_cast<int>(e);
 }
 
-int launch_attention(const AttnLaunch& L, cudaStream_t stream) {
-    const dim3 grid(static_cast<unsigned>(L.N * L.heads), static_cast<unsigned>(L.S / 64));
-    if (L.S == 64)
-        return launch_pdl(attention_f16_wgmma<64>, grid, dim3(128), AttnSmem<64>::BYTES, stream, L.mapQKV, L.mask_add, L.out, L.heads, L.H,
-                          L.out_pitch);
-    if (L.S == 128)
-        return launch_pdl(attention_f16_wgmma<128>, grid, dim3(128), AttnSmem<128>::BYTES, stream, L.mapQKV, L.mask_add, L.out, L.heads, L.H,
-                          L.out_pitch);
-    if (L.S == 256)
-        return launch_pdl(attention_f16_wgmma_ks<256>, grid, dim3(256), AttnKsSmem<256>::BYTES, stream, L.mapQKV, L.mask_add, L.out, L.heads,
-                          L.H, L.out_pitch);
-    if (L.S == 384)
-        return launch_pdl(attention_f16_wgmma_ks<384>, grid, dim3(384), AttnKsSmem<384>::BYTES, stream, L.mapQKV, L.mask_add, L.out, L.heads,
-                          L.H, L.out_pitch);
-    if (L.S == 512)
-        return launch_pdl(attention_f16_wgmma_ks<512>, grid, dim3(512), AttnKsSmem<512>::BYTES, stream, L.mapQKV, L.mask_add, L.out, L.heads,
-                          L.H, L.out_pitch);
+template <int S, bool VARLEN>
+static int launch_attention_s(const AttnLaunch& L, cudaStream_t stream) {
+    const dim3 grid(static_cast<unsigned>(L.N * L.heads), static_cast<unsigned>(S / 64));
+    if constexpr (S <= 128)
+        return launch_pdl(attention_f16_wgmma<S, VARLEN>, grid, dim3(128), AttnSmem<S>::BYTES, stream, L.mapQKV, L.mask_add, L.out, L.heads,
+                          L.H, L.out_pitch, L.seq_off);
+    else
+        return launch_pdl(attention_f16_wgmma_ks<S, VARLEN>, grid, dim3(S), AttnKsSmem<S>::BYTES, stream, L.mapQKV, L.mask_add, L.out,
+                          L.heads, L.H, L.out_pitch, L.seq_off);
+}
+
+template <bool VARLEN>
+static int launch_attention_v(const AttnLaunch& L, cudaStream_t stream) {
+    switch (L.S) {
+        case 64: return launch_attention_s<64, VARLEN>(L, stream);
+        case 128: return launch_attention_s<128, VARLEN>(L, stream);
+        case 256: return launch_attention_s<256, VARLEN>(L, stream);
+        case 384: return launch_attention_s<384, VARLEN>(L, stream);
+        case 512: return launch_attention_s<512, VARLEN>(L, stream);
+    }
     return static_cast<int>(cudaErrorInvalidValue);
 }
 
-int launch_pooler(const __half* h, const __half* w, const float* b, float* out, int N, int S, int C, int C_phys, cudaStream_t stream) {
+int launch_attention(const AttnLaunch& L, cudaStream_t stream) {
+    return L.seq_off ? launch_attention_v<true>(L, stream) : launch_attention_v<false>(L, stream);
+}
+
+int launch_pooler(const __half* h, const __half* w, const float* b, float* out, int N, int S, int C, int C_phys, const int* pos_map,
+                  cudaStream_t stream) {
     if (C % 8 || C > 32 * kLnMaxVec * 8) return static_cast<int>(cudaErrorInvalidValue);
-    return launch_pdl(pooler_kernel, dim3(static_cast<unsigned>((C + 7) / 8)), dim3(256), 0, stream, h, w, b, out, N, S, C, C_phys);
+    return launch_pdl(pooler_kernel, dim3(static_cast<unsigned>((C + 7) / 8)), dim3(256), 0, stream, h, w, b, out, N, S, C, C_phys, pos_map);
 }
 
 int launch_output_cast_rows(const __half* src, float* dst, long long rows, int C, int C_phys, cudaStream_t stream) {
     const long long total = rows * C;
     return launch_pdl(output_cast_rows_kernel, dim3(static_cast<unsigned>((total + 255) / 256)), dim3(256), 0, stream, src, dst, rows, C, C_phys);
+}
+
+int launch_output_unpack_rows(const __half* src, float* dst, const int* pos_map, long long rows, int C, int C_phys, cudaStream_t stream) {
+    const long long total = rows * C;
+    return launch_pdl(output_unpack_rows_kernel, dim3(static_cast<unsigned>((total + 255) / 256)), dim3(256), 0, stream, src, dst, pos_map,
+                      rows, C, C_phys);
 }
 
 }  // namespace b2k

@@ -141,7 +141,7 @@ struct Binding {
 };
 
 enum LKind { L_INPUT_CAST, L_CONV_TC, L_CONV_SIMT, L_MAXPOOL, L_AVGPOOL, L_FC, L_SOFTMAX, L_OUTPUT_CAST, L_NET, L_TAIL, L_QUANTIZE, L_CONV_I8, L_AVGPOOL_I8, L_OUTPUT_CAST_I8,
-             L_EMBED_LN, L_LAYERNORM, L_ATTENTION, L_POOLER, L_OUTPUT_ROWS };
+             L_EMBED_LN, L_LAYERNORM, L_ATTENTION, L_POOLER, L_OUTPUT_ROWS, L_OUTPUT_UNPACK };
 
 // A run of consecutive tcgen05 convolution layers executed by ONE persistent kernel (net_kernel.cu): device-side layer
 // table, dependency ranges and arrival counters live in one allocation owned by the plan.
@@ -179,6 +179,8 @@ struct Launch {
     int in_binding2 = -1, in_binding3 = -1;
     b2k::AttnLaunch attn{};       // L_ATTENTION
     float eps = 0.f;              // L_LAYERNORM
+    const int* live = nullptr;    // L_LAYERNORM of a packed plan: the live row count T (device)
+    const int* pos_map = nullptr; // L_POOLER / L_OUTPUT_UNPACK of a packed plan: the packing index's pos_map (device)
     int N = 0, C = 0, H = 0, W = 0, C_phys = 0, Ho = 0, Wo = 0, k = 0, stride = 0, pad = 0, K = 0, Cout = 0;
 };
 
@@ -277,6 +279,7 @@ struct b2_engine {
     std::map<int, float> requant_r;  // INT8 convs: op index -> r = fl(s_res / s_out) (read from the plan's requantisation block)
     bool tactics_from_plan = false;  // the blob carried a tactic table: nothing left to tune
     bool tuned_at_load = false;      // b2_engine_tune has run
+    int pack_tensor = -1;            // packed transformer plans: the packing index (out2 of the packed OP_EMBED_LN), else -1
     bool half() const { return precision != B2_PREC_FP32; }  // fp16 storage and kernels (INT8 engines: their fp16 part)
     bool int8() const { return precision == B2_PREC_INT8; }
 };
@@ -344,8 +347,12 @@ int validate_transformer_op(b2_engine* e, const Op& op) {
         case OP_EMBED_LN: {
             const Tensor& to = e->tensors[r.out];
             const Tensor& tm = e->tensors[op.out2];
-            if (!act_ok(to) || to.h != 1 || tm.kind != T_VEC || tm.c != to.w || tm.binding >= 0)
-                return fail(B2_EINVAL, "plan: embedding %s: needs an fp16 [1, S, C <= 1024, C %% 8 == 0] output and an fp32 [S] mask tensor", nm);
+            const uint32_t want_c = (op.flags & kOpPacked) ? to.w + 2 : to.w;  // packed: the packing index, S + 2 words per item
+            if (!act_ok(to) || to.h != 1 || tm.kind != T_VEC || tm.c != want_c || tm.binding >= 0)
+                return fail(B2_EINVAL, "plan: embedding %s: needs an fp16 [1, S, C <= 1024, C %% 8 == 0] output and an fp32 [S] mask tensor "
+                            "([S + 2] packing index when packed)", nm);
+            if ((op.flags & kOpPacked) && to.w % 32)
+                return fail(B2_EINVAL, "plan: packed embedding %s: S = %u is not a multiple of 32", nm, to.w);
             if (op.vocab < 1 || op.types < 1 || op.positions < int(to.w))
                 return fail(B2_EINVAL, "plan: embedding %s: vocab %d / positions %d / types %d do not cover S = %u", nm, op.vocab, op.positions,
                             op.types, to.w);
@@ -372,7 +379,7 @@ int validate_transformer_op(b2_engine* e, const Op& op) {
                 return fail(B2_EINVAL, "plan: attention %s: heads * 64 (%d * 64) != hidden size %u", nm, op.heads, to.c);
             if (!act_ok(to) || ti.kind != T_ACT || ti.scale != 0.f || ti.c != 3 * to.c || ti.c_phys != ti.c)
                 return fail(B2_EINVAL, "plan: attention %s: needs a fused fp16 QKV input of 3 x %u channels", nm, to.c);
-            if (ti.h != 1 || to.h != 1 || ti.w != to.w || tm.kind != T_VEC || tm.c != ti.w)
+            if (ti.h != 1 || to.h != 1 || ti.w != to.w || tm.kind != T_VEC || tm.c != ((op.flags & kOpPacked) ? ti.w + 2 : ti.w))
                 return fail(B2_EINVAL, "plan: attention %s: S does not match between QKV, output and mask", nm);
             if (ti.w != 64 && (ti.w == 0 || ti.w % 128 || ti.w > 512))
                 return fail(B2_EINVAL, "plan: attention %s: S = %u (64, or a multiple of 128 up to 512)", nm, ti.w);
@@ -393,6 +400,52 @@ int validate_transformer_op(b2_engine* e, const Op& op) {
         default:
             break;
     }
+    return B2_OK;
+}
+
+// Packed transformer plans (plan_format.h, kOpPacked): one packed embedding ahead of every other transformer op, and
+// every row-wise op of the plan marked, on [1, S, C] tensors of that embedding's S.  Sets e->pack_tensor.
+int validate_packed_ops(b2_engine* e) {
+    using namespace b2plan;
+    int embed = -1;
+    for (size_t i = 0; i < e->ops.size(); ++i) {
+        const Op& op = e->ops[i];
+        if (!(op.flags & kOpPacked) || op.r.type != OP_EMBED_LN) continue;
+        if (embed >= 0) return fail(B2_EINVAL, "plan: packed embedding %s: a plan has one packed embedding", op.name.c_str());
+        embed = int(i);
+    }
+    if (embed < 0) {
+        for (const Op& op : e->ops)
+            if (op.flags & kOpPacked) return fail(B2_EINVAL, "plan: op %s is marked packed in a plan without a packed embedding", op.name.c_str());
+        return B2_OK;
+    }
+    const Op& eo = e->ops[size_t(embed)];
+    const uint32_t S = e->tensors[eo.r.out].w;
+    for (size_t i = 0; i < e->ops.size(); ++i) {
+        const Op& op = e->ops[i];
+        const OpRec& r = op.r;
+        const char* nm = op.name.c_str();
+        const bool packed = (op.flags & kOpPacked) != 0;
+        const bool rowwise = r.type == OP_CONV || r.type == OP_LAYERNORM || r.type == OP_ATTENTION || r.type == OP_POOLER ||
+                             (r.type == OP_OUTPUT_CAST && (op.flags & kOpRowsOut)) || r.type == OP_EMBED_LN;
+        if (!rowwise)
+            return fail(B2_EINVAL, "plan: op %s: a packed plan holds transformer ops, GEMMs and channels-last output casts only", nm);
+        if (!packed) return fail(B2_EINVAL, "plan: op %s of a packed plan is not marked packed", nm);
+        if (r.type != OP_EMBED_LN && int(i) < embed) return fail(B2_EINVAL, "plan: op %s runs before the packed embedding", nm);
+        const int t = r.type == OP_EMBED_LN ? r.out : r.in;
+        const Tensor& tt = e->tensors[size_t(t)];
+        if (tt.kind != T_ACT || tt.h != 1 || tt.w != S)
+            return fail(B2_EINVAL, "plan: packed op %s: its tensor must be [1, S = %u, C] like the embedding's", nm, S);
+        if (r.type == OP_CONV) {
+            const Tensor& to = e->tensors[size_t(r.out)];
+            if (r.k != 1 || r.kw || r.stride != 1 || r.pad_ || !(r.relu & kConvPacked) || (r.relu & (kConvInt8 | kConvRelu)) ||
+                r.cin_phys % 64 || r.cout_phys % 32 || op.groups != 1 || to.h != 1 || to.w != S || (r.res >= 0 && e->tensors[size_t(r.res)].w != S))
+                return fail(B2_EINVAL, "plan: packed conv %s: packed layers are dense 1x1 stride-1 GEMMs with packed weights", nm);
+        }
+        if (r.type == OP_ATTENTION && r.res != eo.out2)
+            return fail(B2_EINVAL, "plan: packed attention %s must read the packing index of embedding %s", nm, eo.name.c_str());
+    }
+    e->pack_tensor = eo.out2;
     return B2_OK;
 }
 
@@ -564,6 +617,7 @@ int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** pa
         }
         e->ops.push_back(op);
     }
+    if (int rc = validate_packed_ops(e)) return rc;
     for (uint32_t i = 0; i < h.n_bindings; ++i, p += sizeof(BindingRec)) {
         BindingRec r;
         memcpy(&r, p, sizeof r);
@@ -679,6 +733,8 @@ void plan_arena(b2_engine* e) {
         const int j = fuse_partner(e, int(i));
         if (j >= 0) e->tensors[r.in].last_use = std::max(e->tensors[r.in].last_use, j);
     }
+    // packed plans: every row-wise op reads the packing index, through the embedding's out2 rather than its own tensors
+    if (e->pack_tensor >= 0) e->tensors[size_t(e->pack_tensor)].last_use = int(e->ops.size()) - 1;
     struct Live {
         size_t off, size;
         int last;
@@ -910,6 +966,8 @@ bool tactic_applies(const b2_context* c, const Op& op, int batch, const ConvConf
     // grouped: one tile per CTA and N tiles inside one span of input channels; GELU: only the one-tile kernel has it
     if (op.groups > 1 && (!span || span % cfg.bn || cfg.splits > 1)) return false;
     if ((op.groups > 1 || (r.relu & b2plan::kConvGelu)) && (cfg.ws || cfg.cn > 1 || cfg.halo)) return false;
+    // packed rows: only the one-tile kernel has the live-row instantiations, and it has no split-K with them
+    if ((op.flags & b2plan::kOpPacked) && (cfg.ws || cfg.cn > 1 || cfg.halo || cfg.splits > 1)) return false;
     if (cfg.halo == 2) {  // one CTA owns all of the 3x3's output channels, i.e. the whole K of the 1x1
         const int j = fuse_partner(c->e, int(&op - &c->e->ops[0]));
         const int R = conv_halo_rows(c, op), cblocks = int(r.cin_phys) / 64;
@@ -1015,7 +1073,9 @@ ConvConfig forced_conv_config(const b2_context* c, const Op& op, int batch) {
     const int M = batch * int(c->e->tensors[r.out].h * c->e->tensors[r.out].w);
     const int kbsz = conv_kb(c, op), nkb = conv_num_kblocks(c, op);
     ConvConfig cfg = pick_conv_config(M, int(r.cout_phys), nkb, kbsz, r.res >= 0, c, true, op.group_span());
-    if (cfg.bn == 0) cfg = pick_conv_config(M, int(r.cout_phys), nkb, kbsz, r.res >= 0, c, false, op.group_span());
+    // (a packed layer has no split-K: a forced split count is dropped there)
+    if (cfg.bn == 0 || ((op.flags & b2plan::kOpPacked) && cfg.splits > 1))
+        cfg = pick_conv_config(M, int(r.cout_phys), nkb, kbsz, r.res >= 0, c, false, op.group_span());
     if (cfg.bn == 0) return cfg;
     auto force = [&](auto set) {
         ConvConfig t = cfg;
@@ -1094,7 +1154,7 @@ int make_conv_launch(b2_context* c, const Op& op, int batch, const ConvConfig& c
     a.wpacked = (r.relu & 2) ? w : nullptr;
     // (GELU layers are always read as a plain matrix: their kernel exists for that operand path only)
     const bool tiled = r.k == 1 && op.kw() == 1 && r.stride == 1 && op.sw() == 1 && r.pad_ == 0 && op.pw_lo() == 0 &&
-                       op.pw_hi() == 0 && kb64 && (!c->force_im2col || gelu);
+                       op.pw_hi() == 0 && kb64 && (!c->force_im2col || gelu || (op.flags & b2plan::kOpPacked));
     a.a_mode = tiled ? b2k::A_TILED : b2k::A_IM2COL;
     if (cfg.halo) {
         const int R = conv_halo_rows(c, op);
@@ -1701,6 +1761,13 @@ int build_plan(b2_context* c, int batch, Plan** out) {
         const Tensor& t = e->tensors[ti];
         return t.binding >= 0 ? nullptr : c->scratch + t.offset;
     };
+    // packed plans: the packing index at this batch, pos_map [batch * S] then seq_off [batch + 1] (seq_off[batch] = T)
+    int* pos_map = nullptr;
+    int* seq_off = nullptr;
+    if (e->pack_tensor >= 0) {
+        pos_map = reinterpret_cast<int*>(tptr(e->pack_tensor));
+        seq_off = pos_map + size_t(batch) * (e->tensors[size_t(e->pack_tensor)].c - 2);
+    }
     for (const Op& op : e->ops) {
         const b2plan::OpRec& r = op.r;
         Launch L;
@@ -1740,7 +1807,8 @@ int build_plan(b2_context* c, int batch, Plan** out) {
             }
             case b2plan::OP_OUTPUT_CAST: {
                 const Tensor& t = e->tensors[r.in];
-                L.kind = t.scale > 0.f ? L_OUTPUT_CAST_I8 : (op.flags & 1) ? L_OUTPUT_ROWS : L_OUTPUT_CAST;
+                L.kind = t.scale > 0.f ? L_OUTPUT_CAST_I8 : (op.flags & b2plan::kOpPacked) ? L_OUTPUT_UNPACK : (op.flags & 1) ? L_OUTPUT_ROWS : L_OUTPUT_CAST;
+                if (L.kind == L_OUTPUT_UNPACK) L.pos_map = pos_map;
                 if (L.kind == L_OUTPUT_ROWS && !half) return fail(B2_EINVAL, "output cast %s: channels-last outputs need an fp16 engine", op.name.c_str());
                 L.qscale = t.scale;
                 L.in = tptr(r.in);
@@ -1789,7 +1857,8 @@ int build_plan(b2_context* c, int batch, Plan** out) {
                     // A grouped layer is never a member: it ends a run
                     const bool net_ok = c->net && !forced && conv_kb(c, op) == 64 && (r.relu & 2) && r.cout_phys % 64 == 0 &&
                                         c->force_ws <= 0 && c->force_cn <= 0 && c->force_halo <= 0 && !c->force_im2col && op.groups == 1 &&
-                                        !(r.relu & b2plan::kConvGelu);  // (the network kernel's epilogue has no GELU)
+                                        !(r.relu & b2plan::kConvGelu) &&  // (the network kernel's epilogue has no GELU ...
+                                        !(op.flags & b2plan::kOpPacked);    // ... and no live-row count)
                     if (net_ok) {
                         int bn = (r.cout_phys % 128 == 0) ? 128 : 64;
                         if (c->net_bn == 64) bn = 64;
@@ -1814,6 +1883,8 @@ int build_plan(b2_context* c, int batch, Plan** out) {
                     if (op.side_join >= 0 && cfg.splits > 1) cfg.splits = 1;  // forced / cached tactic on a side-branch op
                     int rc = make_conv_launch(c, op, batch, cfg, &L.conv);
                     if (rc) return rc;
+                    // packed rows: tiles past the live row count T skip their work (the tuner times the same tactic on all rows)
+                    if (op.flags & b2plan::kOpPacked) L.conv.args.live_rows = seq_off + batch, L.conv.args.live = 1;
                 } else {
                     L.kind = L_CONV_SIMT;
                     b2k::SimtConvArgs& a = L.simt;
@@ -1890,7 +1961,8 @@ int build_plan(b2_context* c, int batch, Plan** out) {
                 a.gamma = reinterpret_cast<const float*>(e->d_payload + r.b_off);
                 a.beta = a.gamma + to.c;
                 a.out = reinterpret_cast<__half*>(tptr(r.out));
-                a.mask_add = reinterpret_cast<float*>(tptr(op.out2));
+                if (op.flags & b2plan::kOpPacked) a.pack = reinterpret_cast<int*>(tptr(op.out2));
+                else a.mask_add = reinterpret_cast<float*>(tptr(op.out2));
                 a.N = batch, a.S = int(to.w), a.C = int(to.c), a.C_phys = int(to.c_phys);
                 a.vocab = op.vocab, a.positions = op.positions, a.types = op.types, a.eps = op.eps;
                 L.bytes = double(batch) * (to.item_bytes + to.w * (12.0 + 3.0 * to.c * 2));
@@ -1902,6 +1974,7 @@ int build_plan(b2_context* c, int batch, Plan** out) {
                 L.in = tptr(r.in), L.out = tptr(r.out);
                 L.bias = reinterpret_cast<const float*>(e->d_payload + r.b_off);
                 L.H = int(ti.h) * int(ti.w), L.C = int(ti.c), L.C_phys = int(ti.c_phys), L.eps = op.eps;
+                if (op.flags & b2plan::kOpPacked) L.live = seq_off + batch;
                 L.bytes = 2.0 * batch * ti.item_bytes;
                 break;
             }
@@ -1910,7 +1983,8 @@ int build_plan(b2_context* c, int batch, Plan** out) {
                 const Tensor& to = e->tensors[r.out];
                 L.kind = L_ATTENTION;
                 b2k::AttnLaunch& a = L.attn;
-                a.mask_add = reinterpret_cast<const float*>(tptr(r.res));
+                if (op.flags & b2plan::kOpPacked) a.seq_off = seq_off;  // the variable-length kernels
+                else a.mask_add = reinterpret_cast<const float*>(tptr(r.res));
                 a.out = reinterpret_cast<__half*>(tptr(r.out));
                 a.N = batch, a.S = int(ti.w), a.heads = op.heads, a.H = int(to.c), a.out_pitch = int(to.c_phys);
                 int rc = make_map_2d(&a.mapQKV, tptr(r.in), ti.c_phys, uint64_t(batch) * ti.w, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B);
@@ -1929,6 +2003,7 @@ int build_plan(b2_context* c, int batch, Plan** out) {
                 L.w = e->d_payload + r.w_off;
                 L.bias = reinterpret_cast<const float*>(e->d_payload + r.b_off);
                 L.W = int(ti.w), L.C = int(ti.c), L.C_phys = int(ti.c_phys);
+                if (op.flags & b2plan::kOpPacked) L.pos_map = pos_map;
                 L.flops = 2.0 * batch * ti.c * ti.c;
                 L.bytes = double(r.w_bytes) + double(batch) * (ti.c * 2.0 + to.item_bytes);
                 break;
@@ -2008,15 +2083,18 @@ int run_launch(const b2_engine* e, const Launch& L, void* const* bindings, cudaS
         }
         case L_LAYERNORM:
             return b2k::launch_layernorm(static_cast<const __half*>(in), static_cast<__half*>(out), L.bias, L.bias + L.C,
-                                         static_cast<long long>(L.N) * L.H, L.C, L.C_phys, L.eps, s);
+                                         static_cast<long long>(L.N) * L.H, L.C, L.C_phys, L.eps, L.live, s);
         case L_ATTENTION:
             return b2k::launch_attention(L.attn, s);
         case L_POOLER:
             return b2k::launch_pooler(static_cast<const __half*>(in), static_cast<const __half*>(L.w), L.bias, static_cast<float*>(out), L.N,
-                                      L.W, L.C, L.C_phys, s);
+                                      L.W, L.C, L.C_phys, L.pos_map, s);
         case L_OUTPUT_ROWS:
             return b2k::launch_output_cast_rows(static_cast<const __half*>(in), static_cast<float*>(out), static_cast<long long>(L.N) * L.H * L.W,
                                                 L.C, L.C_phys, s);
+        case L_OUTPUT_UNPACK:
+            return b2k::launch_output_unpack_rows(static_cast<const __half*>(in), static_cast<float*>(out), L.pos_map,
+                                                  static_cast<long long>(L.N) * L.H * L.W, L.C, L.C_phys, s);
     }
     return int(cudaErrorInvalidValue);
 }
@@ -2116,11 +2194,14 @@ bool patch_layout(const b2_engine* e, const Launch& L, BindPatch* p) {
         case L_EMBED_LN:                                                    // embed_ln_kernel(ids, segs, mask, args)
             p->n_params = 4, p->slots = {{0, L.in_binding}, {1, L.in_binding2}, {2, L.in_binding3}};
             return true;
-        case L_POOLER:                                                      // pooler_kernel(h, w, b, out, N, S, C, C_phys)
-            p->n_params = 8, p->slots = {{3, L.out_binding}};
+        case L_POOLER:                                                      // pooler_kernel(h, w, b, out, N, S, C, C_phys, pos_map)
+            p->n_params = 9, p->slots = {{3, L.out_binding}};
             return true;
         case L_OUTPUT_ROWS:                                                 // output_cast_rows_kernel(src, dst, rows, C, C_phys)
             p->n_params = 5, p->slots = {{1, L.out_binding}};
+            return true;
+        case L_OUTPUT_UNPACK:                                               // output_unpack_rows_kernel(src, dst, pos_map, rows, C, C_phys)
+            p->n_params = 6, p->slots = {{1, L.out_binding}};
             return true;
         default:
             return false;
@@ -2842,8 +2923,9 @@ const char* b2_context_launch_name(b2_context* c, int batch, int i) {
     if (!L) return nullptr;
     static const char* kinds[] = {"input_cast", "conv_tcgen05", "conv_simt", "maxpool", "avgpool", "fc", "softmax", "output_cast", "net_tcgen05", "tail_pool_fc_softmax",
                                   "quantize", "conv_i8_tcgen05", "avgpool_i8", "output_cast_i8", "embed_ln", "layernorm", "attention_f16_wgmma",
-                                  "pooler", "output_cast_rows"};
-    s = std::string(kinds[L->kind]) + (L->kind == L_ATTENTION && L->attn.S > 128 ? "_ks" : "") + ":" + L->name;  // key-split kernel
+                                  "pooler", "output_cast_rows", "output_unpack_rows"};
+    s = std::string(kinds[L->kind]) + (L->kind == L_ATTENTION && L->attn.S > 128 ? "_ks" : "") +  // key-split kernel
+        (L->kind == L_ATTENTION && L->attn.seq_off ? "_varlen" : "") + ":" + L->name;         // variable-length kernel
     if (L->kind == L_CONV_TC)
         s += " bn=" + std::to_string(L->conv.bn) + " kb=" + std::to_string(L->conv.kb) +
              " st=" + std::to_string(L->conv.stages) + "x" + std::to_string(L->conv.sps) +
@@ -2854,7 +2936,7 @@ const char* b2_context_launch_name(b2_context* c, int batch, int i) {
              " grid=" + std::to_string(L->conv.grid_n) + "x" + std::to_string(L->conv.grid_m) + "x" +
              std::to_string(L->conv.args.splits) + " kblk=" + std::to_string(L->conv.args.num_kblocks) +
              (L->conv.args.group_span ? " span=" + std::to_string(L->conv.args.group_span) : std::string()) +
-             ((L->conv.args.relu & b2plan::kConvGelu) ? " gelu" : "");
+             ((L->conv.args.relu & b2plan::kConvGelu) ? " gelu" : "") + (L->conv.args.live ? " live" : "");
     if (L->kind == L_CONV_I8)
         s += " bn=" + std::to_string(L->i8.bn) + " st=" + std::to_string(L->i8.stages) + (L->i8.args.a_mode == b2k::A_TILED ? " tiled" : " im2col") + " grid=" +
              std::to_string(L->i8.grid_n) + "x" + std::to_string(L->i8.grid_m) + " kblk=" + std::to_string(L->i8.args.num_kblocks);

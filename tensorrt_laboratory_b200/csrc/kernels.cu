@@ -72,12 +72,18 @@ struct FragPos {
 // GELU: the epilogue applies GELU (erf form) after bias and residual instead of the optional ReLU.  Instantiated for the
 // tiled, packed-weight operand path only (AV == 2: the 1x1 layers of transformer encoders); the other instantiations keep
 // the ReLU-only epilogue unchanged.
-template <int BN, int KB, int STAGES, int SPS, int CN = 1, bool DBG = false, int AV = 0, bool GELU = false>
+// LIVE (AV == 2, no split-K): packed transformer rows.  Only the first *p.live_rows of the M rows are in use, a count an
+// earlier kernel of the same request wrote, so the grid is sized for all M rows and a tile whose first row is at or past
+// the count does no work.  Each role reads the count after its own pdl_wait(): the weight producer streams the first ring
+// pass before it (constants) and issues nothing more for a dead tile; the activation producer then expects only those
+// weight bytes on the ring's barriers and waits for them to land, so the CTA never retires with bulk copies in flight.
+template <int BN, int KB, int STAGES, int SPS, int CN = 1, bool DBG = false, int AV = 0, bool GELU = false, bool LIVE = false>
 __global__ void __launch_bounds__(kConvThreads, conv_min_ctas(BN))
 conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
                  const __grid_constant__ CUtensorMap mapOut, const __grid_constant__ CUtensorMap mapRes,
                  const ConvArgs p) {
     static_assert(SPS == 1 || KB == 64, "multi-sub-block stages exist for the 64-wide K path only");
+    static_assert(!LIVE || AV == 2, "live-row instantiations exist for the tiled packed-weight path only");
     using Cfg = ConvCfg<BN, STAGES, SPS>;
     constexpr int TPS = 64 / KB;            // TMA sub-tiles per stage: 1 (KB=64), 2 (KB=32 row-folded stem), 8 (KB=8)
     constexpr int A_SUB = 128 * KB * 2;     // bytes of one A sub-tile
@@ -127,6 +133,7 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
         return rem < SPS ? rem : SPS;
     };
     const bool split = p.splits > 1;
+    bool dead = false;  // LIVE: this tile's rows are all past the live row count
     static_assert(AV == 0 || (KB == 64 && CN == 1 && !DBG), "resolved operand paths exist for the plain 64-wide K kernels");
     const bool a_tiled = AV == 2 ? true : (AV == 1 ? false : p.a_mode == A_TILED);
     const bool w_packed = AV != 0 ? true : p.wpacked != nullptr;
@@ -274,7 +281,7 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
             // per TMA instruction, which is what paces the main loop.
             constexpr bool kSplitProducers = KB == 64;
             const int npre = nk < STAGES ? nk : STAGES;
-            if (elect_one_sync()) {
+            if (!LIVE && elect_one_sync()) {
                 for (int i = 0; i < npre; ++i) {  // first ring pass: weights fly while the previous kernel drains
                     mbar_expect_tx(&full_bar[i], stage_bytes(kb_begin + i * SPS));
                     if (!kSplitProducers) load_b(kb_begin + i * SPS, i);
@@ -282,14 +289,23 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
             }
             __syncwarp();
             pdl_wait();
+            if constexpr (LIVE) {
+                dead = m0 >= *p.live_rows;
+                if (elect_one_sync())
+                    for (int i = 0; i < npre; ++i)
+                        mbar_expect_tx(&full_bar[i], dead ? static_cast<uint32_t>(subs_in_step(i) * Cfg::B_SUBBLK) : stage_bytes(kb_begin + i * SPS));
+                __syncwarp();
+                if (dead)
+                    for (int i = 0; i < npre; ++i) mbar_wait(&full_bar[i], 0);  // the weight copies of the first ring pass have landed
+            }
             if (dbg && lane == 0) dbg[2] = clock64();
-            if (elect_one_sync()) {
+            if (!dead && elect_one_sync()) {
                 for (int i = 0; i < npre; ++i) load_a(kb_begin + i * SPS, i);
                 if (has_res && !split) load_residual();
             }
             __syncwarp();
             long long tw = 0, te = 0, tl = 0;
-            for (int i = npre; i < nk; ++i) {
+            for (int i = npre; i < (dead ? 0 : nk); ++i) {
                 const int s = i % STAGES;
                 const uint32_t ph = (i / STAGES) & 1;
                 long long c0 = 0, c1 = 0, c3 = 0;
@@ -317,6 +333,11 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
     const bool consumer = warp < kConsumerWarps;
     float acc[BN / 2];
     if (consumer) {
+        if constexpr (LIVE) {
+            pdl_wait();
+            dead = m0 >= *p.live_rows;
+        }
+        const int nk_mma = dead ? 0 : nk;
         const uint32_t wg = static_cast<uint32_t>(cw >> 2);
         // one arrival per consumer warp (on every CTA of the cluster: a peer refills its slice of our stage)
         auto release_stage = [&](int st) {
@@ -330,7 +351,7 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
             }
         };
         long long mw = 0, mi = 0;
-        for (int i = 0; i < nk; ++i) {
+        for (int i = 0; i < nk_mma; ++i) {
             const int s = i % STAGES;
             const uint32_t ph = (i / STAGES) & 1;
             long long m0c = 0, m1c = 0;
@@ -379,7 +400,7 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
         }
         if constexpr (STAGES > 1) {
             wgmma_wait<0>();
-            if (nk > 0) release_stage((nk - 1) % STAGES);
+            if (nk_mma > 0) release_stage((nk_mma - 1) % STAGES);
         }
         if (dbg && cw == 0 && lane == 0) dbg[4] = clock64(), dbg[14] = mw, dbg[15] = mi;
     }
@@ -388,6 +409,12 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
         // ================= weight producer: constants, so no dependency wait; only the ring's empty barriers ====
         for (int i = 0; i < nk; ++i) {
             const int s = i % STAGES;
+            if constexpr (LIVE) {
+                if (i == STAGES) {  // the first ring pass is out; the rest only for a live tile
+                    pdl_wait();
+                    if (m0 >= *p.live_rows) break;
+                }
+            }
             if (i >= STAGES) mbar_wait(&empty_bar[s], ((i / STAGES) & 1) ^ 1);
             if (elect_one_sync()) load_b(kb_begin + i * SPS, s);
             __syncwarp();
@@ -397,6 +424,9 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
     // ====== epilogue (consumer warpgroups): registers -> bias/residual/ReLU -> fp16 -> swizzled smem tile -> TMA store ======
     pdl_wait();  // every global access below depends on the previous kernel
     __syncthreads();  // every role has left its loop: the pipeline buffers are free to become the output staging tile; s_bias visible
+    if constexpr (LIVE) {
+        if (m0 >= *p.live_rows) return;  // (every thread reads the same count: the whole CTA leaves together)
+    }
     if (dbg && threadIdx.x == 0) dbg[5] = clock64();  // (thread 0: consumer warp 0, lane 0)
     if (p.pdl_trigger == 1) pdl_launch_dependents();
     const FragPos fp(cw, lane);
@@ -1362,6 +1392,18 @@ static int launch_one(const ConvLaunch& L, cudaStream_t stream) {
     dim3 grid(L.grid_n, L.grid_m, L.args.splits);
     const size_t smem = size_t(conv_smem_layout_bytes(BN, STAGES, L.args.residual != nullptr, SPS));
     if (CN > 1 && (KB != 64 || L.grid_n % CN != 0 || L.args.cn != CN)) return static_cast<int>(cudaErrorInvalidValue);
+    if (L.args.live) {  // packed rows: the live-row instantiations of the tiled packed-weight kernel, no split-K
+        if constexpr (CN == 1 && KB == 64) {
+            if (L.args.wpacked != nullptr && L.args.a_mode == A_TILED && L.args.splits == 1 && L.args.dbg == nullptr && L.args.dbg_mode == 0) {
+                if (L.args.relu & 8)
+                    return launch_kernel_cluster(conv_f16_tcgen05<BN, KB, STAGES, SPS, 1, false, 2, true, true>, grid, dim3(kConvThreads), smem,
+                                                 stream, true, 1u, L.mapA, L.mapB, L.mapOut, L.mapRes, L.args);
+                return launch_kernel_cluster(conv_f16_tcgen05<BN, KB, STAGES, SPS, 1, false, 2, false, true>, grid, dim3(kConvThreads), smem,
+                                             stream, true, 1u, L.mapA, L.mapB, L.mapOut, L.mapRes, L.args);
+            }
+        }
+        return static_cast<int>(cudaErrorInvalidValue);
+    }
     if (L.args.relu & 8) {  // GELU: the tiled packed-weight instantiation, one CTA per cluster, no debug stamps
         if constexpr (CN == 1 && KB == 64) {
             if (L.args.wpacked != nullptr && L.args.a_mode == A_TILED && L.args.dbg == nullptr && L.args.dbg_mode == 0)
@@ -1407,6 +1449,8 @@ static int init_one() {
             if ((e = set_conv_smem(conv_f16_tcgen05<BN, KB, STAGES, SPS, 1, false, 1>, bytes))) return e;
             if ((e = set_conv_smem(conv_f16_tcgen05<BN, KB, STAGES, SPS, 1, false, 2>, bytes))) return e;
             if ((e = set_conv_smem(conv_f16_tcgen05<BN, KB, STAGES, SPS, 1, false, 2, true>, bytes))) return e;
+            if ((e = set_conv_smem(conv_f16_tcgen05<BN, KB, STAGES, SPS, 1, false, 2, false, true>, bytes))) return e;
+            if ((e = set_conv_smem(conv_f16_tcgen05<BN, KB, STAGES, SPS, 1, false, 2, true, true>, bytes))) return e;
         }
     }
     return set_conv_smem(conv_f16_tcgen05<BN, KB, STAGES, SPS, CN>, bytes);

@@ -34,7 +34,12 @@ struct ConvArgs {
     int splits;              // split-K factor (gridDim.z); 1 = none
     int kb_per_split;        // k-blocks per split
     float* workspace;        // splits > 1: [tile][split][128][BN] fp32 partial tiles
-    int* tile_counters;      // splits > 1: one arrival counter per output tile (zero between launches)
+    union {
+        int* tile_counters;      // splits > 1: one arrival counter per output tile (zero between launches)
+        const int* live_rows;    // live != 0 (packed transformer rows; tiled, packed weights, one tile per CTA, no split-K):
+                                 // device count of the rows in use, written by an earlier kernel; tiles starting at or past
+                                 // it do no work
+    };
     int pdl_trigger;         // 0: release the dependent kernel right after the prologue, 1: after the main loop
     const uint8_t* wpacked;  // KB==64: weights as pre-swizzled 4 KiB blocks [num_kblocks][Cout/32][32][128 B]; the BN-wide
                              // tile of one k-block is one contiguous cp.async.bulk (nullptr: fetch through mapB)
@@ -45,7 +50,10 @@ struct ConvArgs {
     long long* dbg;          // optional per-CTA phase timestamps (16 x int64 per CTA), nullptr in production
     int group_span;          // grouped convolution (KB==64, one tile per CTA): input channels an N tile reads, max(Cin/g, 64),
                              // starting at channel (n0 / group_span) * group_span; cblocks = group_span / 64.  0 = dense
+    int live;                // 1: the M rows are packed transformer rows and live_rows counts those in use (this field sits
+                             // in the struct's tail padding: the parameter layout of every kernel taking ConvArgs is unchanged)
 };
+static_assert(sizeof(ConvArgs) == 168, "ConvArgs layout");
 
 // The 1x1 / stride-1 convolution a fused bottleneck launch (ConvLaunch::halo == 2) runs on the 3x3's output, with residual
 struct Conv1x1Args {
@@ -247,28 +255,39 @@ struct EmbedArgs {
     const __half* tables;  // [vocab + positions + types][C] word, position, token-type rows
     const float* gamma;    // [C]
     const float* beta;     // [C]
-    __half* out;           // [N][S][C_phys]
-    float* mask_add;       // [N][S]: 0 or -10000
+    __half* out;           // [N][S][C_phys] (packed: [T][C_phys], the valid tokens in (item, position) order)
+    float* mask_add;       // [N][S]: 0 or -10000 (padded plans)
+    int* pack;             // packed plans (mask_add unused): the packing index, int32 [N*S] pos_map then [N + 1] seq_off --
+                           // pos_map[n*S + s] = packed row of token (n, s) or -1 where input_mask is 0, seq_off[n] = first
+                           // packed row of item n, seq_off[N] = T, the live row count.  nullptr: padded plan
     int N, S, C, C_phys, vocab, positions, types;
     float eps;
 };
 int launch_embed_ln(const EmbedArgs& a, cudaStream_t stream);
-// y = (x - mean) / sqrt(var + eps) * gamma + beta over the C channels of each row; fp32 statistics
+// y = (x - mean) / sqrt(var + eps) * gamma + beta over the C channels of each row; fp32 statistics.  live != nullptr: rows
+// at or past *live (a device count) are skipped
 int launch_layernorm(const __half* in, __half* out, const float* gamma, const float* beta, long long rows, int C, int C_phys,
-                     float eps, cudaStream_t stream);
+                     float eps, const int* live, cudaStream_t stream);
 // one CTA per (sequence, head, 64 query rows): S = QK^T * 0.125 + mask, softmax, O = P V (wgmma); S in {64, 128} on one
 // warpgroup, S in {256, 384, 512} on S / 128 warpgroups that split the keys (attention_f16_wgmma_ks)
 struct AttnLaunch {
     CUtensorMap mapQKV;    // 2-D tiled [N*S rows, 3H channels], box 64 x 64, 128B swizzle
-    const float* mask_add; // [N][S]
+    const float* mask_add; // [N][S] (padded plans)
     __half* out;           // [N*S][out_pitch]
     int N, S, heads, H, out_pitch;
+    // packed plans (variable-length kernels): seq_off [N + 1] of the packing index; item n is rows seq_off[n] ...
+    // seq_off[n + 1] - 1 of QKV and of out.  nullptr: padded plan
+    const int* seq_off;
 };
 int init_attention_kernels();
 int launch_attention(const AttnLaunch& L, cudaStream_t stream);
-// pooled[n][j] = tanh(b[j] + sum_k W[j][k] * h[n][0][k])   (h: [N][S][C_phys] fp16, W: [C][C] fp16, out fp32 [N][C])
-int launch_pooler(const __half* h, const __half* w, const float* b, float* out, int N, int S, int C, int C_phys, cudaStream_t stream);
+// pooled[n][j] = tanh(b[j] + sum_k W[j][k] * h[n][0][k])   (h: [N][S][C_phys] fp16, W: [C][C] fp16, out fp32 [N][C]).
+// pos_map != nullptr (packed plans): h[n][0] is packed row pos_map[n*S], and a masked position 0 pools a zero row
+int launch_pooler(const __half* h, const __half* w, const float* b, float* out, int N, int S, int C, int C_phys, const int* pos_map,
+                  cudaStream_t stream);
 // fp16 [rows][C_phys] -> fp32 [rows][C] (channels-last output binding)
 int launch_output_cast_rows(const __half* src, float* dst, long long rows, int C, int C_phys, cudaStream_t stream);
+// packed fp16 [T][C_phys] -> fp32 [N*S][C]: row n*S + s is packed row pos_map[n*S + s], or zeros where that is -1
+int launch_output_unpack_rows(const __half* src, float* dst, const int* pos_map, long long rows, int C, int C_phys, cudaStream_t stream);
 
 }  // namespace b2k

@@ -109,6 +109,21 @@ struct OpRecV2 {  // 192 bytes
 //     512 (S > 128 runs the key-split kernel).
 //   OP_POOLER: in = fp16 [N, 1, S, H]; out = fp32 vector [N, H]; w = fp16 [H][H] (row = output); b = fp32 [H].
 //   OP_OUTPUT_CAST: flags bit 0 = channels-last binding [H * W, C] instead of NCHW.
+// Packed (padding-free) transformer plans: flags bit 1 (kOpPacked) marks an op that works on packed rows -- the tokens
+// with input_mask != 0 of every item, in (item, position) order, T rows in all, T known only on the device.  Tensors keep
+// their [1, S, C] shape per item (the arena holds N * S rows); rows >= T hold no data.  A plan is packed when its
+// OP_EMBED_LN carries the bit; then it is the plan's only embedding, it comes before every other transformer op, and
+// every OP_CONV, OP_LAYERNORM, OP_ATTENTION, OP_POOLER and channels-last OP_OUTPUT_CAST carries the bit too (and no op
+// of an unpacked plan does):
+//   OP_EMBED_LN: out = packed rows; out2 = the packing index, a T_VEC of S + 2 32-bit words per item holding int32 (at
+//     batch N: pos_map [N * S] = packed row of token (n, s) or -1, then seq_off [N + 1] = first packed row of item n,
+//     seq_off[N] = T).  Position embeddings use the token's original position s.
+//   OP_CONV: a dense 1x1 stride-1 convolution with packed weights over [1, S, C] tensors; tiles past row T do no work.
+//   OP_LAYERNORM: rows >= T are not computed.
+//   OP_ATTENTION: res = the packing index (instead of the mask); item n attends over its own seq_off[n + 1] - seq_off[n]
+//     rows.
+//   OP_POOLER: pools packed row pos_map[n * S]; a masked position 0 pools a zero row (tanh(b)).
+//   OP_OUTPUT_CAST (flags bit 0 required): writes the [S, C] binding per item, row s from pos_map, zeros where it is -1.
 struct OpRecV3 {  // 224 bytes
     OpRec v1;
     uint32_t groups;
@@ -121,6 +136,7 @@ struct OpRecV3 {  // 224 bytes
     uint8_t reserved[8];
 };
 enum : uint32_t { kConvRelu = 1, kConvPacked = 2, kConvInt8 = 4, kConvGelu = 8 };
+enum : uint32_t { kOpRowsOut = 1, kOpPacked = 2 };  // OpRecV3::flags
 struct BindingRec {  // 128 bytes
     char name[64];
     uint32_t is_input;

@@ -9,6 +9,7 @@ examples/ONNX/resnet50/build.py:35-67).
   python tools/build_engine.py --model resnet50 --batch 8 --tune -o rn50_tuned.plan      (on a GPU box: tactics in the file)
   python tools/build_engine.py --model resnext50 --precision fp16 --batch 8 --tune -o rx50.plan  (ResNeXt-50 32x4d)
   python tools/build_engine.py --model bert-base --seq 128 --batch 16 [--weights bert.npz] --tune -o bert.plan  (fp16)
+  python tools/build_engine.py --model bert-base --seq 384 --batch 16 --remove-padding -o bert_packed.plan  (masked tokens skipped)
 Weights: deterministic synthetic weights (the reference's benchmark engines are weightless too, models/README.md:6-7),
 unless --caffemodel names a binary NetParameter (trtexec --model=...); MNIST and --onnx carry their own weights.
 --precision int8: post-training quantization, max-abs calibration on --calib (an .npy [N,C,H,W] fp32) or on synthetic images.
@@ -28,6 +29,8 @@ def main():
     ap.add_argument("--model", choices=["resnet50", "resnet152", "resnext50", "mnist", "bert-base"])
     ap.add_argument("--seq", type=int, default=128, help="bert-base: the sequence length of the plan (64, 128, 256, 384 or 512)")
     ap.add_argument("--weights", help="bert-base: .npz of Hugging Face BertModel parameters (default: seeded weights)")
+    ap.add_argument("--remove-padding", action="store_true",
+                    help="bert-base: a packed plan that computes only the tokens with input_mask != 0 (same bindings)")
     ap.add_argument("--prototxt")
     ap.add_argument("--onnx", help="ONNX CNN classifier (Conv / BatchNormalization / Relu / Add / MaxPool / AveragePool / "
                                    "GlobalAveragePool / Flatten / Reshape / Gemm / MatMul / Softmax), e.g. an ONNX-zoo ResNet")
@@ -51,8 +54,8 @@ def main():
     if a.model == "bert-base":  # its own builder: int32 token bindings, fp16 only
         from tensorrt_laboratory_b200 import bert
         cfg = bert.BertConfig(seq=a.seq)
-        blob = builder.build_bert_plan(cfg, a.weights, a.batch, seed=a.seed, precision=prec)
-        net = {"name": f"bert-base S={a.seq}"}
+        blob = builder.build_bert_plan(cfg, a.weights, a.batch, seed=a.seed, precision=prec, remove_padding=a.remove_padding)
+        net = {"name": f"bert-base S={a.seq}" + (" packed" if a.remove_padding else "")}
     elif a.prototxt:
         with open(a.prototxt) as f:
             net = graph.parse_prototxt(f.read())
