@@ -38,7 +38,8 @@ enum {
 enum { B2_DT_FLOAT = 0, B2_DT_HALF = 1, B2_DT_INT8 = 2, B2_DT_INT32 = 3 };
 
 /* engine arithmetic ("precision" of the plan, cf. trtexec --fp16) */
-enum { B2_PREC_FP32 = 0, B2_PREC_FP16 = 1, B2_PREC_INT8 = 2 /* INT8 bottleneck convolutions, fp16 stem / classifier */ };
+enum { B2_PREC_FP32 = 0, B2_PREC_FP16 = 1, B2_PREC_INT8 = 2 /* INT8 bottleneck convolutions, fp16 stem / classifier */,
+       B2_PREC_FP8 = 3 /* FP8 (E4M3) bottleneck convolutions, fp16 stem / classifier */ };
 
 typedef struct b2_runtime b2_runtime;
 typedef struct b2_engine b2_engine;

@@ -14,7 +14,7 @@ import numpy as np
 
 from . import graph as G
 
-PREC_FP32, PREC_FP16, PREC_INT8 = 0, 1, 2
+PREC_FP32, PREC_FP16, PREC_INT8, PREC_FP8 = 0, 1, 2, 3
 OP_INPUT_CAST, OP_CONV, OP_MAXPOOL, OP_AVGPOOL, OP_FC, OP_SOFTMAX, OP_OUTPUT_CAST, OP_QUANTIZE = range(8)
 OP_EMBED_LN, OP_LAYERNORM, OP_ATTENTION, OP_POOLER = range(8, 12)   # transformer ops (version-3 plans)
 CONV_RELU, CONV_PACKED, CONV_INT8, CONV_GELU = 1, 2, 4, 8            # OpRec.relu bits of a convolution
@@ -145,13 +145,16 @@ def build_plan(lowered: dict, precision: int = PREC_FP16, max_batch: int = 8,
     ``outputs``: tensor names to expose as output bindings (default: the graph output).  4-D activation
     outputs get an ``OUTPUT_CAST`` to fp32 NCHW; vector outputs (fc / softmax) are written in place.
     """
-    if precision not in (PREC_FP32, PREC_FP16, PREC_INT8):
-        raise ValueError("precision must be PREC_FP32, PREC_FP16 or PREC_INT8")
+    if precision not in (PREC_FP32, PREC_FP16, PREC_INT8, PREC_FP8):
+        raise ValueError("precision must be PREC_FP32, PREC_FP16, PREC_INT8 or PREC_FP8")
     int8 = precision == PREC_INT8
     if int8 != bool(lowered.get("int8")):
         raise ValueError("PREC_INT8 takes a graph quantized by quantize.quantize_lowered (and only that precision does)")
-    tscale = lowered.get("tensor_scales", {})   # INT8 tensors: name -> scale
-    if int8:  # the fp16 part of an INT8 engine follows the fp16 engine's layout rules
+    if (precision == PREC_FP8) != bool(lowered.get("fp8")):
+        raise ValueError("PREC_FP8 takes a graph quantized by quantize.quantize_lowered(..., fmt='e4m3') (and only that "
+                         "precision does)")
+    tscale = lowered.get("tensor_scales", {})   # 1-byte (INT8 / FP8) tensors: name -> scale
+    if precision in (PREC_INT8, PREC_FP8):  # the fp16 part of an INT8 / FP8 engine follows the fp16 engine's layout rules
         precision_fp = PREC_FP16
     else:
         precision_fp = precision
@@ -169,7 +172,7 @@ def build_plan(lowered: dict, precision: int = PREC_FP16, max_batch: int = 8,
         c, h, w = shapes[tname]
         if tname in vec_tensors:
             rec = dict(name=tname, kind=T_VEC, h=1, w=1, c=c * h * w, c_phys=c * h * w, binding=-1)
-        elif tname in tscale:  # INT8 activations: one 128-byte swizzle row = 128 channels
+        elif tname in tscale:  # 1-byte activations: one 128-byte swizzle row = 128 channels
             rec = dict(name=tname, kind=T_ACT, h=h, w=w, c=c, c_phys=_roundup(c, 128), binding=-1, scale=float(np.float32(tscale[tname])))
         else:
             rec = dict(name=tname, kind=T_ACT, h=h, w=w, c=c, c_phys=phys_channels(c, precision_fp), binding=-1)
@@ -218,12 +221,12 @@ def build_plan(lowered: dict, precision: int = PREC_FP16, max_batch: int = 8,
         rec = dict(name=op["name"], inp=ti, res=-1, out=to, binding=-1)
         if t == "quantize":
             rec.update(type=OP_QUANTIZE)
-        elif t == G.OP_CONV and op.get("int8"):
+        elif t == G.OP_CONV and (op.get("int8") or op.get("fp8")):
             cin_phys, cout_phys = tensors[ti]["c_phys"], tensors[to]["c_phys"]
             k = op["k"]
             taps = k * k
-            Wq = np.zeros((cout_phys, taps, cin_phys), dtype=np.int8)
-            Wq[:op["cout"], :, :op["cin"]] = op["Wq"].reshape(op["cout"], taps, op["cin"])
+            Wq = np.zeros((cout_phys, taps, cin_phys), dtype=np.int8)   # E4M3 codes travel as their bytes; 0x00 is +0
+            Wq[:op["cout"], :, :op["cin"]] = op["Wq"].view(np.int8).reshape(op["cout"], taps, op["cin"])
             w_off, w_bytes = add_payload(pack_weights_sw128_i8(Wq.reshape(cout_phys, taps * cin_phys)))
             rq = np.zeros(2 * cout_phys + 4, dtype=np.float32)   # [m | b | r 0 0 0]; padded channels requantise to 0
             rq[:op["cout"]] = op["m"]
@@ -391,6 +394,8 @@ def build_bert_plan(cfg=None, weights=None, max_batch: int = 16, seed: int = 0, 
         raise ValueError("BERT plans are fp16 only: the attention, LayerNorm and embedding kernels exist for fp16 activations")
     if precision == PREC_INT8:
         raise ValueError("BERT plans are fp16 only: INT8 BERT (quantised GEMMs and attention) is not implemented")
+    if precision == PREC_FP8:
+        raise ValueError("BERT plans are fp16 only: FP8 BERT (quantised GEMMs and attention) is not implemented")
     if precision != PREC_FP16:
         raise ValueError("precision must be PREC_FP16")
     S, H, F = cfg.seq, cfg.hidden, cfg.ffn
@@ -492,14 +497,15 @@ def build_resnext_plan(depth: int = 50, precision: int = PREC_FP16, max_batch: i
 
 def build_resnet_plan(depth: int = 50, precision: int = PREC_FP16, max_batch: int = 8, seed: int = 0,
                       input_dtype: str = "f32", calib_batch: int = 8) -> bytes:
-    """Convenience: generated Caffe-v1 ResNet + deterministic weights -> plan.  PREC_INT8: post-training quantization
-    calibrated (max-abs) on ``calib_batch`` synthetic images (seed 4321), see quantize.py."""
+    """Convenience: generated Caffe-v1 ResNet + deterministic weights -> plan.  PREC_INT8 / PREC_FP8: post-training
+    quantization calibrated (max-abs) on ``calib_batch`` synthetic images (seed 4321), see quantize.py."""
     from . import weights as Wt
     net = G.resnet_caffe(depth)
     low = G.lower(net, Wt.random_weights(net, seed))
-    if precision == PREC_INT8:
+    if precision in (PREC_INT8, PREC_FP8):
         from . import quantize
-        low = quantize.quantize_lowered(low, Wt.synthetic_input(calib_batch, seed=4321))
+        low = quantize.quantize_lowered(low, Wt.synthetic_input(calib_batch, seed=4321),
+                                        fmt="e4m3" if precision == PREC_FP8 else "int8")
     return build_plan(low, precision, max_batch, input_dtype=input_dtype)
 
 

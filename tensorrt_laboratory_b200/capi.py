@@ -108,6 +108,7 @@ SYMBOLS = [
 ]
 
 NP_DTYPES = {0: np.float32, 1: np.float16, 2: np.int8, 3: np.int32}  # B2_DT_* (same order as utils.cc:40-46)
+PRECISIONS = {0: "fp32", 1: "fp16", 2: "int8", 3: "fp8"}  # B2_PREC_* (b200infer.h): what Engine.precision_name reports
 BENCH_KEYS = ["kMaxExecConcurrency", "kMaxCopyConcurrency", "kBatchSize", "kWalltime", "kBatchesComputed",
               "kBatchesPerSecond", "kInferencesPerSecond", "kSecondsPerBatch", "kExecutionTimePerBatch",
               "kLatencyP50", "kLatencyP90", "kLatencyP99", "kLatencyMax", "kGpuComputeTimePerBatch"]
@@ -282,6 +283,7 @@ class Engine:
         self.name = lib.b2_engine_name(self.handle).decode(errors="replace")
         self.max_batch = lib.b2_engine_max_batch(self.handle)
         self.precision = lib.b2_engine_precision(self.handle)
+        self.precision_name = PRECISIONS[self.precision]
         self.bindings: List[dict] = []
         for i in range(lib.b2_engine_nb_bindings(self.handle)):
             dims = (C.c_int32 * 8)()

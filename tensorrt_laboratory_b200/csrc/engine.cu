@@ -96,7 +96,7 @@ struct Tensor {
     std::string name;
     uint32_t kind, h, w, c, c_phys;
     int binding;
-    float scale = 0.f;      // > 0: int8 tensor (INT8 engines), real value = q * scale
+    float scale = 0.f;      // > 0: 1-byte tensor (int8 in INT8 engines, e4m3 in FP8 engines), real value = q * scale
     size_t item_bytes = 0;  // bytes per batch item
     size_t offset = 0;      // arena offset (binding < 0)
     int def = -1, last_use = -1;
@@ -141,7 +141,8 @@ struct Binding {
 };
 
 enum LKind { L_INPUT_CAST, L_CONV_TC, L_CONV_SIMT, L_MAXPOOL, L_AVGPOOL, L_FC, L_SOFTMAX, L_OUTPUT_CAST, L_NET, L_TAIL, L_QUANTIZE, L_CONV_I8, L_AVGPOOL_I8, L_OUTPUT_CAST_I8,
-             L_EMBED_LN, L_LAYERNORM, L_ATTENTION, L_POOLER, L_OUTPUT_ROWS, L_OUTPUT_UNPACK };
+             L_EMBED_LN, L_LAYERNORM, L_ATTENTION, L_POOLER, L_OUTPUT_ROWS, L_OUTPUT_UNPACK, L_QUANTIZE_F8, L_CONV_F8, L_AVGPOOL_F8,
+             L_OUTPUT_CAST_F8 };
 
 // A run of consecutive tcgen05 convolution layers executed by ONE persistent kernel (net_kernel.cu): device-side layer
 // table, dependency ranges and arrival counters live in one allocation owned by the plan.
@@ -171,9 +172,9 @@ struct Launch {
     int side_join = -1;     // see Op::side_join (launch index == op index)
     std::shared_ptr<NetRun> net;  // L_NET
     b2k::TailArgs tail{};         // L_TAIL: pool + fc + softmax in one launch (out = the output binding)
-    b2k::I8ConvLaunch i8{};       // L_CONV_I8
-    float qscale = 0.f;           // L_QUANTIZE: 1/s; L_AVGPOOL_I8: s/HW; L_OUTPUT_CAST_I8: s
-    int C_in_phys = 0;            // L_QUANTIZE / L_AVGPOOL_I8: channel pitch of the source tensor
+    b2k::I8ConvLaunch i8{};       // L_CONV_I8 / L_CONV_F8
+    float qscale = 0.f;           // L_QUANTIZE(_F8): 1/s; L_AVGPOOL_I8 / _F8: s/HW; L_OUTPUT_CAST_I8 / _F8: s
+    int C_in_phys = 0;            // L_QUANTIZE(_F8) / L_AVGPOOL_I8 / _F8: channel pitch of the source tensor
     bool net_member = false;      // L_CONV_TC that build_plan folds into an L_NET launch
     b2k::EmbedArgs embed{};       // L_EMBED_LN (ids / segs / mask are the bindings in_binding, in_binding2, in_binding3)
     int in_binding2 = -1, in_binding3 = -1;
@@ -276,12 +277,13 @@ struct b2_engine {
     std::mutex tune_run_mutex;  // serialises on-device tactic timing across contexts of this engine
     std::map<std::pair<int, int>, ConvConfig> tuned;  // (op index, batch) -> measured-best configuration
     bool tune_cache_loaded = false;
-    std::map<int, float> requant_r;  // INT8 convs: op index -> r = fl(s_res / s_out) (read from the plan's requantisation block)
+    std::map<int, float> requant_r;  // 1-byte convs: op index -> r = fl(s_res / s_out) (read from the plan's requantisation block)
     bool tactics_from_plan = false;  // the blob carried a tactic table: nothing left to tune
     bool tuned_at_load = false;      // b2_engine_tune has run
     int pack_tensor = -1;            // packed transformer plans: the packing index (out2 of the packed OP_EMBED_LN), else -1
-    bool half() const { return precision != B2_PREC_FP32; }  // fp16 storage and kernels (INT8 engines: their fp16 part)
-    bool int8() const { return precision == B2_PREC_INT8; }
+    bool half() const { return precision != B2_PREC_FP32; }  // fp16 storage and kernels (INT8 / FP8 engines: their fp16 part)
+    bool one_byte() const { return precision == B2_PREC_INT8 || precision == B2_PREC_FP8; }  // has 1-byte tensors and convolutions
+    bool fp8() const { return precision == B2_PREC_FP8; }  // ... whose element format is E4M3 (else int8)
 };
 
 struct b2_context {
@@ -318,7 +320,7 @@ struct b2_context {
     int net_ctas = 0;  // CTAs of that kernel (0 = one per SM); a server running N contexts gives each about 1 / N of the SMs
     int net_bn = 0;    // force its N tile (64 / 128); 0 = 128 wherever the channel count allows
     int net_stages = 0;  // force its shared-memory ring depth (2..4); 0 = the deepest that lets two CTAs share an SM
-    int i8_bn = 0;       // INT8 convolutions: force the N tile (128 / 256); 0 = 128
+    int i8_bn = 0;       // 1-byte (INT8 / FP8) convolutions: force the N tile (128 / 256); 0 = 128
     int i8_stages = 0;   // ... and the shared-memory ring depth (2..4); 0 = by rule
     int fuse_tail = 1;   // global average pool + FC + softmax as one launch (tail_f16_kernel)
     int input_ctas = 0;  // grid cap of the input cast (0 = none); set when the input binding is read over PCIe (zero-copy)
@@ -458,7 +460,7 @@ int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** pa
     if (memcmp(h.magic, kMagic, 8) != 0) return fail(B2_EINVAL, "plan: bad magic (not a B2ENGINE blob)");
     if (h.version != kVersion && h.version != kVersionGrouped && h.version != kVersionTransformer)
         return fail(B2_EINVAL, "plan: version %u, this library reads %u, %u and %u", h.version, kVersion, kVersionGrouped, kVersionTransformer);
-    if (h.precision > 2) return fail(B2_EINVAL, "plan: unknown precision %u", h.precision);
+    if (h.precision > B2_PREC_FP8) return fail(B2_EINVAL, "plan: unknown precision %u", h.precision);
     if (h.max_batch == 0 || h.max_batch > 4096) return fail(B2_EINVAL, "plan: bad max_batch %u", h.max_batch);
     const bool v3 = h.version == kVersionTransformer;
     const size_t op_rec_size = v3 ? sizeof(OpRecV3) : h.version == kVersionGrouped ? sizeof(OpRecV2) : sizeof(OpRec);
@@ -473,6 +475,10 @@ int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** pa
     e->max_batch = h.max_batch;
     e->payload_bytes = h.payload_bytes;
     const size_t elt = h.precision == B2_PREC_FP32 ? 4 : 2;
+    // INT8 and FP8 plans share the rules of their 1-byte part; only the element format (and the messages) differ
+    const bool one_byte = h.precision == B2_PREC_INT8 || h.precision == B2_PREC_FP8;
+    const char* qfmt = h.precision == B2_PREC_FP8 ? "fp8" : "int8";
+    const char* qFMT = h.precision == B2_PREC_FP8 ? "FP8" : "INT8";
     const uint8_t* p = base + sizeof(Header);
     for (uint32_t i = 0; i < h.n_tensors; ++i, p += sizeof(TensorRec)) {
         TensorRec r;
@@ -482,9 +488,9 @@ int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** pa
         t.kind = r.kind;
         t.h = r.h, t.w = r.w, t.c = r.c, t.c_phys = r.c_phys;
         t.binding = r.binding;
-        t.scale = h.precision == B2_PREC_INT8 ? r.scale : 0.f;
+        t.scale = one_byte ? r.scale : 0.f;
         if (!(t.scale >= 0.f) || (t.scale > 0.f && (r.kind != T_ACT || r.c_phys % 128)))
-            return fail(B2_EINVAL, "plan: tensor %s has a bad INT8 scale / layout", t.name.c_str());
+            return fail(B2_EINVAL, "plan: tensor %s has a bad %s scale / layout", t.name.c_str(), qFMT);
         if (r.kind == T_ACT) {
             if (r.c_phys < r.c || r.h == 0 || r.w == 0) return fail(B2_EINVAL, "plan: tensor %s has bad dims", t.name.c_str());
             t.item_bytes = size_t(r.h) * r.w * r.c_phys * (t.scale > 0.f ? 1 : elt);
@@ -552,8 +558,8 @@ int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** pa
         if (r.type == OP_QUANTIZE) {
             const Tensor& ti = e->tensors[r.in];
             const Tensor& to = e->tensors[r.out];
-            if (h.precision != B2_PREC_INT8 || ti.scale > 0.f || !(to.scale > 0.f) || ti.h != to.h || ti.w != to.w || ti.c != to.c)
-                return fail(B2_EINVAL, "plan: quantize %s needs an fp16 input and an int8 output of the same shape", op.name.c_str());
+            if (!one_byte || ti.scale > 0.f || !(to.scale > 0.f) || ti.h != to.h || ti.w != to.w || ti.c != to.c)
+                return fail(B2_EINVAL, "plan: quantize %s needs an fp16 input and an %s output of the same shape", op.name.c_str(), qfmt);
         }
         if (r.type == OP_CONV) {
             if (r.k == 0 || r.stride == 0 || int(r.taps) != op.kh() * op.kw() || r.taps_phys < r.taps || op.sw() == 0)
@@ -563,10 +569,10 @@ int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** pa
             if ((r.relu & kConvGelu) && (r.k != 1 || r.kw || r.stride != 1 || r.pad_ || !(r.relu & kConvPacked) ||
                                          r.cin_phys % 64 || op.groups != 1))
                 return fail(B2_EINVAL, "plan: conv %s: GELU layers are dense 1x1 stride-1 convolutions with packed weights", op.name.c_str());
-            const bool i8 = (r.relu & 4) != 0;
+            const bool i8 = (r.relu & kConvInt8) != 0;  // a 1-byte convolution: int8, or e4m3 in an FP8 plan
             if (op.groups > 1) {  // layouts: plan_format.h (OpRecV2)
                 const uint32_t g = uint32_t(op.groups);
-                if (i8) return fail(B2_EINVAL, "plan: conv %s: INT8 grouped convolution is not supported", op.name.c_str());
+                if (i8) return fail(B2_EINVAL, "plan: conv %s: %s grouped convolution is not supported", op.name.c_str(), qFMT);
                 if (r.cin % g || r.cout % g)
                     return fail(B2_EINVAL, "plan: conv %s: %u groups do not divide %u -> %u channels", op.name.c_str(), g, r.cin, r.cout);
                 const uint32_t cpg = r.cin / g;
@@ -586,15 +592,15 @@ int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** pa
             } else if (i8) {
                 const Tensor& qi = e->tensors[r.in];
                 const Tensor& qo = e->tensors[r.out];
-                if (h.precision != B2_PREC_INT8 || !(qi.scale > 0.f) || !(qo.scale > 0.f) || (r.res >= 0 && !(e->tensors[r.res].scale > 0.f)) ||
+                if (!one_byte || !(qi.scale > 0.f) || !(qo.scale > 0.f) || (r.res >= 0 && !(e->tensors[r.res].scale > 0.f)) ||
                     r.cin_phys % 128 || r.cout_phys % 128 || r.taps_phys != r.taps || r.kw != 0 || !(r.relu & 2))
-                    return fail(B2_EINVAL, "plan: int8 conv %s: tensors must be int8 with 128-channel rows", op.name.c_str());
+                    return fail(B2_EINVAL, "plan: %s conv %s: tensors must be %s with 128-channel rows", qfmt, op.name.c_str(), qfmt);
                 if (r.w_bytes != size_t(r.cout_phys) * r.taps_phys * r.cin_phys || r.b_bytes != (size_t(r.cout_phys) * 2 + 4) * 4)
-                    return fail(B2_EINVAL, "plan: int8 conv %s weight / requantisation size mismatch", op.name.c_str());
+                    return fail(B2_EINVAL, "plan: %s conv %s weight / requantisation size mismatch", qfmt, op.name.c_str());
             } else if (r.w_bytes != size_t(r.cout_phys) * r.taps_phys * r.cin_phys * elt || r.b_bytes != size_t(r.cout_phys) * 4)
                 return fail(B2_EINVAL, "plan: conv %s weight size mismatch", op.name.c_str());
             if (!i8 && (e->tensors[r.in].scale > 0.f || e->tensors[r.out].scale > 0.f))
-                return fail(B2_EINVAL, "plan: fp16 conv %s touches an int8 tensor", op.name.c_str());
+                return fail(B2_EINVAL, "plan: fp16 conv %s touches an %s tensor", op.name.c_str(), qfmt);
             const Tensor& ti = e->tensors[r.in];
             const Tensor& to = e->tensors[r.out];
             if (ti.c_phys != r.cin_phys || to.c_phys != r.cout_phys || ti.c != r.cin || to.c != r.cout)
@@ -916,7 +922,7 @@ bool conv_on_tensor_cores(const b2_engine* e, const Op& op);
 // convolution with a residual, no GELU and no groups, whose input is i's output; that tensor is read by nothing else and
 // is not a binding.  Shapes only: whether the fused launch runs is a tactic (ConvConfig::halo == 2 on op i).
 int fuse_partner(const b2_engine* e, int i) {
-    if (!e->half() || e->int8() || i < 0 || size_t(i) + 1 >= e->ops.size()) return -1;
+    if (!e->half() || e->one_byte() || i < 0 || size_t(i) + 1 >= e->ops.size()) return -1;
     const Op &oi = e->ops[size_t(i)], &oj = e->ops[size_t(i) + 1];
     const b2plan::OpRec &ri = oi.r, &rj = oj.r;
     if (ri.type != b2plan::OP_CONV || rj.type != b2plan::OP_CONV || (ri.relu & (4 | b2plan::kConvGelu)) || conv_halo_rows(e, oi) == 0 ||
@@ -1412,13 +1418,16 @@ void tune_cache_append(const b2_engine* e, int op, int batch, const ConvConfig& 
     fclose(f);
 }
 
-// INT8 twin of autotune_conv: times every (N tile, ring depth) of conv_i8_tcgen05 on `c->autotune` concurrent streams.
+// 1-byte twin of autotune_conv: times every (N tile, ring depth) of conv_i8_tcgen05 / conv_f8_tcgen05 on `c->autotune`
+// concurrent streams.
 int autotune_i8_conv(b2_context* c, const Op& op, int batch, ConvConfig* best_out) {
     const b2plan::OpRec& r = op.r;
     TuneTimer tt(c);
     int status = tt.init();
     if (status) return status;
     const int verbose = env_int("B2_TUNE_VERBOSE", 0);
+    const bool fp8 = c->e->fp8();
+    const char* fmt = fp8 ? "fp8" : "int8";
     double best_ms = 1e30;
     ConvConfig best = *best_out;
     for (int bn : {128, 256}) {
@@ -1428,11 +1437,12 @@ int autotune_i8_conv(b2_context* c, const Op& op, int batch, ConvConfig* best_ou
             b2k::I8ConvLaunch cl;
             if ((status = make_i8_conv_launch(c, op, batch, bn, st, &cl))) return status;
             float ms = 0.f;
-            const cudaError_t err = tt.time([&](int, cudaStream_t s) { return b2k::launch_conv_i8_tcgen05(cl, s); }, &ms);
+            const cudaError_t err = tt.time(
+                [&](int, cudaStream_t s) { return fp8 ? b2k::launch_conv_f8_tcgen05(cl, s) : b2k::launch_conv_i8_tcgen05(cl, s); }, &ms);
             if (err != cudaSuccess)
-                return fail(B2_ECUDA, "autotune of %s (int8 bn=%d st=%d) failed: %s", op.name.c_str(), bn, st, cudaGetErrorString(err));
+                return fail(B2_ECUDA, "autotune of %s (%s bn=%d st=%d) failed: %s", op.name.c_str(), fmt, bn, st, cudaGetErrorString(err));
             if (verbose > 1)
-                fprintf(stderr, "[b2 tune]   %s b=%d cand int8 bn=%d st=%d : %.3f us/launch\n", op.name.c_str(), batch, bn, st,
+                fprintf(stderr, "[b2 tune]   %s b=%d cand %s bn=%d st=%d : %.3f us/launch\n", op.name.c_str(), batch, fmt, bn, st,
                         tt.us_per_launch(ms));
             if (ms < best_ms) best_ms = ms, best = ConvConfig{bn, st, 1, 0.0, 1, 0, 1};
         }
@@ -1441,8 +1451,8 @@ int autotune_i8_conv(b2_context* c, const Op& op, int batch, ConvConfig* best_ou
     if (verbose) {
         const Tensor& to = c->e->tensors[r.out];
         const long long M = (long long)batch * to.h * to.w, K = (long long)r.k * r.k * r.cin_phys;
-        fprintf(stderr, "[b2 tune] %s b=%d M=%lld N=%d K=%lld best int8 bn=%d st=%d : %.3f us/launch (%d streams) %.0f TOP/s\n",
-                op.name.c_str(), batch, M, int(r.cout_phys), K, best.bn, best.stages, best.est_us, tt.ns,
+        fprintf(stderr, "[b2 tune] %s b=%d M=%lld N=%d K=%lld best %s bn=%d st=%d : %.3f us/launch (%d streams) %.0f TOP/s\n",
+                op.name.c_str(), batch, M, int(r.cout_phys), K, fmt, best.bn, best.stages, best.est_us, tt.ns,
                 2.0 * M * r.cout_phys * K / best.est_us * 1e-6);
     }
     *best_out = best;
@@ -1457,7 +1467,7 @@ int tune_engine_batch(b2_context* c, int batch) {
         const Op& op = e->ops[i];
         const b2plan::OpRec& r = op.r;
         if (r.type != b2plan::OP_CONV || !e->half()) continue;
-        if (r.relu & 4) {  // INT8 convolution: (N tile, ring depth)
+        if (r.relu & 4) {  // 1-byte convolution: (N tile, ring depth)
             {
                 std::lock_guard<std::mutex> lock(e->tune_mutex);
                 if (e->tuned.count({int(i), batch})) continue;
@@ -1798,7 +1808,7 @@ int build_plan(b2_context* c, int batch, Plan** out) {
             case b2plan::OP_QUANTIZE: {
                 const Tensor& ti = e->tensors[r.in];
                 const Tensor& to = e->tensors[r.out];
-                L.kind = L_QUANTIZE;
+                L.kind = e->fp8() ? L_QUANTIZE_F8 : L_QUANTIZE;
                 L.in = tptr(r.in), L.out = tptr(r.out);
                 L.C = ti.c, L.H = ti.h, L.W = ti.w, L.C_in_phys = ti.c_phys, L.C_phys = to.c_phys;
                 L.qscale = float(1.0 / double(to.scale));
@@ -1807,7 +1817,7 @@ int build_plan(b2_context* c, int batch, Plan** out) {
             }
             case b2plan::OP_OUTPUT_CAST: {
                 const Tensor& t = e->tensors[r.in];
-                L.kind = t.scale > 0.f ? L_OUTPUT_CAST_I8 : (op.flags & b2plan::kOpPacked) ? L_OUTPUT_UNPACK : (op.flags & 1) ? L_OUTPUT_ROWS : L_OUTPUT_CAST;
+                L.kind = t.scale > 0.f ? (e->fp8() ? L_OUTPUT_CAST_F8 : L_OUTPUT_CAST_I8) : (op.flags & b2plan::kOpPacked) ? L_OUTPUT_UNPACK : (op.flags & 1) ? L_OUTPUT_ROWS : L_OUTPUT_CAST;
                 if (L.kind == L_OUTPUT_UNPACK) L.pos_map = pos_map;
                 if (L.kind == L_OUTPUT_ROWS && !half) return fail(B2_EINVAL, "output cast %s: channels-last outputs need an fp16 engine", op.name.c_str());
                 L.qscale = t.scale;
@@ -1825,8 +1835,8 @@ int build_plan(b2_context* c, int batch, Plan** out) {
                 const int M = batch * int(to.h) * int(to.w);
                 L.flops = 2.0 * M * r.cout * op.algo_k();
                 L.bytes = double(batch) * (ti.item_bytes + to.item_bytes * (r.res >= 0 ? 2 : 1)) + double(r.w_bytes);
-                if (r.relu & 4) {  // INT8 tensor path
-                    L.kind = L_CONV_I8;
+                if (r.relu & 4) {  // 1-byte tensor path
+                    L.kind = e->fp8() ? L_CONV_F8 : L_CONV_I8;
                     // one tactic, by rule: the 128-wide N tile with a ring no deeper than the K loop, shallow enough (2-3
                     // stages) that two CTAs share an SM (measured); "i8_bn" / "i8_stages" override
                     // tactic = (N tile, ring depth): timed at load (b2_engine_tune) or carried by the plan; untuned engines use
@@ -1915,10 +1925,10 @@ int build_plan(b2_context* c, int batch, Plan** out) {
             }
             case b2plan::OP_AVGPOOL: {
                 const Tensor& ti = e->tensors[r.in];
-                L.kind = ti.scale > 0.f ? L_AVGPOOL_I8 : L_AVGPOOL;
+                L.kind = ti.scale > 0.f ? (e->fp8() ? L_AVGPOOL_F8 : L_AVGPOOL_I8) : L_AVGPOOL;
                 L.in = tptr(r.in), L.out = tptr(r.out);
                 L.H = ti.h, L.W = ti.w, L.C_phys = ti.c_phys;
-                if (ti.scale > 0.f) {  // int8 in, fp16 out
+                if (ti.scale > 0.f) {  // 1-byte in, fp16 out
                     L.C = ti.c, L.C_in_phys = ti.c_phys, L.C_phys = e->tensors[r.out].c_phys;
                     L.qscale = float(double(ti.scale) / double(ti.h * ti.w));
                 }
@@ -2069,6 +2079,14 @@ int run_launch(const b2_engine* e, const Launch& L, void* const* bindings, cudaS
             return b2k::launch_avgpool_i8(in, out, L.N, L.H * L.W, L.C, L.C_in_phys, L.C_phys, L.qscale, s);
         case L_OUTPUT_CAST_I8:
             return b2k::launch_output_cast_i8(in, static_cast<float*>(out), L.N, L.C, L.H, L.W, L.C_phys, L.qscale, s);
+        case L_QUANTIZE_F8:
+            return b2k::launch_quantize_h_to_f8(in, out, static_cast<long long>(L.N) * L.H * L.W, L.C, L.C_in_phys, L.C_phys, L.qscale, s);
+        case L_CONV_F8:
+            return b2k::launch_conv_f8_tcgen05(L.i8, s);
+        case L_AVGPOOL_F8:
+            return b2k::launch_avgpool_f8(in, out, L.N, L.H * L.W, L.C, L.C_in_phys, L.C_phys, L.qscale, s);
+        case L_OUTPUT_CAST_F8:
+            return b2k::launch_output_cast_f8(in, static_cast<float*>(out), L.N, L.C, L.H, L.W, L.C_phys, L.qscale, s);
         case L_TAIL: {
             b2k::TailArgs t = L.tail;
             t.out = static_cast<float*>(out);
@@ -2178,7 +2196,8 @@ bool patch_layout(const b2_engine* e, const Launch& L, BindPatch* p) {
             p->n_params = 6, p->slots = {{1, L.out_binding}};               // output_cast_kernel(src, dst, N, C, HW, C_phys)
             return true;
         case L_OUTPUT_CAST_I8:
-            p->n_params = 7, p->slots = {{1, L.out_binding}};               // output_cast_i8_kernel(src, dst, N, C, HW, C_phys, s)
+        case L_OUTPUT_CAST_F8:
+            p->n_params = 7, p->slots = {{1, L.out_binding}};               // output_cast_{i8,f8}_kernel(src, dst, N, C, HW, C_phys, s)
             return true;
         case L_FC:
             p->n_params = 7, p->slots = {{3, L.out_binding}};               // fc kernels (in, w, bias, out, N, K, Cout)
@@ -2923,7 +2942,8 @@ const char* b2_context_launch_name(b2_context* c, int batch, int i) {
     if (!L) return nullptr;
     static const char* kinds[] = {"input_cast", "conv_tcgen05", "conv_simt", "maxpool", "avgpool", "fc", "softmax", "output_cast", "net_tcgen05", "tail_pool_fc_softmax",
                                   "quantize", "conv_i8_tcgen05", "avgpool_i8", "output_cast_i8", "embed_ln", "layernorm", "attention_f16_wgmma",
-                                  "pooler", "output_cast_rows", "output_unpack_rows"};
+                                  "pooler", "output_cast_rows", "output_unpack_rows", "quantize_f8", "conv_f8_tcgen05", "avgpool_f8",
+                                  "output_cast_f8"};
     s = std::string(kinds[L->kind]) + (L->kind == L_ATTENTION && L->attn.S > 128 ? "_ks" : "") +  // key-split kernel
         (L->kind == L_ATTENTION && L->attn.seq_off ? "_varlen" : "") + ":" + L->name;         // variable-length kernel
     if (L->kind == L_CONV_TC)
@@ -2937,7 +2957,7 @@ const char* b2_context_launch_name(b2_context* c, int batch, int i) {
              std::to_string(L->conv.args.splits) + " kblk=" + std::to_string(L->conv.args.num_kblocks) +
              (L->conv.args.group_span ? " span=" + std::to_string(L->conv.args.group_span) : std::string()) +
              ((L->conv.args.relu & b2plan::kConvGelu) ? " gelu" : "") + (L->conv.args.live ? " live" : "");
-    if (L->kind == L_CONV_I8)
+    if (L->kind == L_CONV_I8 || L->kind == L_CONV_F8)
         s += " bn=" + std::to_string(L->i8.bn) + " st=" + std::to_string(L->i8.stages) + (L->i8.args.a_mode == b2k::A_TILED ? " tiled" : " im2col") + " grid=" +
              std::to_string(L->i8.grid_n) + "x" + std::to_string(L->i8.grid_m) + " kblk=" + std::to_string(L->i8.args.num_kblocks);
     if (L->kind == L_NET)

@@ -10,6 +10,14 @@
 //  * quantize_h_to_i8_kernel -- fp16 NHWC -> int8 NHWC (channels zero-padded to the 128-channel rows of the INT8 layout)
 //  * avgpool_i8_kernel       -- global average pool: int8 NHWC -> fp16 [N][C]  (exact integer sums)
 //  * output_cast_i8_kernel   -- int8 NHWC -> fp32 NCHW binding (dequantised)
+//
+// FP8 (E4M3) kernels, the same layouts with E4M3 codes in place of int8 values:
+//  * conv_f8_tcgen05<BN> -- the same kernel body (conv_1byte_tile<F8 = true>): wgmma 64 x BN x 32 e4m3 x e4m3 -> f32, then
+//        t = fma(acc, m[c], b[c]);  t = fma(float(q_res), r, t);  t = max(t, 0);  q = e4m3(t)  (RNE, saturating to +-448)
+//  * quantize_h_to_f8_kernel, avgpool_f8_kernel (fp32 sums in pixel order), output_cast_f8_kernel
+#include <cmath>
+#include <type_traits>
+
 #include "kernels.h"
 #include "ptx_sm90.cuh"
 #include "wgmma_sm90.cuh"
@@ -21,16 +29,31 @@ namespace {
 constexpr int kI8Threads = 384;  // warps 0-3: producers, warps 4-11: two consumer warpgroups (rows 0-63 / 64-127)
 constexpr int kI8ASub = 128 * 128;  // 128 rows x 128 K-bytes
 
+// two E4M3 codes (low byte first) -> their exact values; every E4M3 value is an fp16 value
+__device__ __forceinline__ float2 e4m3x2_to_float2(uint16_t v) {
+    uint32_t h2;
+    asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(h2) : "h"(v));
+    return __half22float2(*reinterpret_cast<const __half2*>(&h2));
+}
+// (a, b) -> two E4M3 codes, a in the low byte: round to nearest even, saturating to +-448 (NaN stays NaN)
+__device__ __forceinline__ uint16_t float2_to_e4m3x2(float a, float b) {
+    uint16_t v;
+    asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(v) : "f"(b), "f"(a));
+    return v;
+}
+
 __host__ __device__ constexpr int conv_i8_smem_layout_bytes(int bn, int stages, bool residual) {
     return stages * (kI8ASub + bn * 128) + (residual ? 128 * bn : 0) + 256 + 2 * bn * 4 + 1024;
 }
 
 }  // namespace
 
-template <int BN, int STAGES>
-__global__ void __launch_bounds__(kI8Threads, 1)
-conv_i8_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapOut,
-                const __grid_constant__ CUtensorMap mapRes, const I8ConvArgs p) {
+// The 1-byte convolution, for both element formats: F8 = false is INT8 (s8 operands, exact s32 accumulators, integer
+// requantisation), F8 = true is FP8 (e4m3 operands, fp32 accumulators, satfinite e4m3 conversion).  Producers, ring,
+// padding skips, staging tile and TMA store are the same code.
+template <bool F8, int BN, int STAGES>
+__device__ __forceinline__ void conv_1byte_tile(const CUtensorMap& mapA, const CUtensorMap& mapOut, const CUtensorMap& mapRes,
+                                                const I8ConvArgs& p) {
     constexpr int A_STAGE = kI8ASub, B_STAGE = BN * 128;
     constexpr int PIPE_BYTES = STAGES * (A_STAGE + B_STAGE);
     constexpr int TILE_BYTES = 128 * BN;     // int8 output / residual tile
@@ -84,7 +107,8 @@ conv_i8_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
         }
     }
 
-    int32_t acc[BN / 2];
+    using acc_t = typename std::conditional<F8, float, int32_t>::type;
+    acc_t acc[BN / 2];
     if (warp == 0) {
         // ================= activation producer =================
         int img0 = 0, p0 = 0, q0 = 0;
@@ -139,7 +163,8 @@ conv_i8_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
             wgmma_group_upto<4>(nj, [&](int j) {  // up to 4 x (K = 32 bytes) inside one 128-byte swizzle row
                 const uint64_t ad = make_wgmma_desc(a_addr + j * 32, 16, 1024, WG_SW128);
                 const uint64_t bd = make_wgmma_desc(b_addr + j * 32, 16, 1024, WG_SW128);
-                wgmma_i8<BN>(acc, ad, bd, (i > 0 || j > 0) ? 1u : 0u);
+                if constexpr (F8) wgmma_e4m3<BN>(acc, ad, bd, (i > 0 || j > 0) ? 1u : 0u);
+                else wgmma_i8<BN>(acc, ad, bd, (i > 0 || j > 0) ? 1u : 0u);
             });
             if constexpr (STAGES == 1) {  // the only stage is refilled for step i+1: retire step i first
                 wgmma_wait<0>();
@@ -178,8 +203,8 @@ conv_i8_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
         const int row0 = 64 * ((warp - 4) >> 2) + 16 * ((warp - 4) & 3) + (lane >> 2);
         const float r = p.r;
         // q = clip(rint(max(t, relu ? 0 : -inf)), -127, 127): the lower clamp and the ReLU are ONE fp32 max before the
-        // conversion (rint is monotonic and rint(-127) = -127)
-        const float lo = p.relu != 0 ? 0.0f : -127.0f;
+        // conversion (rint is monotonic and rint(-127) = -127).  FP8 has no lower clamp before its saturating conversion.
+        const float lo = p.relu != 0 ? 0.0f : (F8 ? -INFINITY : -127.0f);
 #pragma unroll
         for (int j = 0; j < BN / 8; ++j) {
 #pragma unroll
@@ -188,7 +213,21 @@ conv_i8_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
                 const int col = 8 * j + 2 * (lane & 3);
                 const uint32_t so = static_cast<uint32_t>((col >> 7) * (128 * 128)) + swz_off<128>(row, (col & 127) >> 4) + (col & 15);
                 uint16_t packed = 0;  // padding channels (col >= nv): zero by construction
-                if (col < nv) {
+                if constexpr (F8) {
+                    // t = fma(acc, m[c], b[c]);  t = fma(float(q_res), r, t);  t = max(t, 0);  q = e4m3(t), satfinite RNE.
+                    if (col < nv) {
+                        float2 rf = make_float2(0.f, 0.f);
+                        if (has_res) rf = e4m3x2_to_float2(*reinterpret_cast<const uint16_t*>(sRes + so));
+                        float t[2];
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            t[e] = __fmaf_rn(acc[4 * j + 2 * h + e], s_m[col + e], s_b[col + e]);
+                            if (has_res) t[e] = __fmaf_rn(e ? rf.y : rf.x, r, t[e]);
+                            t[e] = fmaxf(t[e], lo);
+                        }
+                        packed = float2_to_e4m3x2(t[0], t[1]);
+                    }
+                } else if (col < nv) {
                     char2 rq = make_char2(0, 0);
                     if (has_res) rq = *reinterpret_cast<const char2*>(sRes + so);
                     int q[2];
@@ -213,6 +252,20 @@ conv_i8_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
     }
 }
 
+template <int BN, int STAGES>
+__global__ void __launch_bounds__(kI8Threads, 1)
+conv_i8_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapOut,
+                const __grid_constant__ CUtensorMap mapRes, const I8ConvArgs p) {
+    conv_1byte_tile<false, BN, STAGES>(mapA, mapOut, mapRes, p);
+}
+
+template <int BN, int STAGES>
+__global__ void __launch_bounds__(kI8Threads, 1)
+conv_f8_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapOut,
+                const __grid_constant__ CUtensorMap mapRes, const I8ConvArgs p) {
+    conv_1byte_tile<true, BN, STAGES>(mapA, mapOut, mapRes, p);
+}
+
 int conv_i8_smem_bytes(int bn, int stages, bool residual) { return conv_i8_smem_layout_bytes(bn, stages, residual); }
 bool conv_i8_config_exists(int bn, int stages) {
     return (bn == 128 || bn == 256) && stages >= 1 && stages <= 4 && conv_i8_smem_layout_bytes(bn, stages, true) <= 227 * 1024;
@@ -225,13 +278,19 @@ int init_conv_i8_kernels() {
 #define B2_I8_INIT(BN_, ST_)                                                                                                  \
     if ((e = static_cast<int>(cudaFuncSetAttribute(conv_i8_tcgen05<BN_, ST_>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
                                                    conv_i8_smem_layout_bytes(BN_, ST_, true)))))                             \
+        return e;                                                                                                             \
+    if ((e = static_cast<int>(cudaFuncSetAttribute(conv_f8_tcgen05<BN_, ST_>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
+                                                   conv_i8_smem_layout_bytes(BN_, ST_, true)))))                             \
         return e;
     B2_FOR_EACH_I8(B2_I8_INIT)
 #undef B2_I8_INIT
     return 0;
 }
 
-int launch_conv_i8_tcgen05(const I8ConvLaunch& L, cudaStream_t stream) {
+namespace {
+
+template <bool F8>
+int launch_conv_1byte(const I8ConvLaunch& L, cudaStream_t stream) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(static_cast<unsigned>(L.grid_n), static_cast<unsigned>(L.grid_m), 1);
     cfg.blockDim = dim3(kI8Threads);
@@ -242,12 +301,34 @@ int launch_conv_i8_tcgen05(const I8ConvLaunch& L, cudaStream_t stream) {
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = get_pdl() ? 1 : 0;
-#define B2_I8_CASE(BN_, ST_) \
-    if (L.bn == BN_ && L.stages == ST_) return static_cast<int>(cudaLaunchKernelEx(&cfg, conv_i8_tcgen05<BN_, ST_>, L.mapA, L.mapOut, L.mapRes, L.args));
+#define B2_I8_CASE(BN_, ST_)                                                                                             \
+    if (L.bn == BN_ && L.stages == ST_)                                                                                  \
+        return static_cast<int>(cudaLaunchKernelEx(&cfg, F8 ? conv_f8_tcgen05<BN_, ST_> : conv_i8_tcgen05<BN_, ST_>, L.mapA, \
+                                                   L.mapOut, L.mapRes, L.args));
     B2_FOR_EACH_I8(B2_I8_CASE)
 #undef B2_I8_CASE
     return static_cast<int>(cudaErrorInvalidValue);
 }
+
+// the launch configuration of the SIMT helpers: a 1-D grid, programmatic dependent launch when enabled
+template <class... KArgs, class... Args>
+int launch_simt(void (*kernel)(KArgs...), long long threads_total, int threads, cudaStream_t stream, Args... args) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(static_cast<unsigned>((threads_total + threads - 1) / threads));
+    cfg.blockDim = dim3(threads);
+    cfg.stream = stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = get_pdl() ? 1 : 0;
+    return static_cast<int>(cudaLaunchKernelEx(&cfg, kernel, args...));
+}
+
+}  // namespace
+
+int launch_conv_i8_tcgen05(const I8ConvLaunch& L, cudaStream_t stream) { return launch_conv_1byte<false>(L, stream); }
+int launch_conv_f8_tcgen05(const I8ConvLaunch& L, cudaStream_t stream) { return launch_conv_1byte<true>(L, stream); }
 
 // =================================================================================================
 // SIMT helpers of the INT8 path
@@ -355,6 +436,84 @@ int launch_output_cast_i8(const void* src, float* dst, int N, int C, int H, int 
     cfg.attrs = attr;
     cfg.numAttrs = get_pdl() ? 1 : 0;
     return static_cast<int>(cudaLaunchKernelEx(&cfg, output_cast_i8_kernel, static_cast<const int8_t*>(src), dst, N, C, H * W, C_phys, s));
+}
+
+// =================================================================================================
+// SIMT helpers of the FP8 path (the INT8 helpers' layouts; quantize.py states the arithmetic)
+// =================================================================================================
+// fp16 NHWC [P][C_in_phys] -> e4m3 NHWC [P][C_out_phys]: q = e4m3(fl(float(h) * inv_s)), channels >= C code 0x00.
+// One thread per 16 output channels (one 16-byte store).
+__global__ void quantize_h_to_f8_kernel(const __half* __restrict__ src, uint8_t* __restrict__ dst, long long pixels, int C, int C_in_phys,
+                                        int C_out_phys, float inv_s) {
+    pdl_launch_dependents();
+    pdl_wait();
+    const int groups = C_out_phys / 16;
+    const long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
+    if (idx >= pixels * groups) return;
+    const long long px = idx / groups;
+    const int c0 = static_cast<int>(idx - px * groups) * 16;
+    uint4 o = make_uint4(0u, 0u, 0u, 0u);
+    uint16_t* oq = reinterpret_cast<uint16_t*>(&o);
+    if (c0 < C) {
+        const __half* s = src + px * C_in_phys + c0;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+            const float a = c0 + 2 * i < C ? __fmul_rn(__half2float(s[2 * i]), inv_s) : 0.f;
+            const float b = c0 + 2 * i + 1 < C ? __fmul_rn(__half2float(s[2 * i + 1]), inv_s) : 0.f;
+            oq[i] = float2_to_e4m3x2(a, b);
+        }
+    }
+    reinterpret_cast<uint4*>(dst)[idx] = o;
+}
+
+int launch_quantize_h_to_f8(const void* src, void* dst, long long pixels, int C, int C_in_phys, int C_out_phys, float inv_s,
+                            cudaStream_t stream) {
+    if (C_out_phys % 16 || pixels <= 0) return static_cast<int>(cudaErrorInvalidValue);
+    return launch_simt(quantize_h_to_f8_kernel, pixels * (C_out_phys / 16), 256, stream, static_cast<const __half*>(src), static_cast<uint8_t*>(dst),
+                       pixels, C, C_in_phys, C_out_phys, inv_s);
+}
+
+__device__ __forceinline__ float e4m3_to_float(uint8_t q) { return e4m3x2_to_float2(q).x; }
+
+// global average pool, e4m3 NHWC [N][HW][C_in_phys] -> fp16 [N][C_out_phys]: the values summed in fp32 in pixel order (exact
+// for HW < 73), h = fp16(fl(sum * k)); one thread per channel
+__global__ void avgpool_f8_kernel(const uint8_t* __restrict__ src, __half* __restrict__ dst, int N, int HW, int C, int C_in_phys,
+                                  int C_out_phys, float k) {
+    pdl_launch_dependents();
+    pdl_wait();
+    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= N * C_out_phys) return;
+    const int c = idx % C_out_phys;
+    const int n = idx / C_out_phys;
+    float sum = 0.f;
+    if (c < C) {
+        const uint8_t* s = src + static_cast<size_t>(n) * HW * C_in_phys + c;
+        for (int i = 0; i < HW; ++i) sum = __fadd_rn(sum, e4m3_to_float(s[static_cast<size_t>(i) * C_in_phys]));
+    }
+    dst[idx] = __float2half_rn(__fmul_rn(sum, k));
+}
+
+int launch_avgpool_f8(const void* src, void* dst, int N, int HW, int C, int C_in_phys, int C_out_phys, float k, cudaStream_t stream) {
+    return launch_simt(avgpool_f8_kernel, static_cast<long long>(N) * C_out_phys, 128, stream, static_cast<const uint8_t*>(src),
+                       static_cast<__half*>(dst), N, HW, C, C_in_phys, C_out_phys, k);
+}
+
+// e4m3 NHWC -> fp32 NCHW binding: y = fl(float(q) * s)
+__global__ void output_cast_f8_kernel(const uint8_t* __restrict__ src, float* __restrict__ dst, int N, int C, int HW, int C_phys, float s) {
+    pdl_launch_dependents();
+    pdl_wait();
+    const long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
+    if (idx >= static_cast<long long>(N) * C * HW) return;
+    const int px = static_cast<int>(idx % HW);
+    const long long t = idx / HW;
+    const int c = static_cast<int>(t % C);
+    const int n = static_cast<int>(t / C);
+    dst[idx] = __fmul_rn(e4m3_to_float(src[(static_cast<size_t>(n) * HW + px) * C_phys + c]), s);
+}
+
+int launch_output_cast_f8(const void* src, float* dst, int N, int C, int H, int W, int C_phys, float s, cudaStream_t stream) {
+    return launch_simt(output_cast_f8_kernel, static_cast<long long>(N) * C * H * W, 256, stream, static_cast<const uint8_t*>(src), dst, N, C,
+                       H * W, C_phys, s);
 }
 
 }  // namespace b2k

@@ -179,6 +179,13 @@ int init_conv_i8_kernels();
 bool conv_i8_config_exists(int bn, int stages);
 int conv_i8_smem_bytes(int bn, int stages, bool residual);
 int launch_conv_i8_tcgen05(const I8ConvLaunch& L, cudaStream_t stream);
+// FP8 (E4M3) path, same operand layouts and arguments: conv_f8_tcgen05 (fp32 accumulators, e4m3 = round to nearest even,
+// saturating to +-448), and the E4M3 twins of the three helpers below (quantize.py states the arithmetic)
+int launch_conv_f8_tcgen05(const I8ConvLaunch& L, cudaStream_t stream);
+int launch_quantize_h_to_f8(const void* src, void* dst, long long pixels, int C, int C_in_phys, int C_out_phys, float inv_s,
+                            cudaStream_t stream);
+int launch_avgpool_f8(const void* src, void* dst, int N, int HW, int C, int C_in_phys, int C_out_phys, float k, cudaStream_t stream);
+int launch_output_cast_f8(const void* src, float* dst, int N, int C, int H, int W, int C_phys, float s, cudaStream_t stream);
 // fp16 NHWC -> int8 NHWC, q = clip(rint(fl(float(h) * inv_s)), +-127); channels >= C are written as zeros
 int launch_quantize_h_to_i8(const void* src, void* dst, long long pixels, int C, int C_in_phys, int C_out_phys, float inv_s,
                             cudaStream_t stream);

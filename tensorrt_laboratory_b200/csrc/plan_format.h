@@ -23,8 +23,8 @@ enum OpType : uint32_t {
     OP_AVGPOOL = 3,      // global average pool
     OP_FC = 4,           // inner product -> fp32 vector
     OP_SOFTMAX = 5,      // fp32 vector -> fp32 vector
-    OP_OUTPUT_CAST = 6,  // NHWC activation tensor -> fp32 NCHW binding (dequantised when the tensor is int8)
-    OP_QUANTIZE = 7,     // fp16 NHWC tensor -> int8 NHWC tensor (INT8 engines: in front of the first int8 convolution)
+    OP_OUTPUT_CAST = 6,  // NHWC activation tensor -> fp32 NCHW binding (dequantised when the tensor is int8 / e4m3)
+    OP_QUANTIZE = 7,     // fp16 NHWC tensor -> 1-byte NHWC tensor (INT8 / FP8 engines: in front of the first 1-byte convolution)
     // transformer ops (version-3 plans, fp16 engines only; OpRecV3 below)
     OP_EMBED_LN = 8,     // int32 bindings (ids, segment ids, mask) -> LayerNorm(word + position + type) fp16 [N, 1, S, H]
                          // and the additive attention mask, fp32 [N, S] (tensor `out2`)
@@ -61,7 +61,8 @@ struct TensorRec {  // 96 bytes
     uint32_t kind;
     uint32_t h, w, c, c_phys;
     int32_t binding;  // >= 0: storage is bindings[binding] (T_VEC only), -1: activation arena
-    float scale;      // INT8 engines: > 0 marks an int8 tensor (1 byte per element, real value = q * scale); 0 = fp16 / fp32
+    float scale;      // INT8 / FP8 engines: > 0 marks a 1-byte tensor, int8 or E4M3 by the plan's precision (real value =
+                      // q * scale); 0 = fp16 / fp32
     uint8_t pad[4];
 };
 struct OpRec {  // 176 bytes
@@ -70,8 +71,9 @@ struct OpRec {  // 176 bytes
     int32_t in, res, out;  // tensor indices (-1 = none)
     int32_t binding;       // cast ops: binding index
     uint32_t k, stride, pad_;
-    uint32_t relu;         // bit 0: fused ReLU.  bit 2 (convs): INT8 convolution -- int8 weights in 128-byte K blocks, and the
-                           // "bias" region holds [m: cout_phys fp32][b: cout_phys fp32][r, 0, 0, 0] (quantize.py).
+    uint32_t relu;         // bit 0: fused ReLU.  bit 2 (convs): 1-byte convolution -- int8 weights (E4M3 codes in an FP8 plan)
+                           // in 128-byte K blocks, and the "bias" region holds [m: cout_phys fp32][b: cout_phys fp32][r, 0, 0, 0]
+                           // (quantize.py).
                            // bit 1 (convs): weights are stored as pre-swizzled 4 KiB blocks
                            // [K/64][Cout/32][32 rows][128 B] (builder.pack_weights_sw128) instead of row-major [Cout][K]
     uint32_t ceil_mode;    // pools: Caffe ceil mode.  convs: algorithmic K (Cin*kh*kw of the ORIGINAL conv) when the
@@ -91,7 +93,7 @@ struct OpRec {  // 176 bytes
 //     (o / cpg) * cpg - (o / span) * span ... and the other columns are zero.  w_bytes = Cout_phys * taps * span * 2.
 //   relu bit 1 clear (every other geometry, and fp32 engines): row-major [Cout_phys][taps_phys][Cin/groups];
 //     w_bytes = Cout_phys * taps_phys * (Cin / groups) * element size.
-// INT8 grouped convolutions do not exist.
+// 1-byte (INT8 / FP8) grouped convolutions do not exist.
 struct OpRecV2 {  // 192 bytes
     OpRec v1;
     uint32_t groups;

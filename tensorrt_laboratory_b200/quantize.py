@@ -16,6 +16,25 @@ Scheme (what the INT8 kernels of this repository implement, bit for bit):
 
 A convolution runs in INT8 when both its channel counts are multiples of 64 (all bottleneck convolutions of the ResNets).
 
+FP8 (``fmt="e4m3"``): the same split and the same layouts, with E4M3 codes (the ``e4m3fn`` format: no infinities,
+subnormals kept, largest value 448) in place of int8 values.  ``e4m3()`` is round-to-nearest-even, saturating to +-448
+(the ``satfinite`` conversion of the tensor-core epilogue):
+  * activations: symmetric per-tensor scale ``s = fl32(max(amax, 1e-12) / 448)`` from max-abs calibration;
+  * quantize op: ``q = e4m3(fl(float(h) * fl(1/s)))``;
+  * weights: symmetric per-OUTPUT-CHANNEL scale ``s_w[c] = max|W[c]| / 448``, ``Wq = e4m3(clamp(fl32(W / s_w), +-448))``,
+    stored as raw E4M3 bytes in the ``pack_weights_sw128_i8`` block layout;
+  * convolution: ``acc = sum(Wq * q)`` on the tensor core with fp32 accumulators.  Every product is exact in fp32, but the
+    order and width of the tensor core's internal accumulation belong to the hardware (Hopper's FP8 MMA keeps fewer bits
+    than fp32 there), so the GPU result is not bit-reproducible on the CPU; the tests bound it from the exact sum instead;
+  * epilogue: INT8's, except for the last step
+        t = fma(acc, m[c], b[c])                      m[c] = fl(s_in * s_w[c] / s_out),  b[c] = fl(bias[c] / s_out)
+        t = fma(float(q_res), r, t)                   r = fl(s_res / s_out)                      (fused residual)
+        t = max(t, 0)                                                                           (fused ReLU)
+        q_out = e4m3(t)                               padding output channels are code 0x00
+  * average pool: each code converted to fp32 and summed in fp32 in pixel order, ``h = fp16(fl(sum * fl(s / HW)))`` (the
+    sum is exact for HW < 73: E4M3 values are multiples of 2^-9 and at most 448);
+  * output cast of an FP8 tensor to an fp32 binding: ``y = fl(float(q) * s)``.
+
 The calibration forward pass runs on the host (torch CPU, fp32) -- build-time work like the rest of this module, never
 part of the request path.
 """
@@ -29,6 +48,16 @@ import numpy as np
 from . import graph as G
 
 QMAX = 127.0
+E4M3_MAX = 448.0
+FORMATS = {"int8": "INT8", "e4m3": "FP8"}
+
+
+def e4m3(x: np.ndarray) -> np.ndarray:
+    """float32 values -> E4M3 codes (uint8): round to nearest even, saturating to +-448.  torch's cast is round-to-nearest-
+    even but turns values from 464 up into NaN, hence the clamp."""
+    import torch
+    t = torch.from_numpy(np.ascontiguousarray(x, dtype=np.float32)).clamp(-E4M3_MAX, E4M3_MAX)
+    return t.to(torch.float8_e4m3fn).view(torch.uint8).numpy()
 
 
 def _is_int8_conv(op: dict) -> bool:
@@ -78,27 +107,36 @@ def calibrate(lowered: dict, calib_inputs: np.ndarray) -> Dict[str, float]:
     return amax
 
 
-def quantize_lowered(lowered: dict, calib_inputs: np.ndarray, amax: Optional[Dict[str, float]] = None) -> dict:
+def quantize_lowered(lowered: dict, calib_inputs: np.ndarray, amax: Optional[Dict[str, float]] = None,
+                     fmt: str = "int8") -> dict:
     """-> a lowered graph whose eligible convolutions carry INT8 parameters (``Wq`` int8 OHWI, ``m`` / ``b`` fp32 per
     output channel, ``r`` fp32 or None, ``in_scale`` / ``out_scale``), with ``quantize`` ops inserted where an INT8
     convolution reads an fp16 tensor, ``in_scale`` on an average pool that reads INT8, and ``tensor_scales`` {name: s}
     for every INT8 tensor.  ``lowered`` itself is not modified.  Grouped convolutions have no INT8 path: a graph that
-    contains one is rejected before calibration."""
+    contains one is rejected before calibration.
+
+    ``fmt="e4m3"``: the FP8 scheme above instead -- ``Wq`` holds E4M3 codes (uint8), and the graph and its quantized
+    convolutions are marked ``fp8`` rather than ``int8``."""
+    if fmt not in FORMATS:
+        raise ValueError(f"fmt must be one of {sorted(FORMATS)}, not {fmt!r}")
+    name = FORMATS[fmt]
+    fp8 = fmt == "e4m3"
+    qmax = E4M3_MAX if fp8 else QMAX
     for op in lowered["ops"]:
         if op["type"] == G.OP_CONV and op.get("groups", 1) != 1:
-            raise ValueError(f"conv {op['name']}: INT8 grouped convolution is not supported ({op['groups']} groups); "
+            raise ValueError(f"conv {op['name']}: {name} grouped convolution is not supported ({op['groups']} groups); "
                              "build this model in fp16 or fp32")
     amax = amax or calibrate(lowered, calib_inputs)
     q = copy.copy(lowered)
     q["tensors"] = dict(lowered["tensors"])
-    q["int8"] = True
-    scales: Dict[str, float] = {}   # INT8 tensors only
+    q["fp8" if fp8 else "int8"] = True
+    scales: Dict[str, float] = {}   # 1-byte tensors only
     ops = []
     alias: Dict[str, str] = {}      # fp16 tensor -> its quantized copy
 
     def scale_of(name: str) -> float:
         # scales are fp32 numbers (that is what the plan stores); everything derived from them starts from the rounded value
-        return float(np.float32(max(amax[name], 1e-12) / QMAX))
+        return float(np.float32(max(amax[name], 1e-12) / qmax))
 
     for op in lowered["ops"]:
         op = dict(op)
@@ -115,22 +153,25 @@ def quantize_lowered(lowered: dict, calib_inputs: np.ndarray, amax: Optional[Dic
                 op["input"] = alias[src]
             if op["residual"] is not None:
                 if op["residual"] not in scales:
-                    raise ValueError(f"conv {op['name']}: the residual input of an INT8 convolution must be an INT8 tensor")
+                    raise ValueError(f"conv {op['name']}: the residual input of an {name} convolution must be an {name} tensor")
             s_in = scales[op["input"]]
             s_out = scale_of(op["output"])
             W = np.asarray(op["W"], dtype=np.float64)                      # [O, kh, kw, I]
-            s_w = np.maximum(np.abs(W).reshape(W.shape[0], -1).max(axis=1), 1e-12) / QMAX
-            op["Wq"] = np.clip(np.rint(W / s_w[:, None, None, None]), -QMAX, QMAX).astype(np.int8)
+            s_w = np.maximum(np.abs(W).reshape(W.shape[0], -1).max(axis=1), 1e-12) / qmax
+            if fp8:
+                op["Wq"] = e4m3(np.clip((W / s_w[:, None, None, None]).astype(np.float32), -E4M3_MAX, E4M3_MAX))
+            else:
+                op["Wq"] = np.clip(np.rint(W / s_w[:, None, None, None]), -QMAX, QMAX).astype(np.int8)
             op["m"] = (s_in * s_w / s_out).astype(np.float32)
             op["b"] = (np.asarray(op["bias"], dtype=np.float64) / s_out).astype(np.float32)
             op["r"] = np.float32(scales[op["residual"]] / s_out) if op["residual"] is not None else None
             op["in_scale"], op["out_scale"], op["w_scale"] = s_in, s_out, s_w
-            op["int8"] = True
+            op["fp8" if fp8 else "int8"] = True
             scales[op["output"]] = s_out
         else:
             for key in ("input", "residual"):
                 if op.get(key) in scales and op["type"] != G.OP_AVGPOOL:
-                    raise ValueError(f"{op['name']}: an fp16 operator reads the INT8 tensor {op[key]}")
+                    raise ValueError(f"{op['name']}: an fp16 operator reads the {name} tensor {op[key]}")
             if op["type"] == G.OP_AVGPOOL and op["input"] in scales:
                 c, h, w = q["tensors"][op["input"]]
                 op["in_scale"] = scales[op["input"]]

@@ -6,13 +6,15 @@ examples/ONNX/resnet50/build.py:35-67).
   python tools/build_engine.py --prototxt /path/ResNet-152-deploy.prototxt --precision fp16 --batch 32 -o rn152.plan
   python tools/build_engine.py --model mnist --precision fp32 --batch 1 -o mnist.plan
   python tools/build_engine.py --prototxt deploy.prototxt --caffemodel weights.caffemodel --precision int8 --batch 32 -o rn.plan
+  python tools/build_engine.py --model resnet50 --precision fp8 --batch 8 -o rn50_fp8.plan  (E4M3 bottleneck convolutions)
   python tools/build_engine.py --model resnet50 --batch 8 --tune -o rn50_tuned.plan      (on a GPU box: tactics in the file)
   python tools/build_engine.py --model resnext50 --precision fp16 --batch 8 --tune -o rx50.plan  (ResNeXt-50 32x4d)
   python tools/build_engine.py --model bert-base --seq 128 --batch 16 [--weights bert.npz] --tune -o bert.plan  (fp16)
   python tools/build_engine.py --model bert-base --seq 384 --batch 16 --remove-padding -o bert_packed.plan  (masked tokens skipped)
 Weights: deterministic synthetic weights (the reference's benchmark engines are weightless too, models/README.md:6-7),
 unless --caffemodel names a binary NetParameter (trtexec --model=...); MNIST and --onnx carry their own weights.
---precision int8: post-training quantization, max-abs calibration on --calib (an .npy [N,C,H,W] fp32) or on synthetic images.
+--precision int8 / fp8: post-training quantization (fp8: E4M3), max-abs calibration on --calib (an .npy [N,C,H,W] fp32) or on
+synthetic images.
 --tune: time the kernel configurations on this machine's GPU (what trtexec does while building) and store the tactic table
 in the plan file; an engine deserialized from it never tunes at load.
 """
@@ -34,16 +36,16 @@ def main():
     ap.add_argument("--prototxt")
     ap.add_argument("--onnx", help="ONNX CNN classifier (Conv / BatchNormalization / Relu / Add / MaxPool / AveragePool / "
                                    "GlobalAveragePool / Flatten / Reshape / Gemm / MatMul / Softmax), e.g. an ONNX-zoo ResNet")
-    ap.add_argument("--precision", choices=["fp16", "fp32", "int8"], default="fp16")
+    ap.add_argument("--precision", choices=["fp16", "fp32", "int8", "fp8"], default="fp16")
     ap.add_argument("--caffemodel", help="binary caffe NetParameter with the weights of --prototxt / --model resnetNN")
-    ap.add_argument("--calib", help="int8: .npy of calibration inputs [N, C, H, W] fp32 (default: 8 synthetic images)")
+    ap.add_argument("--calib", help="int8 / fp8: .npy of calibration inputs [N, C, H, W] fp32 (default: 8 synthetic images)")
     ap.add_argument("--tune", action="store_true", help="needs a GPU: tune kernel tactics now and embed them in the plan")
     ap.add_argument("--tune-all-batches", action="store_true", help="with --tune: one tactic set per batch size 1..max")
     ap.add_argument("--batch", type=int, default=8)
     ap.add_argument("--seed", type=int, default=0)
     ap.add_argument("-o", "--output", required=True)
     a = ap.parse_args()
-    prec = {"fp16": builder.PREC_FP16, "fp32": builder.PREC_FP32, "int8": builder.PREC_INT8}[a.precision]
+    prec = {"fp16": builder.PREC_FP16, "fp32": builder.PREC_FP32, "int8": builder.PREC_INT8, "fp8": builder.PREC_FP8}[a.precision]
 
     def weights_for(net):
         if a.caffemodel:
@@ -67,7 +69,7 @@ def main():
         sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
         from tests import helpers
         net, wts, _, _ = helpers.load_mnist_golden()
-    elif a.model == "resnext50":  # 32x4d: grouped 3x3 convolutions (fp16 / fp32 only: INT8 has no grouped convolution)
+    elif a.model == "resnext50":  # 32x4d: grouped 3x3 convolutions (fp16 / fp32 only: INT8 and FP8 have no grouped convolution)
         net = graph.resnext_caffe(50)
         wts = weights_for(net)
     else:
@@ -75,14 +77,14 @@ def main():
         wts = weights_for(net)
     if a.model != "bert-base":
         low = graph.lower(net, wts)
-        if prec == builder.PREC_INT8:
+        if prec in (builder.PREC_INT8, builder.PREC_FP8):
             import numpy as np
             from tensorrt_laboratory_b200 import quantize
             if a.calib:
                 calib = np.load(a.calib).astype(np.float32)
             else:
                 calib = weights.synthetic_input(8, chw=tuple(net["input_dims"][1:]), seed=4321)
-            low = quantize.quantize_lowered(low, calib)
+            low = quantize.quantize_lowered(low, calib, fmt="e4m3" if prec == builder.PREC_FP8 else "int8")
         blob = builder.build_plan(low, prec, a.batch)
     if a.tune:
         from tensorrt_laboratory_b200 import capi
