@@ -48,6 +48,18 @@ def grouped_tc_span(cin: int, cout: int, groups: int, cin_phys: int, cout_phys: 
     return max(cpg, 64)
 
 
+def grouped_1byte_span(cin: int, cout: int, groups: int) -> int:
+    """K bytes per filter tap in the weight row of a grouped INT8 / FP8 convolution, or 0 when the 1-byte kernels do not
+    run its geometry.  They need Cin/g == Cout/g == cpg with cpg | 128 (a group lies inside one 128-channel row of the
+    1-byte layout: span 128) or 128 | cpg (span cpg)."""
+    if groups <= 1 or cin != cout or cin % groups:
+        return 0
+    cpg = cin // groups
+    if 128 % cpg and cpg % 128:
+        return 0
+    return max(cpg, 128)
+
+
 def expand_grouped_weights(W: np.ndarray, groups: int, span: int, cout_phys: int) -> np.ndarray:
     """Block-diagonal weight rows of a tensor-core grouped convolution: W [Cout, taps, cpg] -> [Cout_phys, taps, span].
     Row o is read against the `span` input channels starting at channel (o // span) * span, so its cpg real weights sit
@@ -225,9 +237,19 @@ def build_plan(lowered: dict, precision: int = PREC_FP16, max_batch: int = 8,
             cin_phys, cout_phys = tensors[ti]["c_phys"], tensors[to]["c_phys"]
             k = op["k"]
             taps = k * k
-            Wq = np.zeros((cout_phys, taps, cin_phys), dtype=np.int8)   # E4M3 codes travel as their bytes; 0x00 is +0
-            Wq[:op["cout"], :, :op["cin"]] = op["Wq"].view(np.int8).reshape(op["cout"], taps, op["cin"])
-            w_off, w_bytes = add_payload(pack_weights_sw128_i8(Wq.reshape(cout_phys, taps * cin_phys)))
+            groups = op.get("groups", 1)
+            if groups > 1:  # block-diagonal rows [Cout_phys][taps][span], packed as a dense [Cout_phys, taps * span] matrix
+                span = grouped_1byte_span(op["cin"], op["cout"], groups)
+                if not span:
+                    raise ValueError(f"conv {op['name']}: no 1-byte kernel for {op['cin']} -> {op['cout']} channels in {groups} groups")
+                Wg = op["Wq"].view(np.int8).reshape(op["cout"], taps, op["cin"] // groups)
+                Wx = expand_grouped_weights(Wg, groups, span, cout_phys)
+                w_off, w_bytes = add_payload(pack_weights_sw128_i8(Wx.reshape(cout_phys, taps * span)))
+                rec["groups"] = groups
+            else:
+                Wq = np.zeros((cout_phys, taps, cin_phys), dtype=np.int8)   # E4M3 codes travel as their bytes; 0x00 is +0
+                Wq[:op["cout"], :, :op["cin"]] = op["Wq"].view(np.int8).reshape(op["cout"], taps, op["cin"])
+                w_off, w_bytes = add_payload(pack_weights_sw128_i8(Wq.reshape(cout_phys, taps * cin_phys)))
             rq = np.zeros(2 * cout_phys + 4, dtype=np.float32)   # [m | b | r 0 0 0]; padded channels requantise to 0
             rq[:op["cout"]] = op["m"]
             rq[cout_phys:cout_phys + op["cout"]] = op["b"]
@@ -488,11 +510,17 @@ def build_bert_plan(cfg=None, weights=None, max_batch: int = 16, seed: int = 0, 
 
 
 def build_resnext_plan(depth: int = 50, precision: int = PREC_FP16, max_batch: int = 8, seed: int = 0,
-                       input_dtype: str = "f32", groups: int = 32, width_per_group: int = 4) -> bytes:
-    """Convenience: generated ResNeXt (:func:`graph.resnext_caffe`) + deterministic weights -> plan (fp16 or fp32)."""
+                       input_dtype: str = "f32", groups: int = 32, width_per_group: int = 4, calib_batch: int = 8) -> bytes:
+    """Convenience: generated ResNeXt (:func:`graph.resnext_caffe`) + deterministic weights -> plan.  PREC_INT8 / PREC_FP8:
+    post-training quantization with the grouped convolutions included, calibrated like :func:`build_resnet_plan`."""
     from . import weights as Wt
     net = G.resnext_caffe(depth, groups, width_per_group)
-    return build_plan(G.lower(net, Wt.random_weights(net, seed)), precision, max_batch, input_dtype=input_dtype)
+    low = G.lower(net, Wt.random_weights(net, seed))
+    if precision in (PREC_INT8, PREC_FP8):
+        from . import quantize
+        low = quantize.quantize_lowered(low, Wt.synthetic_input(calib_batch, seed=4321),
+                                        fmt="e4m3" if precision == PREC_FP8 else "int8", grouped=True)
+    return build_plan(low, precision, max_batch, input_dtype=input_dtype)
 
 
 def build_resnet_plan(depth: int = 50, precision: int = PREC_FP16, max_batch: int = 8, seed: int = 0,

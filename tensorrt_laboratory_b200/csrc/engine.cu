@@ -124,9 +124,10 @@ struct Op {
     int pw_hi() const { return int(r.kw ? r.pad_w_hi : r.pad_); }
     double algo_k() const { return r.ceil_mode ? double(r.ceil_mode) : double(r.cin / uint32_t(groups)) * r.taps; }
     // grouped convolution with the packed block-diagonal weight layout (plan_format.h): input channels per N tile, the
-    // K extent of one tap; 0 = dense, or grouped on the SIMT convolution
+    // K extent of one tap -- max(cpg, 64) in fp16, max(cpg, 128) for a 1-byte convolution; 0 = dense, or grouped on the
+    // SIMT convolution
     int group_span() const {
-        return groups > 1 && (r.relu & 2) ? std::max(int(r.cin) / groups, 64) : 0;
+        return groups > 1 && (r.relu & 2) ? std::max(int(r.cin) / groups, (r.relu & 4) ? 128 : 64) : 0;
     }
 };
 
@@ -570,9 +571,23 @@ int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** pa
                                          r.cin_phys % 64 || op.groups != 1))
                 return fail(B2_EINVAL, "plan: conv %s: GELU layers are dense 1x1 stride-1 convolutions with packed weights", op.name.c_str());
             const bool i8 = (r.relu & kConvInt8) != 0;  // a 1-byte convolution: int8, or e4m3 in an FP8 plan
-            if (op.groups > 1) {  // layouts: plan_format.h (OpRecV2)
+            if (op.groups > 1 && i8) {  // 1-byte grouped convolution: packed block-diagonal rows [Cout_phys][taps][span]
+                const uint32_t g = uint32_t(op.groups), cpg = r.cin / g;
+                const Tensor& qi = e->tensors[r.in];
+                const Tensor& qo = e->tensors[r.out];
+                if (!one_byte || r.cin % g || r.cin != r.cout || cpg == 0 || (128 % cpg && cpg % 128) || !(qi.scale > 0.f) || !(qo.scale > 0.f) ||
+                    (r.res >= 0 && !(e->tensors[r.res].scale > 0.f)) || r.cin_phys % 128 || r.cin_phys != r.cout_phys ||
+                    r.taps_phys != r.taps || r.kw != 0 || !(r.relu & 2))
+                    return fail(B2_EINVAL,
+                                "plan: conv %s: %s grouped convolution needs Cin/g == Cout/g dividing 128 or a multiple of 128, %s "
+                                "tensors with 128-channel rows and packed weights (%u -> %u channels, %u groups)",
+                                op.name.c_str(), qFMT, qfmt, r.cin, r.cout, g);
+                const size_t want = size_t(r.cout_phys) * r.taps * std::max<uint32_t>(cpg, 128);
+                if (r.w_bytes != want || r.b_bytes != (size_t(r.cout_phys) * 2 + 4) * 4)
+                    return fail(B2_EINVAL, "plan: %s grouped conv %s weight / requantisation size mismatch (%llu weight bytes, layout needs %zu)",
+                                qfmt, op.name.c_str(), (unsigned long long)r.w_bytes, want);
+            } else if (op.groups > 1) {  // layouts: plan_format.h (OpRecV2)
                 const uint32_t g = uint32_t(op.groups);
-                if (i8) return fail(B2_EINVAL, "plan: conv %s: %s grouped convolution is not supported", op.name.c_str(), qFMT);
                 if (r.cin % g || r.cout % g)
                     return fail(B2_EINVAL, "plan: conv %s: %u groups do not divide %u -> %u channels", op.name.c_str(), g, r.cin, r.cout);
                 const uint32_t cpg = r.cin / g;
@@ -1241,7 +1256,12 @@ int make_i8_conv_launch(b2_context* c, const Op& op, int batch, int bn, int stag
     a.has_res = r.res >= 0 ? 1 : 0;
     a.relu = int(r.relu & 1);
     a.M = M, a.Cout = int(r.cout_phys);
-    a.cblocks = int(r.cin_phys) / 128;
+    // grouped: each N tile reads its own span of input channels (kernels.h); the diagonal modes take their padding skip
+    // from the tile's real channels, the dense mode's spans are whole 128-channel blocks
+    const int span = op.group_span(), cpg = int(r.cin) / op.groups;
+    a.group_span = span;
+    cl.group_mode = !span ? 0 : cpg <= 32 ? 32 : cpg == 64 ? 64 : 128;
+    a.cblocks = (span ? span : int(r.cin_phys)) / 128;
     a.last_cb_mmas = (int(r.cin) % 128) ? (int(r.cin) % 128 + 31) / 32 : 4;
     a.cout_real = int(r.cout);
     a.num_kblocks = int(r.taps) * a.cblocks;
@@ -1418,6 +1438,15 @@ void tune_cache_append(const b2_engine* e, int op, int batch, const ConvConfig& 
     fclose(f);
 }
 
+// The (N tile, ring depth) of a 1-byte convolution: an instantiated configuration whose N tile divides the output
+// channels and, for a grouped layer, the span of input channels a tile reads.  The tuner, tactic tables and the forced
+// "i8_bn" / "i8_stages" options all go through these two rules.
+bool i8_bn_fits(const Op& op, int bn) {
+    const int span = op.group_span();
+    return int(op.r.cout_phys) % bn == 0 && (!span || span % bn == 0);
+}
+bool i8_tactic_ok(const Op& op, int bn, int stages) { return i8_bn_fits(op, bn) && b2k::conv_i8_config_exists(bn, stages); }
+
 // 1-byte twin of autotune_conv: times every (N tile, ring depth) of conv_i8_tcgen05 / conv_f8_tcgen05 on `c->autotune`
 // concurrent streams.
 int autotune_i8_conv(b2_context* c, const Op& op, int batch, ConvConfig* best_out) {
@@ -1431,9 +1460,8 @@ int autotune_i8_conv(b2_context* c, const Op& op, int batch, ConvConfig* best_ou
     double best_ms = 1e30;
     ConvConfig best = *best_out;
     for (int bn : {128, 256}) {
-        if (int(r.cout_phys) % bn) continue;
         for (int st = 1; st <= 4; ++st) {
-            if (!b2k::conv_i8_config_exists(bn, st)) continue;
+            if (!i8_tactic_ok(op, bn, st)) continue;
             b2k::I8ConvLaunch cl;
             if ((status = make_i8_conv_launch(c, op, batch, bn, st, &cl))) return status;
             float ms = 0.f;
@@ -1853,8 +1881,9 @@ int build_plan(b2_context* c, int batch, Plan** out) {
                     }
                     if (c->i8_bn > 0) bn = c->i8_bn;
                     if (c->i8_stages > 0) st = c->i8_stages;
-                    if (int(r.cout_phys) % bn) bn = 128;
-                    if (!b2k::conv_i8_config_exists(bn, st)) bn = 128, st = 2;
+                    // an N tile that does not fit falls back to 128, a configuration that does not exist to (128, 2)
+                    if (!i8_bn_fits(op, bn)) bn = 128;
+                    if (!i8_tactic_ok(op, bn, st)) bn = 128, st = 2;
                     int rc = make_i8_conv_launch(c, op, batch, bn, st, &L.i8);
                     if (rc) return rc;
                 } else if (!c->force_simt && conv_on_tensor_cores(e, op)) {
@@ -2959,7 +2988,10 @@ const char* b2_context_launch_name(b2_context* c, int batch, int i) {
              ((L->conv.args.relu & b2plan::kConvGelu) ? " gelu" : "") + (L->conv.args.live ? " live" : "");
     if (L->kind == L_CONV_I8 || L->kind == L_CONV_F8)
         s += " bn=" + std::to_string(L->i8.bn) + " st=" + std::to_string(L->i8.stages) + (L->i8.args.a_mode == b2k::A_TILED ? " tiled" : " im2col") + " grid=" +
-             std::to_string(L->i8.grid_n) + "x" + std::to_string(L->i8.grid_m) + " kblk=" + std::to_string(L->i8.args.num_kblocks);
+             std::to_string(L->i8.grid_n) + "x" + std::to_string(L->i8.grid_m) + " kblk=" + std::to_string(L->i8.args.num_kblocks) +
+             (L->i8.group_mode ? " span=" + std::to_string(L->i8.args.group_span) + " mode=" +
+                                     (L->i8.group_mode == 128 ? std::string("dense") : std::to_string(L->i8.group_mode))
+                               : std::string());
     if (L->kind == L_NET)
         s += " layers=" + std::to_string(L->net->args.n_layers) + " tiles=" + std::to_string(L->net->args.total_tiles) +
              " ctas=" + std::to_string(L->net->ctas) + " stages=" + std::to_string(L->net->args.stages);

@@ -7,6 +7,11 @@
 //        t = fma(float(acc), m[c], b[c]);  t = fma(float(q_res), r, t);  t = max(t, 0);  q = clip(rint(t), +-127)
 //    -> int8 -> 128-byte-swizzled staging tile -> TMA store.  Same warp roles as conv_f16_tcgen05 (warp 0 activation
 //    producer, warp 3 weight producer, warps 4-11 = two consumer warpgroups doing wgmma and the epilogue), PDL throughout.
+//  * conv_i8_grouped_tcgen05<BN, STAGES, GM>, conv_f8_grouped_tcgen05 -- the same kernel for a grouped convolution with
+//    Cin/g == Cout/g == cpg, cpg | 128 or 128 | cpg: the N tile at n0 reads the span = max(cpg, 128) input channels from
+//    channel (n0 / span) * span against block-diagonal weight rows [Cout][taps][span].  GM = 32 (cpg | 32) / 64 (cpg = 64): K-slice j of a 128-channel block
+//    only reaches output columns 32j ... (resp. 64 (j/2) ...), so each slice is one m64n32k32 (m64n64k32) onto its own
+//    accumulator columns instead of an n128 over the whole tile; GM = 128 (128 | cpg): the dense MMA sequence.
 //  * quantize_h_to_i8_kernel -- fp16 NHWC -> int8 NHWC (channels zero-padded to the 128-channel rows of the INT8 layout)
 //  * avgpool_i8_kernel       -- global average pool: int8 NHWC -> fp16 [N][C]  (exact integer sums)
 //  * output_cast_i8_kernel   -- int8 NHWC -> fp32 NCHW binding (dequantised)
@@ -50,8 +55,9 @@ __host__ __device__ constexpr int conv_i8_smem_layout_bytes(int bn, int stages, 
 
 // The 1-byte convolution, for both element formats: F8 = false is INT8 (s8 operands, exact s32 accumulators, integer
 // requantisation), F8 = true is FP8 (e4m3 operands, fp32 accumulators, satfinite e4m3 conversion).  Producers, ring,
-// padding skips, staging tile and TMA store are the same code.
-template <bool F8, int BN, int STAGES>
+// padding skips, staging tile and TMA store are the same code.  GM: 0 = dense; else grouped (I8ConvArgs::group_span) with
+// GM the N of each slice's MMA -- 32 / 64 (diagonal slices, BN = 128) or 128 (the dense sequence over the tile's span).
+template <bool F8, int BN, int STAGES, int GM = 0>
 __device__ __forceinline__ void conv_1byte_tile(const CUtensorMap& mapA, const CUtensorMap& mapOut, const CUtensorMap& mapRes,
                                                 const I8ConvArgs& p) {
     constexpr int A_STAGE = kI8ASub, B_STAGE = BN * 128;
@@ -59,6 +65,7 @@ __device__ __forceinline__ void conv_1byte_tile(const CUtensorMap& mapA, const C
     constexpr int TILE_BYTES = 128 * BN;     // int8 output / residual tile
     constexpr int NBOX = BN / 128;           // 128-column TMA boxes per tile row
     static_assert(TILE_BYTES <= PIPE_BYTES, "the output staging tile reuses the pipeline buffers");
+    static_assert(GM == 0 || GM == 128 || BN == 128, "diagonal slices: one 128-channel block per N tile");
 
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -85,6 +92,8 @@ __device__ __forceinline__ void conv_1byte_tile(const CUtensorMap& mapA, const C
     int nv = p.cout_real - n0;
     nv = nv >= BN ? BN : (nv <= 0 ? 32 : ((nv + 31) / 32) * 32);
     const uint32_t b_bytes = static_cast<uint32_t>(nv) * 128u;
+    // grouped: the tile's first input channel block (its span's first); dense: 0
+    const int cb0 = GM ? (n0 / p.group_span) * (p.group_span / 128) : 0;
 
     // ---------------- prologue: nothing here depends on the previous kernel's output ----------------
     if (threadIdx.x == 0) {
@@ -135,9 +144,9 @@ __device__ __forceinline__ void conv_1byte_tile(const CUtensorMap& mapA, const C
             if (elect_one_sync()) {
                 mbar_expect_tx(&full_bar[s], A_STAGE + b_bytes);
                 if (tiled)
-                    tma_load_2d(&mapA, &full_bar[s], sA + s * A_STAGE, cur_cb * 128, m0);
+                    tma_load_2d(&mapA, &full_bar[s], sA + s * A_STAGE, (cb0 + cur_cb) * 128, m0);
                 else
-                    tma_load_im2col_4d(&mapA, &full_bar[s], sA + s * A_STAGE, cur_cb * 128, base_w, base_h, img0,
+                    tma_load_im2col_4d(&mapA, &full_bar[s], sA + s * A_STAGE, (cb0 + cur_cb) * 128, base_w, base_h, img0,
                                        static_cast<uint16_t>(cur_sx), static_cast<uint16_t>(cur_r));
             }
             __syncwarp();
@@ -158,14 +167,33 @@ __device__ __forceinline__ void conv_1byte_tile(const CUtensorMap& mapA, const C
             mbar_wait(&full_bar[s], (i / STAGES) & 1);
             const uint32_t a_addr = smem_u32(sA + s * A_STAGE) + wg * 8192;
             const uint32_t b_addr = smem_u32(sB + s * B_STAGE);
-            // all-zero 32-byte slices at the end of a tap's last channel block contribute nothing: not issued
-            const int nj = (cur_cb == p.cblocks - 1) ? p.last_cb_mmas : 4;
-            wgmma_group_upto<4>(nj, [&](int j) {  // up to 4 x (K = 32 bytes) inside one 128-byte swizzle row
-                const uint64_t ad = make_wgmma_desc(a_addr + j * 32, 16, 1024, WG_SW128);
-                const uint64_t bd = make_wgmma_desc(b_addr + j * 32, 16, 1024, WG_SW128);
-                if constexpr (F8) wgmma_e4m3<BN>(acc, ad, bd, (i > 0 || j > 0) ? 1u : 0u);
-                else wgmma_i8<BN>(acc, ad, bd, (i > 0 || j > 0) ? 1u : 0u);
-            });
+            if constexpr (GM == 0 || GM == 128) {
+                // all-zero 32-byte slices at the end of a tap's last channel block contribute nothing: not issued
+                const int nj = (cur_cb == p.cblocks - 1) ? p.last_cb_mmas : 4;
+                wgmma_group_upto<4>(nj, [&](int j) {  // up to 4 x (K = 32 bytes) inside one 128-byte swizzle row
+                    const uint64_t ad = make_wgmma_desc(a_addr + j * 32, 16, 1024, WG_SW128);
+                    const uint64_t bd = make_wgmma_desc(b_addr + j * 32, 16, 1024, WG_SW128);
+                    if constexpr (F8) wgmma_e4m3<BN>(acc, ad, bd, (i > 0 || j > 0) ? 1u : 0u);
+                    else wgmma_i8<BN>(acc, ad, bd, (i > 0 || j > 0) ? 1u : 0u);
+                });
+            } else {
+                // Diagonal slices.  Slice j holds the tile's input channels 32j ... 32j + 31, whose groups are output
+                // channels 32j ... (GM = 32) or 64 (j/2) ... 64 (j/2) + 63 (GM = 64): one MMA of GM columns onto registers
+                // GM/2 * (j / (GM/32)) ..., weight rows from that column on (4 KiB per 32 rows).  Cin == Cout, so the
+                // tile's real input slices are its nv / 32 real output columns' (the rest of the block is padding and not
+                // issued; the registers of columns >= nv are then never written, and the epilogue writes zeros there).
+                // Every register block is first written at K-block 0 by its first slice.
+                constexpr int SPAN = GM / 32;  // slices per MMA
+                wgmma_group_upto<4>(nv / 32, [&](int j) {
+                    const int blk = j / SPAN;
+                    const uint64_t ad = make_wgmma_desc(a_addr + j * 32, 16, 1024, WG_SW128);
+                    const uint64_t bd = make_wgmma_desc(b_addr + blk * (GM * 128) + j * 32, 16, 1024, WG_SW128);
+                    const uint32_t accumulate = (i > 0 || j % SPAN != 0) ? 1u : 0u;
+                    auto& d = *reinterpret_cast<acc_t(*)[GM / 2]>(acc + blk * (GM / 2));
+                    if constexpr (F8) wgmma_e4m3<GM>(d, ad, bd, accumulate);
+                    else wgmma_i8<GM>(d, ad, bd, accumulate);
+                });
+            }
             if constexpr (STAGES == 1) {  // the only stage is refilled for step i+1: retire step i first
                 wgmma_wait<0>();
                 __syncwarp();
@@ -266,12 +294,31 @@ conv_f8_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
     conv_1byte_tile<true, BN, STAGES>(mapA, mapOut, mapRes, p);
 }
 
+// grouped twins (GM: see conv_1byte_tile)
+template <int BN, int STAGES, int GM>
+__global__ void __launch_bounds__(kI8Threads, 1)
+conv_i8_grouped_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapOut,
+                        const __grid_constant__ CUtensorMap mapRes, const I8ConvArgs p) {
+    conv_1byte_tile<false, BN, STAGES, GM>(mapA, mapOut, mapRes, p);
+}
+
+template <int BN, int STAGES, int GM>
+__global__ void __launch_bounds__(kI8Threads, 1)
+conv_f8_grouped_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapOut,
+                        const __grid_constant__ CUtensorMap mapRes, const I8ConvArgs p) {
+    conv_1byte_tile<true, BN, STAGES, GM>(mapA, mapOut, mapRes, p);
+}
+
 int conv_i8_smem_bytes(int bn, int stages, bool residual) { return conv_i8_smem_layout_bytes(bn, stages, residual); }
 bool conv_i8_config_exists(int bn, int stages) {
     return (bn == 128 || bn == 256) && stages >= 1 && stages <= 4 && conv_i8_smem_layout_bytes(bn, stages, true) <= 227 * 1024;
 }
 
 #define B2_FOR_EACH_I8(X) X(128, 1) X(128, 2) X(128, 3) X(128, 4) X(256, 1) X(256, 2) X(256, 3)
+// grouped: the diagonal modes have BN = 128 (a span of 128 channels); the dense mode every (BN, ring depth) above
+#define B2_FOR_EACH_I8_GROUPED(X)                                                                                    \
+    X(128, 1, 32) X(128, 2, 32) X(128, 3, 32) X(128, 4, 32) X(128, 1, 64) X(128, 2, 64) X(128, 3, 64) X(128, 4, 64) \
+    X(128, 1, 128) X(128, 2, 128) X(128, 3, 128) X(128, 4, 128) X(256, 1, 128) X(256, 2, 128) X(256, 3, 128)
 
 int init_conv_i8_kernels() {
     int e = 0;
@@ -284,6 +331,17 @@ int init_conv_i8_kernels() {
         return e;
     B2_FOR_EACH_I8(B2_I8_INIT)
 #undef B2_I8_INIT
+#define B2_I8G_INIT(BN_, ST_, GM_)                                                                                   \
+    if ((e = static_cast<int>(cudaFuncSetAttribute(conv_i8_grouped_tcgen05<BN_, ST_, GM_>,                          \
+                                                   cudaFuncAttributeMaxDynamicSharedMemorySize,                     \
+                                                   conv_i8_smem_layout_bytes(BN_, ST_, true)))))                    \
+        return e;                                                                                                    \
+    if ((e = static_cast<int>(cudaFuncSetAttribute(conv_f8_grouped_tcgen05<BN_, ST_, GM_>,                          \
+                                                   cudaFuncAttributeMaxDynamicSharedMemorySize,                     \
+                                                   conv_i8_smem_layout_bytes(BN_, ST_, true)))))                    \
+        return e;
+    B2_FOR_EACH_I8_GROUPED(B2_I8G_INIT)
+#undef B2_I8G_INIT
     return 0;
 }
 
@@ -301,6 +359,15 @@ int launch_conv_1byte(const I8ConvLaunch& L, cudaStream_t stream) {
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = get_pdl() ? 1 : 0;
+#define B2_I8G_CASE(BN_, ST_, GM_)                                                                                  \
+    if (L.bn == BN_ && L.stages == ST_ && L.group_mode == GM_)                                                      \
+        return static_cast<int>(cudaLaunchKernelEx(&cfg, F8 ? conv_f8_grouped_tcgen05<BN_, ST_, GM_> : conv_i8_grouped_tcgen05<BN_, ST_, GM_>, \
+                                                   L.mapA, L.mapOut, L.mapRes, L.args));
+    if (L.group_mode) {
+        B2_FOR_EACH_I8_GROUPED(B2_I8G_CASE)
+        return static_cast<int>(cudaErrorInvalidValue);
+    }
+#undef B2_I8G_CASE
 #define B2_I8_CASE(BN_, ST_)                                                                                             \
     if (L.bn == BN_ && L.stages == ST_)                                                                                  \
         return static_cast<int>(cudaLaunchKernelEx(&cfg, F8 ? conv_f8_tcgen05<BN_, ST_> : conv_i8_tcgen05<BN_, ST_>, L.mapA, \

@@ -167,6 +167,10 @@ struct I8ConvArgs {
     // padding that need not be computed: the LAST 128-channel block of every tap holds `last_cb_mmas` (1..4) 32-byte MMA
     // slices of real input channels (the rest is zero), and output channels >= cout_real are padding whose result is zero
     int last_cb_mmas, cout_real;
+    // grouped convolution (Cin/g == Cout/g == cpg, cpg | 128 or 128 | cpg; 0 = dense): the input channels an N tile reads,
+    // max(cpg, 128), starting at channel (n0 / group_span) * group_span; cblocks = group_span / 128 and num_kblocks =
+    // taps * cblocks, against block-diagonal weight rows [Cout][taps][group_span] packed as a dense [Cout, K] matrix
+    int group_span;
 };
 struct I8ConvLaunch {
     CUtensorMap mapA;    // int8 activations: 2-D tiled [M, Cin] (box 128 rows x 128 B) or 4-D im2col
@@ -174,6 +178,8 @@ struct I8ConvLaunch {
     CUtensorMap mapRes;  // int8 residual load, same geometry
     I8ConvArgs args;
     int bn, stages, grid_m, grid_n;  // N tile 128 / 256, shared-memory ring depth 2..4
+    int group_mode;  // grouped (args.group_span > 0): the N of each K-slice's MMA, 32 (cpg | 32), 64 (cpg = 64) or 128 (128 | cpg,
+                     // the dense sequence; BN must divide the span); 0 = dense
 };
 int init_conv_i8_kernels();
 bool conv_i8_config_exists(int bn, int stages);

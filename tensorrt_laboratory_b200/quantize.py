@@ -15,6 +15,9 @@ Scheme (what the INT8 kernels of this repository implement, bit for bit):
     convolution; the global average pool reads INT8 and writes fp16: ``h = fp16(fl(float(sum q) * fl(s / HW)))``.
 
 A convolution runs in INT8 when both its channel counts are multiples of 64 (all bottleneck convolutions of the ResNets).
+With ``grouped=True`` a grouped convolution runs in INT8 / FP8 too, when Cin/g == Cout/g == cpg and cpg divides 128 or is a
+multiple of 128 (``builder.grouped_1byte_span``: every grouped layer of ResNeXt-50 32x4d, ResNeXt-101 32x8d / 64x4d, and
+depthwise layers); its weights are scaled per output channel over that channel's taps * cpg weights.
 
 FP8 (``fmt="e4m3"``): the same split and the same layouts, with E4M3 codes (the ``e4m3fn`` format: no infinities,
 subnormals kept, largest value 448) in place of int8 values.  ``e4m3()`` is round-to-nearest-even, saturating to +-448
@@ -80,7 +83,8 @@ def calibrate(lowered: dict, calib_inputs: np.ndarray) -> Dict[str, float]:
             t = op["type"]
             if t == G.OP_CONV:
                 w = torch.from_numpy(np.ascontiguousarray(op["W"], dtype=np.float32)).permute(0, 3, 1, 2).contiguous()
-                y = F.conv2d(a, w, torch.from_numpy(np.asarray(op["bias"], dtype=np.float32)), stride=op["stride"], padding=op["pad"])
+                y = F.conv2d(a, w, torch.from_numpy(np.asarray(op["bias"], dtype=np.float32)), stride=op["stride"], padding=op["pad"],
+                             groups=op.get("groups", 1))
                 if op["residual"] is not None:
                     y = y + blobs[op["residual"]]
                 if op["relu"]:
@@ -108,12 +112,13 @@ def calibrate(lowered: dict, calib_inputs: np.ndarray) -> Dict[str, float]:
 
 
 def quantize_lowered(lowered: dict, calib_inputs: np.ndarray, amax: Optional[Dict[str, float]] = None,
-                     fmt: str = "int8") -> dict:
+                     fmt: str = "int8", grouped: bool = False) -> dict:
     """-> a lowered graph whose eligible convolutions carry INT8 parameters (``Wq`` int8 OHWI, ``m`` / ``b`` fp32 per
     output channel, ``r`` fp32 or None, ``in_scale`` / ``out_scale``), with ``quantize`` ops inserted where an INT8
     convolution reads an fp16 tensor, ``in_scale`` on an average pool that reads INT8, and ``tensor_scales`` {name: s}
-    for every INT8 tensor.  ``lowered`` itself is not modified.  Grouped convolutions have no INT8 path: a graph that
-    contains one is rejected before calibration.
+    for every INT8 tensor.  ``lowered`` itself is not modified.  A graph with a grouped convolution is rejected before
+    calibration unless ``grouped=True``; then every grouped convolution is quantized like a dense one, and one whose
+    geometry the 1-byte kernels do not run (see above) is rejected before calibration instead.
 
     ``fmt="e4m3"``: the FP8 scheme above instead -- ``Wq`` holds E4M3 codes (uint8), and the graph and its quantized
     convolutions are marked ``fp8`` rather than ``int8``."""
@@ -122,10 +127,16 @@ def quantize_lowered(lowered: dict, calib_inputs: np.ndarray, amax: Optional[Dic
     name = FORMATS[fmt]
     fp8 = fmt == "e4m3"
     qmax = E4M3_MAX if fp8 else QMAX
+    from .builder import grouped_1byte_span
     for op in lowered["ops"]:
         if op["type"] == G.OP_CONV and op.get("groups", 1) != 1:
-            raise ValueError(f"conv {op['name']}: {name} grouped convolution is not supported ({op['groups']} groups); "
-                             "build this model in fp16 or fp32")
+            if not grouped:
+                raise ValueError(f"conv {op['name']}: {name} grouped convolution is not supported ({op['groups']} groups); "
+                                 "build this model in fp16 or fp32")
+            if not grouped_1byte_span(op["cin"], op["cout"], op["groups"]):
+                raise ValueError(f"conv {op['name']}: {name} grouped convolution needs Cin/g == Cout/g dividing 128 or a multiple "
+                                 f"of 128 ({op['cin']} -> {op['cout']} channels, {op['groups']} groups); build this model in "
+                                 "fp16 or fp32")
     amax = amax or calibrate(lowered, calib_inputs)
     q = copy.copy(lowered)
     q["tensors"] = dict(lowered["tensors"])
@@ -140,7 +151,7 @@ def quantize_lowered(lowered: dict, calib_inputs: np.ndarray, amax: Optional[Dic
 
     for op in lowered["ops"]:
         op = dict(op)
-        if _is_int8_conv(op):
+        if _is_int8_conv(op) or (op["type"] == G.OP_CONV and op.get("groups", 1) != 1):  # grouped: admitted above
             src = op["input"]
             if src not in scales:  # produced by the fp16 part: quantize it once
                 if src not in alias:

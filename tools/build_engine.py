@@ -9,12 +9,14 @@ examples/ONNX/resnet50/build.py:35-67).
   python tools/build_engine.py --model resnet50 --precision fp8 --batch 8 -o rn50_fp8.plan  (E4M3 bottleneck convolutions)
   python tools/build_engine.py --model resnet50 --batch 8 --tune -o rn50_tuned.plan      (on a GPU box: tactics in the file)
   python tools/build_engine.py --model resnext50 --precision fp16 --batch 8 --tune -o rx50.plan  (ResNeXt-50 32x4d)
+  python tools/build_engine.py --model resnext50 --precision int8 --batch 8 -o rx50_int8.plan  (grouped 1-byte convolutions)
   python tools/build_engine.py --model bert-base --seq 128 --batch 16 [--weights bert.npz] --tune -o bert.plan  (fp16)
   python tools/build_engine.py --model bert-base --seq 384 --batch 16 --remove-padding -o bert_packed.plan  (masked tokens skipped)
 Weights: deterministic synthetic weights (the reference's benchmark engines are weightless too, models/README.md:6-7),
 unless --caffemodel names a binary NetParameter (trtexec --model=...); MNIST and --onnx carry their own weights.
 --precision int8 / fp8: post-training quantization (fp8: E4M3), max-abs calibration on --calib (an .npy [N,C,H,W] fp32) or on
-synthetic images.
+synthetic images.  Grouped convolutions are quantized too when Cin/g == Cout/g divides 128 or is a multiple of 128; a
+model with any other grouped geometry builds in fp16 or fp32 only.
 --tune: time the kernel configurations on this machine's GPU (what trtexec does while building) and store the tactic table
 in the plan file; an engine deserialized from it never tunes at load.
 """
@@ -69,7 +71,7 @@ def main():
         sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
         from tests import helpers
         net, wts, _, _ = helpers.load_mnist_golden()
-    elif a.model == "resnext50":  # 32x4d: grouped 3x3 convolutions (fp16 / fp32 only: INT8 and FP8 have no grouped convolution)
+    elif a.model == "resnext50":  # 32x4d: grouped 3x3 convolutions, cpg 4 ... 32 (every precision)
         net = graph.resnext_caffe(50)
         wts = weights_for(net)
     else:
@@ -84,7 +86,7 @@ def main():
                 calib = np.load(a.calib).astype(np.float32)
             else:
                 calib = weights.synthetic_input(8, chw=tuple(net["input_dims"][1:]), seed=4321)
-            low = quantize.quantize_lowered(low, calib, fmt="e4m3" if prec == builder.PREC_FP8 else "int8")
+            low = quantize.quantize_lowered(low, calib, fmt="e4m3" if prec == builder.PREC_FP8 else "int8", grouped=True)
         blob = builder.build_plan(low, prec, a.batch)
     if a.tune:
         from tensorrt_laboratory_b200 import capi
