@@ -17,6 +17,7 @@ from . import graph as G
 PREC_FP32, PREC_FP16, PREC_INT8, PREC_FP8 = 0, 1, 2, 3
 OP_INPUT_CAST, OP_CONV, OP_MAXPOOL, OP_AVGPOOL, OP_FC, OP_SOFTMAX, OP_OUTPUT_CAST, OP_QUANTIZE = range(8)
 OP_EMBED_LN, OP_LAYERNORM, OP_ATTENTION, OP_POOLER = range(8, 12)   # transformer ops (version-3 plans)
+OP_PATCHIFY, OP_TOKENS, OP_CLS_HEAD = range(12, 15)                  # Vision Transformer ops (version-3 plans)
 CONV_RELU, CONV_PACKED, CONV_INT8, CONV_GELU = 1, 2, 4, 8            # OpRec.relu bits of a convolution
 FLAG_ROWS_OUT, FLAG_PACKED = 1, 2  # OpRecV3.flags: channels-last output cast; op on packed (padding-free) rows
 T_ACT, T_VEC = 0, 1
@@ -506,6 +507,129 @@ def build_bert_plan(cfg=None, weights=None, max_batch: int = 16, seed: int = 0, 
         bindings.append(dict(name=tap, is_input=0, dtype=0, tensor=ti, dims=[S, tensors[ti]["c"]]))
         ops.append(dict(name="cast:" + tap, type=OP_OUTPUT_CAST, inp=ti, res=-1, out=-1, binding=len(bindings) - 1, flags=FLAG_ROWS_OUT | pk))
     default_name = f"bert_l{cfg.layers}_h{H}_s{S}" + ("_packed" if remove_padding else "")
+    return _serialize(tensors, ops, bindings, payload, PREC_FP16, max_batch, name or default_name)
+
+
+def build_vit_plan(cfg=None, weights=None, max_batch: int = 8, seed: int = 0, precision: int = PREC_FP16,
+                   name: Optional[str] = None, taps: Sequence[str] = ()) -> bytes:
+    """Vision Transformer classifier (``vit.VitConfig``; default ViT-B/16 at 224 x 224, 1000 classes) -> fp16 plan
+    (version 3).
+
+    ``weights``: a dict or ``.npz`` path in Hugging Face ``ViTForImageClassification`` names (``vit.load_weights``);
+    default: seeded ``vit.random_weights(cfg, seed)``.  Bindings: fp32 ``data`` [3, image, width] (input, as ResNet's),
+    fp32 ``prob`` [classes] and ``logits`` [classes] (outputs).  Ops: ``OP_PATCHIFY`` (the image as fp16 patch rows
+    [P, 3 p^2], column c p^2 + dy p + dx), the patch projection as a 1x1 GEMM with the [H, 3 p^2] reshape of the
+    convolution weight, ``OP_TOKENS`` (class token and position embeddings, and the packing index), then per pre-LN layer
+    ln1 = LN(x), qkv = GEMM(ln1) (Q, K, V fused as in ``build_bert_plan``), ctx = attention(qkv), x1 = GEMM(ctx) + x,
+    ln2 = LN(x1), f = GELU(GEMM(ln2)), x2 = GEMM(f) + x1; then ``OP_CLS_HEAD`` (final LayerNorm of the class token and the
+    classifier) and the softmax.  Every item has L = P + 1 tokens, so the plan is a packed plan whose index says so:
+    every encoder op runs on packed rows and attention on the variable-length kernels.
+
+    ``taps``: activation tensors (``patches``, ``patch_embed``, ``tokens``, ``l{i}.ln1``, ``l{i}.qkv``, ``l{i}.context``,
+    ``l{i}.attn_sum``, ``l{i}.ln2``, ``l{i}.ffn``, ``l{i}.out``, ``final_ln``) to expose as extra fp32 [rows, C] output
+    bindings of the same names.  ``final_ln`` is the final LayerNorm of every token, computed by an extra LayerNorm op
+    only when it is tapped; the head computes the class token's row with the same arithmetic.
+
+    Geometry: image divisible by p, L <= 512, H = 64 heads <= 1024, FFN a multiple of 64, 3 p^2 a multiple of 64."""
+    from . import vit as Vm
+    cfg = cfg or Vm.VIT_B16
+    for prec, what in ((PREC_FP32, "fp32"), (PREC_INT8, "INT8"), (PREC_FP8, "FP8")):
+        if precision == prec:
+            raise ValueError(f"ViT plans are fp16 only: {what} ViT is not implemented")
+    if precision != PREC_FP16:
+        raise ValueError("precision must be PREC_FP16")
+    H, F, p, L, P = cfg.hidden, cfg.ffn, cfg.patch, cfg.tokens, cfg.patches
+    if cfg.image % p or cfg.width % p:
+        raise ValueError(f"the image size ({cfg.image} x {cfg.width}) must be divisible by the patch size ({p})")
+    if (3 * p * p) % 64:
+        raise ValueError(f"3 p^2 must be a multiple of 64 (p = {p}: 3 p^2 = {3 * p * p}), the K block of the patch GEMM")
+    if L > 512:
+        raise ValueError(f"{L} tokens: a plan takes at most 512 (patches + the class token)")
+    if cfg.heads * 64 != H or H > 1024:
+        raise ValueError(f"the hidden size must be heads * 64 and at most 1024 ({cfg.heads} * 64, H = {H})")
+    if F % 64:
+        raise ValueError(f"the FFN width must be a multiple of 64 (F = {F})")
+    W = Vm.load_weights(weights if weights is not None else Vm.random_weights(cfg, seed), cfg)
+
+    tensors: List[dict] = []
+    ops: List[dict] = []
+    payload = bytearray()
+
+    def add_payload(arr: np.ndarray):
+        while len(payload) % 256:
+            payload.append(0)
+        off = len(payload)
+        raw = np.ascontiguousarray(arr).tobytes()
+        payload.extend(raw)
+        return off, len(raw)
+
+    def act(tname: str, c: int, rows: int = L) -> int:
+        tensors.append(dict(name=tname, kind=T_ACT, h=1, w=rows, c=c, c_phys=c, binding=-1))
+        return len(tensors) - 1
+
+    def vec(tname: str, c: int, binding: int = -1) -> int:
+        tensors.append(dict(name=tname, kind=T_VEC, h=1, w=1, c=c, c_phys=c, binding=binding))
+        return len(tensors) - 1
+
+    def gemm(oname: str, ti: int, to: int, Wm: np.ndarray, b: np.ndarray, res: int = -1, gelu: bool = False, flags: int = FLAG_PACKED):
+        cout, cin = Wm.shape
+        w_off, w_bytes = add_payload(pack_weights_sw128(Wm.astype(np.float16)))
+        b_off, b_bytes = add_payload(b.astype(np.float32))
+        return dict(name=oname, type=OP_CONV, inp=ti, res=res, out=to, binding=-1, k=1, stride=1, pad=0,
+                    relu=CONV_PACKED | (CONV_GELU if gelu else 0), cin=cin, cout=cout, cin_phys=cin, cout_phys=cout, taps=1,
+                    taps_phys=1, w_off=w_off, w_bytes=w_bytes, b_off=b_off, b_bytes=b_bytes, flags=flags)
+
+    def layernorm(oname: str, ti: int, to: int, prefix: str) -> dict:
+        b_off, b_bytes = add_payload(np.concatenate([W[prefix + ".weight"], W[prefix + ".bias"]]).astype(np.float32))
+        return dict(name=oname, type=OP_LAYERNORM, inp=ti, res=-1, out=to, binding=-1, eps=cfg.eps, b_off=b_off, b_bytes=b_bytes,
+                    flags=FLAG_PACKED)
+
+    # bindings: 0 data, 1 prob, 2 logits, then the taps
+    patches, pe = act("patches", 3 * p * p, P), act("patch_embed", H, P)
+    ops.append(dict(name="patchify", type=OP_PATCHIFY, inp=-1, res=-1, out=patches, binding=0, k=p))
+    ops.append(gemm("patch_embed", patches, pe, W["embeddings.patch_embeddings.projection.weight"].reshape(H, 3 * p * p),
+                    W["embeddings.patch_embeddings.projection.bias"], flags=0))
+    x = act("tokens", H)
+    index = vec("packing_index", L + 2)
+    table = np.concatenate([W["embeddings.cls_token"].reshape(1, H), W["embeddings.position_embeddings"].reshape(L, H)])
+    w_off, w_bytes = add_payload(table.astype(np.float16))
+    ops.append(dict(name="tokens", type=OP_TOKENS, inp=pe, res=-1, out=x, out2=index, binding=-1, cin=H, cout=H, cin_phys=H,
+                    cout_phys=H, w_off=w_off, w_bytes=w_bytes, flags=FLAG_PACKED))
+    for i in range(cfg.layers):
+        q = f"encoder.layer.{i}."
+        ln1, qkv, ctx, x1 = act(f"l{i}.ln1", H), act(f"l{i}.qkv", 3 * H), act(f"l{i}.context", H), act(f"l{i}.attn_sum", H)
+        ln2, f, x2 = act(f"l{i}.ln2", H), act(f"l{i}.ffn", F), act(f"l{i}.out", H)
+        Wqkv = np.concatenate([W[q + f"attention.attention.{m}.weight"] for m in ("query", "key", "value")])
+        bqkv = np.concatenate([W[q + f"attention.attention.{m}.bias"] for m in ("query", "key", "value")])
+        ops.append(layernorm(f"l{i}.ln1", x, ln1, q + "layernorm_before"))
+        ops.append(gemm(f"l{i}.qkv", ln1, qkv, Wqkv, bqkv))
+        ops.append(dict(name=f"l{i}.attention", type=OP_ATTENTION, inp=qkv, res=index, out=ctx, binding=-1, heads=cfg.heads,
+                        flags=FLAG_PACKED))
+        ops.append(gemm(f"l{i}.attn_out", ctx, x1, W[q + "attention.output.dense.weight"], W[q + "attention.output.dense.bias"], res=x))
+        ops.append(layernorm(f"l{i}.ln2", x1, ln2, q + "layernorm_after"))
+        ops.append(gemm(f"l{i}.ffn1", ln2, f, W[q + "intermediate.dense.weight"], W[q + "intermediate.dense.bias"], gelu=True))
+        ops.append(gemm(f"l{i}.ffn2", f, x2, W[q + "output.dense.weight"], W[q + "output.dense.bias"], res=x1))
+        x = x2
+    if "final_ln" in taps:
+        ops.append(layernorm("final_ln", x, act("final_ln", H), "layernorm"))
+    prob, logits = vec("prob", cfg.classes, binding=1), vec("logits", cfg.classes, binding=2)
+    w_off, w_bytes = add_payload(W["classifier.weight"].astype(np.float16))
+    b_off, b_bytes = add_payload(np.concatenate([W["layernorm.weight"], W["layernorm.bias"], W["classifier.bias"]]).astype(np.float32))
+    ops.append(dict(name="cls_head", type=OP_CLS_HEAD, inp=x, res=-1, out=logits, binding=-1, cin=H, cout=cfg.classes, cin_phys=H,
+                    cout_phys=cfg.classes, eps=cfg.eps, w_off=w_off, w_bytes=w_bytes, b_off=b_off, b_bytes=b_bytes, flags=FLAG_PACKED))
+    ops.append(dict(name="softmax", type=OP_SOFTMAX, inp=logits, res=-1, out=prob, binding=-1))
+    bindings = [dict(name="data", is_input=1, dtype=0, tensor=patches, dims=[3, cfg.image, cfg.width]),
+                dict(name="prob", is_input=0, dtype=0, tensor=prob, dims=[cfg.classes]),
+                dict(name="logits", is_input=0, dtype=0, tensor=logits, dims=[cfg.classes])]
+    for tap in taps:
+        ti = next((k for k, t in enumerate(tensors) if t["name"] == tap and t["kind"] == T_ACT), None)
+        if ti is None:
+            raise ValueError(f"tap {tap!r}: no such activation tensor")
+        bindings.append(dict(name=tap, is_input=0, dtype=0, tensor=ti, dims=[tensors[ti]["w"], tensors[ti]["c"]]))
+        front = ti in (patches, pe)  # made before the tokens op: plain rows, not packed ones
+        ops.append(dict(name="cast:" + tap, type=OP_OUTPUT_CAST, inp=ti, res=-1, out=-1, binding=len(bindings) - 1,
+                        flags=FLAG_ROWS_OUT | (0 if front else FLAG_PACKED)))
+    default_name = f"vit_l{cfg.layers}_h{H}_p{p}_i{cfg.image}" + (f"x{cfg.width}" if cfg.width != cfg.image else "")
     return _serialize(tensors, ops, bindings, payload, PREC_FP16, max_batch, name or default_name)
 
 

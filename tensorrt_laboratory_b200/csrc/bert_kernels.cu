@@ -12,6 +12,9 @@
 //  Packed (padding-free) plans: embed_ln_packed_kernel writes only the valid tokens, to consecutive rows, and the packing
 //  index; the attention kernels' VARLEN variants run each item over its own rows; output_unpack_rows_kernel and the
 //  pooler read packed rows through the index (DESIGN.md, "Packed BERT").
+//  Vision Transformer plans (DESIGN.md, "ViT"): patchify_kernel turns the fp32 image into fp16 patch rows, tokens_kernel
+//  adds the class token and position embeddings and writes the packing index of equal-length items, cls_head_kernel
+//  runs the final LayerNorm on each class token and the classifier.
 //
 // Numerics (DESIGN.md, "BERT numerics"): every sum below runs in a fixed order -- a lane adds its own elements in index
 // order, then the warp combines lanes with an xor butterfly -- so a row's result does not depend on the batch, the grid
@@ -646,6 +649,140 @@ __global__ void output_unpack_rows_kernel(const __half* __restrict__ src, float*
     dst[idx] = pr < 0 ? 0.0f : __half2float(src[static_cast<long long>(pr) * C_phys + (idx - r * C)]);
 }
 
+// ---- Vision Transformer front and back end (DESIGN.md, "ViT") -----------------------------------------------------------
+// fp32 NCHW image [N][3][Himg][Wimg] -> fp16 patch rows [N * P][3 p^2]: patch t = (py, px) in row-major order, element
+// (c, dy, dx) at column c p^2 + dy p + dx (the flattening of a [H, 3, p, p] weight).  One thread per 8 consecutive floats of
+// an image row (p % 8 == 0): two 16-byte loads, coalesced along the row, and one 16-byte store.  Grid-stride, so a cast
+// that reads zero-copy host memory may run on a capped grid (the input cast's `max_blocks`).
+__global__ void patchify_kernel(const float* __restrict__ src, uint4* __restrict__ dst, int N, int Himg, int Wimg, int p) {
+    pdl_launch_dependents();
+    pdl_wait();
+    const int w8 = Wimg >> 3, pw = Wimg / p, P = (Himg / p) * pw, K = 3 * p * p;
+    const long long total = static_cast<long long>(N) * 3 * Himg * w8, step = static_cast<long long>(gridDim.x) * blockDim.x;
+    for (long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; idx < total; idx += step) {
+        const int x = static_cast<int>(idx % w8) * 8;
+        const long long t = idx / w8;
+        const int y = static_cast<int>(t % Himg);
+        const long long nc = t / Himg;
+        const int c = static_cast<int>(nc % 3), n = static_cast<int>(nc / 3);
+        const float4* s = reinterpret_cast<const float4*>(src + (static_cast<size_t>(nc) * Himg + y) * Wimg + x);
+        const float4 a = __ldg(s), b = __ldg(s + 1);
+        uint4 o;
+        __half2* o2 = reinterpret_cast<__half2*>(&o);
+        o2[0] = __floats2half2_rn(a.x, a.y);
+        o2[1] = __floats2half2_rn(a.z, a.w);
+        o2[2] = __floats2half2_rn(b.x, b.y);
+        o2[3] = __floats2half2_rn(b.z, b.w);
+        const int row = n * P + (y / p) * pw + x / p;
+        const int col = c * p * p + (y % p) * p + x % p;
+        dst[(static_cast<size_t>(row) * K + col) >> 3] = o;
+    }
+}
+
+// Token rows x [N][L][C] from the patch projection y [N][L - 1][C]: row 0 = fp16(cls + pos_0), row t = fp16(y[t - 1] +
+// pos_t), sums in fp32; `table` = fp16 [cls | pos_0 ... pos_{L-1}] rows.  Also the packing index of a batch whose items
+// all have L tokens: pos_map[r] = r, seq_off[n] = n L (n = 0 ... N).  One warp per row; the table rows are constants and
+// are read before the dependency wait.
+__global__ void __launch_bounds__(32 * kRowWarps) tokens_kernel(const __half* __restrict__ y, __half* __restrict__ x, int* __restrict__ pack,
+                                                             const __half* __restrict__ table, int N, int L, int C) {
+    const int lane = threadIdx.x & 31;
+    const long long row = static_cast<long long>(blockIdx.x) * kRowWarps + (threadIdx.x >> 5);
+    const bool valid = row < static_cast<long long>(N) * L;
+    const int n = valid ? static_cast<int>(row / L) : 0, t = valid ? static_cast<int>(row - static_cast<long long>(n) * L) : 0;
+    const int nv = (C / 8 - lane + 31) / 32;
+    float pos[kLnMaxVec][8], cls[kLnMaxVec][8];
+    if (valid) {
+        const uint4* pr = reinterpret_cast<const uint4*>(table + static_cast<size_t>(1 + t) * C);
+        const uint4* cr = reinterpret_cast<const uint4*>(table);
+#pragma unroll
+        for (int k = 0; k < kLnMaxVec; ++k)
+            if (k < nv) {
+                unpack8(__ldg(pr + lane + 32 * k), pos[k]);
+                if (t == 0) unpack8(__ldg(cr + lane + 32 * k), cls[k]);
+            }
+    }
+    pdl_launch_dependents();
+    pdl_wait();
+    if (!valid) return;
+    if (lane == 0) pack[row] = static_cast<int>(row);
+    int* seq_off = pack + static_cast<size_t>(N) * L;
+    if (lane == 1 && t == 0) seq_off[n] = n * L;
+    if (lane == 1 && row == static_cast<long long>(N) * L - 1) seq_off[N] = N * L;
+    const uint4* src = reinterpret_cast<const uint4*>(y + (static_cast<size_t>(n) * (L - 1) + (t > 0 ? t - 1 : 0)) * C);
+    uint4* dst = reinterpret_cast<uint4*>(x + static_cast<size_t>(row) * C);
+#pragma unroll
+    for (int k = 0; k < kLnMaxVec; ++k) {
+        if (k >= nv) continue;
+        float a[8];
+        if (t == 0) {
+#pragma unroll
+            for (int e = 0; e < 8; ++e) a[e] = cls[k][e];
+        } else {
+            unpack8(src[lane + 32 * k], a);
+        }
+        uint4 o;
+        __half2* o2 = reinterpret_cast<__half2*>(&o);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) o2[i] = __floats2half2_rn(__fadd_rn(a[2 * i], pos[k][2 * i]), __fadd_rn(a[2 * i + 1], pos[k][2 * i + 1]));
+        dst[lane + 32 * k] = o;
+    }
+}
+
+// Classifier head: logits[n][j] = b[j] + W[j] . LN(x[n][0]).  One warp per class j, its weight row in registers (loaded
+// before the dependency wait); per group of kHeadWarps items, warp w computes the LayerNorm of item w's class-token row
+// into shared memory exactly as layernorm_h8_kernel does (fp16 result), once per CTA.  The dot product runs in the
+// pooler's order: each lane sums its own products in index order, the warp adds lanes by an xor butterfly, then + b[j].
+// `gbb` = fp32 [gamma C | beta C | b classes].  pos_map (packed plans): the class token of item n is row pos_map[n * S].
+constexpr int kHeadWarps = 8;
+__global__ void __launch_bounds__(32 * kHeadWarps) cls_head_kernel(const __half* __restrict__ x, const __half* __restrict__ w,
+                                                                 const float* __restrict__ gbb, float* __restrict__ out, int N, int S, int C,
+                                                                 int classes, float eps, const int* __restrict__ pos_map) {
+    __shared__ __align__(16) __half h[kHeadWarps][32 * kLnMaxVec * 8];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int j = blockIdx.x * kHeadWarps + warp;
+    const int nv = (C / 8 - lane + 31) / 32;
+    float wr[kLnMaxVec][8];
+    if (j < classes) {
+        const uint4* wrow = reinterpret_cast<const uint4*>(w + static_cast<size_t>(j) * C);
+#pragma unroll
+        for (int k = 0; k < kLnMaxVec; ++k)
+            if (k < nv) unpack8(__ldg(wrow + lane + 32 * k), wr[k]);
+    }
+    pdl_launch_dependents();
+    pdl_wait();
+    const float bj = j < classes ? __ldg(gbb + 2 * C + j) : 0.f;
+    for (int n0 = 0; n0 < N; n0 += kHeadWarps) {
+        const int items = min(kHeadWarps, N - n0);
+        if (warp < items) {
+            const int n = n0 + warp;
+            const long long r = pos_map ? pos_map[static_cast<size_t>(n) * S] : static_cast<long long>(n) * S;
+            const uint4* src = reinterpret_cast<const uint4*>(x + r * C);
+            float v[kLnMaxVec][8];
+#pragma unroll
+            for (int k = 0; k < kLnMaxVec; ++k)
+                if (k < nv) unpack8(src[lane + 32 * k], v[k]);
+            ln_row_store(v, nv, lane, C, eps, gbb, gbb + C, h[warp], C);
+        }
+        __syncthreads();
+        if (j < classes)
+            for (int i = 0; i < items; ++i) {
+                const uint4* hrow = reinterpret_cast<const uint4*>(h[i]);
+                float acc = 0.f;
+#pragma unroll
+                for (int k = 0; k < kLnMaxVec; ++k) {
+                    if (k >= nv) continue;
+                    float v[8];
+                    unpack8(hrow[lane + 32 * k], v);
+#pragma unroll
+                    for (int e = 0; e < 8; ++e) acc = __fadd_rn(acc, __fmul_rn(wr[k][e], v[e]));
+                }
+                acc = warp_sum(acc);
+                if (lane == 0) out[static_cast<size_t>(n0 + i) * classes + j] = __fadd_rn(acc, bj);
+            }
+        __syncthreads();
+    }
+}
+
 }  // namespace
 
 int launch_embed_ln(const EmbedArgs& a, cudaStream_t stream) {
@@ -727,6 +864,28 @@ int launch_output_unpack_rows(const __half* src, float* dst, const int* pos_map,
     const long long total = rows * C;
     return launch_pdl(output_unpack_rows_kernel, dim3(static_cast<unsigned>((total + 255) / 256)), dim3(256), 0, stream, src, dst, pos_map,
                       rows, C, C_phys);
+}
+
+int launch_patchify(const float* src, __half* dst, int N, int Himg, int Wimg, int p, int max_blocks, cudaStream_t stream) {
+    if (p < 8 || p % 8 || Himg % p || Wimg % p) return static_cast<int>(cudaErrorInvalidValue);
+    const long long total = static_cast<long long>(N) * 3 * Himg * (Wimg / 8);
+    unsigned blocks = static_cast<unsigned>((total + 255) / 256);
+    if (max_blocks > 0 && blocks > static_cast<unsigned>(max_blocks)) blocks = static_cast<unsigned>(max_blocks);
+    return launch_pdl(patchify_kernel, dim3(blocks), dim3(256), 0, stream, src, reinterpret_cast<uint4*>(dst), N, Himg, Wimg, p);
+}
+
+int launch_tokens(const __half* y, __half* x, int* pack, const __half* table, int N, int L, int C, cudaStream_t stream) {
+    if (C % 8 || C > 32 * kLnMaxVec * 8 || L < 2) return static_cast<int>(cudaErrorInvalidValue);
+    const long long rows = static_cast<long long>(N) * L;
+    return launch_pdl(tokens_kernel, dim3(static_cast<unsigned>((rows + kRowWarps - 1) / kRowWarps)), dim3(32 * kRowWarps), 0, stream, y, x,
+                      pack, table, N, L, C);
+}
+
+int launch_cls_head(const __half* x, const __half* w, const float* gbb, float* out, int N, int S, int C, int classes, float eps,
+                    const int* pos_map, cudaStream_t stream) {
+    if (C % 8 || C > 32 * kLnMaxVec * 8) return static_cast<int>(cudaErrorInvalidValue);
+    return launch_pdl(cls_head_kernel, dim3(static_cast<unsigned>((classes + kHeadWarps - 1) / kHeadWarps)), dim3(32 * kHeadWarps), 0, stream, x,
+                      w, gbb, out, N, S, C, classes, eps, pos_map);
 }
 
 }  // namespace b2k

@@ -143,7 +143,15 @@ struct Binding {
 
 enum LKind { L_INPUT_CAST, L_CONV_TC, L_CONV_SIMT, L_MAXPOOL, L_AVGPOOL, L_FC, L_SOFTMAX, L_OUTPUT_CAST, L_NET, L_TAIL, L_QUANTIZE, L_CONV_I8, L_AVGPOOL_I8, L_OUTPUT_CAST_I8,
              L_EMBED_LN, L_LAYERNORM, L_ATTENTION, L_POOLER, L_OUTPUT_ROWS, L_OUTPUT_UNPACK, L_QUANTIZE_F8, L_CONV_F8, L_AVGPOOL_F8,
-             L_OUTPUT_CAST_F8 };
+             L_OUTPUT_CAST_F8, L_PATCHIFY, L_TOKENS, L_CLS_HEAD };
+
+// Attention kernel of a packed plan's S tokens: the smallest instantiated sequence length S_k >= S (the variable-length
+// kernels attend each item over its own rows, so the rows S ... S_k - 1 of an item's tile are never used)
+int attention_keys(int S) {
+    for (int sk : {64, 128, 256, 384, 512})
+        if (S <= sk) return sk;
+    return 0;
+}
 
 // A run of consecutive tcgen05 convolution layers executed by ONE persistent kernel (net_kernel.cu): device-side layer
 // table, dependency ranges and arrival counters live in one allocation owned by the plan.
@@ -384,7 +392,9 @@ int validate_transformer_op(b2_engine* e, const Op& op) {
                 return fail(B2_EINVAL, "plan: attention %s: needs a fused fp16 QKV input of 3 x %u channels", nm, to.c);
             if (ti.h != 1 || to.h != 1 || ti.w != to.w || tm.kind != T_VEC || tm.c != ((op.flags & kOpPacked) ? ti.w + 2 : ti.w))
                 return fail(B2_EINVAL, "plan: attention %s: S does not match between QKV, output and mask", nm);
-            if (ti.w != 64 && (ti.w == 0 || ti.w % 128 || ti.w > 512))
+            if ((op.flags & kOpPacked) && (ti.w == 0 || ti.w > 512))
+                return fail(B2_EINVAL, "plan: packed attention %s: S = %u (1 ... 512)", nm, ti.w);
+            if (!(op.flags & kOpPacked) && ti.w != 64 && (ti.w == 0 || ti.w % 128 || ti.w > 512))
                 return fail(B2_EINVAL, "plan: attention %s: S = %u (64, or a multiple of 128 up to 512)", nm, ti.w);
             if (r.w_bytes || r.b_bytes) return fail(B2_EINVAL, "plan: attention %s carries no weights", nm);
             e->flops_per_item += 4.0 * double(ti.w) * ti.w * to.c;  // Q K^T and P V
@@ -400,9 +410,59 @@ int validate_transformer_op(b2_engine* e, const Op& op) {
             e->flops_per_item += 2.0 * ti.c * ti.c;
             break;
         }
+        case OP_PATCHIFY: {  // the image binding's geometry is checked with the bindings (validate_patchify_binding)
+            const Tensor& to = e->tensors[r.out];
+            const uint32_t p = r.k;
+            if (r.in != -1 || p < 8 || p % 8 || to.kind != T_ACT || to.scale != 0.f || to.h != 1 || to.c != 3 * p * p || to.c_phys != to.c)
+                return fail(B2_EINVAL, "plan: patchify %s: patch size %u needs p %% 8 == 0 and an fp16 [1, P, 3 p^2 = %u] output", nm, p,
+                            3 * p * p);
+            if (r.w_bytes || r.b_bytes || op.flags) return fail(B2_EINVAL, "plan: patchify %s carries no weights and no flags", nm);
+            break;
+        }
+        case OP_TOKENS: {
+            const Tensor& ti = e->tensors[r.in];
+            const Tensor& to = e->tensors[r.out];
+            const Tensor& tm = e->tensors[op.out2];
+            if (!(op.flags & kOpPacked)) return fail(B2_EINVAL, "plan: tokens %s: writes a packing index, so it must be marked packed", nm);
+            if (!act_ok(ti) || !act_ok(to) || ti.h != 1 || to.h != 1 || ti.c != to.c || ti.c_phys != ti.c || to.c_phys != to.c ||
+                to.w != ti.w + 1 || to.w > 512)
+                return fail(B2_EINVAL, "plan: tokens %s: needs fp16 [1, P, H] in and [1, P + 1 <= 512, H] out, H %% 8 == 0, H <= 1024", nm);
+            if (tm.kind != T_VEC || tm.c != to.w + 2 || tm.binding >= 0)
+                return fail(B2_EINVAL, "plan: tokens %s: the packing index must be a [L + 2 = %u] vector, not [%u]", nm, to.w + 2, tm.c);
+            if (r.w_bytes != uint64_t(to.w + 1) * to.c * 2 || r.b_bytes)
+                return fail(B2_EINVAL, "plan: tokens %s: class-token and position tables must be H + L x H = %u fp16 values", nm, (to.w + 1) * to.c);
+            e->flops_per_item += double(to.w) * to.c;
+            break;
+        }
+        case OP_CLS_HEAD: {
+            const Tensor& ti = e->tensors[r.in];
+            const Tensor& to = e->tensors[r.out];
+            if (!act_ok(ti) || ti.h != 1 || ti.c_phys != ti.c || r.cin != ti.c || r.cout == 0 || to.kind != T_VEC || to.c != r.cout)
+                return fail(B2_EINVAL, "plan: cls_head %s: needs an fp16 [1, S, H] input and an fp32 [classes] output", nm);
+            if (r.w_bytes != uint64_t(r.cout) * ti.c * 2 || r.b_bytes != (2 * uint64_t(ti.c) + r.cout) * 4)
+                return fail(B2_EINVAL, "plan: cls_head %s: weight must be classes x H = %u x %u fp16, gamma / beta / bias %u fp32", nm, r.cout, ti.c,
+                            2 * ti.c + r.cout);
+            if (!(op.eps >= 0.f && op.eps < 1.f)) return fail(B2_EINVAL, "plan: cls_head %s: bad eps", nm);
+            e->flops_per_item += 2.0 * r.cout * ti.c;
+            break;
+        }
         default:
             break;
     }
+    return B2_OK;
+}
+
+// OP_PATCHIFY reads an fp32 input binding [3, Himg, Wimg] whose patches fill its output tensor
+int validate_patchify_binding(const b2_engine* e, const Op& op) {
+    const b2plan::OpRec& r = op.r;
+    const Binding& b = e->bindings[size_t(r.binding)];
+    const Tensor& to = e->tensors[size_t(r.out)];
+    const int p = int(r.k);
+    if (!b.is_input || b.dtype != B2_DT_FLOAT || b.nd != 3 || b.dims[0] != 3 || b.dims[1] <= 0 || b.dims[2] <= 0)
+        return fail(B2_EINVAL, "plan: patchify %s: binding %s must be an fp32 input image [3, H, W]", op.name.c_str(), b.name.c_str());
+    if (b.dims[1] % p || b.dims[2] % p || uint32_t((b.dims[1] / p) * (b.dims[2] / p)) != to.w)
+        return fail(B2_EINVAL, "plan: patchify %s: a %d x %d image in %d x %d patches does not give the %u patch rows of tensor %s", op.name.c_str(),
+                    b.dims[1], b.dims[2], p, p, to.w, to.name.c_str());
     return B2_OK;
 }
 
@@ -413,29 +473,52 @@ int validate_packed_ops(b2_engine* e) {
     int embed = -1;
     for (size_t i = 0; i < e->ops.size(); ++i) {
         const Op& op = e->ops[i];
-        if (!(op.flags & kOpPacked) || op.r.type != OP_EMBED_LN) continue;
+        if (!(op.flags & kOpPacked) || (op.r.type != OP_EMBED_LN && op.r.type != OP_TOKENS)) continue;
         if (embed >= 0) return fail(B2_EINVAL, "plan: packed embedding %s: a plan has one packed embedding", op.name.c_str());
         embed = int(i);
     }
     if (embed < 0) {
         for (const Op& op : e->ops)
             if (op.flags & kOpPacked) return fail(B2_EINVAL, "plan: op %s is marked packed in a plan without a packed embedding", op.name.c_str());
+        for (const Op& op : e->ops)
+            if (op.r.type == OP_PATCHIFY || op.r.type == OP_CLS_HEAD)
+                return fail(B2_EINVAL, "plan: op %s belongs to a ViT plan, which has a packed OP_TOKENS", op.name.c_str());
         return B2_OK;
     }
     const Op& eo = e->ops[size_t(embed)];
     const uint32_t S = e->tensors[eo.r.out].w;
+    // ViT plans (OP_TOKENS): the patch front end -- one OP_PATCHIFY and one unpacked dense 1x1 GEMM -- runs before the
+    // embedding; after it, the classifier's softmax and channels-last casts of the patch tensors run unpacked
+    const bool vit = eo.r.type == OP_TOKENS;
+    int front_patchify = 0, front_gemm = 0;
+    auto made_before_embed = [&](int t) {
+        for (int k = 0; k < embed; ++k)
+            if (e->ops[size_t(k)].r.out == t) return true;
+        return false;
+    };
     for (size_t i = 0; i < e->ops.size(); ++i) {
         const Op& op = e->ops[i];
         const OpRec& r = op.r;
         const char* nm = op.name.c_str();
         const bool packed = (op.flags & kOpPacked) != 0;
+        if (vit && int(i) < embed) {
+            const bool dense1x1 = r.type == OP_CONV && r.k == 1 && !r.kw && r.stride == 1 && !r.pad_ && (r.relu & kConvPacked) &&
+                                  !(r.relu & (kConvInt8 | kConvRelu | kConvGelu)) && op.groups == 1;
+            if (!packed && r.type == OP_PATCHIFY && !front_patchify++) continue;
+            if (!packed && dense1x1 && !front_gemm++) continue;
+            return fail(B2_EINVAL, "plan: op %s runs before the packed embedding %s (a ViT plan runs one OP_PATCHIFY and one unpacked "
+                        "dense 1x1 GEMM there)", nm, eo.name.c_str());
+        }
+        if (vit && !packed && (r.type == OP_SOFTMAX || (r.type == OP_OUTPUT_CAST && (op.flags & kOpRowsOut) && made_before_embed(r.in))))
+            continue;
         const bool rowwise = r.type == OP_CONV || r.type == OP_LAYERNORM || r.type == OP_ATTENTION || r.type == OP_POOLER ||
-                             (r.type == OP_OUTPUT_CAST && (op.flags & kOpRowsOut)) || r.type == OP_EMBED_LN;
+                             (r.type == OP_OUTPUT_CAST && (op.flags & kOpRowsOut)) || r.type == OP_EMBED_LN || r.type == OP_TOKENS ||
+                             r.type == OP_CLS_HEAD;
         if (!rowwise)
             return fail(B2_EINVAL, "plan: op %s: a packed plan holds transformer ops, GEMMs and channels-last output casts only", nm);
         if (!packed) return fail(B2_EINVAL, "plan: op %s of a packed plan is not marked packed", nm);
-        if (r.type != OP_EMBED_LN && int(i) < embed) return fail(B2_EINVAL, "plan: op %s runs before the packed embedding", nm);
-        const int t = r.type == OP_EMBED_LN ? r.out : r.in;
+        if (int(i) < embed) return fail(B2_EINVAL, "plan: op %s runs before the packed embedding", nm);
+        const int t = (r.type == OP_EMBED_LN || r.type == OP_TOKENS) ? r.out : r.in;
         const Tensor& tt = e->tensors[size_t(t)];
         if (tt.kind != T_ACT || tt.h != 1 || tt.w != S)
             return fail(B2_EINVAL, "plan: packed op %s: its tensor must be [1, S = %u, C] like the embedding's", nm, S);
@@ -528,17 +611,18 @@ int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** pa
         }
         op.name = fixed_str(op.r.name, 64);
         const OpRec& r = op.r;
-        if (r.type > OP_POOLER) return fail(B2_EINVAL, "plan: op %s has unknown type %u", op.name.c_str(), r.type);
+        if (r.type > OP_CLS_HEAD) return fail(B2_EINVAL, "plan: op %s has unknown type %u", op.name.c_str(), r.type);
         const bool transformer_op = r.type >= OP_EMBED_LN;
         if (transformer_op && (!v3 || h.precision != B2_PREC_FP16))
             return fail(B2_EINVAL, "plan: op %s: transformer ops need a version-3 fp16 plan", op.name.c_str());
-        const bool in_opt = r.type == OP_INPUT_CAST || r.type == OP_EMBED_LN, out_opt = r.type == OP_OUTPUT_CAST;
-        if (!tensor_ok(r.in, in_opt) || !tensor_ok(r.out, out_opt) || !tensor_ok(r.res, true) || !tensor_ok(op.out2, r.type != OP_EMBED_LN))
+        const bool in_opt = r.type == OP_INPUT_CAST || r.type == OP_EMBED_LN || r.type == OP_PATCHIFY, out_opt = r.type == OP_OUTPUT_CAST;
+        const bool has_out2 = r.type == OP_EMBED_LN || r.type == OP_TOKENS;
+        if (!tensor_ok(r.in, in_opt) || !tensor_ok(r.out, out_opt) || !tensor_ok(r.res, true) || !tensor_ok(op.out2, !has_out2))
             return fail(B2_EINVAL, "plan: op %s references a missing tensor", op.name.c_str());
-        if (r.type != OP_EMBED_LN && (op.out2 != -1 || op.binding2 != -1 || op.binding3 != -1))
-            return fail(B2_EINVAL, "plan: op %s: second output / extra bindings exist for the embedding op only", op.name.c_str());
+        if ((!has_out2 && op.out2 != -1) || (r.type != OP_EMBED_LN && (op.binding2 != -1 || op.binding3 != -1)))
+            return fail(B2_EINVAL, "plan: op %s: second output / extra bindings exist for the embedding ops only", op.name.c_str());
         if (r.type == OP_EMBED_LN && r.in != -1) return fail(B2_EINVAL, "plan: embedding %s reads bindings, not a tensor", op.name.c_str());
-        if ((r.type == OP_INPUT_CAST || r.type == OP_OUTPUT_CAST) && (r.binding < 0 || r.binding >= int(h.n_bindings)))
+        if ((r.type == OP_INPUT_CAST || r.type == OP_OUTPUT_CAST || r.type == OP_PATCHIFY) && (r.binding < 0 || r.binding >= int(h.n_bindings)))
             return fail(B2_EINVAL, "plan: cast op %s has a bad binding", op.name.c_str());
         if (r.w_off > h.payload_bytes || r.w_bytes > h.payload_bytes - r.w_off || r.b_off > h.payload_bytes ||
             r.b_bytes > h.payload_bytes - r.b_off)
@@ -677,6 +761,9 @@ int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** pa
             return fail(B2_EINVAL, "plan: cast op %s reads int32 binding %s (int32 bindings feed the embedding op only)", op.name.c_str(),
                         b.name.c_str());
     }
+    for (const Op& op : e->ops)
+        if (op.r.type == OP_PATCHIFY)
+            if (int rc = validate_patchify_binding(e, op)) return rc;
     // int32 bindings: the token inputs of OP_EMBED_LN, [S] per item, and nothing else reads them
     std::vector<int> int32_readers(e->bindings.size(), 0);
     for (const Op& op : e->ops) {
@@ -2026,6 +2113,8 @@ int build_plan(b2_context* c, int batch, Plan** out) {
                 else a.mask_add = reinterpret_cast<const float*>(tptr(r.res));
                 a.out = reinterpret_cast<__half*>(tptr(r.out));
                 a.N = batch, a.S = int(ti.w), a.heads = op.heads, a.H = int(to.c), a.out_pitch = int(to.c_phys);
+                if (op.flags & b2plan::kOpPacked) a.S = attention_keys(int(ti.w));
+                L.W = int(ti.w);
                 int rc = make_map_2d(&a.mapQKV, tptr(r.in), ti.c_phys, uint64_t(batch) * ti.w, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B);
                 if (rc) return rc;
                 L.flops = 4.0 * batch * double(ti.w) * ti.w * to.c;
@@ -2044,6 +2133,44 @@ int build_plan(b2_context* c, int batch, Plan** out) {
                 L.W = int(ti.w), L.C = int(ti.c), L.C_phys = int(ti.c_phys);
                 if (op.flags & b2plan::kOpPacked) L.pos_map = pos_map;
                 L.flops = 2.0 * batch * ti.c * ti.c;
+                L.bytes = double(r.w_bytes) + double(batch) * (ti.c * 2.0 + to.item_bytes);
+                break;
+            }
+            case b2plan::OP_PATCHIFY: {
+                const Tensor& to = e->tensors[r.out];
+                const Binding& b = e->bindings[r.binding];
+                L.kind = L_PATCHIFY;
+                L.in_binding = r.binding;
+                L.out = tptr(r.out);
+                L.H = b.dims[1], L.W = b.dims[2], L.k = int(r.k);
+                L.max_blocks = c->input_ctas;
+                L.bytes = double(batch) * (3.0 * b.dims[1] * b.dims[2] * 4 + to.item_bytes);
+                break;
+            }
+            case b2plan::OP_TOKENS: {
+                const Tensor& ti = e->tensors[r.in];
+                const Tensor& to = e->tensors[r.out];
+                L.kind = L_TOKENS;
+                L.in = tptr(r.in), L.out = tptr(r.out);
+                L.w = e->d_payload + r.w_off;
+                L.pos_map = pos_map;  // the packing index this op writes
+                L.W = int(to.w), L.C = int(to.c);
+                L.flops = double(batch) * to.w * to.c;
+                L.bytes = double(batch) * (ti.item_bytes + to.item_bytes + (to.w + 2) * 4.0) + double(r.w_bytes);
+                break;
+            }
+            case b2plan::OP_CLS_HEAD: {
+                const Tensor& ti = e->tensors[r.in];
+                const Tensor& to = e->tensors[r.out];
+                L.kind = L_CLS_HEAD;
+                L.in = tptr(r.in);
+                L.out = tptr(r.out);
+                L.out_binding = to.binding;
+                L.w = e->d_payload + r.w_off;
+                L.bias = reinterpret_cast<const float*>(e->d_payload + r.b_off);
+                L.W = int(ti.w), L.C = int(ti.c), L.Cout = int(r.cout), L.eps = op.eps;
+                if (op.flags & b2plan::kOpPacked) L.pos_map = pos_map;
+                L.flops = 2.0 * batch * double(r.cout) * ti.c;
                 L.bytes = double(r.w_bytes) + double(batch) * (ti.c * 2.0 + to.item_bytes);
                 break;
             }
@@ -2142,6 +2269,14 @@ int run_launch(const b2_engine* e, const Launch& L, void* const* bindings, cudaS
         case L_OUTPUT_UNPACK:
             return b2k::launch_output_unpack_rows(static_cast<const __half*>(in), static_cast<float*>(out), L.pos_map,
                                                   static_cast<long long>(L.N) * L.H * L.W, L.C, L.C_phys, s);
+        case L_PATCHIFY:
+            return b2k::launch_patchify(static_cast<const float*>(in), static_cast<__half*>(out), L.N, L.H, L.W, L.k, L.max_blocks, s);
+        case L_TOKENS:
+            return b2k::launch_tokens(static_cast<const __half*>(in), static_cast<__half*>(out), const_cast<int*>(L.pos_map),
+                                      static_cast<const __half*>(L.w), L.N, L.W, L.C, s);
+        case L_CLS_HEAD:
+            return b2k::launch_cls_head(static_cast<const __half*>(in), static_cast<const __half*>(L.w), L.bias, static_cast<float*>(out), L.N,
+                                        L.W, L.C, L.Cout, L.eps, L.pos_map, s);
     }
     return int(cudaErrorInvalidValue);
 }
@@ -2250,6 +2385,12 @@ bool patch_layout(const b2_engine* e, const Launch& L, BindPatch* p) {
             return true;
         case L_OUTPUT_UNPACK:                                               // output_unpack_rows_kernel(src, dst, pos_map, rows, C, C_phys)
             p->n_params = 6, p->slots = {{1, L.out_binding}};
+            return true;
+        case L_PATCHIFY:                                                    // patchify_kernel(src, dst, N, Himg, Wimg, p)
+            p->n_params = 6, p->slots = {{0, L.in_binding}};
+            return true;
+        case L_CLS_HEAD:                                                    // cls_head_kernel(x, w, gbb, out, N, S, C, classes, eps, pos_map)
+            p->n_params = 10, p->slots = {{3, L.out_binding}};
             return true;
         default:
             return false;
@@ -2972,9 +3113,10 @@ const char* b2_context_launch_name(b2_context* c, int batch, int i) {
     static const char* kinds[] = {"input_cast", "conv_tcgen05", "conv_simt", "maxpool", "avgpool", "fc", "softmax", "output_cast", "net_tcgen05", "tail_pool_fc_softmax",
                                   "quantize", "conv_i8_tcgen05", "avgpool_i8", "output_cast_i8", "embed_ln", "layernorm", "attention_f16_wgmma",
                                   "pooler", "output_cast_rows", "output_unpack_rows", "quantize_f8", "conv_f8_tcgen05", "avgpool_f8",
-                                  "output_cast_f8"};
+                                  "output_cast_f8", "patchify", "tokens", "cls_head"};
     s = std::string(kinds[L->kind]) + (L->kind == L_ATTENTION && L->attn.S > 128 ? "_ks" : "") +  // key-split kernel
         (L->kind == L_ATTENTION && L->attn.seq_off ? "_varlen" : "") + ":" + L->name;         // variable-length kernel
+    if (L->kind == L_ATTENTION && L->attn.S != L->W) s += " sk=" + std::to_string(L->attn.S);  // kernel of a longer sequence
     if (L->kind == L_CONV_TC)
         s += " bn=" + std::to_string(L->conv.bn) + " kb=" + std::to_string(L->conv.kb) +
              " st=" + std::to_string(L->conv.stages) + "x" + std::to_string(L->conv.sps) +

@@ -302,5 +302,15 @@ int launch_pooler(const __half* h, const __half* w, const float* b, float* out, 
 int launch_output_cast_rows(const __half* src, float* dst, long long rows, int C, int C_phys, cudaStream_t stream);
 // packed fp16 [T][C_phys] -> fp32 [N*S][C]: row n*S + s is packed row pos_map[n*S + s], or zeros where that is -1
 int launch_output_unpack_rows(const __half* src, float* dst, const int* pos_map, long long rows, int C, int C_phys, cudaStream_t stream);
+// Vision Transformer front and back end (bert_kernels.cu).  fp32 NCHW [N][3][Himg][Wimg] -> fp16 patch rows [N * P][3 p^2]
+// (p % 8 == 0, p | Himg, p | Wimg; column c p^2 + dy p + dx), round to nearest; max_blocks > 0 caps the grid
+int launch_patchify(const float* src, __half* dst, int N, int Himg, int Wimg, int p, int max_blocks, cudaStream_t stream);
+// token rows [N][L][C] from the patch projection y [N][L - 1][C] and fp16 table [cls | pos_0 .. pos_{L-1}]: row 0 =
+// fp16(cls + pos_0), row t = fp16(y[t - 1] + pos_t); and the packing index (pos_map [N L] identity, seq_off[n] = n L, n <= N)
+int launch_tokens(const __half* y, __half* x, int* pack, const __half* table, int N, int L, int C, cudaStream_t stream);
+// logits[n][j] = b[j] + W[j] . LayerNorm(x[n][0]) (LayerNorm as launch_layernorm, fp16 result); gbb = fp32 [gamma C | beta C |
+// b classes], W fp16 [classes][C], out fp32 [N][classes]; pos_map != nullptr: item n's token 0 is row pos_map[n * S]
+int launch_cls_head(const __half* x, const __half* w, const float* gbb, float* out, int N, int S, int C, int classes, float eps,
+                    const int* pos_map, cudaStream_t stream);
 
 }  // namespace b2k

@@ -12,7 +12,7 @@ constexpr char kMagic[8] = {'B', '2', 'E', 'N', 'G', 'I', 'N', 'E'};
 // grouped, so every plan without one stays version 1.  The engine reads both.
 constexpr uint32_t kVersion = 1;
 constexpr uint32_t kVersionGrouped = 2;
-// Version 3: OpRecV3 (224 bytes), written only for plans with transformer ops (OP_EMBED_LN ... OP_POOLER), so every CNN
+// Version 3: OpRecV3 (224 bytes), written only for plans with transformer ops (OP_EMBED_LN ... OP_CLS_HEAD), so every CNN
 // plan keeps version 1 / 2.
 constexpr uint32_t kVersionTransformer = 3;
 
@@ -31,6 +31,11 @@ enum OpType : uint32_t {
     OP_LAYERNORM = 9,    // fp16 [.., C] -> fp16 [.., C] over the channels
     OP_ATTENTION = 10,   // fused QKV tensor [N, 1, S, 3H] + additive mask (tensor `res`) -> context [N, 1, S, H]
     OP_POOLER = 11,      // tanh(W h[CLS] + b): fp16 [N, 1, S, H] -> fp32 vector [N, H]
+    // Vision Transformer ops (version-3 plans)
+    OP_PATCHIFY = 12,    // fp32 NCHW image binding [3, Himg, Wimg] -> fp16 patch rows [N, 1, P, 3 p^2]
+    OP_TOKENS = 13,      // patch projection [N, 1, P, H] -> tokens [N, 1, P + 1, H] (class token, + position embeddings)
+                         // and the packing index (tensor `out2`)
+    OP_CLS_HEAD = 14,    // LayerNorm of token 0, then the classifier: fp16 [N, 1, S, H] -> fp32 logits [N, classes]
 };
 
 enum TensorKind : uint32_t { T_ACT = 0 /* NHWC, engine precision */, T_VEC = 1 /* [N, c] fp32 */ };
@@ -108,7 +113,8 @@ struct OpRecV2 {  // 192 bytes
 //   OP_LAYERNORM: in / out fp16 of the same shape; b = fp32 [gamma C | beta C]; eps.
 //   OP_ATTENTION: in = QKV [N, 1, S, 3H] with channel (part * H + head * 64 + d), part 0 = Q, 1 = K, 2 = V; res = the fp32
 //     mask [N, S]; out = [N, 1, S, H], head h at channels 64h ...; heads * 64 == H, S = 64 or a multiple of 128 up to
-//     512 (S > 128 runs the key-split kernel).
+//     512 (S > 128 runs the key-split kernel).  Packed plans take any S <= 512: the kernel of the smallest S_k in {64, 128,
+//     256, 384, 512} with S_k >= S runs each item over its own rows.
 //   OP_POOLER: in = fp16 [N, 1, S, H]; out = fp32 vector [N, H]; w = fp16 [H][H] (row = output); b = fp32 [H].
 //   OP_OUTPUT_CAST: flags bit 0 = channels-last binding [H * W, C] instead of NCHW.
 // Packed (padding-free) transformer plans: flags bit 1 (kOpPacked) marks an op that works on packed rows -- the tokens
@@ -126,6 +132,19 @@ struct OpRecV2 {  // 192 bytes
 //     rows.
 //   OP_POOLER: pools packed row pos_map[n * S]; a masked position 0 pools a zero row (tanh(b)).
 //   OP_OUTPUT_CAST (flags bit 0 required): writes the [S, C] binding per item, row s from pos_map, zeros where it is -1.
+// Vision Transformer plans are packed plans whose embedding is OP_TOKENS; every item has L = S tokens, so the packing
+// index is pos_map = identity, seq_off[n] = n S.  Before OP_TOKENS a plan holds exactly one OP_PATCHIFY and one unpacked
+// dense 1x1 GEMM (the patch projection); after it, besides the packed ops above, OP_CLS_HEAD (packed), OP_SOFTMAX and
+// unpacked channels-last output casts of the patch tensors:
+//   OP_PATCHIFY: binding = the fp32 input [3, Himg, Wimg]; k = p (a multiple of 8 dividing Himg and Wimg); out = fp16
+//     [1, P, 3 p^2], P = (Himg / p)(Wimg / p), patch t = (py, px) in row-major order, element (c, dy, dx) at column
+//     c p^2 + dy p + dx; each value rounded to nearest.  No weights.
+//   OP_TOKENS (flags bit 1 required): in = the patch projection [1, S - 1, H]; out = [1, S, H]: row 0 = fp16(cls + pos_0),
+//     row t = fp16(in[t - 1] + pos_t), fp32 sums; w = fp16 [1 + S][H] (the class token, then S position rows); out2 = the
+//     packing index, a T_VEC of S + 2 words per item (at batch N: pos_map [N S] = identity, seq_off [N + 1] = n S).
+//   OP_CLS_HEAD: in = fp16 [1, S, H]; out = fp32 vector [classes] (cout = classes, cin = H); w = fp16 [classes][H]; b = fp32
+//     [gamma H | beta H | bias classes]; eps.  LayerNorm of each item's token 0 as OP_LAYERNORM computes it (fp16 result),
+//     then logits = bias + W h in fp32.  Packed: token 0 of item n is row pos_map[n S].
 struct OpRecV3 {  // 224 bytes
     OpRec v1;
     uint32_t groups;

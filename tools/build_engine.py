@@ -12,6 +12,7 @@ examples/ONNX/resnet50/build.py:35-67).
   python tools/build_engine.py --model resnext50 --precision int8 --batch 8 -o rx50_int8.plan  (grouped 1-byte convolutions)
   python tools/build_engine.py --model bert-base --seq 128 --batch 16 [--weights bert.npz] --tune -o bert.plan  (fp16)
   python tools/build_engine.py --model bert-base --seq 384 --batch 16 --remove-padding -o bert_packed.plan  (masked tokens skipped)
+  python tools/build_engine.py --model vit-b16 --batch 8 [--weights vit.npz] --tune -o vit.plan  (ViT-B/16, also vit-b32 / vit-l16; fp16)
 Weights: deterministic synthetic weights (the reference's benchmark engines are weightless too, models/README.md:6-7),
 unless --caffemodel names a binary NetParameter (trtexec --model=...); MNIST and --onnx carry their own weights.
 --precision int8 / fp8: post-training quantization (fp8: E4M3), max-abs calibration on --calib (an .npy [N,C,H,W] fp32) or on
@@ -30,9 +31,10 @@ from tensorrt_laboratory_b200 import builder, graph, weights  # noqa: E402
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--model", choices=["resnet50", "resnet152", "resnext50", "mnist", "bert-base"])
+    ap.add_argument("--model", choices=["resnet50", "resnet152", "resnext50", "mnist", "bert-base", "vit-b16", "vit-b32", "vit-l16"])
     ap.add_argument("--seq", type=int, default=128, help="bert-base: the sequence length of the plan (64, 128, 256, 384 or 512)")
-    ap.add_argument("--weights", help="bert-base: .npz of Hugging Face BertModel parameters (default: seeded weights)")
+    ap.add_argument("--weights", help="bert-base / vit-*: .npz of Hugging Face BertModel / ViTForImageClassification parameters "
+                                        "(default: seeded weights)")
     ap.add_argument("--remove-padding", action="store_true",
                     help="bert-base: a packed plan that computes only the tokens with input_mask != 0 (same bindings)")
     ap.add_argument("--prototxt")
@@ -60,6 +62,11 @@ def main():
         cfg = bert.BertConfig(seq=a.seq)
         blob = builder.build_bert_plan(cfg, a.weights, a.batch, seed=a.seed, precision=prec, remove_padding=a.remove_padding)
         net = {"name": f"bert-base S={a.seq}" + (" packed" if a.remove_padding else "")}
+    elif a.model in ("vit-b16", "vit-b32", "vit-l16"):  # its own builder: patch and token ops, fp16 only
+        from tensorrt_laboratory_b200 import vit
+        cfg = {"vit-b16": vit.VIT_B16, "vit-b32": vit.VIT_B32, "vit-l16": vit.VIT_L16}[a.model]
+        blob = builder.build_vit_plan(cfg, a.weights, a.batch, seed=a.seed, precision=prec)
+        net = {"name": a.model}
     elif a.prototxt:
         with open(a.prototxt) as f:
             net = graph.parse_prototxt(f.read())
@@ -77,7 +84,7 @@ def main():
     else:
         net = graph.resnet_caffe(int(a.model[6:]))
         wts = weights_for(net)
-    if a.model != "bert-base":
+    if a.model not in ("bert-base", "vit-b16", "vit-b32", "vit-l16"):
         low = graph.lower(net, wts)
         if prec in (builder.PREC_INT8, builder.PREC_FP8):
             import numpy as np
