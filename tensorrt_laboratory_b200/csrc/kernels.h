@@ -107,53 +107,6 @@ void set_pdl(bool on);
 bool get_pdl();
 
 // ---------------------------------------------------------------------------------------------
-// net_f16_tcgen05 -- ONE persistent kernel for a whole run of consecutive convolution layers (net_kernel.cu).
-//   The tiles (128 output pixels x BN output channels) of every layer of the run form one ordered work list; CTAs draw
-//   tickets from it.  A tile of layer L+1 starts as soon as the 128-row tiles of layer L that it reads are stored
-//   (per-(layer, M-tile) arrival counters in global memory) instead of waiting for the whole layer.
-// ---------------------------------------------------------------------------------------------
-constexpr int kNetMaxLayers = 160;   // layer descriptors are copied to shared memory
-
-struct NetLayerInfo {
-    const uint8_t* wpacked;   // pre-swizzled weights [num_kblocks][Cout/32][32][128 B]
-    const float* bias;        // [Cout]
-    __half* out;              // [M][Cout] NHWC
-    const __half* residual;   // [M][Cout] or nullptr
-    int M, Cout, num_kblocks, cblocks;
-    int kw, HoWo, Wo, stride_h;
-    int stride_w, pad_h, pad_w, relu;
-    int a_mode, bn, tiles_m, tiles_n;
-    int tile_begin, total_tiles;
-    int in_flag_off;         // first M-tile counter of the layer that produces the input (-1: produced before this kernel)
-    int in_need;             // N tiles per M tile of that layer = value of a complete counter
-    int res_flag_off, res_need;  // same for the residual input
-    int out_flag_off;        // first M-tile counter of this layer
-    int dep_off;             // first entry of this layer in NetArgs::deps
-    int war_upto;            // every layer of the run up to this index must be COMPLETE before this layer may store: its output
-                             // buffer is recycled arena memory those layers read or wrote (-1: none)
-    int pad_[3];
-};
-static_assert(sizeof(NetLayerInfo) % 16 == 0, "NetLayerInfo is copied to shared memory in 16-byte words");
-struct alignas(64) NetLayer {
-    CUtensorMap mapA;    // activations: 2-D tiled [M, Cin] (box 128 x 64) or 4-D im2col
-    NetLayerInfo info;
-};
-struct NetArgs {
-    const NetLayer* layers;  // device memory
-    const short2* deps;      // device: per (layer, M tile) first / last M tile of the input it reads
-    int* mt_done;            // device: per (layer, M tile) finished-tile counters (zero between launches)
-    int* layer_done;         // device: per layer finished-tile counters (zero between launches)
-    int* ctrl;               // device: [0] ticket counter, [1] exited CTAs (zero between launches)
-    int n_layers, total_tiles, n_flags;
-    int stages;              // shared-memory ring depth (2..4 stages of one 64-wide K-block: 16 KiB of activations + 16 KiB of weights)
-    long long* dbg;          // optional (debug instantiation): 8 roles x 8 int64 counters per CTA
-};
-int init_net_kernel();
-int net_smem_bytes(int n_layers, int stages);
-// persistent launch with `ctas` CTAs (up to two per SM when the ring is shallow enough); returns 0 or a cudaError_t
-int launch_net_f16_tcgen05(const NetArgs& a, int ctas, cudaStream_t stream);
-
-// ---------------------------------------------------------------------------------------------
 // INT8 path (i8_kernels.cu): wgmma s8 convolution with a requantising epilogue + its SIMT helpers
 // ---------------------------------------------------------------------------------------------
 struct I8ConvArgs {

@@ -447,13 +447,6 @@ int trt_device_throughput(const void* blob, size_t nbytes, int contexts, int bat
     for (auto& x : ctx) {
         if (status != B2_OK) break;
         if ((status = b2_context_create(eng, &x.c))) break;
-        // the contexts share the GPU: each persistent network kernel gets its share of the SMs (one CTA each; B2_NET_CTAS overrides)
-        if (!getenv("B2_NET_CTAS")) {
-            int dev = 0, sms = 0;
-            cudaGetDevice(&dev);
-            cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-            b2_context_set_option(x.c, "net_ctas", std::max(1, sms / contexts));
-        }
         if (!cuda_ok(cudaMalloc(&x.scratch, std::max<size_t>(b2_engine_device_memory_size(eng), 1024)), "cudaMalloc scratch")) break;
         if ((status = b2_context_set_device_memory(x.c, x.scratch))) break;
         x.bind.assign(nb, nullptr);

@@ -465,7 +465,6 @@ void InferenceManager::PrepareModel(const Model* model) {
         for (size_t k = 0; k < n; k++) held.push_back(pool->PopWithoutReturn());
         for (auto& ctx : held) {
             TRT_CHECK_B2(b2_context_set_device_memory(ctx->handle, m_Lanes[lane]->workspace));
-            if (!getenv("B2_NET_CTAS")) b2_context_set_option(ctx->handle, "net_ctas", std::max(1, sms / std::max(1, m_MaxExecutions)));
             if (ZeroCopyInput() && !getenv("B2_INPUT_CTAS")) {  // a PCIe-paced cast must not hold every thread slot of the GPU
                 const char* v = getenv("TRTLAB_ZERO_COPY_CTAS");
                 b2_context_set_option(ctx->handle, "input_ctas", v ? atoi(v) : std::max(1, sms / 2));

@@ -102,15 +102,14 @@ def test_gelu_gemm_tactics_bit_identical(gpu):
         assert rel_err(taps["ffn"], want["ffn"]) <= TOL, opt
 
 
-def test_gelu_layer_never_takes_the_persistent_or_network_kernel(gpu):
+def test_gelu_layer_never_takes_the_persistent_kernel(gpu):
     cfg = bert.BertConfig(**{**SMALL.__dict__, "layers": 1})
     eng = capi.Engine(builder.build_bert_plan(cfg, max_batch=4))
-    for opt in ({"ws": 1}, {"net": 1}):
-        s = capi.Session(eng, opt)
-        names = [s._lib.b2_context_launch_name(s.ctx, 4, i).decode() for i in range(s.nb_launches(4))]
-        s.close()
-        ffn1 = [n for n in names if ":l0.ffn1" in n]
-        assert len(ffn1) == 1 and ffn1[0].startswith("conv_tcgen05:") and " ws=" not in ffn1[0] and " gelu" in ffn1[0], names
+    s = capi.Session(eng, {"ws": 1})
+    names = [s._lib.b2_context_launch_name(s.ctx, 4, i).decode() for i in range(s.nb_launches(4))]
+    s.close()
+    ffn1 = [n for n in names if ":l0.ffn1" in n]
+    assert len(ffn1) == 1 and ffn1[0].startswith("conv_tcgen05:") and " ws=" not in ffn1[0] and " gelu" in ffn1[0], names
     eng.destroy()
 
 

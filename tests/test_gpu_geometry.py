@@ -643,14 +643,6 @@ def test_resnet50_200x264_tuned_tactics_change_no_bit(wide):
         np.testing.assert_array_equal(got[t], wide["out"][t], err_msg=t)
 
 
-def test_resnet50_200x264_network_kernel(wide):
-    """The opt-in persistent network kernel (net=1) runs the same MMAs per tile: bit-identical to net=0."""
-    got, names = _run_blob(wide["blob"], wide["x"], {"net": 1})
-    assert any(n.startswith("net_tcgen05:") for n in names), names
-    for t in WIDE_TAPS:
-        np.testing.assert_array_equal(got[t], wide["out"][t], err_msg=t)
-
-
 def test_resnet50_200x264_int8(wide):
     """The _full_net_check scheme of tests/test_int8.py: the fp16 stem within fp16 tolerance, everything INT8 downstream of
     the GPU's own pool1 bit for bit."""

@@ -114,7 +114,7 @@ def _check_names(names, fmt, span, cpg, n_grouped=1):
     grouped = [n for n in names if n.startswith(KERNEL[fmt]) and " span=" in n]
     assert len(grouped) == n_grouped, names
     assert all(f" span={span} mode={_mode(cpg)}" in n for n in grouped), grouped
-    assert not any(n.startswith(("conv_simt", "conv_tcgen05", "net_tcgen05")) for n in names), names
+    assert not any(n.startswith(("conv_simt", "conv_tcgen05")) for n in names), names
 
 
 def _within(op, q_in, got, res, steps):

@@ -130,22 +130,6 @@ def test_simt_reads_the_packed_grouped_layout(gpu):
     _check(256, 14, 1, 2, batch=2, options={"simt": 1}, kernel="conv_simt")
 
 
-def test_grouped_layer_ends_a_network_kernel_run(gpu):
-    """net=1 folds runs of dense convolutions into one persistent kernel; a grouped layer is never a member."""
-    net = graph.resnext_caffe(50)
-    wts = weights.random_weights(net, 0)
-    low = graph.lower(net, wts)
-    x = weights.synthetic_input(2)
-    ref = helpers.run_engine(low, x, builder.PREC_FP16, options={"autotune": 0})["prob"]
-    got = helpers.run_engine(low, x, builder.PREC_FP16, options={"net": 1})["prob"]
-    names = helpers.LAST_LAUNCH_NAMES
-    runs = [n for n in names if n.startswith("net_tcgen05")]
-    grouped = [n for n in names if n.startswith("conv_tcgen05:") and " span=" in n]
-    assert runs and len(grouped) == 16, names
-    assert not any("branch2b" in n.split(" ")[0] for n in runs), runs  # runs are named first..last: none spans a 3x3
-    np.testing.assert_array_equal(got, ref)
-
-
 def test_fp32_engine_grouped_conv_matches_fp32_oracle(gpu):
     import torch
     for cin, cout, groups, stride in ((32, 32, 8, 1), (48, 96, 3, 2), (64, 64, 64, 1)):

@@ -6,6 +6,8 @@ Tolerances (stated per the north star):
   * ResNet-50 fp16 engine vs the fp32 CPU oracle: <= 1e-3 relative on `prob` (relative to the row max),
     identical argmax for every image; vs the fp16-emulating oracle: <= 1e-4.
 """
+import threading
+
 import numpy as np
 import pytest
 
@@ -184,6 +186,38 @@ def test_side_branches_run_forked_and_change_nothing(rn50, rn50_session):
     np.testing.assert_array_equal(outs[(1, 1)], outs[(0, 1)])
     np.testing.assert_array_equal(outs[(1, 0)], outs[(0, 1)])
     np.testing.assert_array_equal(outs[(1, 1)], rn50_session["sess"].infer(rn50["x"])["prob"])
+
+
+def test_four_contexts_share_the_gpu(rn50, rn50_session):
+    """BASELINE configs[1]: four ExecutionContexts on four streams, driven from four threads at once."""
+    eng = rn50_session["eng"]
+    sessions = [capi.Session(eng) for _ in range(4)]
+    xs = [weights.synthetic_input(8, seed=100 + i) for i in range(4)]
+    try:
+        ref = [sessions[0].infer(x)["prob"] for x in xs]
+        results = [[None] * 6 for _ in range(4)]
+
+        def work(i):
+            for k in range(6):
+                results[i][k] = sessions[i].infer(xs[i])["prob"]
+
+        ts = [threading.Thread(target=work, args=(i,)) for i in range(4)]
+        for t in ts:
+            t.start()
+        for t in ts:
+            t.join()
+        for i in range(4):
+            for k in range(6):
+                assert np.array_equal(results[i][k], ref[i]), (i, k)
+    finally:
+        for s in sessions:
+            s.close()
+
+
+def test_removed_network_kernel_options_are_rejected(rn50_session):
+    for key in ("net", "net_ctas", "net_bn", "net_stages"):
+        with pytest.raises(capi.B2Error):
+            rn50_session["sess"].set_option(key, 1)
 
 
 def test_dynamic_batching_runner(rn50, rn50_session):
