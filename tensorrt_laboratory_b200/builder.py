@@ -18,6 +18,7 @@ PREC_FP32, PREC_FP16, PREC_INT8, PREC_FP8 = 0, 1, 2, 3
 OP_INPUT_CAST, OP_CONV, OP_MAXPOOL, OP_AVGPOOL, OP_FC, OP_SOFTMAX, OP_OUTPUT_CAST, OP_QUANTIZE = range(8)
 OP_EMBED_LN, OP_LAYERNORM, OP_ATTENTION, OP_POOLER = range(8, 12)   # transformer ops (version-3 plans)
 OP_PATCHIFY, OP_TOKENS, OP_CLS_HEAD = range(12, 15)                  # Vision Transformer ops (version-3 plans)
+OP_LRN = 15                                                          # local response normalisation (version-4 plans)
 CONV_RELU, CONV_PACKED, CONV_INT8, CONV_GELU = 1, 2, 4, 8            # OpRec.relu bits of a convolution
 FLAG_ROWS_OUT, FLAG_PACKED = 1, 2  # OpRecV3.flags: channels-last output cast; op on packed (padding-free) rows
 T_ACT, T_VEC = 0, 1
@@ -25,6 +26,7 @@ MAGIC = b"B2ENGINE"
 VERSION = 1           # plans without grouped convolutions: 176-byte op records
 VERSION_GROUPED = 2   # a plan with at least one grouped convolution: 192-byte op records (+ groups)
 VERSION_TRANSFORMER = 3  # a plan with transformer ops or a GELU convolution: 224-byte op records (plan_format.h OpRecV3)
+VERSION_CONCAT = 4    # a plan with channel-slice convolutions or LRN: 192-byte op records (+ groups, out_c0, out_cw)
 
 _HEADER = struct.Struct("<8sIIIIIIQQ64s16x")
 _TENSOR = struct.Struct("<64sIIIIIif4x")  # ... binding, scale (INT8 tensors: real value = q * scale; 0 = fp16 / fp32 tensor)
@@ -32,8 +34,9 @@ _OP = struct.Struct("<64sIiiiiIIIIIIIIIIIQQQQIIII")
 _OP_V2 = struct.Struct("<64sIiiiiIIIIIIIIIIIQQQQIIIII12x")  # version 2: _OP + groups + 12 reserved bytes
 # version 3: _OP + groups, heads, vocab, positions, types, binding2, binding3, out2, eps, flags + 8 reserved bytes
 _OP_V3 = struct.Struct("<64sIiiiiIIIIIIIIIIIQQQQIIIIIIIIIiiifI8x")
+_OP_V4 = struct.Struct("<64sIiiiiIIIIIIIIIIIQQQQIIIIIII4x")  # version 4: _OP + groups, out_c0, out_cw + 4 reserved bytes
 _BINDING = struct.Struct("<64sIIiI8i16x")
-assert _HEADER.size == 128 and _TENSOR.size == 96 and _OP.size == 176 and _OP_V2.size == 192 and _OP_V3.size == 224
+assert _HEADER.size == 128 and _TENSOR.size == 96 and _OP.size == 176 and _OP_V2.size == 192 and _OP_V3.size == 224 and _OP_V4.size == 192
 assert _BINDING.size == 128
 
 
@@ -173,6 +176,10 @@ def build_plan(lowered: dict, precision: int = PREC_FP16, max_batch: int = 8,
         precision_fp = precision
     wdtype = np.float16 if precision_fp == PREC_FP16 else np.float32
     outputs = list(outputs) if outputs else [lowered["output"]]
+    concat = any("out_c0" in op for op in lowered["ops"])
+    if (concat or any(op["type"] == G.OP_LRN for op in lowered["ops"])) and precision != PREC_FP16:
+        raise ValueError("a graph with a Concat or LRN layer builds in fp16 only: channel concatenation and LRN have no fp32, "
+                         "INT8 or FP8 kernels")
     shapes: Dict[str, tuple] = dict(lowered["tensors"])
     vec_tensors = {op["output"] for op in lowered["ops"] if op["type"] in (G.OP_FC, G.OP_SOFTMAX)}
 
@@ -226,6 +233,22 @@ def build_plan(lowered: dict, precision: int = PREC_FP16, max_batch: int = 8,
         # kw taps are contiguous in memory: the engine reads a whole filter row as one 64-byte TMA "pixel"
         tensors[t_in].update(w=win // 2 + s2d_lo + s2d_hi, c=8, c_phys=8)
         ops[0].update(k=2, pad=s2d_lo, stride=s2d_hi)
+
+    # concatenated tensors: each input convolution writes [out_c0, out_c0 + width); the last one's width runs to c_phys, so
+    # its zero weight rows rewrite the tail padding on every pass
+    slice_width: Dict[str, int] = {}
+    writers: Dict[str, List[dict]] = {}
+    for op in lowered["ops"]:
+        if "out_c0" in op:
+            writers.setdefault(op["output"], []).append(op)
+    for tname, ws in writers.items():
+        c_phys = phys_channels(shapes[tname][0], PREC_FP16)
+        ws = sorted(ws, key=lambda o: o["out_c0"])
+        for k, op in enumerate(ws):
+            if op["out_c0"] % 8:
+                raise ValueError(f"Concat {tname}: input {op['name']} starts at channel {op['out_c0']}, not a multiple of 8 "
+                                 "(the 16-byte alignment of the convolution's output store)")
+            slice_width[op["name"]] = c_phys - op["out_c0"] if k + 1 == len(ws) else op["cout"]
 
     for op in lowered["ops"]:
         t = op["type"]
@@ -295,6 +318,13 @@ def build_plan(lowered: dict, precision: int = PREC_FP16, max_batch: int = 8,
             cout_phys = tensors[to]["c_phys"]
             k = op["k"]
             Wsrc, cin_eff, extra = op["W"], op["cin"], {}
+            if op["name"] in slice_width:  # weight rows = the slice width rounded up to 64; rows past cout are zero
+                cw = slice_width[op["name"]]
+                cout_phys = _roundup(cw, 64)
+                extra = dict(out_c0=op["out_c0"], out_cw=cw)
+                if cin_phys % 64 or not pack_weights or op is s2d_op:
+                    raise ValueError(f"conv {op['name']}: a concatenated convolution needs a multiple of 64 input channels "
+                                     "and packed weights")
             taps = k * k
             if op is s2d_op:
                 Wsrc, kw2, pad_lo, pad_hi = stem_s2d_transform(op["W"], k, op["pad"], win)
@@ -332,6 +362,9 @@ def build_plan(lowered: dict, precision: int = PREC_FP16, max_batch: int = 8,
                        w_off=w_off, w_bytes=w_bytes, b_off=b_off, b_bytes=b_bytes)
         elif t == G.OP_SOFTMAX:
             rec.update(type=OP_SOFTMAX)
+        elif t == G.OP_LRN:
+            b_off, b_bytes = add_payload(np.array([op["alpha"], op["beta"], op["k"]], dtype=np.float32))
+            rec.update(type=OP_LRN, k=op["local_size"], b_off=b_off, b_bytes=b_bytes)
         else:
             raise ValueError(f"unsupported lowered op {t}")
         ops.append(rec)
@@ -358,10 +391,14 @@ def _serialize(tensors: List[dict], ops: List[dict], bindings: List[dict], paylo
                name: str) -> bytes:
     # version 1 unless a convolution is grouped (2) or the plan has transformer ops / GELU (3): every plan without them
     # stays byte-identical to what older builders wrote
-    transformer = any(o["type"] >= OP_EMBED_LN or (o["type"] == OP_CONV and o.get("relu", 0) & CONV_GELU) for o in ops)
+    # version 4 when a convolution writes a channel slice or an op is an LRN
+    concat = any(o["type"] == OP_LRN or "out_cw" in o for o in ops)
+    transformer = any(OP_EMBED_LN <= o["type"] <= OP_CLS_HEAD or (o["type"] == OP_CONV and o.get("relu", 0) & CONV_GELU) for o in ops)
+    if concat and transformer:
+        raise ValueError("a plan holds channel slices / LRN or transformer ops, not both")
     grouped = any(o.get("groups", 1) > 1 for o in ops)
-    op_struct = _OP_V3 if transformer else _OP_V2 if grouped else _OP
-    version = VERSION_TRANSFORMER if transformer else VERSION_GROUPED if grouped else VERSION
+    op_struct = _OP_V4 if concat else _OP_V3 if transformer else _OP_V2 if grouped else _OP
+    version = VERSION_CONCAT if concat else VERSION_TRANSFORMER if transformer else VERSION_GROUPED if grouped else VERSION
     tables = _HEADER.size + len(tensors) * _TENSOR.size + len(ops) * op_struct.size + len(bindings) * _BINDING.size
     payload_offset = _roundup(tables, 256)
     blob = bytearray()
@@ -380,6 +417,8 @@ def _serialize(tensors: List[dict], ops: List[dict], bindings: List[dict], paylo
             blob += op_struct.pack(*fields, o.get("groups", 1), o.get("heads", 0), o.get("vocab", 0), o.get("positions", 0),
                                    o.get("types", 0), o.get("binding2", -1), o.get("binding3", -1), o.get("out2", -1),
                                    o.get("eps", 0.0), o.get("flags", 0))
+        elif concat:
+            blob += op_struct.pack(*fields, o.get("groups", 1), o.get("out_c0", 0), o.get("out_cw", 0))
         else:
             blob += op_struct.pack(*fields, o.get("groups", 1)) if grouped else op_struct.pack(*fields)
     for b in bindings:
@@ -644,6 +683,19 @@ def build_resnext_plan(depth: int = 50, precision: int = PREC_FP16, max_batch: i
         from . import quantize
         low = quantize.quantize_lowered(low, Wt.synthetic_input(calib_batch, seed=4321),
                                         fmt="e4m3" if precision == PREC_FP8 else "int8", grouped=True)
+    return build_plan(low, precision, max_batch, input_dtype=input_dtype)
+
+
+def build_googlenet_plan(precision: int = PREC_FP16, max_batch: int = 8, seed: int = 0, input_dtype: str = "f32",
+                         weights: Optional[dict] = None) -> bytes:
+    """Convenience: generated BVLC GoogLeNet (:func:`graph.googlenet_caffe`) + deterministic (or given, BVLC-named) weights
+    -> fp16 plan.  Each inception module's four branch convolutions write their channel slices of the module's output
+    directly; the two LRN layers run lrn_h8_kernel.  fp16 only."""
+    if precision != PREC_FP16:
+        raise ValueError("GoogLeNet builds in fp16 only: channel concatenation and LRN have no fp32, INT8 or FP8 kernels")
+    from . import weights as Wt
+    net = G.googlenet_caffe()
+    low = G.lower(net, weights if weights is not None else Wt.random_weights(net, seed))
     return build_plan(low, precision, max_batch, input_dtype=input_dtype)
 
 

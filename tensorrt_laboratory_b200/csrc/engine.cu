@@ -12,6 +12,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <cmath>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -114,6 +115,9 @@ struct Op {
     // >= 0: this op's only consumer is the residual input of op `side_join`, and nothing in between depends on it (the
     // shortcut convolution of a ResNet "a" block): it may run on a forked stream, concurrently with the ops up to there
     int side_join = -1;
+    // version-4 convolutions: output channels [c0, c0 + cw) of a tensor several convolutions write (cw == 0: all of it)
+    int c0 = 0, cw = 0;
+    float lrn[3] = {0.f, 0.f, 0.f};  // OP_LRN: alpha, beta, k (host copy of the op's parameter block)
     // conv geometry with the "0 = square" defaults resolved
     int kh() const { return int(r.k); }
     int kw() const { return int(r.kw ? r.kw : r.k); }
@@ -143,7 +147,7 @@ struct Binding {
 
 enum LKind { L_INPUT_CAST, L_CONV_TC, L_CONV_SIMT, L_MAXPOOL, L_AVGPOOL, L_FC, L_SOFTMAX, L_OUTPUT_CAST, L_TAIL, L_QUANTIZE, L_CONV_I8, L_AVGPOOL_I8, L_OUTPUT_CAST_I8,
              L_EMBED_LN, L_LAYERNORM, L_ATTENTION, L_POOLER, L_OUTPUT_ROWS, L_OUTPUT_UNPACK, L_QUANTIZE_F8, L_CONV_F8, L_AVGPOOL_F8,
-             L_OUTPUT_CAST_F8, L_PATCHIFY, L_TOKENS, L_CLS_HEAD };
+             L_OUTPUT_CAST_F8, L_PATCHIFY, L_TOKENS, L_CLS_HEAD, L_LRN };
 
 // Attention kernel of a packed plan's S tokens: the smallest instantiated sequence length S_k >= S (the variable-length
 // kernels attend each item over its own rows, so the rows S ... S_k - 1 of an item's tile are never used)
@@ -178,6 +182,8 @@ struct Launch {
     const int* live = nullptr;    // L_LAYERNORM of a packed plan: the live row count T (device)
     const int* pos_map = nullptr; // L_POOLER / L_OUTPUT_UNPACK of a packed plan: the packing index's pos_map (device)
     int N = 0, C = 0, H = 0, W = 0, C_phys = 0, Ho = 0, Wo = 0, k = 0, stride = 0, pad = 0, K = 0, Cout = 0;
+    int c0 = 0, cw = 0;                       // L_CONV_TC of a slice writer: its output channels (Op::c0, Op::cw)
+    float alpha = 0.f, beta = 0.f, kk = 0.f;  // L_LRN (k = n)
 };
 
 // A maximal run of launches that touch no binding: captured ONCE per plan (= per context, arena and batch) into a CUDA
@@ -515,6 +521,37 @@ int validate_packed_ops(b2_engine* e) {
     return B2_OK;
 }
 
+// Output channel slices (plan_format.h, version 4): the slices of every tensor they write tile [0, c_phys) exactly, and
+// the real channels they carry are the tensor's first c.
+int validate_slices(b2_engine* e) {
+    std::map<int, std::vector<const Op*>> writers;  // tensor -> its slice writers
+    for (const Op& op : e->ops)
+        if (op.cw) writers[op.r.out].push_back(&op);
+    for (auto& [t, ws] : writers) {
+        const Tensor& to = e->tensors[size_t(t)];
+        for (const Op& op : e->ops)
+            if (!op.cw && (op.r.out == t || op.out2 == t))
+                return fail(B2_EINVAL, "plan: op %s writes %s, whose channels slice writers share", op.name.c_str(), to.name.c_str());
+        std::sort(ws.begin(), ws.end(), [](const Op* a, const Op* b) { return a->c0 < b->c0; });
+        int next = 0;
+        for (size_t i = 0; i < ws.size(); ++i) {
+            const Op& op = *ws[i];
+            if (op.c0 < next)
+                return fail(B2_EINVAL, "plan: conv %s: slice [%d, %d) of %s overlaps another slice", op.name.c_str(), op.c0, op.c0 + op.cw, to.name.c_str());
+            if (op.c0 > next)
+                return fail(B2_EINVAL, "plan: conv %s: slice [%d, %d) of %s leaves channels [%d, %d) unwritten", op.name.c_str(), op.c0, op.c0 + op.cw,
+                            to.name.c_str(), next, op.c0);
+            const bool last = i + 1 == ws.size();
+            if (last ? (uint32_t(op.c0 + op.cw) != to.c_phys || op.c0 + int(op.r.cout) != int(to.c)) : int(op.r.cout) != op.cw)
+                return fail(B2_EINVAL, "plan: conv %s: slice [%d, %d) of %s: slices carry their real channels back to back, and the last one "
+                            "ends at channel %u (c_phys) after the tensor's %u real ones", op.name.c_str(), op.c0, op.c0 + op.cw, to.name.c_str(),
+                            to.c_phys, to.c);
+            next = op.c0 + op.cw;
+        }
+    }
+    return B2_OK;
+}
+
 int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** payload) {
     using namespace b2plan;
     if (!blob || nbytes < sizeof(Header)) return fail(B2_EINVAL, "plan: blob too small (%zu bytes)", nbytes);
@@ -522,12 +559,14 @@ int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** pa
     Header h;
     memcpy(&h, base, sizeof h);
     if (memcmp(h.magic, kMagic, 8) != 0) return fail(B2_EINVAL, "plan: bad magic (not a B2ENGINE blob)");
-    if (h.version != kVersion && h.version != kVersionGrouped && h.version != kVersionTransformer)
-        return fail(B2_EINVAL, "plan: version %u, this library reads %u, %u and %u", h.version, kVersion, kVersionGrouped, kVersionTransformer);
+    if (h.version != kVersion && h.version != kVersionGrouped && h.version != kVersionTransformer && h.version != kVersionConcat)
+        return fail(B2_EINVAL, "plan: version %u, this library reads %u, %u, %u and %u", h.version, kVersion, kVersionGrouped, kVersionTransformer,
+                    kVersionConcat);
     if (h.precision > B2_PREC_FP8) return fail(B2_EINVAL, "plan: unknown precision %u", h.precision);
     if (h.max_batch == 0 || h.max_batch > 4096) return fail(B2_EINVAL, "plan: bad max_batch %u", h.max_batch);
     const bool v3 = h.version == kVersionTransformer;
-    const size_t op_rec_size = v3 ? sizeof(OpRecV3) : h.version == kVersionGrouped ? sizeof(OpRecV2) : sizeof(OpRec);
+    const bool v4 = h.version == kVersionConcat;
+    const size_t op_rec_size = v3 ? sizeof(OpRecV3) : (h.version == kVersionGrouped || v4) ? sizeof(OpRecV2) : sizeof(OpRec);
     const size_t tbl = sizeof(Header) + size_t(h.n_tensors) * sizeof(TensorRec) + size_t(h.n_ops) * op_rec_size +
                        size_t(h.n_bindings) * sizeof(BindingRec);
     // (overflow-safe: a > n || b > n - a instead of a + b > n)
@@ -570,12 +609,19 @@ int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** pa
     for (uint32_t i = 0; i < h.n_ops; ++i, p += op_rec_size) {
         Op op;
         memcpy(&op.r, p, sizeof(OpRec));
-        if (h.version == kVersionGrouped) {
+        if (h.version == kVersionGrouped || v4) {
             OpRecV2 r2;
             memcpy(&r2, p, sizeof r2);
             if (r2.v1.type == OP_CONV && (r2.groups == 0 || r2.groups > 65536))
                 return fail(B2_EINVAL, "plan: conv %s has %u groups", fixed_str(r2.v1.name, 64).c_str(), r2.groups);
             if (r2.v1.type == OP_CONV) op.groups = int(r2.groups);
+            if (v4 && (r2.out_c0 || r2.out_cw)) {
+                if (r2.v1.type != OP_CONV)
+                    return fail(B2_EINVAL, "plan: op %s: only a convolution writes an output channel slice", fixed_str(r2.v1.name, 64).c_str());
+                if (r2.out_cw == 0 || r2.out_c0 > (1u << 20) || r2.out_cw > (1u << 20))
+                    return fail(B2_EINVAL, "plan: conv %s: bad output channel slice [%u, +%u)", fixed_str(r2.v1.name, 64).c_str(), r2.out_c0, r2.out_cw);
+                op.c0 = int(r2.out_c0), op.cw = int(r2.out_cw);
+            }
         }
         if (v3) {
             OpRecV3 r3;
@@ -591,8 +637,10 @@ int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** pa
         }
         op.name = fixed_str(op.r.name, 64);
         const OpRec& r = op.r;
-        if (r.type > OP_CLS_HEAD) return fail(B2_EINVAL, "plan: op %s has unknown type %u", op.name.c_str(), r.type);
-        const bool transformer_op = r.type >= OP_EMBED_LN;
+        if (r.type > OP_LRN) return fail(B2_EINVAL, "plan: op %s has unknown type %u", op.name.c_str(), r.type);
+        if (r.type == OP_LRN && (!v4 || h.precision != B2_PREC_FP16))
+            return fail(B2_EINVAL, "plan: lrn %s: LRN needs a version-4 fp16 plan", op.name.c_str());
+        const bool transformer_op = r.type >= OP_EMBED_LN && r.type <= OP_CLS_HEAD;
         if (transformer_op && (!v3 || h.precision != B2_PREC_FP16))
             return fail(B2_EINVAL, "plan: op %s: transformer ops need a version-3 fp16 plan", op.name.c_str());
         const bool in_opt = r.type == OP_INPUT_CAST || r.type == OP_EMBED_LN || r.type == OP_PATCHIFY, out_opt = r.type == OP_OUTPUT_CAST;
@@ -682,7 +730,19 @@ int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** pa
                 return fail(B2_EINVAL, "plan: fp16 conv %s touches an %s tensor", op.name.c_str(), qfmt);
             const Tensor& ti = e->tensors[r.in];
             const Tensor& to = e->tensors[r.out];
-            if (ti.c_phys != r.cin_phys || to.c_phys != r.cout_phys || ti.c != r.cin || to.c != r.cout)
+            if (op.cw) {  // a slice writer (plan_format.h, version 4); how the slices tile the tensor is checked below
+                if (h.precision != B2_PREC_FP16 || i8)
+                    return fail(B2_EINVAL, "plan: conv %s: output channel slices exist in fp16 plans only", op.name.c_str());
+                if (r.res >= 0) return fail(B2_EINVAL, "plan: conv %s: a slice writer has no residual", op.name.c_str());
+                if (op.c0 % 8) return fail(B2_EINVAL, "plan: conv %s: slice offset %d is not a multiple of 8", op.name.c_str(), op.c0);
+                if (uint64_t(op.c0) + uint64_t(op.cw) > to.c_phys)
+                    return fail(B2_EINVAL, "plan: conv %s: slice [%d, %d) runs past the %u channels of %s", op.name.c_str(), op.c0, op.c0 + op.cw,
+                                to.c_phys, to.name.c_str());
+                if (op.groups != 1 || !(r.relu & kConvPacked) || r.cout > uint32_t(op.cw) || r.cout_phys != (uint32_t(op.cw) + 63) / 64 * 64 ||
+                    ti.c_phys != r.cin_phys || ti.c != r.cin || to.kind != T_ACT || to.binding >= 0 || r.in == r.out)
+                    return fail(B2_EINVAL, "plan: conv %s: a slice writer is a dense packed-weight convolution with cout <= width and "
+                                "cout_phys = width rounded up to 64, into an arena activation it does not read", op.name.c_str());
+            } else if (ti.c_phys != r.cin_phys || to.c_phys != r.cout_phys || ti.c != r.cin || to.c != r.cout)
                 return fail(B2_EINVAL, "plan: conv %s channel mismatch with its tensors", op.name.c_str());
             if (uint64_t(ti.h) + 2 * uint64_t(r.pad_) < r.k || int64_t(ti.w) + op.pw_lo() + op.pw_hi() < op.kw())
                 return fail(B2_EINVAL, "plan: conv %s window larger than its padded input", op.name.c_str());
@@ -696,6 +756,19 @@ int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** pa
             if (r.w_bytes != size_t(r.cout) * K * elt || r.b_bytes != size_t(r.cout) * 4)
                 return fail(B2_EINVAL, "plan: fc %s weight size mismatch", op.name.c_str());
             e->flops_per_item += 2.0 * ti.h * ti.w * ti.c * r.cout;
+        } else if (r.type == OP_LRN) {
+            const Tensor& ti = e->tensors[r.in];
+            const Tensor& to = e->tensors[r.out];
+            if (ti.kind != T_ACT || to.kind != T_ACT || ti.h != to.h || ti.w != to.w || ti.c != to.c || ti.c_phys != to.c_phys || ti.c_phys % 8 ||
+                r.in == r.out)
+                return fail(B2_EINVAL, "plan: lrn %s: needs an fp16 input and a distinct output of the same shape", op.name.c_str());
+            if (r.k < 1 || r.k > uint32_t(b2k::kLrnMaxSize) || r.k % 2 == 0)
+                return fail(B2_EINVAL, "plan: lrn %s: local size %u (odd, 1 ... %d)", op.name.c_str(), r.k, b2k::kLrnMaxSize);
+            if (r.w_bytes != 0 || r.b_bytes != 12) return fail(B2_EINVAL, "plan: lrn %s: parameters must be fp32 [alpha, beta, k]", op.name.c_str());
+            float* prm = op.lrn;
+            memcpy(prm, base + h.payload_offset + r.b_off, sizeof op.lrn);
+            if (!(std::isfinite(prm[0]) && std::isfinite(prm[1]) && std::isfinite(prm[2]) && prm[2] > 0.f && prm[0] >= 0.f))
+                return fail(B2_EINVAL, "plan: lrn %s: alpha, beta and k must be finite, alpha >= 0 and k > 0", op.name.c_str());
         } else if (transformer_op) {
             int rc = validate_transformer_op(e, op);
             if (rc) return rc;
@@ -703,6 +776,7 @@ int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** pa
         e->ops.push_back(op);
     }
     if (int rc = validate_packed_ops(e)) return rc;
+    if (int rc = validate_slices(e)) return rc;
     for (uint32_t i = 0; i < h.n_bindings; ++i, p += sizeof(BindingRec)) {
         BindingRec r;
         memcpy(&r, p, sizeof r);
@@ -796,7 +870,8 @@ void plan_arena(b2_engine* e) {
     for (size_t i = 0; i < e->ops.size(); ++i) {
         Op& op = e->ops[i];
         op.side_join = -1;
-        if (int(i) <= busy_until || op.r.type != b2plan::OP_CONV || op.r.out < 0 || e->tensors[op.r.out].binding >= 0) continue;
+        // (a slice writer's tensor is read as a whole by later ops, never as one residual: it is not a side branch)
+        if (int(i) <= busy_until || op.r.type != b2plan::OP_CONV || op.r.out < 0 || e->tensors[op.r.out].binding >= 0 || op.cw) continue;
         int consumers = 0, join = -1;
         bool as_residual_only = true;
         for (size_t k = i + 1; k < e->ops.size(); ++k) {
@@ -813,6 +888,8 @@ void plan_arena(b2_engine* e) {
         const auto& r = e->ops[i].r;
         for (int t : {r.out, e->ops[i].out2})
             if (t >= 0 && e->tensors[t].def < 0) e->tensors[t].def = int(i);
+        // a tensor several slice writers share lives from its first writer to its last reader, and past its last writer
+        if (e->ops[i].cw) e->tensors[r.out].last_use = std::max(e->tensors[r.out].last_use, int(i));
         for (int t : {r.in, r.res})
             if (t >= 0) e->tensors[t].last_use = std::max(e->tensors[t].last_use, int(i));
         // a side op may still be READING its input while the ops before the join run: keep that buffer until the join
@@ -855,10 +932,11 @@ void plan_arena(b2_engine* e) {
 }
 
 // ---- tensor maps ------------------------------------------------------------------------------
+// `pitch`: elements from one outer row to the next (0 = inner; a channel slice of a wider tensor passes the tensor's)
 int make_map_2d(CUtensorMap* map, const void* base, uint64_t inner, uint64_t outer, uint32_t box_inner,
-                uint32_t box_outer, CUtensorMapSwizzle swz, bool int8 = false) {
+                uint32_t box_outer, CUtensorMapSwizzle swz, bool int8 = false, uint64_t pitch = 0) {
     cuuint64_t dims[2] = {inner, outer};
-    cuuint64_t strides[1] = {inner * (int8 ? 1u : 2u)};
+    cuuint64_t strides[1] = {(pitch ? pitch : inner) * (int8 ? 1u : 2u)};
     cuuint32_t box[2] = {box_inner, box_outer};
     cuuint32_t estr[2] = {1, 1};
     CUresult r = g_encode_tiled(map, int8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims, strides, box,
@@ -871,9 +949,11 @@ int make_map_2d(CUtensorMap* map, const void* base, uint64_t inner, uint64_t out
 }
 
 // NHWC activation tensor as a 4-D tiled map {C, W, H, N} with a {64 ch, box_w, box_h, 1} box (3x3 halo kernel)
-int make_map_nhwc(CUtensorMap* map, const void* base, int C, int W, int H, int N, uint32_t box_w, uint32_t box_h) {
+// (`pitch`: channels per pixel in memory, 0 = C; a channel slice of a wider tensor passes the tensor's)
+int make_map_nhwc(CUtensorMap* map, const void* base, int C, int W, int H, int N, uint32_t box_w, uint32_t box_h, int pitch = 0) {
+    const cuuint64_t P = cuuint64_t(pitch ? pitch : C);
     cuuint64_t dims[4] = {cuuint64_t(C), cuuint64_t(W), cuuint64_t(H), cuuint64_t(N)};
-    cuuint64_t strides[3] = {cuuint64_t(C) * 2, cuuint64_t(C) * 2 * W, cuuint64_t(C) * 2 * W * H};
+    cuuint64_t strides[3] = {P * 2, P * 2 * W, P * 2 * W * H};
     cuuint32_t box[4] = {64, box_w, box_h, 1};
     cuuint32_t estr[4] = {1, 1, 1, 1};
     CUresult r = g_encode_tiled(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims, strides, box, estr,
@@ -1002,6 +1082,8 @@ int fuse_partner(const b2_engine* e, int i) {
     if (!e->half() || e->one_byte() || i < 0 || size_t(i) + 1 >= e->ops.size()) return -1;
     const Op &oi = e->ops[size_t(i)], &oj = e->ops[size_t(i) + 1];
     const b2plan::OpRec &ri = oi.r, &rj = oj.r;
+    // a slice writer is neither: it has no residual (so no 1x1 of a pair), and its tensor has other readers (no 3x3 of one)
+    if (oi.cw || oj.cw) return -1;
     if (ri.type != b2plan::OP_CONV || rj.type != b2plan::OP_CONV || (ri.relu & (4 | b2plan::kConvGelu)) || conv_halo_rows(e, oi) == 0 ||
         !b2k::conv_halo_config_exists(int(ri.cout_phys)) || ri.cin_phys / 64 > 8)
         return -1;
@@ -1198,6 +1280,10 @@ int make_conv_launch(b2_context* c, const Op& op, int batch, const ConvConfig& c
     const bool gelu = (r.relu & b2plan::kConvGelu) != 0;
     b2k::ConvLaunch& cl = *out;
     memset(&cl, 0, sizeof cl);
+    // the output as the kernels' store sees it: all of the tensor, or the slice [c0, c0 + cw) of a wider one (columns of
+    // the tile past the slice are clipped by the map)
+    uint8_t* const out_base = tptr(r.out) + size_t(op.c0) * 2;
+    const int out_c = op.cw ? op.cw : int(r.cout_phys), out_pitch = op.cw ? int(to.c_phys) : 0;
     cl.kb = conv_kb(c, op);
     cl.grid_m = (M + 127) / 128;
     const int nkb = conv_num_kblocks(c, op);
@@ -1260,7 +1346,7 @@ int make_conv_launch(b2_context* c, const Op& op, int batch, const ConvConfig& c
             if (!rc) rc = make_map_nhwc(&cl.mapRes, tptr(rj.res), int(rj.cout_phys), int(to.w), int(to.h), batch, uint32_t(to.w) + 2, uint32_t(R));
             return rc;
         }
-        rc = make_map_nhwc(&cl.mapOut, tptr(r.out), int(r.cout_phys), int(to.w), int(to.h), batch, uint32_t(to.w) + 2, uint32_t(R));
+        rc = make_map_nhwc(&cl.mapOut, out_base, out_c, int(to.w), int(to.h), batch, uint32_t(to.w) + 2, uint32_t(R), out_pitch);
         cl.mapRes = cl.mapOut;
         return rc;
     }
@@ -1282,14 +1368,14 @@ int make_conv_launch(b2_context* c, const Op& op, int batch, const ConvConfig& c
         rc = make_map_2d(&cl.mapB, w, uint64_t(r.taps_phys) * r.cin_phys, r.cout_phys, uint32_t(cl.kb), uint32_t(cl.bn), swz);
     if (rc) return rc;
     if (cfg.ws && fold) {  // persistent stem: one output row per M tile, a {C, W, H, N} map clips the pixels past Wo
-        rc = make_map_nhwc(&cl.mapOut, tptr(r.out), int(r.cout_phys), int(to.w), int(to.h), batch, 128, 1);
+        rc = make_map_nhwc(&cl.mapOut, out_base, out_c, int(to.w), int(to.h), batch, 128, 1, out_pitch);
         cl.mapRes = cl.mapOut;
         return rc;
     }
     // epilogue maps: 128-row x min(64, BN)-column boxes, 128B (or 64B for BN=32) swizzle = conflict-free staging
     const uint32_t ow = cl.bn >= 64 ? 64 : 32;
     const CUtensorMapSwizzle oswz = cl.bn >= 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
-    rc = make_map_2d(&cl.mapOut, tptr(r.out), r.cout_phys, uint64_t(M), ow, 128, oswz);
+    rc = make_map_2d(&cl.mapOut, out_base, uint64_t(out_c), uint64_t(M), ow, 128, oswz, false, uint64_t(out_pitch));
     if (rc) return rc;
     if (r.res >= 0) rc = make_map_2d(&cl.mapRes, tptr(r.res), r.cout_phys, uint64_t(M), ow, 128, oswz);
     else cl.mapRes = cl.mapOut;
@@ -1802,8 +1888,13 @@ int build_plan(b2_context* c, int batch, Plan** out) {
                     if (!i8_tactic_ok(op, bn, st)) bn = 128, st = 2;
                     int rc = make_i8_conv_launch(c, op, batch, bn, st, &L.i8);
                     if (rc) return rc;
+                } else if (op.cw && (c->force_simt || !conv_on_tensor_cores(e, op))) {
+                    // the SIMT convolution addresses its output rows by the layer's own channel count
+                    return fail(B2_EINVAL, "conv %s: writes channel slice [%d, %d) of %s, which only the tensor-core kernels do", op.name.c_str(),
+                                op.c0, op.c0 + op.cw, to.name.c_str());
                 } else if (!c->force_simt && conv_on_tensor_cores(e, op)) {
                     L.kind = L_CONV_TC;
+                    L.c0 = op.c0, L.cw = op.cw;
                     ConvConfig cfg = forced_conv_config(c, op, batch);
                     if (cfg.bn == 0) return fail(B2_EINVAL, "conv %s: no kernel configuration", op.name.c_str());
                     const bool forced = c->force_bn || c->force_stages || c->force_splits || c->force_sps;
@@ -1991,6 +2082,16 @@ int build_plan(b2_context* c, int batch, Plan** out) {
                 L.bytes = double(r.w_bytes) + double(batch) * (ti.c * 2.0 + to.item_bytes);
                 break;
             }
+            case b2plan::OP_LRN: {
+                const Tensor& ti = e->tensors[r.in];
+                L.kind = L_LRN;
+                L.in = tptr(r.in), L.out = tptr(r.out);
+                L.H = int(ti.h), L.W = int(ti.w), L.C = int(ti.c), L.C_phys = int(ti.c_phys), L.k = int(r.k);
+                L.alpha = op.lrn[0], L.beta = op.lrn[1], L.kk = op.lrn[2];  // (checked when the plan was read)
+                L.flops = double(batch) * ti.h * ti.w * ti.c * (2.0 * r.k + 4.0);
+                L.bytes = 2.0 * batch * ti.item_bytes;
+                break;
+            }
             default:
                 return fail(B2_EINVAL, "op %s: unknown type", op.name.c_str());
         }
@@ -2034,6 +2135,8 @@ int run_launch(const b2_engine* e, const Launch& L, void* const* bindings, cudaS
             return b2k::launch_conv_simt(L.simt, half, s);
         case L_MAXPOOL:
             return b2k::launch_maxpool(in, out, L.N, L.H, L.W, L.C_phys, L.Ho, L.Wo, L.k, L.stride, L.pad, half, s);
+        case L_LRN:
+            return b2k::launch_lrn_f16(in, out, static_cast<long long>(L.N) * L.H * L.W, L.C, L.C_phys, L.k, L.alpha, L.beta, L.kk, s);
         case L_AVGPOOL:
             return b2k::launch_avgpool(in, out, L.N, L.H * L.W, L.C_phys, half, s);
         case L_FC:
@@ -2888,8 +2991,8 @@ const char* b2_context_launch_name(b2_context* c, int batch, int i) {
     static const char* kinds[] = {"input_cast", "conv_tcgen05", "conv_simt", "maxpool", "avgpool", "fc", "softmax", "output_cast", "tail_pool_fc_softmax",
                                   "quantize", "conv_i8_tcgen05", "avgpool_i8", "output_cast_i8", "embed_ln", "layernorm", "attention_f16_wgmma",
                                   "pooler", "output_cast_rows", "output_unpack_rows", "quantize_f8", "conv_f8_tcgen05", "avgpool_f8",
-                                  "output_cast_f8", "patchify", "tokens", "cls_head"};
-    static_assert(sizeof(kinds) / sizeof(kinds[0]) == L_CLS_HEAD + 1, "kinds[] is indexed by LKind");
+                                  "output_cast_f8", "patchify", "tokens", "cls_head", "lrn"};
+    static_assert(sizeof(kinds) / sizeof(kinds[0]) == L_LRN + 1, "kinds[] is indexed by LKind");
     s = std::string(kinds[L->kind]) + (L->kind == L_ATTENTION && L->attn.S > 128 ? "_ks" : "") +  // key-split kernel
         (L->kind == L_ATTENTION && L->attn.seq_off ? "_varlen" : "") + ":" + L->name;         // variable-length kernel
     if (L->kind == L_ATTENTION && L->attn.S != L->W) s += " sk=" + std::to_string(L->attn.S);  // kernel of a longer sequence
@@ -2903,7 +3006,8 @@ const char* b2_context_launch_name(b2_context* c, int batch, int i) {
              " grid=" + std::to_string(L->conv.grid_n) + "x" + std::to_string(L->conv.grid_m) + "x" +
              std::to_string(L->conv.args.splits) + " kblk=" + std::to_string(L->conv.args.num_kblocks) +
              (L->conv.args.group_span ? " span=" + std::to_string(L->conv.args.group_span) : std::string()) +
-             ((L->conv.args.relu & b2plan::kConvGelu) ? " gelu" : "") + (L->conv.args.live ? " live" : "");
+             ((L->conv.args.relu & b2plan::kConvGelu) ? " gelu" : "") + (L->conv.args.live ? " live" : "") +
+             (L->cw ? " c0=" + std::to_string(L->c0) + " cw=" + std::to_string(L->cw) : std::string());
     if (L->kind == L_CONV_I8 || L->kind == L_CONV_F8)
         s += " bn=" + std::to_string(L->i8.bn) + " st=" + std::to_string(L->i8.stages) + (L->i8.args.a_mode == b2k::A_TILED ? " tiled" : " im2col") + " grid=" +
              std::to_string(L->i8.grid_n) + "x" + std::to_string(L->i8.grid_m) + " kblk=" + std::to_string(L->i8.args.num_kblocks) +

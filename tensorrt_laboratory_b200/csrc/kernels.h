@@ -186,6 +186,10 @@ int launch_output_cast(const void* src, float* dst, int N, int C, int H, int W, 
                        bool half_storage, cudaStream_t stream);
 int launch_maxpool(const void* src, void* dst, int N, int H, int W, int C_phys, int Ho, int Wo, int k,
                    int stride, int pad, bool half_storage, cudaStream_t stream);
+// Caffe LRN across channels (lrn_kernels.cu): fp16 NHWC [pixels][C_phys] -> same shape; n odd, 1 ... kLrnMaxSize
+constexpr int kLrnMaxSize = 15;
+int launch_lrn_f16(const void* src, void* dst, long long pixels, int C, int C_phys, int n, float alpha, float beta, float k,
+                   cudaStream_t stream);
 // global average pool: NHWC [N,HW,C] -> [N,1,1,C]
 int launch_avgpool(const void* src, void* dst, int N, int HW, int C_phys, bool half_storage,
                    cudaStream_t stream);

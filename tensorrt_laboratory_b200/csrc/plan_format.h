@@ -15,6 +15,9 @@ constexpr uint32_t kVersionGrouped = 2;
 // Version 3: OpRecV3 (224 bytes), written only for plans with transformer ops (OP_EMBED_LN ... OP_CLS_HEAD), so every CNN
 // plan keeps version 1 / 2.
 constexpr uint32_t kVersionTransformer = 3;
+// Version 4: OpRecV2 records whose reserved bytes carry output channel slices (out_c0, out_cw), written only for plans
+// that concatenate channels or hold an OP_LRN, so every other plan keeps version 1 / 2 / 3 and its bytes.
+constexpr uint32_t kVersionConcat = 4;
 
 enum OpType : uint32_t {
     OP_INPUT_CAST = 0,   // fp32 NCHW binding -> NHWC activation tensor
@@ -36,6 +39,7 @@ enum OpType : uint32_t {
     OP_TOKENS = 13,      // patch projection [N, 1, P, H] -> tokens [N, 1, P + 1, H] (class token, + position embeddings)
                          // and the packing index (tensor `out2`)
     OP_CLS_HEAD = 14,    // LayerNorm of token 0, then the classifier: fp16 [N, 1, S, H] -> fp32 logits [N, classes]
+    OP_LRN = 15,         // local response normalisation across channels (version-4 fp16 plans; OpRecV2 below)
 };
 
 enum TensorKind : uint32_t { T_ACT = 0 /* NHWC, engine precision */, T_VEC = 1 /* [N, c] fp32 */ };
@@ -99,10 +103,26 @@ struct OpRec {  // 176 bytes
 //   relu bit 1 clear (every other geometry, and fp32 engines): row-major [Cout_phys][taps_phys][Cin/groups];
 //     w_bytes = Cout_phys * taps_phys * (Cin / groups) * element size.
 // 1-byte (INT8 / FP8) grouped convolutions do not exist.
+//
+// Version-4 plans (kVersionConcat) use OpRecV2 and give its reserved bytes a meaning:
+//   out_c0, out_cw (OP_CONV only; 0 / 0 = the convolution writes all of its output tensor): the convolution writes output
+//     channels [out_c0, out_c0 + out_cw) of `out`, a tensor the outputs of several convolutions share (a channel
+//     concatenation with no copy).  Its own channel o lands at channel out_c0 + o; channels o >= out_cw are not written.
+//     Rules: fp16 plans only; no residual, no groups, packed weights; out_c0 % 8 == 0 (the TMA store's 16-byte aligned base);
+//     cout <= out_cw and cout_phys == roundup(out_cw, 64) (weight rows and bias past cout are zero); the slices of a tensor
+//     tile [0, c_phys) exactly, in any op order -- no gap, no overlap, every writer a slice writer -- and every slice but
+//     the last (highest out_c0) has out_cw == cout, while the last one ends at c_phys with out_c0 + cout == c.  Its zero
+//     weight rows so rewrite the tensor's tail padding [c, c_phys) with zeros on every pass.
+//   OP_LRN: Caffe ACROSS_CHANNELS local response normalisation of an fp16 tensor into one of the same shape:
+//     y_c = x_c * (k + alpha / n * sum_{|j - c| <= (n - 1) / 2} x_j^2)^(-beta), x_j = 0 outside [0, c).  `k` (the record
+//     field) = n, odd, 1 ... 15; b = fp32 [alpha, beta, k] (b_bytes = 12); no weights.  Numerics: the squares summed in
+//     fp32 in channel order, scale = fmaf(fp32(alpha / n), sum, k) in fp32, powf(scale, -beta) in fp32, x times that in
+//     fp32 and one rounding to fp16.  Channels >= c are written as zero.
 struct OpRecV2 {  // 192 bytes
     OpRec v1;
     uint32_t groups;
-    uint8_t reserved[12];
+    uint32_t out_c0, out_cw;  // version 4 only (zero in version-2 plans)
+    uint8_t reserved[4];
 };
 // Version-3 op record (plans with transformer ops).  OP_CONV: `relu` bit 3 = fused GELU (erf form) after bias and residual;
 // it excludes bit 0 and bit 2 (INT8).

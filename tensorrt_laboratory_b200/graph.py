@@ -149,7 +149,20 @@ def parse_prototxt(text: str) -> dict:
         elif ltype == "Eltwise":
             p = _one(L, "eltwise_param", {})
             rec.update(operation=_one(p, "operation", "SUM"))
-        elif ltype in ("ReLU", "Softmax"):
+        elif ltype == "Concat":
+            p = _one(L, "concat_param", {})
+            axis = _one(p, "axis", _one(p, "concat_dim", 1))
+            if axis != 1:
+                raise ValueError(f"prototxt: Concat {rec['name']}: concatenation along axis {axis}; only channels (axis 1) are supported")
+            rec.update(axis=1)
+        elif ltype == "LRN":
+            p = _one(L, "lrn_param", {})
+            region = _one(p, "norm_region", "ACROSS_CHANNELS")
+            if region != "ACROSS_CHANNELS":
+                raise ValueError(f"prototxt: LRN {rec['name']}: norm_region {region}; only ACROSS_CHANNELS is supported")
+            rec.update(local_size=_one(p, "local_size", 5), alpha=float(_one(p, "alpha", 1.0)), beta=float(_one(p, "beta", 0.75)),
+                       k=float(_one(p, "k", 1.0)))
+        elif ltype in ("ReLU", "Softmax", "Dropout"):
             pass
         else:
             raise ValueError(f"prototxt: unsupported layer type {ltype!r} ({rec['name']})")
@@ -253,6 +266,64 @@ def _bottleneck_net(name: str, depth: int, widths: List[int], group: int) -> dic
     return {"name": name, "input": "data", "input_dims": [1, 3, 224, 224], "layers": L}
 
 
+# BVLC GoogLeNet inception modules (Szegedy et al., "Going Deeper with Convolutions", Table 1):
+# name -> (#1x1, #3x3 reduce, #3x3, #5x5 reduce, #5x5, pool proj)
+_INCEPTION = {
+    "3a": (64, 96, 128, 16, 32, 32), "3b": (128, 128, 192, 32, 96, 64),
+    "4a": (192, 96, 208, 16, 48, 64), "4b": (160, 112, 224, 24, 64, 64), "4c": (128, 128, 256, 24, 64, 64),
+    "4d": (112, 144, 288, 32, 64, 64), "4e": (256, 160, 320, 32, 128, 128),
+    "5a": (256, 160, 320, 32, 128, 128), "5b": (384, 192, 384, 48, 128, 128),
+}
+
+
+def googlenet_caffe() -> dict:
+    """The raw layer list of BVLC GoogLeNet's deploy net (``models/bvlc_googlenet/deploy.prototxt`` of Caffe), without the
+    auxiliary classifiers, under the BVLC layer and blob names, so that ``bvlc_googlenet.caffemodel`` loads by name.
+    Every convolution has a bias and a ReLU; the LRN layers are local_size 5, alpha 1e-4, beta 0.75."""
+    L: List[dict] = []
+
+    def conv(name, bottom, nout, k, pad=0, stride=1, relu="relu"):
+        L.append(dict(name=name, type="Convolution", bottoms=[bottom], tops=[name], num_output=nout, kernel_size=k, pad=pad,
+                      stride=stride, bias_term=True))
+        L.append(dict(name=name.rsplit("/", 1)[0] + "/" + relu, type="ReLU", bottoms=[name], tops=[name]))
+
+    def pool(name, bottom, k, stride, pad=0, kind="MAX"):
+        L.append(dict(name=name, type="Pooling", bottoms=[bottom], tops=[name], pool=kind, kernel_size=k, stride=stride, pad=pad))
+
+    def lrn(name, bottom):
+        L.append(dict(name=name, type="LRN", bottoms=[bottom], tops=[name], local_size=5, alpha=1e-4, beta=0.75, k=1.0))
+
+    conv("conv1/7x7_s2", "data", 64, 7, 3, 2, "relu_7x7")
+    pool("pool1/3x3_s2", "conv1/7x7_s2", 3, 2)
+    lrn("pool1/norm1", "pool1/3x3_s2")
+    conv("conv2/3x3_reduce", "pool1/norm1", 64, 1, relu="relu_3x3_reduce")
+    conv("conv2/3x3", "conv2/3x3_reduce", 192, 3, 1, relu="relu_3x3")
+    lrn("conv2/norm2", "conv2/3x3")
+    pool("pool2/3x3_s2", "conv2/norm2", 3, 2)
+    prev = "pool2/3x3_s2"
+    for tag, (n1, r3, n3, r5, n5, pp) in _INCEPTION.items():
+        m = f"inception_{tag}"
+        conv(f"{m}/1x1", prev, n1, 1, relu="relu_1x1")
+        conv(f"{m}/3x3_reduce", prev, r3, 1, relu="relu_3x3_reduce")
+        conv(f"{m}/3x3", f"{m}/3x3_reduce", n3, 3, 1, relu="relu_3x3")
+        conv(f"{m}/5x5_reduce", prev, r5, 1, relu="relu_5x5_reduce")
+        conv(f"{m}/5x5", f"{m}/5x5_reduce", n5, 5, 2, relu="relu_5x5")
+        pool(f"{m}/pool", prev, 3, 1, 1)
+        conv(f"{m}/pool_proj", f"{m}/pool", pp, 1, relu="relu_pool_proj")
+        L.append(dict(name=f"{m}/output", type="Concat", bottoms=[f"{m}/1x1", f"{m}/3x3", f"{m}/5x5", f"{m}/pool_proj"],
+                      tops=[f"{m}/output"], axis=1))
+        prev = f"{m}/output"
+        if tag in ("3b", "4e"):
+            pool(f"pool{tag[0]}/3x3_s2", prev, 3, 2)
+            prev = f"pool{tag[0]}/3x3_s2"
+    pool("pool5/7x7_s1", prev, 7, 1, kind="AVE")
+    L.append(dict(name="pool5/drop_7x7_s1", type="Dropout", bottoms=["pool5/7x7_s1"], tops=["pool5/7x7_s1"]))
+    L.append(dict(name="loss3/classifier", type="InnerProduct", bottoms=["pool5/7x7_s1"], tops=["loss3/classifier"], num_output=1000,
+                  bias_term=True))
+    L.append(dict(name="prob", type="Softmax", bottoms=["loss3/classifier"], tops=["prob"]))
+    return {"name": "GoogleNet", "input": "data", "input_dims": [1, 3, 224, 224], "layers": L}
+
+
 # --------------------------------------------------------------------------------------------------
 # shape inference on raw layers
 # --------------------------------------------------------------------------------------------------
@@ -293,7 +364,12 @@ def infer_shapes(net: dict) -> Dict[str, Tuple[int, int, int]]:
                 if shapes[b] != (c, h, w):
                     raise ValueError(f"Eltwise {L['name']}: shape mismatch {shapes[b]} vs {(c, h, w)}")
             shapes[L["tops"][0]] = (c, h, w)
-        else:  # BatchNorm / Scale / ReLU / Softmax
+        elif t == "Concat":
+            for b in L["bottoms"][1:]:
+                if shapes[b][1:] != (h, w):
+                    raise ValueError(f"Concat {L['name']}: input {b} is {shapes[b][1]}x{shapes[b][2]}, not {h}x{w} like {L['bottoms'][0]}")
+            shapes[L["tops"][0]] = (sum(shapes[b][0] for b in L["bottoms"]), h, w)
+        else:  # BatchNorm / Scale / ReLU / Softmax / LRN / Dropout
             shapes[L["tops"][0]] = (c, h, w)
     return shapes
 
@@ -303,6 +379,23 @@ def infer_shapes(net: dict) -> Dict[str, Tuple[int, int, int]]:
 # --------------------------------------------------------------------------------------------------
 
 OP_CONV, OP_MAXPOOL, OP_AVGPOOL, OP_FC, OP_SOFTMAX = "conv", "maxpool", "avgpool", "fc", "softmax"
+OP_LRN = "lrn"
+
+
+def _drop_dropout(net: dict) -> dict:
+    """``net`` without its Dropout layers (identity at inference): a layer that reads a Dropout's top reads its bottom."""
+    if not any(L["type"] == "Dropout" for L in net["layers"]):
+        return net
+    alias: Dict[str, str] = {}
+    layers = []
+    for L in net["layers"]:
+        bottoms = [alias.get(b, b) for b in L["bottoms"]]
+        if L["type"] == "Dropout":
+            if L["tops"][0] != bottoms[0]:
+                alias[L["tops"][0]] = bottoms[0]
+            continue
+        layers.append(dict(L, bottoms=bottoms))
+    return dict(net, layers=layers)
 
 
 def lower(net: dict, weights: Optional[dict] = None) -> dict:
@@ -315,6 +408,7 @@ def lower(net: dict, weights: Optional[dict] = None) -> dict:
     """
     import numpy as np
 
+    net = _drop_dropout(net)
     layers = net["layers"]
     shapes = infer_shapes(net)
     # last writer of each blob decides the SSA tensor that consumers see
@@ -424,6 +518,44 @@ def lower(net: dict, weights: Optional[dict] = None) -> dict:
             ops.append(op)
             producer[L["tops"][0]] = op
             tensors[L["tops"][0]] = shapes[L["tops"][0]]
+        elif t == "LRN":
+            n = L.get("local_size", 5)
+            if n < 1 or n % 2 == 0:
+                raise ValueError(f"LRN {name}: local_size {n} must be odd")
+            if L["tops"][0] == L["bottoms"][0]:
+                raise ValueError(f"LRN {name}: in-place LRN is not supported (give the layer its own top)")
+            op = dict(type=OP_LRN, name=name, input=L["bottoms"][0], output=L["tops"][0], local_size=n,
+                      alpha=float(L.get("alpha", 1.0)), beta=float(L.get("beta", 0.75)), k=float(L.get("k", 1.0)))
+            ops.append(op)
+            producer[L["tops"][0]] = op
+            tensors[L["tops"][0]] = shapes[L["tops"][0]]
+        elif t == "Concat":
+            # no op: each input convolution writes its own channel range of the output (op["out_c0"])
+            top = L["tops"][0]
+            if len(set(L["bottoms"])) != len(L["bottoms"]) or top in L["bottoms"]:
+                raise ValueError(f"Concat {name}: an input appears twice, or the output overwrites an input")
+            c0 = 0
+            for b in L["bottoms"]:
+                op = producer.get(b)
+                if op is None or op["type"] != OP_CONV or op["residual"] is not None or op["output"] != b:
+                    raise ValueError(f"Concat {name}: input {b} is not the output of a convolution (only convolutions, "
+                                     "without a residual, can be concatenated)")
+                # (the convolution's own in-place BatchNorm / Scale / ReLU before the Concat are part of it)
+                readers = [M["name"] for j, M in enumerate(layers) if j != i and b in M["bottoms"] and
+                           not (j < i and M["type"] in ("BatchNorm", "Scale", "ReLU") and M["tops"] == [b])]
+                if readers:
+                    raise ValueError(f"Concat {name}: input {b} is also read by {readers[0]}; a concatenated convolution "
+                                     "output may have no other reader")
+                if b == net["input"]:
+                    raise ValueError(f"Concat {name}: the network input cannot be concatenated")
+                op["output"] = top
+                op["out_c0"] = c0
+                op["_sealed"] = True
+                c0 += op["cout"]
+                del tensors[b]
+                del producer[b]
+            tensors[top] = shapes[top]
+            producer[top] = dict(type="concat", name=name)
         else:
             raise ValueError(f"unsupported layer type {t}")
         i += 1

@@ -178,6 +178,18 @@ def import_onnx(model: dict, input_dims: Optional[List[int]] = None, name: str =
         elif op == "Softmax":
             layers.append(dict(name=uname(node, out), type="Softmax", bottoms=[ins[0]], tops=[out]))
             shapes[out] = shapes[ins[0]]
+        elif op == "Concat":
+            if int(attrs.get("axis", 1)) != 1:
+                raise ValueError(f"onnx import: Concat {node['name'] or out} along axis {attrs.get('axis')}; only channels (axis 1)")
+            layers.append(dict(name=uname(node, out), type="Concat", bottoms=ins, tops=[out], axis=1))
+            shapes[out] = (sum(shapes[x][0] for x in ins),) + shapes[ins[0]][1:]
+        elif op == "LRN":
+            size = int(attrs["size"])
+            if size % 2 == 0:
+                raise ValueError(f"onnx import: LRN {node['name'] or out}: even size {size} (the window is centred only for odd sizes)")
+            layers.append(dict(name=uname(node, out), type="LRN", bottoms=[ins[0]], tops=[out], local_size=size,
+                               alpha=float(attrs.get("alpha", 1e-4)), beta=float(attrs.get("beta", 0.75)), k=float(attrs.get("bias", 1.0))))
+            shapes[out] = shapes[ins[0]]
         else:
             raise ValueError(f"onnx import: unsupported operator {op}")
     net = {"name": name, "input": inp, "input_dims": input_dims, "layers": layers}
@@ -311,6 +323,15 @@ def export_onnx(net: dict, weights: Dict[str, dict], opset: int = 11) -> bytes:
         elif ty == "Softmax":
             src = t(L["bottoms"][0])
             nodes.append(_node("Softmax", [src], [fresh(L["tops"][0])], name, axis=1))
+        elif ty == "Concat":
+            srcs = [t(b) for b in L["bottoms"]]
+            nodes.append(_node("Concat", srcs, [fresh(L["tops"][0])], name, axis=1))
+        elif ty == "LRN":
+            src = t(L["bottoms"][0])
+            nodes.append(_node("LRN", [src], [fresh(L["tops"][0])], name, size=int(L["local_size"]), alpha=float(L["alpha"]),
+                               beta=float(L["beta"]), bias=float(L["k"])))
+        elif ty == "Dropout":  # identity at inference
+            cur[L["tops"][0]] = t(L["bottoms"][0])
         else:
             raise ValueError(f"export_onnx: unsupported layer type {ty}")
         i += 1

@@ -129,6 +129,10 @@ def quantize_lowered(lowered: dict, calib_inputs: np.ndarray, amax: Optional[Dic
     qmax = E4M3_MAX if fp8 else QMAX
     from .builder import grouped_1byte_span
     for op in lowered["ops"]:
+        if "out_c0" in op or op["type"] == G.OP_LRN:
+            raise ValueError(f"{op['name']}: a graph with a Concat or LRN layer builds in fp16 only; {name} channel "
+                             "concatenation and LRN are not supported")
+    for op in lowered["ops"]:
         if op["type"] == G.OP_CONV and op.get("groups", 1) != 1:
             if not grouped:
                 raise ValueError(f"conv {op['name']}: {name} grouped convolution is not supported ({op['groups']} groups); "

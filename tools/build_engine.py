@@ -13,6 +13,7 @@ examples/ONNX/resnet50/build.py:35-67).
   python tools/build_engine.py --model bert-base --seq 128 --batch 16 [--weights bert.npz] --tune -o bert.plan  (fp16)
   python tools/build_engine.py --model bert-base --seq 384 --batch 16 --remove-padding -o bert_packed.plan  (masked tokens skipped)
   python tools/build_engine.py --model vit-b16 --batch 8 [--weights vit.npz] --tune -o vit.plan  (ViT-B/16, also vit-b32 / vit-l16; fp16)
+  python tools/build_engine.py --model googlenet --batch 8 [--caffemodel bvlc_googlenet.caffemodel] --tune -o googlenet.plan  (fp16)
 Weights: deterministic synthetic weights (the reference's benchmark engines are weightless too, models/README.md:6-7),
 unless --caffemodel names a binary NetParameter (trtexec --model=...); MNIST and --onnx carry their own weights.
 --precision int8 / fp8: post-training quantization (fp8: E4M3), max-abs calibration on --calib (an .npy [N,C,H,W] fp32) or on
@@ -31,7 +32,7 @@ from tensorrt_laboratory_b200 import builder, graph, weights  # noqa: E402
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--model", choices=["resnet50", "resnet152", "resnext50", "mnist", "bert-base", "vit-b16", "vit-b32", "vit-l16"])
+    ap.add_argument("--model", choices=["resnet50", "resnet152", "resnext50", "mnist", "bert-base", "vit-b16", "vit-b32", "vit-l16", "googlenet"])
     ap.add_argument("--seq", type=int, default=128, help="bert-base: the sequence length of the plan (64, 128, 256, 384 or 512)")
     ap.add_argument("--weights", help="bert-base / vit-*: .npz of Hugging Face BertModel / ViTForImageClassification parameters "
                                         "(default: seeded weights)")
@@ -78,6 +79,9 @@ def main():
         sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
         from tests import helpers
         net, wts, _, _ = helpers.load_mnist_golden()
+    elif a.model == "googlenet":  # BVLC GoogLeNet (no auxiliary classifiers): Concat and LRN, fp16 only
+        net = graph.googlenet_caffe()
+        wts = weights_for(net)
     elif a.model == "resnext50":  # 32x4d: grouped 3x3 convolutions, cpg 4 ... 32 (every precision)
         net = graph.resnext_caffe(50)
         wts = weights_for(net)
