@@ -20,6 +20,7 @@ OP_EMBED_LN, OP_LAYERNORM, OP_ATTENTION, OP_POOLER = range(8, 12)   # transforme
 OP_PATCHIFY, OP_TOKENS, OP_CLS_HEAD = range(12, 15)                  # Vision Transformer ops (version-3 plans)
 OP_LRN = 15                                                          # local response normalisation (version-4 plans)
 CONV_RELU, CONV_PACKED, CONV_INT8, CONV_GELU = 1, 2, 4, 8            # OpRec.relu bits of a convolution
+CONV_PREACT = 16  # OpRec.relu bit of a convolution or average pool: BatchNorm + ReLU input prologue (version-4 plans)
 FLAG_ROWS_OUT, FLAG_PACKED = 1, 2  # OpRecV3.flags: channels-last output cast; op on packed (padding-free) rows
 T_ACT, T_VEC = 0, 1
 MAGIC = b"B2ENGINE"
@@ -78,6 +79,12 @@ def expand_grouped_weights(W: np.ndarray, groups: int, span: int, cout_phys: int
 
 def _roundup(v: int, m: int) -> int:
     return (v + m - 1) // m * m
+
+
+def _pad_vec(v: np.ndarray, n: int) -> np.ndarray:
+    out = np.zeros(n, dtype=np.float32)
+    out[:len(v)] = v
+    return out
 
 
 def phys_channels(c: int, precision: int) -> int:
@@ -248,7 +255,10 @@ def build_plan(lowered: dict, precision: int = PREC_FP16, max_batch: int = 8,
             if op["out_c0"] % 8:
                 raise ValueError(f"Concat {tname}: input {op['name']} starts at channel {op['out_c0']}, not a multiple of 8 "
                                  "(the 16-byte alignment of the convolution's output store)")
-            slice_width[op["name"]] = c_phys - op["out_c0"] if k + 1 == len(ws) else op["cout"]
+            if op["type"] == G.OP_MAXPOOL and k + 1 < len(ws):  # a max pool writes its input's padded channels
+                slice_width[op["name"]] = phys_channels(shapes[op["input"]][0], PREC_FP16)
+            else:
+                slice_width[op["name"]] = c_phys - op["out_c0"] if k + 1 == len(ws) else op["cout"]
 
     for op in lowered["ops"]:
         t = op["type"]
@@ -315,6 +325,8 @@ def build_plan(lowered: dict, precision: int = PREC_FP16, max_batch: int = 8,
             if "W" not in op:
                 raise ValueError(f"conv {op['name']}: lowered graph carries no weights")
             cin_phys = tensors[ti]["c_phys"]
+            if op["input"] in writers and op["cin"] < shapes[op["input"]][0]:  # input prefix: channels [0, cin) of a concatenation
+                cin_phys = _roundup(op["cin"], 64)
             cout_phys = tensors[to]["c_phys"]
             k = op["k"]
             Wsrc, cin_eff, extra = op["W"], op["cin"], {}
@@ -340,8 +352,14 @@ def build_plan(lowered: dict, precision: int = PREC_FP16, max_batch: int = 8,
                 w_off, w_bytes = add_payload(pack_weights_sw128(W.astype(np.float16).reshape(cout_phys, taps_phys * cin_phys)))
             else:
                 w_off, w_bytes = add_payload(W.astype(wdtype))
+            pre = 0
+            if op.get("pre"):  # b = [bias cout_phys][scale cin_phys][shift cin_phys]
+                if precision_fp != PREC_FP16 or not packed:
+                    raise ValueError(f"conv {op['name']}: a BatchNorm + ReLU input prologue needs an fp16 plan with packed weights")
+                bias = np.concatenate([bias, _pad_vec(op["pre_scale"], cin_phys), _pad_vec(op["pre_shift"], cin_phys)])
+                pre = CONV_PREACT
             b_off, b_bytes = add_payload(bias)
-            rec.update(type=OP_CONV, k=k, stride=op["stride"], pad=op["pad"], relu=int(op["relu"]) | (2 if packed else 0),
+            rec.update(type=OP_CONV, k=k, stride=op["stride"], pad=op["pad"], relu=int(op["relu"]) | (2 if packed else 0) | pre,
                        cin=cin_eff, cout=op["cout"], cin_phys=cin_phys, cout_phys=cout_phys,
                        taps=taps, taps_phys=taps_phys, w_off=w_off, w_bytes=w_bytes, b_off=b_off, b_bytes=b_bytes)
             rec.update(extra)
@@ -349,7 +367,19 @@ def build_plan(lowered: dict, precision: int = PREC_FP16, max_batch: int = 8,
                 rec["res"] = add_tensor(op["residual"])
         elif t == G.OP_MAXPOOL:
             rec.update(type=OP_MAXPOOL, k=op["k"], stride=op["stride"], pad=op["pad"], ceil_mode=int(op["ceil_mode"]))
+            if op["name"] in slice_width:
+                if precision_fp != PREC_FP16:
+                    raise ValueError(f"maxpool {op['name']}: a concatenated max pool needs an fp16 plan")
+                rec.update(out_c0=op["out_c0"], out_cw=slice_width[op["name"]])
+        elif t == G.OP_AVGPOOL and op.get("pre"):  # b = [scale c_phys][shift c_phys]
+            if precision_fp != PREC_FP16:
+                raise ValueError(f"avgpool {op['name']}: a BatchNorm + ReLU input prologue needs an fp16 plan")
+            c_phys = tensors[ti]["c_phys"]
+            b_off, b_bytes = add_payload(np.concatenate([_pad_vec(op["pre_scale"], c_phys), _pad_vec(op["pre_shift"], c_phys)]))
+            rec.update(type=OP_AVGPOOL, k=op["k"], stride=op["k"], relu=CONV_PREACT, b_off=b_off, b_bytes=b_bytes)
         elif t == G.OP_AVGPOOL:
+            if tensors[to]["h"] != 1 or tensors[to]["w"] != 1:
+                raise ValueError(f"avgpool {op['name']}: a windowed average pool runs only with a BatchNorm + ReLU input prologue")
             rec.update(type=OP_AVGPOOL, k=op["k"], stride=op["stride"])
         elif t == G.OP_FC:
             c, h, w = op["in_chw"]
@@ -695,6 +725,21 @@ def build_googlenet_plan(precision: int = PREC_FP16, max_batch: int = 8, seed: i
         raise ValueError("GoogLeNet builds in fp16 only: channel concatenation and LRN have no fp32, INT8 or FP8 kernels")
     from . import weights as Wt
     net = G.googlenet_caffe()
+    low = G.lower(net, weights if weights is not None else Wt.random_weights(net, seed))
+    return build_plan(low, precision, max_batch, input_dtype=input_dtype)
+
+
+def build_densenet_plan(depth: int = 121, max_batch: int = 8, seed: int = 0, weights: Optional[dict] = None,
+                        precision: int = PREC_FP16, input_dtype: str = "f32") -> bytes:
+    """Convenience: generated DenseNet-{121,169,201} (:func:`graph.densenet_caffe`) + deterministic (or given, Caffe-named:
+    ``weights.random_weights``, ``caffemodel``, ``densenet.load_weights``) weights -> fp16 plan.  Each dense block is one
+    tensor: the stem's max pool or the transition convolution writes its first channels and every 3x3 its 32, and every
+    1x1 reads the channel prefix written so far through a BatchNorm + ReLU input prologue.  fp16 only."""
+    if precision != PREC_FP16:
+        raise ValueError("DenseNet builds in fp16 only: the BatchNorm + ReLU prologue and channel concatenation have no fp32, "
+                         "INT8 or FP8 kernels")
+    from . import weights as Wt
+    net = G.densenet_caffe(depth)
     low = G.lower(net, weights if weights is not None else Wt.random_weights(net, seed))
     return build_plan(low, precision, max_batch, input_dtype=input_dtype)
 

@@ -117,6 +117,8 @@ struct Op {
     int side_join = -1;
     // version-4 convolutions: output channels [c0, c0 + cw) of a tensor several convolutions write (cw == 0: all of it)
     int c0 = 0, cw = 0;
+    // version-4 convolutions: reads channels [0, r.cin) of a wider, slice-written input (plan_format.h, input prefix)
+    bool prefix = false;
     float lrn[3] = {0.f, 0.f, 0.f};  // OP_LRN: alpha, beta, k (host copy of the op's parameter block)
     // conv geometry with the "0 = square" defaults resolved
     int kh() const { return int(r.k); }
@@ -147,7 +149,7 @@ struct Binding {
 
 enum LKind { L_INPUT_CAST, L_CONV_TC, L_CONV_SIMT, L_MAXPOOL, L_AVGPOOL, L_FC, L_SOFTMAX, L_OUTPUT_CAST, L_TAIL, L_QUANTIZE, L_CONV_I8, L_AVGPOOL_I8, L_OUTPUT_CAST_I8,
              L_EMBED_LN, L_LAYERNORM, L_ATTENTION, L_POOLER, L_OUTPUT_ROWS, L_OUTPUT_UNPACK, L_QUANTIZE_F8, L_CONV_F8, L_AVGPOOL_F8,
-             L_OUTPUT_CAST_F8, L_PATCHIFY, L_TOKENS, L_CLS_HEAD, L_LRN };
+             L_OUTPUT_CAST_F8, L_PATCHIFY, L_TOKENS, L_CLS_HEAD, L_LRN, L_AVGPOOL_PRE };
 
 // Attention kernel of a packed plan's S tokens: the smallest instantiated sequence length S_k >= S (the variable-length
 // kernels attend each item over its own rows, so the rows S ... S_k - 1 of an item's tile are never used)
@@ -182,7 +184,8 @@ struct Launch {
     const int* live = nullptr;    // L_LAYERNORM of a packed plan: the live row count T (device)
     const int* pos_map = nullptr; // L_POOLER / L_OUTPUT_UNPACK of a packed plan: the packing index's pos_map (device)
     int N = 0, C = 0, H = 0, W = 0, C_phys = 0, Ho = 0, Wo = 0, k = 0, stride = 0, pad = 0, K = 0, Cout = 0;
-    int c0 = 0, cw = 0;                       // L_CONV_TC of a slice writer: its output channels (Op::c0, Op::cw)
+    int c0 = 0, cw = 0;                       // L_CONV_TC / L_MAXPOOL of a slice writer: its output channels (Op::c0, Op::cw)
+    int out_pitch = 0;                        // L_MAXPOOL of a slice writer: channels per pixel of its output tensor
     float alpha = 0.f, beta = 0.f, kk = 0.f;  // L_LRN (k = n)
 };
 
@@ -527,6 +530,8 @@ int validate_slices(b2_engine* e) {
     std::map<int, std::vector<const Op*>> writers;  // tensor -> its slice writers
     for (const Op& op : e->ops)
         if (op.cw) writers[op.r.out].push_back(&op);
+    // real channels of a slice writer: a convolution's cout, a max pool's input channels
+    auto real = [&](const Op& op) { return op.r.type == b2plan::OP_CONV ? int(op.r.cout) : int(e->tensors[size_t(op.r.in)].c); };
     for (auto& [t, ws] : writers) {
         const Tensor& to = e->tensors[size_t(t)];
         for (const Op& op : e->ops)
@@ -542,12 +547,30 @@ int validate_slices(b2_engine* e) {
                 return fail(B2_EINVAL, "plan: conv %s: slice [%d, %d) of %s leaves channels [%d, %d) unwritten", op.name.c_str(), op.c0, op.c0 + op.cw,
                             to.name.c_str(), next, op.c0);
             const bool last = i + 1 == ws.size();
-            if (last ? (uint32_t(op.c0 + op.cw) != to.c_phys || op.c0 + int(op.r.cout) != int(to.c)) : int(op.r.cout) != op.cw)
+            if (last ? (uint32_t(op.c0 + op.cw) != to.c_phys || op.c0 + real(op) != int(to.c)) : real(op) != op.cw)
                 return fail(B2_EINVAL, "plan: conv %s: slice [%d, %d) of %s: slices carry their real channels back to back, and the last one "
                             "ends at channel %u (c_phys) after the tensor's %u real ones", op.name.c_str(), op.c0, op.c0 + op.cw, to.name.c_str(),
                             to.c_phys, to.c);
             next = op.c0 + op.cw;
         }
+    }
+    // input prefixes: [0, cin) of a slice-written tensor, ending at a slice boundary, read after every writer of those slices
+    for (size_t i = 0; i < e->ops.size(); ++i) {
+        const Op& op = e->ops[i];
+        if (!op.prefix) continue;
+        const auto it = writers.find(op.r.in);
+        const Tensor& ti = e->tensors[size_t(op.r.in)];
+        if (it == writers.end())
+            return fail(B2_EINVAL, "plan: conv %s: reads channels [0, %u) of %s, which is not slice-written", op.name.c_str(), op.r.cin, ti.name.c_str());
+        bool boundary = false;
+        for (const Op* w : it->second) {
+            if (w->c0 + real(*w) == int(op.r.cin)) boundary = true;
+            if (w->c0 < int(op.r.cin) && w >= &op)
+                return fail(B2_EINVAL, "plan: conv %s: reads channels [0, %u) of %s before %s writes its slice [%d, %d)", op.name.c_str(), op.r.cin,
+                            ti.name.c_str(), w->name.c_str(), w->c0, w->c0 + w->cw);
+        }
+        if (!boundary)
+            return fail(B2_EINVAL, "plan: conv %s: prefix [0, %u) of %s does not end at a slice boundary", op.name.c_str(), op.r.cin, ti.name.c_str());
     }
     return B2_OK;
 }
@@ -616,8 +639,8 @@ int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** pa
                 return fail(B2_EINVAL, "plan: conv %s has %u groups", fixed_str(r2.v1.name, 64).c_str(), r2.groups);
             if (r2.v1.type == OP_CONV) op.groups = int(r2.groups);
             if (v4 && (r2.out_c0 || r2.out_cw)) {
-                if (r2.v1.type != OP_CONV)
-                    return fail(B2_EINVAL, "plan: op %s: only a convolution writes an output channel slice", fixed_str(r2.v1.name, 64).c_str());
+                if (r2.v1.type != OP_CONV && r2.v1.type != OP_MAXPOOL)
+                    return fail(B2_EINVAL, "plan: op %s: only a convolution writes an output channel slice (and a max pool, its input's channels)", fixed_str(r2.v1.name, 64).c_str());
                 if (r2.out_cw == 0 || r2.out_c0 > (1u << 20) || r2.out_cw > (1u << 20))
                     return fail(B2_EINVAL, "plan: conv %s: bad output channel slice [%u, +%u)", fixed_str(r2.v1.name, 64).c_str(), r2.out_c0, r2.out_cw);
                 op.c0 = int(r2.out_c0), op.cw = int(r2.out_cw);
@@ -657,12 +680,39 @@ int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** pa
             return fail(B2_EINVAL, "plan: op %s weights outside payload", op.name.c_str());
         if ((r.type == OP_MAXPOOL || r.type == OP_AVGPOOL) && (r.k == 0 || r.stride == 0))
             return fail(B2_EINVAL, "plan: pool %s has a zero window or stride", op.name.c_str());
+        if (r.type == OP_MAXPOOL && op.cw) {  // a slice writer (plan_format.h, version 4)
+            const Tensor& ti = e->tensors[r.in];
+            const Tensor& to = e->tensors[r.out];
+            if (h.precision != B2_PREC_FP16 || op.c0 % 8 || uint32_t(op.cw) != ti.c_phys || uint64_t(op.c0) + uint64_t(op.cw) > to.c_phys ||
+                ti.kind != T_ACT || to.kind != T_ACT || to.binding >= 0 || r.in == r.out)
+                return fail(B2_EINVAL, "plan: op %s: only a convolution writes an output channel slice, and a max pool all %u channels of its "
+                            "input, at a multiple of 8, into an fp16 arena activation it does not read", op.name.c_str(), ti.c_phys);
+        }
         if (r.type == OP_MAXPOOL) {
             const Tensor& ti = e->tensors[r.in];
             const Tensor& to = e->tensors[r.out];
-            if (ti.kind != T_ACT || to.kind != T_ACT || ti.c_phys != to.c_phys || to.h == 0 || to.w == 0 ||
+            if (ti.kind != T_ACT || to.kind != T_ACT || (!op.cw && ti.c_phys != to.c_phys) || to.h == 0 || to.w == 0 ||
                 uint64_t(to.h - 1) * r.stride >= uint64_t(ti.h) + r.pad_ || uint64_t(to.w - 1) * r.stride >= uint64_t(ti.w) + r.pad_)
                 return fail(B2_EINVAL, "plan: pool %s output dims do not fit its input", op.name.c_str());
+        }
+        if (r.type == OP_AVGPOOL) {
+            // a prologue pool, or a k x k / stride k window (plan_format.h, version 4); without a prologue, only the global pool
+            const Tensor& ti = e->tensors[r.in];
+            const Tensor& to = e->tensors[r.out];
+            const bool pre = (r.relu & kConvPreAct) != 0;
+            if (r.relu & ~kConvPreAct) return fail(B2_EINVAL, "plan: avgpool %s: unknown flags 0x%x", op.name.c_str(), r.relu);
+            if (pre && !(v4 && h.precision == B2_PREC_FP16))
+                return fail(B2_EINVAL, "plan: avgpool %s: a BatchNorm + ReLU prologue needs a version-4 fp16 plan", op.name.c_str());
+            if (!pre && (to.h != 1 || to.w != 1))
+                return fail(B2_EINVAL, "plan: avgpool %s: a windowed average pool carries a BatchNorm + ReLU prologue", op.name.c_str());
+            if (pre) {
+                if (ti.kind != T_ACT || to.kind != T_ACT || r.stride != r.k || r.pad_ || ti.h % r.k || ti.w % r.k || to.h != ti.h / r.k ||
+                    to.w != ti.w / r.k || to.c != ti.c || to.c_phys != ti.c_phys || ti.c % 8 || ti.c_phys % 8 || r.in == r.out)
+                    return fail(B2_EINVAL, "plan: avgpool %s: a prologue pool is a k x k / stride k window without padding that tiles its "
+                                "input, into a distinct tensor of the same channels", op.name.c_str());
+                if (r.w_bytes != 0 || r.b_bytes != size_t(ti.c_phys) * 8)
+                    return fail(B2_EINVAL, "plan: avgpool %s: the prologue parameters must be fp32 [scale c_phys][shift c_phys]", op.name.c_str());
+            }
         }
         if (r.type == OP_INPUT_CAST || r.type == OP_OUTPUT_CAST) {  // the caller's Buffers are sized from the BINDING dims
             const Tensor& tt = e->tensors[r.type == OP_INPUT_CAST ? r.out : r.in];
@@ -677,6 +727,19 @@ int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** pa
         if (r.type == OP_CONV) {
             if (r.k == 0 || r.stride == 0 || int(r.taps) != op.kh() * op.kw() || r.taps_phys < r.taps || op.sw() == 0)
                 return fail(B2_EINVAL, "plan: conv %s has bad geometry", op.name.c_str());
+            if (v4 && (r.relu & ~(kConvRelu | kConvPacked | kConvInt8 | kConvGelu | kConvPreAct)))
+                return fail(B2_EINVAL, "plan: conv %s: unknown flags 0x%x", op.name.c_str(), r.relu);
+            const bool pre = (r.relu & kConvPreAct) != 0;
+            if (pre && (!v4 || h.precision != B2_PREC_FP16 || (r.relu & (kConvInt8 | kConvGelu))))
+                return fail(B2_EINVAL, "plan: conv %s: a BatchNorm + ReLU prologue needs a version-4 fp16 plan", op.name.c_str());
+            if (pre && (r.k != 1 || r.kw || r.stride != 1 || r.pad_ || !(r.relu & kConvPacked) || op.groups != 1 || r.res >= 0))
+                return fail(B2_EINVAL, "plan: conv %s: a BatchNorm + ReLU prologue exists for dense 1x1 stride-1 unpadded convolutions with "
+                            "packed weights and no residual", op.name.c_str());
+            op.prefix = v4 && r.cin < e->tensors[r.in].c;
+            if (op.prefix && (r.k != 1 || r.kw || r.stride != 1 || r.pad_ || !(r.relu & kConvPacked) || op.groups != 1 || (r.relu & kConvInt8) ||
+                              r.cin == 0 || r.cin_phys != (r.cin + 63) / 64 * 64 || r.cin_phys > e->tensors[r.in].c_phys))
+                return fail(B2_EINVAL, "plan: conv %s: an input prefix reader is a dense 1x1 stride-1 convolution with packed weights and "
+                            "cin_phys = cin rounded up to 64", op.name.c_str());
             if ((r.relu & kConvGelu) && (!v3 || (r.relu & (kConvRelu | kConvInt8))))
                 return fail(B2_EINVAL, "plan: conv %s: GELU excludes ReLU and INT8 and needs a version-3 plan", op.name.c_str());
             if ((r.relu & kConvGelu) && (r.k != 1 || r.kw || r.stride != 1 || r.pad_ || !(r.relu & kConvPacked) ||
@@ -724,7 +787,8 @@ int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** pa
                     return fail(B2_EINVAL, "plan: %s conv %s: tensors must be %s with 128-channel rows", qfmt, op.name.c_str(), qfmt);
                 if (r.w_bytes != size_t(r.cout_phys) * r.taps_phys * r.cin_phys || r.b_bytes != (size_t(r.cout_phys) * 2 + 4) * 4)
                     return fail(B2_EINVAL, "plan: %s conv %s weight / requantisation size mismatch", qfmt, op.name.c_str());
-            } else if (r.w_bytes != size_t(r.cout_phys) * r.taps_phys * r.cin_phys * elt || r.b_bytes != size_t(r.cout_phys) * 4)
+            } else if (r.w_bytes != size_t(r.cout_phys) * r.taps_phys * r.cin_phys * elt ||
+                       r.b_bytes != (size_t(r.cout_phys) + (pre ? 2 * size_t(r.cin_phys) : 0)) * 4)
                 return fail(B2_EINVAL, "plan: conv %s weight size mismatch", op.name.c_str());
             if (!i8 && (e->tensors[r.in].scale > 0.f || e->tensors[r.out].scale > 0.f))
                 return fail(B2_EINVAL, "plan: fp16 conv %s touches an %s tensor", op.name.c_str(), qfmt);
@@ -739,10 +803,10 @@ int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** pa
                     return fail(B2_EINVAL, "plan: conv %s: slice [%d, %d) runs past the %u channels of %s", op.name.c_str(), op.c0, op.c0 + op.cw,
                                 to.c_phys, to.name.c_str());
                 if (op.groups != 1 || !(r.relu & kConvPacked) || r.cout > uint32_t(op.cw) || r.cout_phys != (uint32_t(op.cw) + 63) / 64 * 64 ||
-                    ti.c_phys != r.cin_phys || ti.c != r.cin || to.kind != T_ACT || to.binding >= 0 || r.in == r.out)
+                    (!op.prefix && (ti.c_phys != r.cin_phys || ti.c != r.cin)) || to.kind != T_ACT || to.binding >= 0 || r.in == r.out)
                     return fail(B2_EINVAL, "plan: conv %s: a slice writer is a dense packed-weight convolution with cout <= width and "
                                 "cout_phys = width rounded up to 64, into an arena activation it does not read", op.name.c_str());
-            } else if (ti.c_phys != r.cin_phys || to.c_phys != r.cout_phys || ti.c != r.cin || to.c != r.cout)
+            } else if ((!op.prefix && (ti.c_phys != r.cin_phys || ti.c != r.cin)) || to.c_phys != r.cout_phys || to.c != r.cout)
                 return fail(B2_EINVAL, "plan: conv %s channel mismatch with its tensors", op.name.c_str());
             if (uint64_t(ti.h) + 2 * uint64_t(r.pad_) < r.k || int64_t(ti.w) + op.pw_lo() + op.pw_hi() < op.kw())
                 return fail(B2_EINVAL, "plan: conv %s window larger than its padded input", op.name.c_str());
@@ -871,7 +935,7 @@ void plan_arena(b2_engine* e) {
         Op& op = e->ops[i];
         op.side_join = -1;
         // (a slice writer's tensor is read as a whole by later ops, never as one residual: it is not a side branch)
-        if (int(i) <= busy_until || op.r.type != b2plan::OP_CONV || op.r.out < 0 || e->tensors[op.r.out].binding >= 0 || op.cw) continue;
+        if (int(i) <= busy_until || op.r.type != b2plan::OP_CONV || op.r.out < 0 || e->tensors[op.r.out].binding >= 0 || op.cw || op.prefix) continue;
         int consumers = 0, join = -1;
         bool as_residual_only = true;
         for (size_t k = i + 1; k < e->ops.size(); ++k) {
@@ -1084,6 +1148,8 @@ int fuse_partner(const b2_engine* e, int i) {
     const b2plan::OpRec &ri = oi.r, &rj = oj.r;
     // a slice writer is neither: it has no residual (so no 1x1 of a pair), and its tensor has other readers (no 3x3 of one)
     if (oi.cw || oj.cw) return -1;
+    // nor are a prefix reader and a prologue convolution (they run the one-tile kernel only)
+    if (oi.prefix || oj.prefix || ((ri.relu | rj.relu) & b2plan::kConvPreAct)) return -1;
     if (ri.type != b2plan::OP_CONV || rj.type != b2plan::OP_CONV || (ri.relu & (4 | b2plan::kConvGelu)) || conv_halo_rows(e, oi) == 0 ||
         !b2k::conv_halo_config_exists(int(ri.cout_phys)) || ri.cin_phys / 64 > 8)
         return -1;
@@ -1128,6 +1194,13 @@ bool tactic_applies(const b2_context* c, const Op& op, int batch, const ConvConf
     const Tensor& to = c->e->tensors[r.out];
     const int span = op.group_span(), kb = conv_kb(c, op);
     if (cfg.bn <= 0 || int(r.cout_phys) % cfg.bn || cfg.splits < 1 || cfg.sps < 1 || cfg.ws < 0) return false;
+    // a prologue convolution or a prefix reader: the tiled packed-weight one-tile kernel only, its prologue's scale and
+    // shift in shared memory too
+    if ((r.relu & b2plan::kConvPreAct) || op.prefix)
+        return !cfg.ws && cfg.cn <= 1 && !cfg.halo && cfg.splits == 1 && kb == 64 && (r.relu & b2plan::kConvPacked) &&
+               b2k::conv_config_exists(cfg.bn, kb, cfg.stages, cfg.sps) &&
+               b2k::conv_smem_bytes(cfg.bn, cfg.stages, r.res >= 0, cfg.sps) +
+                       ((r.relu & b2plan::kConvPreAct) ? b2k::conv_pre_smem_bytes(int(r.cin_phys) / 64) : 0) <= kSmemLimit;
     // grouped: one tile per CTA and N tiles inside one span of input channels; GELU: only the one-tile kernel has it
     if (op.groups > 1 && (!span || span % cfg.bn || cfg.splits > 1)) return false;
     if ((op.groups > 1 || (r.relu & b2plan::kConvGelu)) && (cfg.ws || cfg.cn > 1 || cfg.halo)) return false;
@@ -1239,7 +1312,8 @@ ConvConfig forced_conv_config(const b2_context* c, const Op& op, int batch) {
     const int kbsz = conv_kb(c, op), nkb = conv_num_kblocks(c, op);
     ConvConfig cfg = pick_conv_config(M, int(r.cout_phys), nkb, kbsz, r.res >= 0, c, true, op.group_span());
     // (a packed layer has no split-K: a forced split count is dropped there)
-    if (cfg.bn == 0 || ((op.flags & b2plan::kOpPacked) && cfg.splits > 1))
+    if (cfg.bn == 0 || ((op.flags & b2plan::kOpPacked) && cfg.splits > 1) ||
+        (((r.relu & b2plan::kConvPreAct) || op.prefix) && !tactic_applies(c, op, batch, cfg)))
         cfg = pick_conv_config(M, int(r.cout_phys), nkb, kbsz, r.res >= 0, c, false, op.group_span());
     if (cfg.bn == 0) return cfg;
     auto force = [&](auto set) {
@@ -1323,7 +1397,9 @@ int make_conv_launch(b2_context* c, const Op& op, int batch, const ConvConfig& c
     a.wpacked = (r.relu & 2) ? w : nullptr;
     // (GELU layers are always read as a plain matrix: their kernel exists for that operand path only)
     const bool tiled = r.k == 1 && op.kw() == 1 && r.stride == 1 && op.sw() == 1 && r.pad_ == 0 && op.pw_lo() == 0 &&
-                       op.pw_hi() == 0 && kb64 && (!c->force_im2col || gelu || (op.flags & b2plan::kOpPacked));
+                       op.pw_hi() == 0 && kb64 &&
+                       (!c->force_im2col || gelu || (op.flags & b2plan::kOpPacked) || (r.relu & b2plan::kConvPreAct) || op.prefix);
+    a.pre = (r.relu & b2plan::kConvPreAct) ? 1 : 0;
     a.a_mode = tiled ? b2k::A_TILED : b2k::A_IM2COL;
     if (cfg.halo) {
         const int R = conv_halo_rows(c, op);
@@ -1353,7 +1429,9 @@ int make_conv_launch(b2_context* c, const Op& op, int batch, const ConvConfig& c
     const CUtensorMapSwizzle swz = kb64 ? CU_TENSOR_MAP_SWIZZLE_128B : (fold ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_NONE);
     const uint64_t pix = uint64_t(r.cin_phys) * 2, rowb = uint64_t(ti.w) * pix, imgb = uint64_t(ti.h) * rowb;
     int rc;
-    if (tiled)
+    if (tiled && op.prefix)  // channels [0, cin) of rows c_phys apart; the TMA reads [cin, cin_phys) as zeros
+        rc = make_map_2d(&cl.mapA, tptr(r.in), r.cin, uint64_t(M), 64, 128, swz, false, ti.c_phys);
+    else if (tiled)
         rc = make_map_2d(&cl.mapA, tptr(r.in), r.cin_phys, uint64_t(M), 64, uint32_t(128 / cl.cn), swz);
     else if (fold)  // kw pixels x 8 channels = 32 contiguous K-elements per window; windows advance by ONE pixel
         rc = make_map_im2col(&cl.mapA, tptr(r.in), int(r.cin_phys) * op.kw(), int(ti.w) - op.kw() + 1, int(ti.h), batch, pix,
@@ -1943,12 +2021,22 @@ int build_plan(b2_context* c, int batch, Plan** out) {
                 L.kind = L_MAXPOOL;
                 L.in = tptr(r.in), L.out = tptr(r.out);
                 L.H = ti.h, L.W = ti.w, L.C_phys = ti.c_phys, L.Ho = to.h, L.Wo = to.w;
+                if (op.cw) L.c0 = op.c0, L.cw = op.cw, L.out_pitch = int(to.c_phys);
                 L.k = r.k, L.stride = r.stride, L.pad = r.pad_;
                 L.bytes = double(batch) * (ti.item_bytes + to.item_bytes);
                 break;
             }
             case b2plan::OP_AVGPOOL: {
                 const Tensor& ti = e->tensors[r.in];
+                if (r.relu & b2plan::kConvPreAct) {  // windowed or global, with the BatchNorm + ReLU prologue
+                    const Tensor& to = e->tensors[r.out];
+                    L.kind = L_AVGPOOL_PRE;
+                    L.in = tptr(r.in), L.out = tptr(r.out);
+                    L.bias = reinterpret_cast<const float*>(e->d_payload + r.b_off);
+                    L.H = ti.h, L.W = ti.w, L.C = ti.c, L.C_phys = ti.c_phys, L.k = int(r.k);
+                    L.bytes = double(batch) * (ti.item_bytes + to.item_bytes);
+                    break;
+                }
                 L.kind = ti.scale > 0.f ? (e->fp8() ? L_AVGPOOL_F8 : L_AVGPOOL_I8) : L_AVGPOOL;
                 L.in = tptr(r.in), L.out = tptr(r.out);
                 L.H = ti.h, L.W = ti.w, L.C_phys = ti.c_phys;
@@ -2134,9 +2222,12 @@ int run_launch(const b2_engine* e, const Launch& L, void* const* bindings, cudaS
         case L_CONV_SIMT:
             return b2k::launch_conv_simt(L.simt, half, s);
         case L_MAXPOOL:
+            if (L.cw) return b2k::launch_maxpool_pitched(in, out, L.N, L.H, L.W, L.C_phys, L.Ho, L.Wo, L.k, L.stride, L.pad, L.out_pitch, L.c0, s);
             return b2k::launch_maxpool(in, out, L.N, L.H, L.W, L.C_phys, L.Ho, L.Wo, L.k, L.stride, L.pad, half, s);
         case L_LRN:
             return b2k::launch_lrn_f16(in, out, static_cast<long long>(L.N) * L.H * L.W, L.C, L.C_phys, L.k, L.alpha, L.beta, L.kk, s);
+        case L_AVGPOOL_PRE:
+            return b2k::launch_avgpool_bnrelu(in, out, L.bias, L.N, L.H, L.W, L.C, L.C_phys, L.k, s);
         case L_AVGPOOL:
             return b2k::launch_avgpool(in, out, L.N, L.H * L.W, L.C_phys, half, s);
         case L_FC:
@@ -2991,8 +3082,8 @@ const char* b2_context_launch_name(b2_context* c, int batch, int i) {
     static const char* kinds[] = {"input_cast", "conv_tcgen05", "conv_simt", "maxpool", "avgpool", "fc", "softmax", "output_cast", "tail_pool_fc_softmax",
                                   "quantize", "conv_i8_tcgen05", "avgpool_i8", "output_cast_i8", "embed_ln", "layernorm", "attention_f16_wgmma",
                                   "pooler", "output_cast_rows", "output_unpack_rows", "quantize_f8", "conv_f8_tcgen05", "avgpool_f8",
-                                  "output_cast_f8", "patchify", "tokens", "cls_head", "lrn"};
-    static_assert(sizeof(kinds) / sizeof(kinds[0]) == L_LRN + 1, "kinds[] is indexed by LKind");
+                                  "output_cast_f8", "patchify", "tokens", "cls_head", "lrn", "avgpool_bnrelu"};
+    static_assert(sizeof(kinds) / sizeof(kinds[0]) == L_AVGPOOL_PRE + 1, "kinds[] is indexed by LKind");
     s = std::string(kinds[L->kind]) + (L->kind == L_ATTENTION && L->attn.S > 128 ? "_ks" : "") +  // key-split kernel
         (L->kind == L_ATTENTION && L->attn.seq_off ? "_varlen" : "") + ":" + L->name;         // variable-length kernel
     if (L->kind == L_ATTENTION && L->attn.S != L->W) s += " sk=" + std::to_string(L->attn.S);  // kernel of a longer sequence
@@ -3007,6 +3098,7 @@ const char* b2_context_launch_name(b2_context* c, int batch, int i) {
              std::to_string(L->conv.args.splits) + " kblk=" + std::to_string(L->conv.args.num_kblocks) +
              (L->conv.args.group_span ? " span=" + std::to_string(L->conv.args.group_span) : std::string()) +
              ((L->conv.args.relu & b2plan::kConvGelu) ? " gelu" : "") + (L->conv.args.live ? " live" : "") +
+             (L->conv.args.pre ? " pre" : "") +
              (L->cw ? " c0=" + std::to_string(L->c0) + " cw=" + std::to_string(L->cw) : std::string());
     if (L->kind == L_CONV_I8 || L->kind == L_CONV_F8)
         s += " bn=" + std::to_string(L->i8.bn) + " st=" + std::to_string(L->i8.stages) + (L->i8.args.a_mode == b2k::A_TILED ? " tiled" : " im2col") + " grid=" +

@@ -77,13 +77,20 @@ struct FragPos {
 // the count does no work.  Each role reads the count after its own pdl_wait(): the weight producer streams the first ring
 // pass before it (constants) and issues nothing more for a dead tile; the activation producer then expects only those
 // weight bytes on the ring's barriers and waits for them to land, so the CTA never retires with bulk copies in flight.
-template <int BN, int KB, int STAGES, int SPS, int CN = 1, bool DBG = false, int AV = 0, bool GELU = false, bool LIVE = false>
+// PRE (AV == 2, no split-K): a BatchNorm + ReLU input prologue (plan_format.h, kConvPreAct).  The fp32 scale and shift
+// (cin_phys each, behind the bias in global memory) are staged in shared memory once per CTA.  When a stage lands, each
+// consumer warpgroup rewrites its own 64 rows of every A sub-block in place, a = fp16_rn(max(fmaf(x, scale, shift), 0)),
+// then fences the generic-proxy stores against the async proxy and syncs on its own named barrier before its wgmmas.  The
+// transform of step i overlaps the wgmmas of step i - 1 that are still in flight (they read another stage).
+template <int BN, int KB, int STAGES, int SPS, int CN = 1, bool DBG = false, int AV = 0, bool GELU = false, bool LIVE = false,
+          bool PRE = false>
 __global__ void __launch_bounds__(kConvThreads, conv_min_ctas(BN))
 conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
                  const __grid_constant__ CUtensorMap mapOut, const __grid_constant__ CUtensorMap mapRes,
                  const ConvArgs p) {
     static_assert(SPS == 1 || KB == 64, "multi-sub-block stages exist for the 64-wide K path only");
     static_assert(!LIVE || AV == 2, "live-row instantiations exist for the tiled packed-weight path only");
+    static_assert(!PRE || (AV == 2 && !LIVE && !GELU), "prologue instantiations exist for the tiled packed-weight path only");
     using Cfg = ConvCfg<BN, STAGES, SPS>;
     constexpr int TPS = 64 / KB;            // TMA sub-tiles per stage: 1 (KB=64), 2 (KB=32 row-folded stem), 8 (KB=8)
     constexpr int A_SUB = 128 * KB * 2;     // bytes of one A sub-tile
@@ -160,6 +167,11 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
         mbar_init(res_bar, 1);
         fence_barrier_init();
         fence_proxy_async();
+    }
+    if constexpr (PRE) {  // [scale cin_phys][shift cin_phys] behind s_bias; constants, so legal before pdl_wait()
+        const int n4 = p.cblocks * 32;  // float4s in 2 * cin_phys floats
+        const float4* src = reinterpret_cast<const float4*>(p.bias + p.Cout);
+        for (int i = threadIdx.x; i < n4; i += kConvThreads) reinterpret_cast<float4*>(s_bias + BN)[i] = __ldg(src + i);
     }
     __syncthreads();
     if (cn > 1) cluster_sync_all();  // peers' barriers exist before anything is multicast at them
@@ -359,6 +371,40 @@ conv_f16_tcgen05(const __grid_constant__ CUtensorMap mapA, const __grid_constant
             mbar_wait(&full_bar[s], ph);
             if (dbg) m1c = clock64(), mw += m1c - m0c;
             if (dbg && i == 0 && cw == 0 && lane == 0) dbg[3] = clock64();
+            if constexpr (PRE) {
+                // thread t of the warpgroup owns 16-byte chunk t % 8 of rows t / 8 + 16 j (j < 4): those rows share
+                // row % 8, so under the 128-byte swizzle (chunk XOR row % 8) all four hold the same 8 channels
+                const int t = threadIdx.x & 127;
+                const int ch8 = ((t & 7) ^ ((t >> 3) & 7)) * 8;
+                const float* s_scale = s_bias + BN;
+                const float* s_shift = s_scale + p.cblocks * 64;
+#pragma unroll
+                for (int u = 0; u < SPS; ++u) {
+                    if (u >= subs_in_step(i)) break;
+                    const int c = (kb_begin + i * SPS + u) * 64 + ch8;
+                    float sc[8], sh[8];
+                    *reinterpret_cast<float4*>(sc) = *reinterpret_cast<const float4*>(s_scale + c);
+                    *reinterpret_cast<float4*>(sc + 4) = *reinterpret_cast<const float4*>(s_scale + c + 4);
+                    *reinterpret_cast<float4*>(sh) = *reinterpret_cast<const float4*>(s_shift + c);
+                    *reinterpret_cast<float4*>(sh + 4) = *reinterpret_cast<const float4*>(s_shift + c + 4);
+                    uint8_t* rows = sA + s * Cfg::A_STAGE + u * Cfg::A_SUBBLK + wg * 8192 + (t >> 3) * 128 + (t & 7) * 16;
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) {
+                        uint4* q = reinterpret_cast<uint4*>(rows + j * 16 * 128);
+                        uint4 v = *q;
+                        __half2* h2 = reinterpret_cast<__half2*>(&v);
+#pragma unroll
+                        for (int e = 0; e < 4; ++e) {
+                            const float2 f = __half22float2(h2[e]);
+                            h2[e] = __floats2half2_rn(fmaxf(fmaf(f.x, sc[2 * e], sh[2 * e]), 0.0f),
+                                                      fmaxf(fmaf(f.y, sc[2 * e + 1], sh[2 * e + 1]), 0.0f));
+                        }
+                        *q = v;
+                    }
+                }
+                fence_proxy_async();                 // generic stores -> the wgmma (async proxy) reads below
+                named_bar_sync(1 + wg, 128);         // the warpgroup's 64 rows are all transformed
+            }
             const uint32_t a_addr = smem_u32(sA + s * Cfg::A_STAGE);
             const uint32_t b_addr = smem_u32(sB + s * Cfg::B_STAGE);
             // one wgmma per K = 16; the number of them in a step is resolved outside the group (wgmma_group)
@@ -1392,6 +1438,16 @@ static int launch_one(const ConvLaunch& L, cudaStream_t stream) {
     dim3 grid(L.grid_n, L.grid_m, L.args.splits);
     const size_t smem = size_t(conv_smem_layout_bytes(BN, STAGES, L.args.residual != nullptr, SPS));
     if (CN > 1 && (KB != 64 || L.grid_n % CN != 0 || L.args.cn != CN)) return static_cast<int>(cudaErrorInvalidValue);
+    if (L.args.pre) {  // BatchNorm + ReLU prologue: the tiled packed-weight instantiation, no split-K; scale + shift behind the bias
+        if constexpr (CN == 1 && KB == 64) {
+            if (L.args.wpacked != nullptr && L.args.a_mode == A_TILED && L.args.splits == 1 && !L.args.live && !(L.args.relu & 8) &&
+                L.args.dbg == nullptr && L.args.dbg_mode == 0)
+                return launch_kernel_cluster(conv_f16_tcgen05<BN, KB, STAGES, SPS, 1, false, 2, false, false, true>, grid, dim3(kConvThreads),
+                                             smem + size_t(conv_pre_smem_bytes(L.args.cblocks)), stream, true, 1u, L.mapA, L.mapB, L.mapOut,
+                                             L.mapRes, L.args);
+        }
+        return static_cast<int>(cudaErrorInvalidValue);
+    }
     if (L.args.live) {  // packed rows: the live-row instantiations of the tiled packed-weight kernel, no split-K
         if constexpr (CN == 1 && KB == 64) {
             if (L.args.wpacked != nullptr && L.args.a_mode == A_TILED && L.args.splits == 1 && L.args.dbg == nullptr && L.args.dbg_mode == 0) {
@@ -1451,6 +1507,8 @@ static int init_one() {
             if ((e = set_conv_smem(conv_f16_tcgen05<BN, KB, STAGES, SPS, 1, false, 2, true>, bytes))) return e;
             if ((e = set_conv_smem(conv_f16_tcgen05<BN, KB, STAGES, SPS, 1, false, 2, false, true>, bytes))) return e;
             if ((e = set_conv_smem(conv_f16_tcgen05<BN, KB, STAGES, SPS, 1, false, 2, true, true>, bytes))) return e;
+            // (the prologue's scale and shift grow with cin: the engine admits a tactic only where the total fits)
+            if ((e = set_conv_smem(conv_f16_tcgen05<BN, KB, STAGES, SPS, 1, false, 2, false, false, true>, 227 * 1024))) return e;
         }
     }
     return set_conv_smem(conv_f16_tcgen05<BN, KB, STAGES, SPS, CN>, bytes);
@@ -1959,6 +2017,52 @@ __global__ void maxpool_h8_kernel(const uint4* __restrict__ src, uint4* __restri
     dst[idx] = o;
 }
 
+// maxpool_h8_kernel into channels [c0, c0 + C_phys) of a wider fp16 tensor with out_pitch channels per pixel (a channel
+// slice of a concatenation); its own kernel, so the unpitched one keeps its code
+__global__ void maxpool_h8_pitched_kernel(const uint4* __restrict__ src, uint4* __restrict__ dst, int N, int H, int W, int C8, int Ho,
+                                          int Wo, int k, int stride, int pad, int out_pitch8, int out_c08) {
+    pdl_launch_dependents();
+    pdl_wait();
+    const long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
+    if (idx >= static_cast<long long>(N) * Ho * Wo * C8) return;
+    const int c = static_cast<int>(idx % C8);
+    const long long pix = idx / C8;
+    const int wo = static_cast<int>(pix % Wo);
+    const long long t = pix / Wo;
+    const int ho = static_cast<int>(t % Ho);
+    const int n = static_cast<int>(t / Ho);
+    const __half2 ninf = __float2half2_rn(-INFINITY);
+    __half2 m[4] = {ninf, ninf, ninf, ninf};
+    for (int r = 0; r < k; ++r) {
+        const int hi = ho * stride - pad + r;
+        if (hi < 0 || hi >= H) continue;
+        for (int s = 0; s < k; ++s) {
+            const int wi = wo * stride - pad + s;
+            if (wi < 0 || wi >= W) continue;
+            const uint4 v = __ldg(src + ((static_cast<size_t>(n) * H + hi) * W + wi) * C8 + c);
+            const __half2* v2 = reinterpret_cast<const __half2*>(&v);
+#pragma unroll
+            for (int i = 0; i < 4; ++i) m[i] = __hmax2(m[i], v2[i]);
+        }
+    }
+    uint4 o;
+    __half2* o2 = reinterpret_cast<__half2*>(&o);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) o2[i] = m[i];
+    dst[static_cast<size_t>(pix) * out_pitch8 + out_c08 + c] = o;
+}
+
+int launch_maxpool_pitched(const void* src, void* dst, int N, int H, int W, int C_phys, int Ho, int Wo, int k, int stride, int pad,
+                           int out_pitch, int out_c0, cudaStream_t stream) {
+    if (C_phys % 8 || out_pitch % 8 || out_c0 % 8) return static_cast<int>(cudaErrorInvalidValue);
+    const int threads = 256;
+    const long long total = static_cast<long long>(N) * Ho * Wo * (C_phys / 8);
+    B2_LAUNCH_RC = launch_kernel(maxpool_h8_pitched_kernel, dim3(static_cast<unsigned>((total + threads - 1) / threads)), dim3(threads), 0, stream,
+                                 true, reinterpret_cast<const uint4*>(src), reinterpret_cast<uint4*>(dst), N, H, W, C_phys / 8, Ho, Wo, k, stride,
+                                 pad, out_pitch / 8, out_c0 / 8);
+    return B2_LAUNCH_RC;
+}
+
 int launch_maxpool(const void* src, void* dst, int N, int H, int W, int C_phys, int Ho, int Wo, int k, int stride,
                    int pad, bool half_storage, cudaStream_t stream) {
     const int threads = 256;
@@ -2037,6 +2141,61 @@ __global__ void __launch_bounds__(256) avgpool_h8_kernel(const uint4* __restrict
         for (int i = 0; i < 4; ++i) o2[i] = __floats2half2_rn(tot[2 * i], tot[2 * i + 1]);
         dst[static_cast<size_t>(n) * C8 + cg] = o;
     }
+}
+
+// fp16 k x k / stride k average pool (k = H = W: the global pool) with a BatchNorm + ReLU input prologue, 8 channels
+// (16 bytes) per thread: y = fp16_rn(fp32(1 / k^2) * sum over the window in row-major order of max(fmaf(x, scale, shift), 0)),
+// the sum in fp32.  Channels >= C are written as zeros.
+__global__ void __launch_bounds__(256) avgpool_bnrelu_h8_kernel(const uint4* __restrict__ src, uint4* __restrict__ dst,
+                                                               const float* __restrict__ scale, const float* __restrict__ shift, int N,
+                                                               int H, int W, int C8, int C, int Ho, int Wo, int k, float inv) {
+    pdl_launch_dependents();
+    pdl_wait();
+    const long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
+    if (idx >= static_cast<long long>(N) * Ho * Wo * C8) return;
+    const int c = static_cast<int>(idx % C8);
+    long long t = idx / C8;
+    const int wo = static_cast<int>(t % Wo);
+    t /= Wo;
+    const int ho = static_cast<int>(t % Ho);
+    const int n = static_cast<int>(t / Ho);
+    uint4 o = make_uint4(0u, 0u, 0u, 0u);
+    if (c * 8 < C) {
+        float sc[8], sh[8], acc[8];
+        *reinterpret_cast<float4*>(sc) = __ldg(reinterpret_cast<const float4*>(scale) + 2 * c);
+        *reinterpret_cast<float4*>(sc + 4) = __ldg(reinterpret_cast<const float4*>(scale) + 2 * c + 1);
+        *reinterpret_cast<float4*>(sh) = __ldg(reinterpret_cast<const float4*>(shift) + 2 * c);
+        *reinterpret_cast<float4*>(sh + 4) = __ldg(reinterpret_cast<const float4*>(shift) + 2 * c + 1);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) acc[i] = 0.f;
+        const uint4* base = src + ((static_cast<size_t>(n) * H + static_cast<size_t>(ho) * k) * W + static_cast<size_t>(wo) * k) * C8 + c;
+        for (int r = 0; r < k; ++r)
+            for (int s = 0; s < k; ++s) {
+                const uint4 v = __ldg(base + (static_cast<size_t>(r) * W + s) * C8);
+                const __half2* h2 = reinterpret_cast<const __half2*>(&v);
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const float2 f = __half22float2(h2[i]);
+                    acc[2 * i] += fmaxf(fmaf(f.x, sc[2 * i], sh[2 * i]), 0.f);
+                    acc[2 * i + 1] += fmaxf(fmaf(f.y, sc[2 * i + 1], sh[2 * i + 1]), 0.f);
+                }
+            }
+        __half2* o2 = reinterpret_cast<__half2*>(&o);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) o2[i] = __floats2half2_rn(acc[2 * i] * inv, acc[2 * i + 1] * inv);
+    }
+    dst[idx] = o;
+}
+
+int launch_avgpool_bnrelu(const void* src, void* dst, const float* scale_shift, int N, int H, int W, int C, int C_phys, int k,
+                          cudaStream_t stream) {
+    if (C_phys % 8 || C % 8 || k < 1 || H % k || W % k) return static_cast<int>(cudaErrorInvalidValue);
+    const int Ho = H / k, Wo = W / k, threads = 256;
+    const long long total = static_cast<long long>(N) * Ho * Wo * (C_phys / 8);
+    B2_LAUNCH_RC = launch_kernel(avgpool_bnrelu_h8_kernel, dim3(static_cast<unsigned>((total + threads - 1) / threads)), dim3(threads), 0, stream,
+                                 true, reinterpret_cast<const uint4*>(src), reinterpret_cast<uint4*>(dst), scale_shift, scale_shift + C_phys, N,
+                                 H, W, C_phys / 8, C, Ho, Wo, k, 1.0f / static_cast<float>(k * k));
+    return B2_LAUNCH_RC;
 }
 
 int launch_avgpool(const void* src, void* dst, int N, int HW, int C_phys, bool half_storage, cudaStream_t stream) {

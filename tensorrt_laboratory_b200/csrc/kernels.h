@@ -4,6 +4,7 @@
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
+#include <stddef.h>
 #include <stdint.h>
 
 namespace b2k {
@@ -47,13 +48,16 @@ struct ConvArgs {
     int cn;                  // CTAs per cluster along N sharing one activation tile by TMA multicast (1 = no cluster)
     int tiles_m, tiles_n;    // persistent variant: output tile grid (128-row x BN-column tiles)
     int dbg_mode;            // bottleneck isolation (debug only): bit1 skip A loads, bit2 skip B loads
-    long long* dbg;          // optional per-CTA phase timestamps (16 x int64 per CTA), nullptr in production
+    int pre;                 // 1: BatchNorm + ReLU input prologue (tiled, packed weights, one tile per CTA, no split-K); the
+                             // fp32 [scale cin_phys][shift cin_phys] follow the bias (Cout floats).  (This field fills the
+                             // alignment gap before `dbg`: every other field keeps its offset.)
+    long long* dbg;         // optional per-CTA phase timestamps (16 x int64 per CTA), nullptr in production
     int group_span;          // grouped convolution (KB==64, one tile per CTA): input channels an N tile reads, max(Cin/g, 64),
                              // starting at channel (n0 / group_span) * group_span; cblocks = group_span / 64.  0 = dense
     int live;                // 1: the M rows are packed transformer rows and live_rows counts those in use (this field sits
                              // in the struct's tail padding: the parameter layout of every kernel taking ConvArgs is unchanged)
 };
-static_assert(sizeof(ConvArgs) == 168, "ConvArgs layout");
+static_assert(sizeof(ConvArgs) == 168 && offsetof(ConvArgs, dbg) == 152, "ConvArgs layout");
 
 // The 1x1 / stride-1 convolution a fused bottleneck launch (ConvLaunch::halo == 2) runs on the 3x3's output, with residual
 struct Conv1x1Args {
@@ -89,6 +93,8 @@ int launch_conv_f16_tcgen05(const ConvLaunch& L, cudaStream_t stream);
 int init_conv_kernels();
 bool conv_config_exists(int bn, int kb, int stages, int sps = 1);  // is this configuration instantiated?
 int conv_smem_bytes(int bn, int stages, bool residual, int sps = 1);  // dynamic shared memory of one CTA
+// ... plus this much for a BatchNorm + ReLU prologue (ConvArgs::pre) over cblocks 64-channel blocks: its scale and shift
+inline int conv_pre_smem_bytes(int cblocks) { return cblocks * 64 * 2 * 4; }
 bool conv_cluster_config_exists(int bn, int stages, int sps, int cn);  // cluster-multicast instantiations
 bool conv_halo_config_exists(int bn);                                // 3x3 halo variant
 int conv_halo_smem(int bn, int w, int r, int cblocks);
@@ -190,6 +196,13 @@ int launch_maxpool(const void* src, void* dst, int N, int H, int W, int C_phys, 
 constexpr int kLrnMaxSize = 15;
 int launch_lrn_f16(const void* src, void* dst, long long pixels, int C, int C_phys, int n, float alpha, float beta, float k,
                    cudaStream_t stream);
+// fp16 max pool into channels [out_c0, out_c0 + C_phys) of a tensor with out_pitch channels per pixel (multiples of 8)
+int launch_maxpool_pitched(const void* src, void* dst, int N, int H, int W, int C_phys, int Ho, int Wo, int k, int stride, int pad,
+                           int out_pitch, int out_c0, cudaStream_t stream);
+// fp16 k x k / stride k average pool (H % k == W % k == 0; k = H = W is the global pool) with a BatchNorm + ReLU input
+// prologue; scale_shift = fp32 [scale C_phys][shift C_phys]; numerics in plan_format.h (OP_AVGPOOL, kConvPreAct)
+int launch_avgpool_bnrelu(const void* src, void* dst, const float* scale_shift, int N, int H, int W, int C, int C_phys, int k,
+                          cudaStream_t stream);
 // global average pool: NHWC [N,HW,C] -> [N,1,1,C]
 int launch_avgpool(const void* src, void* dst, int N, int HW, int C_phys, bool half_storage,
                    cudaStream_t stream);

@@ -23,7 +23,7 @@ enum OpType : uint32_t {
     OP_INPUT_CAST = 0,   // fp32 NCHW binding -> NHWC activation tensor
     OP_CONV = 1,         // conv + folded BN/Scale bias (+ residual) (+ ReLU)
     OP_MAXPOOL = 2,
-    OP_AVGPOOL = 3,      // global average pool
+    OP_AVGPOOL = 3,      // global average pool (version 4: also k x k / stride k, with a BatchNorm + ReLU prologue)
     OP_FC = 4,           // inner product -> fp32 vector
     OP_SOFTMAX = 5,      // fp32 vector -> fp32 vector
     OP_OUTPUT_CAST = 6,  // NHWC activation tensor -> fp32 NCHW binding (dequantised when the tensor is int8 / e4m3)
@@ -105,7 +105,7 @@ struct OpRec {  // 176 bytes
 // 1-byte (INT8 / FP8) grouped convolutions do not exist.
 //
 // Version-4 plans (kVersionConcat) use OpRecV2 and give its reserved bytes a meaning:
-//   out_c0, out_cw (OP_CONV only; 0 / 0 = the convolution writes all of its output tensor): the convolution writes output
+//   out_c0, out_cw (OP_CONV, and OP_MAXPOOL as below; 0 / 0 = the convolution writes all of its output tensor): the convolution writes output
 //     channels [out_c0, out_c0 + out_cw) of `out`, a tensor the outputs of several convolutions share (a channel
 //     concatenation with no copy).  Its own channel o lands at channel out_c0 + o; channels o >= out_cw are not written.
 //     Rules: fp16 plans only; no residual, no groups, packed weights; out_c0 % 8 == 0 (the TMA store's 16-byte aligned base);
@@ -118,6 +118,23 @@ struct OpRec {  // 176 bytes
 //     field) = n, odd, 1 ... 15; b = fp32 [alpha, beta, k] (b_bytes = 12); no weights.  Numerics: the squares summed in
 //     fp32 in channel order, scale = fmaf(fp32(alpha / n), sum, k) in fp32, powf(scale, -beta) in fp32, x times that in
 //     fp32 and one rounding to fp16.  Channels >= c are written as zero.
+//   OP_MAXPOOL may write a channel slice too (fp16 plans): out_c0 / out_cw with out_c0 % 8 == 0 and out_cw == the input's
+//     c_phys; it writes its input's c_phys channels at out_c0 and takes part in the tiling rules above as a writer whose
+//     real channel count ("cout") is its input's c.
+//   Input prefix (OP_CONV): cin < c of the input tensor means the convolution reads channels [0, cin) of it, with
+//     cin_phys = roundup(cin, 64); the engine's A operand then has channel extent cin and pitch c_phys, and the channels
+//     [cin, cin_phys) read as zeros.  Legal only for a dense 1x1 stride-1 unpadded convolution with packed weights, whose
+//     input is slice-written, where cin ends exactly at a slice boundary (the end of some writer's real channels), and
+//     which comes after every writer of the slices it reads.
+//   kConvPreAct (`relu` bit 4, OP_CONV and OP_AVGPOOL, fp16 plans): a BatchNorm + ReLU input prologue.
+//     OP_CONV (dense 1x1 stride-1 unpadded, packed weights, no residual): b = fp32 [bias cout_phys][scale cin_phys][shift
+//     cin_phys], zeros past cout / cin; b_bytes = (cout_phys + 2 cin_phys) * 4.  Numerics: the wgmma operand is
+//     a = fp16_rn(max(fmaf(float(x), scale_c, shift_c), 0)); everything else as for a plain convolution.  Any other
+//     unknown `relu` bit of a version-4 convolution is refused.
+//   OP_AVGPOOL: a k x k / stride k window (pad 0, H and W multiples of k; k = H = W is the global pool) over an fp16 tensor
+//     into one of the same c and c_phys.  Without kConvPreAct only the global pool exists (b_bytes = 0).  With it, b = fp32
+//     [scale c_phys][shift c_phys], zeros past c; y = fp16_rn(fp32(1 / k^2) * sum of max(fmaf(x, scale, shift), 0)) with the
+//     sum in fp32 in row-major window order; channels >= c are written as 0.
 struct OpRecV2 {  // 192 bytes
     OpRec v1;
     uint32_t groups;
@@ -176,7 +193,7 @@ struct OpRecV3 {  // 224 bytes
     uint32_t flags;
     uint8_t reserved[8];
 };
-enum : uint32_t { kConvRelu = 1, kConvPacked = 2, kConvInt8 = 4, kConvGelu = 8 };
+enum : uint32_t { kConvRelu = 1, kConvPacked = 2, kConvInt8 = 4, kConvGelu = 8, kConvPreAct = 16 };
 enum : uint32_t { kOpRowsOut = 1, kOpPacked = 2 };  // OpRecV3::flags
 struct BindingRec {  // 128 bytes
     char name[64];

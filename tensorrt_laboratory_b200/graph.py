@@ -143,6 +143,11 @@ def parse_prototxt(text: str) -> dict:
                 stride=_one(p, "stride", 1),
                 pad=_one(p, "pad", 0),
             )
+            round_mode = _one(p, "round_mode", "CEIL")  # absent = Caffe's CEIL
+            if round_mode not in ("CEIL", "FLOOR"):
+                raise ValueError(f"prototxt: Pooling {rec['name']}: round_mode {round_mode}; CEIL or FLOOR")
+            if round_mode == "FLOOR":
+                rec["ceil_mode"] = False
         elif ltype == "InnerProduct":
             p = _one(L, "inner_product_param", {})
             rec.update(num_output=_one(p, "num_output"), bias_term=_one(p, "bias_term", True))
@@ -324,6 +329,58 @@ def googlenet_caffe() -> dict:
     return {"name": "GoogleNet", "input": "data", "input_dims": [1, 3, 224, 224], "layers": L}
 
 
+# DenseNet (Huang et al., "Densely Connected Convolutional Networks"): dense layers per block, growth 32, a 4 x 32
+# bottleneck, compression 1/2 -- torchvision's geometry
+_DENSENET_BLOCKS = {121: (6, 12, 24, 16), 169: (6, 12, 32, 32), 201: (6, 12, 48, 32)}
+
+
+def densenet_caffe(depth: int = 121) -> dict:
+    """The raw layer list of DenseNet-{121,169,201} in the usual Caffe form: blocks 2 ... 5, each dense layer
+    ``conv{b}_{l}/x1/bn|scale``, ``relu{b}_{l}/x1``, ``conv{b}_{l}/x1`` (1x1, 128), the same with ``x2`` (3x3, 32), then
+    ``concat_{b}_{l}`` of the previous concatenation (or ``pool1`` / ``pool{b-1}``) and ``conv{b}_{l}/x2``; transitions
+    ``conv{b}_blk/bn|scale``, ``relu{b}_blk``, ``conv{b}_blk`` (1x1, half the channels) and ``pool{b}`` (AVE 2x2/2); the
+    stem ``conv1`` (7x7/2, 64), ``conv1/bn|scale``, ``relu1``, ``pool1`` (MAX 3x3/2, pad 1, FLOOR); the head
+    ``conv5_blk/bn|scale``, ``relu5_blk``, ``pool5`` (global AVE), ``fc6`` and ``prob``.  Every BatchNorm writes a new blob
+    named after it; Scale and ReLU run in place on it.  No convolution has a bias."""
+    if depth not in _DENSENET_BLOCKS:
+        raise ValueError(f"unsupported DenseNet depth {depth}")
+    L: List[dict] = []
+
+    def conv(name, bottom, nout, k, pad=0, stride=1):
+        L.append(dict(name=name, type="Convolution", bottoms=[bottom], tops=[name], num_output=nout, kernel_size=k, pad=pad,
+                      stride=stride, bias_term=False))
+
+    def bn_scale_relu(prefix, relu, bottom):
+        bn = prefix + "/bn"
+        L.append(dict(name=bn, type="BatchNorm", bottoms=[bottom], tops=[bn], use_global_stats=True, eps=1e-5))
+        L.append(dict(name=prefix + "/scale", type="Scale", bottoms=[bn], tops=[bn], bias_term=True))
+        L.append(dict(name=relu, type="ReLU", bottoms=[bn], tops=[bn]))
+        return bn
+
+    conv("conv1", "data", 64, 7, 3, 2)
+    L.append(dict(name="pool1", type="Pooling", bottoms=[bn_scale_relu("conv1", "relu1", "conv1")], tops=["pool1"], pool="MAX",
+                  kernel_size=3, stride=2, pad=1, ceil_mode=False))
+    prev, c = "pool1", 64
+    for b, n in enumerate(_DENSENET_BLOCKS[depth], 2):
+        for l in range(1, n + 1):
+            x1, x2 = f"conv{b}_{l}/x1", f"conv{b}_{l}/x2"
+            conv(x1, bn_scale_relu(x1, f"relu{b}_{l}/x1", prev), 128, 1)
+            conv(x2, bn_scale_relu(x2, f"relu{b}_{l}/x2", x1), 32, 3, 1)
+            L.append(dict(name=f"concat_{b}_{l}", type="Concat", bottoms=[prev, x2], tops=[f"concat_{b}_{l}"], axis=1))
+            prev, c = f"concat_{b}_{l}", c + 32
+        if b < 5:
+            c //= 2
+            conv(f"conv{b}_blk", bn_scale_relu(f"conv{b}_blk", f"relu{b}_blk", prev), c, 1)
+            L.append(dict(name=f"pool{b}", type="Pooling", bottoms=[f"conv{b}_blk"], tops=[f"pool{b}"], pool="AVE", kernel_size=2,
+                          stride=2, pad=0))
+            prev = f"pool{b}"
+    L.append(dict(name="pool5", type="Pooling", bottoms=[bn_scale_relu("conv5_blk", "relu5_blk", prev)], tops=["pool5"], pool="AVE",
+                  kernel_size=7, stride=1, pad=0))
+    L.append(dict(name="fc6", type="InnerProduct", bottoms=["pool5"], tops=["fc6"], num_output=1000, bias_term=True))
+    L.append(dict(name="prob", type="Softmax", bottoms=["fc6"], tops=["prob"]))
+    return {"name": f"DenseNet-{depth}", "input": "data", "input_dims": [1, 3, 224, 224], "layers": L}
+
+
 # --------------------------------------------------------------------------------------------------
 # shape inference on raw layers
 # --------------------------------------------------------------------------------------------------
@@ -419,13 +476,51 @@ def lower(net: dict, weights: Optional[dict] = None) -> dict:
     def fold_state(op):
         return op.setdefault("_fold", {"scale": None, "shift": None})
 
+    def readers_of(blob, i):
+        """Layers other than layer i that read ``blob``, less the in-place BatchNorm / Scale / ReLU before layer i."""
+        return [(j, M) for j, M in enumerate(layers) if j != i and blob in M["bottoms"] and
+                not (j < i and M["type"] in ("BatchNorm", "Scale", "ReLU") and M["tops"] == [blob])]
+
+    # Pre-activations: a BatchNorm (+ Scale) + ReLU chain that cannot fold into the convolution before it becomes the input
+    # prologue of its one reader.  blob -> {name, input, relu, scale, shift} (scale / shift fp64 while folding)
+    preact: Dict[str, dict] = {}
+    grown: Dict[str, str] = {}  # nested concatenation: blob -> the Concat top that extends it (channel prefix)
+
+    def take_preact(blob, i, reader):
+        pa = preact.pop(blob)
+        if not pa["relu"]:
+            raise ValueError(f"BatchNorm {pa['name']}: a pre-activation without ReLU is not supported ({reader} reads it)")
+        n = len(readers_of(blob, i)) + 1
+        if n != 1:
+            raise ValueError(f"BatchNorm {pa['name']}: its output {blob} has {n} readers; a pre-activation has exactly one")
+        return pa
+
+    def attach_preact(op, pa):
+        op["pre"] = True
+        if "scale" in pa:
+            op["pre_scale"] = pa["scale"].astype(np.float32)
+            op["pre_shift"] = pa["shift"].astype(np.float32)
+
     consumed_by_eltwise = set()
     i = 0
     while i < len(layers):
         L = layers[i]
         t = L["type"]
         name = L["name"]
+        for b in L["bottoms"]:
+            if b in preact and not (t in ("Scale", "ReLU") and L["tops"] == [b]) and not (
+                    t == "Convolution" or (t == "Pooling" and L["pool"] == "AVE")):
+                raise ValueError(f"BatchNorm {preact[b]['name']}: a pre-activation is the input prologue of a 1x1 convolution or an "
+                                 f"average pool, not of {t} {name}")
+        pa_in = None
+        if t in ("Convolution", "Pooling") and L["bottoms"][0] in preact:
+            pa_in = take_preact(L["bottoms"][0], i, name)
+            L = dict(L, bottoms=[pa_in["input"]] + L["bottoms"][1:])
         if t == "Convolution":
+            if pa_in is not None and (L["kernel_size"] != 1 or L["stride"] != 1 or L["pad"] != 0 or L.get("group", 1) != 1):
+                raise ValueError(f"BatchNorm {pa_in['name']}: a pre-activation before {name}, a {L['kernel_size']}x{L['kernel_size']} "
+                                 "convolution, is not supported (only dense 1x1 stride-1 unpadded ones: with padding, "
+                                 "relu(shift) != 0 at a zero-padded pixel)")
             cin = tensors[L["bottoms"][0]][0]
             groups = L.get("group", 1)
             if groups < 1 or cin % groups or L["num_output"] % groups:
@@ -438,19 +533,48 @@ def lower(net: dict, weights: Optional[dict] = None) -> dict:
                 b = (np.asarray(weights[name]["b"], dtype=np.float64) if L["bias_term"]
                      else np.zeros(L["num_output"], dtype=np.float64))
                 op["_w"], op["_b"] = w, b
+            if pa_in is not None:
+                attach_preact(op, pa_in)
             ops.append(op)
             producer[L["tops"][0]] = op
             tensors[L["tops"][0]] = shapes[L["tops"][0]]
         elif t == "BatchNorm":
-            op = producer[L["bottoms"][0]]
-            if op["type"] != OP_CONV or op.get("_sealed"):
+            bottom, top = L["bottoms"][0], L["tops"][0]
+            op = producer.get(bottom)
+            if (op is None or op["type"] != OP_CONV or op.get("_sealed") or op["output"] != bottom) and top != bottom:
+                # a pre-activation (into a new blob): folded into the input prologue of the blob's one reader
+                pa = preact[top] = dict(name=name, input=bottom, relu=False)
+                if weights is not None:
+                    pa["scale"] = 1.0 / np.sqrt(np.asarray(weights[name]["var"], dtype=np.float64) + L.get("eps", 1e-5))
+                    pa["shift"] = -np.asarray(weights[name]["mean"], dtype=np.float64) * pa["scale"]
+                i += 1
+                continue
+            if op is None or op["type"] != OP_CONV or op.get("_sealed"):
                 raise ValueError(f"BatchNorm {name} does not follow a foldable Convolution")
+            if top != bottom:  # folded into the convolution, whose output takes the new blob's name
+                others = readers_of(bottom, i)
+                if others:
+                    raise ValueError(f"BatchNorm {name}: the convolution output {bottom} it normalises is also read by {others[0][1]['name']}")
+                op["output"] = top
+                del tensors[bottom]
+                del producer[bottom]
+                tensors[top] = shapes[top]
+                producer[top] = op
             if weights is not None:
                 mean = np.asarray(weights[name]["mean"], dtype=np.float64)
                 var = np.asarray(weights[name]["var"], dtype=np.float64)
                 inv = 1.0 / np.sqrt(var + L.get("eps", 1e-5))
                 op["_w"] = op["_w"] * inv[:, None, None, None]
                 op["_b"] = (op["_b"] - mean) * inv
+        elif t == "Scale" and L["bottoms"][0] in preact and L["tops"] == L["bottoms"]:
+            pa = preact[L["bottoms"][0]]
+            if pa["relu"]:
+                raise ValueError(f"Scale {name}: a pre-activation applies its Scale before its ReLU")
+            if weights is not None:
+                g = np.asarray(weights[name]["gamma"], dtype=np.float64)
+                pa["scale"], pa["shift"] = pa["scale"] * g, pa["shift"] * g
+                if L.get("bias_term"):
+                    pa["shift"] = pa["shift"] + np.asarray(weights[name]["beta"], dtype=np.float64)
         elif t == "Scale":
             op = producer[L["bottoms"][0]]
             if op["type"] != OP_CONV or op.get("_sealed"):
@@ -461,6 +585,8 @@ def lower(net: dict, weights: Optional[dict] = None) -> dict:
                 op["_b"] = op["_b"] * g
                 if L.get("bias_term"):
                     op["_b"] = op["_b"] + np.asarray(weights[name]["beta"], dtype=np.float64)
+        elif t == "ReLU" and L["bottoms"][0] in preact and L["tops"] == L["bottoms"]:
+            preact[L["bottoms"][0]]["relu"] = True
         elif t == "ReLU":
             op = producer[L["bottoms"][0]]
             if op["type"] != OP_CONV:
@@ -493,10 +619,37 @@ def lower(net: dict, weights: Optional[dict] = None) -> dict:
                           k=L["kernel_size"], stride=L["stride"], pad=L["pad"],
                           ceil_mode=L.get("ceil_mode", True))
             else:
-                if not (L["kernel_size"] == h == w and L["pad"] == 0):
-                    raise ValueError(f"Pooling {name}: only global AVE pooling is supported")
+                k = L["kernel_size"]
+                glob = k == h == w and L["pad"] == 0
+                if not glob and not (L["stride"] == k and L["pad"] == 0 and h % k == 0 and w % k == 0):
+                    raise ValueError(f"Pooling {name}: only global AVE pooling, or a k x k / stride k window without padding that "
+                                     "tiles the input, is supported")
+                conv = producer.get(L["bottoms"][0])
+                if (not glob and pa_in is None and conv is not None and conv["type"] == OP_CONV and conv.get("pre") and
+                        conv["output"] == L["bottoms"][0] and conv["residual"] is None and not conv["relu"] and
+                        not conv.get("_sealed") and not readers_of(L["bottoms"][0], i)):
+                    # pre-activation -> 1x1 convolution -> average pool: the two commute exactly, so the pool runs first with
+                    # the prologue and the convolution on the pooled tensor (4x less work; the convolution writes the output)
+                    mid = conv["name"] + "/pool"
+                    pool = dict(type=OP_AVGPOOL, name=name, input=conv["input"], output=mid, k=k, stride=k, pad=0, ceil_mode=True,
+                                pre=True)
+                    for key in ("pre_scale", "pre_shift"):
+                        if key in conv:
+                            pool[key] = conv.pop(key)
+                    del conv["pre"]
+                    ops.insert(ops.index(conv), pool)
+                    tensors[mid] = (conv["cin"], h // k, w // k)
+                    del tensors[conv["output"]]
+                    del producer[conv["output"]]
+                    conv.update(input=mid, output=L["tops"][0], commuted=True, _sealed=True)
+                    producer[L["tops"][0]] = conv
+                    tensors[L["tops"][0]] = shapes[L["tops"][0]]
+                    i += 1
+                    continue
                 op = dict(type=OP_AVGPOOL, name=name, input=L["bottoms"][0], output=L["tops"][0],
-                          k=L["kernel_size"], stride=L["stride"], pad=0, ceil_mode=True)
+                          k=k, stride=k if not glob else L["stride"], pad=0, ceil_mode=True)
+                if pa_in is not None:
+                    attach_preact(op, pa_in)
             ops.append(op)
             producer[L["tops"][0]] = op
             tensors[L["tops"][0]] = shapes[L["tops"][0]]
@@ -535,7 +688,29 @@ def lower(net: dict, weights: Optional[dict] = None) -> dict:
             if len(set(L["bottoms"])) != len(L["bottoms"]) or top in L["bottoms"]:
                 raise ValueError(f"Concat {name}: an input appears twice, or the output overwrites an input")
             c0 = 0
-            for b in L["bottoms"]:
+            b0 = L["bottoms"][0]
+            p0 = producer.get(b0)
+            r0 = readers_of(b0, i)
+            # a Concat that grows its first input: an earlier Concat's top, a max pool's output, or a convolution's output
+            # that pre-activations (before this Concat) read too.  The whole chain is one tensor, the last Concat's top; each
+            # earlier top is a channel prefix of it, and the first input's producer writes its first slice.
+            if p0 is not None and (p0["type"] in ("concat", OP_MAXPOOL) or (p0["type"] == OP_CONV and r0)):
+                for j, M in r0:
+                    if not (j < i and M["type"] == "BatchNorm" and M["tops"][0] != b0 and M["tops"][0] not in tensors):
+                        raise ValueError(f"Concat {name}: input {b0} is also read by {M['name']}; the first input of a growing "
+                                         "concatenation may be read only by pre-activation BatchNorms before the Concat")
+                if p0["type"] != "concat":
+                    if p0.get("residual") is not None or p0["output"] != b0 or b0 == net["input"]:
+                        raise ValueError(f"Concat {name}: input {b0} is not the output of a convolution without a residual or of a max pool")
+                    p0["out_c0"] = 0
+                    p0["_sealed"] = True
+                    if p0["type"] == OP_MAXPOOL:
+                        p0["cout"] = tensors[b0][0]
+                grown[b0] = top
+                c0 = tensors[b0][0]
+            elif p0 is not None and p0["type"] not in (OP_CONV, "concat") and b0 != net["input"]:
+                raise ValueError(f"Concat {name}: input {b0} is not the output of a convolution, a max pool or a concatenation")
+            for b in (L["bottoms"][1:] if b0 in grown else L["bottoms"]):
                 op = producer.get(b)
                 if op is None or op["type"] != OP_CONV or op["residual"] is not None or op["output"] != b:
                     raise ValueError(f"Concat {name}: input {b} is not the output of a convolution (only convolutions, "
@@ -560,6 +735,22 @@ def lower(net: dict, weights: Optional[dict] = None) -> dict:
             raise ValueError(f"unsupported layer type {t}")
         i += 1
 
+    if preact:
+        pa = next(iter(preact.values()))
+        raise ValueError(f"BatchNorm {pa['name']}: its pre-activation has no reader")
+
+    def phys(b):
+        while b in grown:
+            b = grown[b]
+        return b
+
+    for op in ops:  # nested concatenations: every blob of a chain is its last top (the readers' cin keeps the prefix)
+        if op.get("input") in grown:
+            op["input"] = phys(op["input"])
+        if op.get("output") in grown:
+            op["output"] = phys(op["output"])
+    for b in grown:
+        tensors.pop(b, None)
     for op in ops:
         if op["type"] == OP_CONV and "_w" in op:
             op["W"] = np.ascontiguousarray(op.pop("_w").transpose(0, 2, 3, 1)).astype(np.float32)  # OHWI

@@ -14,6 +14,8 @@ examples/ONNX/resnet50/build.py:35-67).
   python tools/build_engine.py --model bert-base --seq 384 --batch 16 --remove-padding -o bert_packed.plan  (masked tokens skipped)
   python tools/build_engine.py --model vit-b16 --batch 8 [--weights vit.npz] --tune -o vit.plan  (ViT-B/16, also vit-b32 / vit-l16; fp16)
   python tools/build_engine.py --model googlenet --batch 8 [--caffemodel bvlc_googlenet.caffemodel] --tune -o googlenet.plan  (fp16)
+  python tools/build_engine.py --model densenet121 --batch 8 [--caffemodel F | --weights tv.npz] --tune -o densenet.plan  (fp16;
+      also densenet169 / densenet201; --weights: a torchvision densenetNNN state_dict saved as .npz)
 Weights: deterministic synthetic weights (the reference's benchmark engines are weightless too, models/README.md:6-7),
 unless --caffemodel names a binary NetParameter (trtexec --model=...); MNIST and --onnx carry their own weights.
 --precision int8 / fp8: post-training quantization (fp8: E4M3), max-abs calibration on --calib (an .npy [N,C,H,W] fp32) or on
@@ -32,10 +34,11 @@ from tensorrt_laboratory_b200 import builder, graph, weights  # noqa: E402
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--model", choices=["resnet50", "resnet152", "resnext50", "mnist", "bert-base", "vit-b16", "vit-b32", "vit-l16", "googlenet"])
+    ap.add_argument("--model", choices=["resnet50", "resnet152", "resnext50", "mnist", "bert-base", "vit-b16", "vit-b32", "vit-l16", "googlenet",
+                                        "densenet121", "densenet169", "densenet201"])
     ap.add_argument("--seq", type=int, default=128, help="bert-base: the sequence length of the plan (64, 128, 256, 384 or 512)")
-    ap.add_argument("--weights", help="bert-base / vit-*: .npz of Hugging Face BertModel / ViTForImageClassification parameters "
-                                        "(default: seeded weights)")
+    ap.add_argument("--weights", help="bert-base / vit-*: .npz of Hugging Face BertModel / ViTForImageClassification parameters; "
+                                        "densenet*: .npz of a torchvision state_dict (default: seeded weights)")
     ap.add_argument("--remove-padding", action="store_true",
                     help="bert-base: a packed plan that computes only the tokens with input_mask != 0 (same bindings)")
     ap.add_argument("--prototxt")
@@ -82,6 +85,15 @@ def main():
     elif a.model == "googlenet":  # BVLC GoogLeNet (no auxiliary classifiers): Concat and LRN, fp16 only
         net = graph.googlenet_caffe()
         wts = weights_for(net)
+    elif a.model.startswith("densenet"):  # pre-activation 1x1s and growing concatenations, fp16 only
+        net = graph.densenet_caffe(int(a.model[8:]))
+        if prec != builder.PREC_FP16:
+            raise SystemExit("DenseNet builds in fp16 only")
+        if a.weights:
+            from tensorrt_laboratory_b200 import densenet
+            wts = densenet.load_weights(a.weights, int(a.model[8:]))
+        else:
+            wts = weights_for(net)
     elif a.model == "resnext50":  # 32x4d: grouped 3x3 convolutions, cpg 4 ... 32 (every precision)
         net = graph.resnext_caffe(50)
         wts = weights_for(net)
