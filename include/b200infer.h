@@ -121,17 +121,18 @@ int b2_engine_nb_tactics(const b2_engine* e);
 /* exports the tactic table, 10 x uint32 per record {op, batch, bn, stages, splits, sps, ws, cn, halo, 0} (the TacticRec
  * layout of the plan format); builder.attach_tactics() appends it to a plan blob.  Returns the records written. */
 int b2_engine_get_tactics(const b2_engine* e, uint32_t* out, int cap_records);
-/* Builds the launch plan of `batch` for the context's current device memory and instantiates its CUDA-graph segments
+/* Builds the launch plan of `batch` for the context's current device memory and instantiates its CUDA graph
  * (one graph per context and batch, independent of the binding pointers).  `stream` may be NULL. */
 int b2_context_prepare(b2_context* c, int batch, b2_stream_t stream);
-/* knobs: "graph"=0/1 replay the forward as a cached CUDA graph (default 1); "simt"=0/1 force the
- * SIMT reference kernels instead of the tcgen05 path (debug); "bn"/"stages"/"splits" force the conv tile,
- * pipeline depth and split-K factor (0 = cost model); "pdl"=0/1 programmatic dependent launch (process-wide);
+/* knobs: "graph"=0/1 replay the forward as a cached CUDA graph (default 1; any other value is B2_EINVAL);
+ * "simt"=0/1 force the SIMT reference kernels instead of the tcgen05 path (debug); "bn"/"stages"/"splits" force the
+ * conv tile, pipeline depth and split-K factor (0 = cost model); "pdl"=0/1 programmatic dependent launch (process-wide);
  * "pdl_trigger"=0/1 release point of the dependent kernel; "autotune"=0 (cost model) / 1 (latency) / N>=2 (N-stream
  * throughput, default 4) on-device tactic selection; "sps"=2 double-width pipeline stages; tactic switches
  * "halo"=1/-1 (3x3 halo kernel everywhere it applies / never; 0 = tuner decides), "ws"=1/N/-1 (persistent
- * warp-specialised kernel), "cn"=2/4/-1 (cluster multicast of the activation tile), "fork"=0/1 (shortcut convolutions
- * on a parallel graph branch); returns B2_EINVAL for unknown keys.  Every tactic computes bit-identical results.
+ * warp-specialised kernel), "cn"=2/4/-1 (cluster multicast of the activation tile); "fork"=0 only (every launch runs
+ * on the request's stream; other values are B2_EINVAL); returns B2_EINVAL for unknown keys.  Every tactic computes
+ * bit-identical results.
  * Environment: B2_TUNE_CACHE=<file> persists tuned tactics across processes (timing cache). */
 int b2_context_set_option(b2_context* c, const char* key, int value);
 

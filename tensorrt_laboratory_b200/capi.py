@@ -443,7 +443,7 @@ class Session:
         return self._lib.b2_context_nb_launches(self.ctx, batch)
 
     def prepare(self, batch: int):
-        """Build the launch plan and instantiate its graph segments ahead of the first request."""
+        """Build the launch plan and instantiate its CUDA graph ahead of the first request."""
         check(self._lib.b2_context_prepare(self.ctx, batch, self.stream.handle))
 
     def close(self):

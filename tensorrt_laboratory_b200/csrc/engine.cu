@@ -112,9 +112,6 @@ struct Op {
     float eps = 0.f;
     uint32_t flags = 0;
     std::string name;
-    // >= 0: this op's only consumer is the residual input of op `side_join`, and nothing in between depends on it (the
-    // shortcut convolution of a ResNet "a" block): it may run on a forked stream, concurrently with the ops up to there
-    int side_join = -1;
     // version-4 convolutions: output channels [c0, c0 + cw) of a tensor several convolutions write (cw == 0: all of it)
     int c0 = 0, cw = 0;
     // version-4 convolutions: reads channels [0, r.cin) of a wider, slice-written input (plan_format.h, input prefix)
@@ -172,7 +169,6 @@ struct Launch {
     int in_binding = -1, out_binding = -1;
     bool src_half = false;  // input cast: the binding is fp16
     int max_blocks = 0;     // input cast: grid cap (option input_ctas), 0 = one thread per element group
-    int side_join = -1;     // see Op::side_join (launch index == op index)
     b2k::TailArgs tail{};         // L_TAIL: pool + fc + softmax in one launch (out = the output binding)
     b2k::I8ConvLaunch i8{};       // L_CONV_I8 / L_CONV_F8
     float qscale = 0.f;           // L_QUANTIZE(_F8): 1/s; L_AVGPOOL_I8 / _F8: s/HW; L_OUTPUT_CAST_I8 / _F8: s
@@ -189,14 +185,6 @@ struct Launch {
     float alpha = 0.f, beta = 0.f, kk = 0.f;  // L_LRN (k = n)
 };
 
-// A maximal run of launches that touch no binding: captured ONCE per plan (= per context, arena and batch) into a CUDA
-// graph that is valid for any binding pointers.  Launches that read or write a binding (the input cast, the classifier
-// tail, output casts) are issued directly around it, so the engine never captures or instantiates per Buffers object.
-struct Segment {
-    int begin = 0, end = 0;  // [begin, end) launch indices
-    bool graphable = false;
-    cudaGraphExec_t exec = nullptr;
-};
 // One kernel node of the plan's graph that reads or writes a binding: its pointer argument is re-pointed at the caller's
 // buffer before every launch (cudaGraphExecKernelNodeSetParams) -- the graph itself is captured and instantiated once.
 struct BindPatch {
@@ -213,14 +201,10 @@ struct BindPatch {
 struct Plan {
     int batch = 0;
     std::vector<Launch> launches;
-    std::vector<Segment> segments;   // graph mode 3: binding-free runs as graphs, binding-dependent launches direct
-    bool graph_failed = false;       // the plan could not be captured as one patchable graph: segments instead
     cudaGraph_t graph = nullptr;     // graph mode 1 (default): the whole plan, binding arguments patched per launch
     cudaGraphExec_t exec = nullptr;
     std::vector<BindPatch> patches;
     ~Plan() {
-        for (Segment& sg : segments)
-            if (sg.exec) cudaGraphExecDestroy(sg.exec);
         if (exec) cudaGraphExecDestroy(exec);
         if (graph) cudaGraphDestroy(graph);
     }
@@ -292,7 +276,7 @@ struct b2_engine {
 struct b2_context {
     b2_engine* e = nullptr;
     uint8_t* scratch = nullptr;
-    // Launch plans (TMA maps embed arena addresses) and their captured graph segments are cached PER SCRATCH pointer:
+    // Launch plans (TMA maps embed arena addresses) and their captured graphs are cached PER SCRATCH pointer:
     // the reference pairs a pooled IExecutionContext with whichever pooled activation block the request drew
     // (inference_manager.cc:254-273), so the same context may see several scratch pointers over its life.
     struct ScratchState {
@@ -315,16 +299,11 @@ struct b2_context {
     int pdl_trigger = 1;
     int no_fold = 0;    // 1: run the stem through the generic 8-channel tap path instead of the row-folded one
     int autotune = 4;  // 0 off (cost model), 1 latency mode, N>=2 throughput mode over N streams
-    int fork = 0;      // 1: run side branches (Op::side_join) on a forked stream / a parallel graph branch.  Off by default:
-                       // measured neutral (4-context throughput within noise) -- the fork and
-                       // join turn the programmatic (PDL) edges around them into full dependencies, which eats the overlap
     int i8_bn = 0;       // 1-byte (INT8 / FP8) convolutions: force the N tile (128 / 256); 0 = 128
     int i8_stages = 0;   // ... and the shared-memory ring depth (2..4); 0 = by rule
     int fuse_tail = 1;   // global average pool + FC + softmax as one launch (tail_f16_kernel)
     int input_ctas = 0;  // grid cap of the input cast (0 = none); set when the input binding is read over PCIe (zero-copy)
     int* d_tail_ctrl = nullptr;  // its ticket / arrival counters (zero between launches)
-    cudaStream_t side = nullptr;
-    cudaEvent_t fork_ev = nullptr, join_ev = nullptr;
 };
 
 namespace {
@@ -928,26 +907,6 @@ int fuse_partner(const b2_engine* e, int i);
 
 // ---- activation arena: first-fit over live intervals ------------------------------------------
 void plan_arena(b2_engine* e) {
-    // side branches: a conv whose output is consumed exactly once, as the residual of a later op, with at least one
-    // independent op in between.  Regions do not nest or overlap.
-    int busy_until = -1;
-    for (size_t i = 0; i < e->ops.size(); ++i) {
-        Op& op = e->ops[i];
-        op.side_join = -1;
-        // (a slice writer's tensor is read as a whole by later ops, never as one residual: it is not a side branch)
-        if (int(i) <= busy_until || op.r.type != b2plan::OP_CONV || op.r.out < 0 || e->tensors[op.r.out].binding >= 0 || op.cw || op.prefix) continue;
-        int consumers = 0, join = -1;
-        bool as_residual_only = true;
-        for (size_t k = i + 1; k < e->ops.size(); ++k) {
-            const auto& rk = e->ops[k].r;
-            if (rk.in == op.r.out) ++consumers, as_residual_only = false;
-            if (rk.res == op.r.out) ++consumers, join = int(k);
-        }
-        if (consumers == 1 && as_residual_only && join > int(i) + 1) {
-            op.side_join = join;
-            busy_until = join;
-        }
-    }
     for (size_t i = 0; i < e->ops.size(); ++i) {
         const auto& r = e->ops[i].r;
         for (int t : {r.out, e->ops[i].out2})
@@ -956,8 +915,6 @@ void plan_arena(b2_engine* e) {
         if (e->ops[i].cw) e->tensors[r.out].last_use = std::max(e->tensors[r.out].last_use, int(i));
         for (int t : {r.in, r.res})
             if (t >= 0) e->tensors[t].last_use = std::max(e->tensors[t].last_use, int(i));
-        // a side op may still be READING its input while the ops before the join run: keep that buffer until the join
-        if (e->ops[i].side_join >= 0 && r.in >= 0) e->tensors[r.in].last_use = std::max(e->tensors[r.in].last_use, e->ops[i].side_join);
         // a 3x3 that may run fused with the next op reads its input while that op's output is written
         const int j = fuse_partner(e, int(i));
         if (j >= 0) e->tensors[r.in].last_use = std::max(e->tensors[r.in].last_use, j);
@@ -1741,8 +1698,7 @@ int tune_engine_batch(b2_context* c, int batch) {
         }
         const Tensor& to = e->tensors[r.out];
         const int kbsz = conv_kb(c, op), nkb = conv_num_kblocks(c, op);
-        const bool side = op.side_join >= 0;
-        const bool no_split = side || op.groups > 1;  // side branches and grouped convolutions never split K
+        const bool no_split = op.groups > 1;  // grouped convolutions never split K
         // Split-K is the ONE tactic that changes the fp32 summation order (every other one -- N tile, ring depth, halo,
         // persistent -- adds the same products in the same order), so letting the timing pick it would make the BITS of a
         // model depend on the load-time measurement of that process: seen once as a 4e-3 relative difference between a tuned
@@ -1804,15 +1760,12 @@ int tune_engine_batch(b2_context* c, int batch) {
 }
 
 // Every 3x3 launch whose tactic is the fused one (halo == 2) absorbs the launch of the next op, the 1x1 its kernel runs
-// (launch index == op index on entry).  The fused launch does both ops' work less the tensor between them; a side branch
-// that joined at the 1x1 joins at the fused launch.
+// (launch index == op index on entry).  The fused launch does both ops' work less the tensor between them.
 void fuse_bottlenecks(b2_context* c, Plan* plan, int batch) {
     std::vector<Launch>& ls = plan->launches;
     if (std::none_of(ls.begin(), ls.end(), [](const Launch& L) { return L.kind == L_CONV_TC && L.conv.halo == 2; })) return;
-    std::vector<int> new_index(ls.size());
     std::vector<Launch> out;
     for (size_t k = 0; k < ls.size(); ++k) {
-        new_index[k] = int(out.size());
         if (ls[k].kind == L_CONV_TC && ls[k].conv.halo == 2 && k + 1 < ls.size()) {
             Launch& J = ls[k + 1];
             Launch L = std::move(ls[k]);
@@ -1820,15 +1773,12 @@ void fuse_bottlenecks(b2_context* c, Plan* plan, int batch) {
             L.name += "+" + J.name;
             L.flops += J.flops;
             L.bytes += J.bytes - 2.0 * batch * double(mid.item_bytes);
-            new_index[k + 1] = new_index[k];
             ++k;
             out.push_back(std::move(L));
             continue;
         }
         out.push_back(std::move(ls[k]));
     }
-    for (Launch& L : out)
-        if (L.side_join >= 0) L.side_join = new_index[size_t(L.side_join)];
     ls = std::move(out);
 }
 
@@ -1856,7 +1806,7 @@ void fuse_tail(b2_context* c, Plan* plan, int batch) {
         T.tail.ctrl = c->d_tail_ctrl;
         T.tail.N = batch, T.tail.HW = P.H * P.W, T.tail.C = P.C_phys, T.tail.Cout = F.Cout;
         ls[i] = std::move(T);
-        ls.erase(ls.begin() + long(i) + 1, ls.begin() + long(i) + 3);  // (launches before i keep their indices: side joins stay valid)
+        ls.erase(ls.begin() + long(i) + 1, ls.begin() + long(i) + 3);
         return;
     }
 }
@@ -1891,7 +1841,6 @@ int build_plan(b2_context* c, int batch, Plan** out) {
         Launch L;
         L.name = op.name;
         L.N = batch;
-        L.side_join = op.side_join;
         switch (r.type) {
             case b2plan::OP_INPUT_CAST: {
                 const Tensor& t = e->tensors[r.out];
@@ -1992,7 +1941,6 @@ int build_plan(b2_context* c, int batch, Plan** out) {
                         const ConvConfig f = fused_conv_config(op);
                         if (tactic_applies(c, op, batch, f)) cfg = f;
                     }
-                    if (op.side_join >= 0 && cfg.splits > 1) cfg.splits = 1;  // forced / cached tactic on a side-branch op
                     int rc = make_conv_launch(c, op, batch, cfg, &L.conv);
                     if (rc) return rc;
                     // packed rows: tiles past the live row count T skip their work (the tuner times the same tactic on all rows)
@@ -2187,21 +2135,6 @@ int build_plan(b2_context* c, int batch, Plan** out) {
     }
     fuse_bottlenecks(c, plan.get(), batch);
     fuse_tail(c, plan.get(), batch);
-    {   // split into binding-dependent launches and binding-independent (graphable) runs
-        const std::vector<Launch>& ls = plan->launches;
-        size_t i = 0;
-        while (i < ls.size()) {
-            const bool dep = ls[i].in_binding >= 0 || ls[i].out_binding >= 0;
-            size_t j = i + 1;
-            if (!dep)
-                while (j < ls.size() && ls[j].in_binding < 0 && ls[j].out_binding < 0) ++j;
-            Segment sg;
-            sg.begin = int(i), sg.end = int(j);
-            sg.graphable = !dep && (j - i) >= 3;
-            plan->segments.push_back(sg);
-            i = j;
-        }
-    }
     *out = plan.get();
     c->cur->plans[batch] = std::move(plan);
     return B2_OK;
@@ -2288,67 +2221,11 @@ int run_launch(const b2_engine* e, const Launch& L, void* const* bindings, cudaS
     return int(cudaErrorInvalidValue);
 }
 
-// Launches the plan on `s`.  Side branches go to the context's second stream between a fork and a join event: inside
-// a stream capture that becomes a parallel branch of the graph, outside it is plain two-stream concurrency.
-int run_range(b2_context* c, const Plan& plan, size_t first, size_t last, void* const* bindings, cudaStream_t s);
-int run_all(b2_context* c, const Plan& plan, void* const* bindings, cudaStream_t s) {
-    return run_range(c, plan, 0, plan.launches.size(), bindings, s);
-}
-int run_range(b2_context* c, const Plan& plan, size_t first, size_t last, void* const* bindings, cudaStream_t s) {
-    const b2_engine* e = c->e;
-    bool fork = c->fork != 0;
-    if (fork && !c->side) {
-        if (cudaStreamCreateWithFlags(&c->side, cudaStreamNonBlocking) != cudaSuccess ||
-            cudaEventCreateWithFlags(&c->fork_ev, cudaEventDisableTiming) != cudaSuccess ||
-            cudaEventCreateWithFlags(&c->join_ev, cudaEventDisableTiming) != cudaSuccess) {
-            cudaGetLastError();
-            fork = false;
-        }
-    }
-    int pending_join = -1;
-    for (size_t i = first; i < last; ++i) {
-        const Launch& L = plan.launches[i];
-        if (pending_join == int(i)) {
-            B2_CUDA(cudaStreamWaitEvent(s, c->join_ev, 0));
-            pending_join = -1;
-        }
-        int rc;
-        if (fork && pending_join < 0 && L.side_join > int(i) && L.side_join < int(last)) {
-            B2_CUDA(cudaEventRecord(c->fork_ev, s));
-            B2_CUDA(cudaStreamWaitEvent(c->side, c->fork_ev, 0));
-            rc = run_launch(e, L, bindings, c->side);
-            if (rc == 0) {
-                B2_CUDA(cudaEventRecord(c->join_ev, c->side));
-                pending_join = L.side_join;
-            }
-        } else {
-            rc = run_launch(e, L, bindings, s);
-        }
-        if (rc != 0)
+// Launches the plan on `s`, in order.
+int run_all(const b2_engine* e, const Plan& plan, void* const* bindings, cudaStream_t s) {
+    for (const Launch& L : plan.launches)
+        if (int rc = run_launch(e, L, bindings, s))
             return fail(B2_ECUDA, "launch of %s failed: %s", L.name.c_str(), cudaGetErrorString(cudaError_t(rc)));
-    }
-    if (pending_join >= 0) B2_CUDA(cudaStreamWaitEvent(s, c->join_ev, 0));  // never leave the branch dangling
-    return B2_OK;
-}
-
-// Captures launches [begin, end) of the plan -- none of which touches a binding -- on `stream` (which must be idle-able:
-// capture only records) and instantiates the graph once for the life of the plan.
-int instantiate_segment(b2_context* c, Plan* plan, Segment* sg, void* const* bindings, cudaStream_t stream) {
-    cudaGraph_t graph = nullptr;
-    B2_CUDA(cudaStreamBeginCapture(stream, cudaStreamCaptureModeThreadLocal));
-    int rc = run_range(c, *plan, size_t(sg->begin), size_t(sg->end), bindings, stream);
-    cudaError_t ce = cudaStreamEndCapture(stream, &graph);
-    if (rc) {
-        if (graph) cudaGraphDestroy(graph);
-        return rc;
-    }
-    if (ce != cudaSuccess) return fail(B2_ECUDA, "cudaStreamEndCapture failed: %s", cudaGetErrorString(ce));
-    ce = cudaGraphInstantiate(&sg->exec, graph, 0);
-    cudaGraphDestroy(graph);
-    if (ce != cudaSuccess) {
-        sg->exec = nullptr;
-        return fail(B2_ECUDA, "cudaGraphInstantiate failed: %s", cudaGetErrorString(ce));
-    }
     return B2_OK;
 }
 
@@ -2405,30 +2282,32 @@ bool patch_layout(const b2_engine* e, const Launch& L, BindPatch* p) {
 }
 
 // Captures the WHOLE plan once (programmatic edges between all kernels survive) and remembers the kernel nodes that touch
-// a binding.  Returns B2_OK with plan->exec == nullptr if the plan cannot be patched (then graph mode 3 takes over).
+// a binding, so that each request can re-point them at its buffers.
 int instantiate_plan_graph(b2_context* c, Plan* plan, void* const* bindings, cudaStream_t stream) {
     std::vector<BindPatch> patches;
     cudaGraph_t graph = nullptr;
-    bool patchable = true;
     B2_CUDA(cudaStreamBeginCapture(stream, cudaStreamCaptureModeThreadLocal));
     int rc = B2_OK;
-    for (size_t i = 0; i < plan->launches.size() && !rc; ++i) {
+    for (size_t i = 0; i < plan->launches.size(); ++i) {
         const Launch& L = plan->launches[i];
-        rc = run_range(c, *plan, i, i + 1, bindings, stream);
-        if (rc || (L.in_binding < 0 && L.out_binding < 0)) continue;
+        if (int lr = run_launch(c->e, L, bindings, stream)) {
+            rc = fail(B2_ECUDA, "launch of %s failed: %s", L.name.c_str(), cudaGetErrorString(cudaError_t(lr)));
+            break;
+        }
+        if (L.in_binding < 0 && L.out_binding < 0) continue;
         BindPatch p;
         p.launch = int(i);
         if (!patch_layout(c->e, L, &p)) {
-            patchable = false;
-            continue;
+            rc = fail(B2_EINVAL, "launch %s reads or writes a binding the graph cannot re-point", L.name.c_str());
+            break;
         }
         cudaStreamCaptureStatus st;
         const cudaGraphNode_t* deps = nullptr;
         size_t ndeps = 0;
         if (cudaStreamGetCaptureInfo_v2(stream, &st, nullptr, nullptr, &deps, &ndeps) != cudaSuccess || ndeps != 1) {
             cudaGetLastError();
-            patchable = false;
-            continue;
+            rc = fail(B2_ECUDA, "launch %s: no single captured node to re-point", L.name.c_str());
+            break;
         }
         p.node = deps[0];
         patches.push_back(p);
@@ -2441,17 +2320,13 @@ int instantiate_plan_graph(b2_context* c, Plan* plan, void* const* bindings, cud
     if (ce != cudaSuccess) return fail(B2_ECUDA, "cudaStreamEndCapture failed: %s", cudaGetErrorString(ce));
     for (BindPatch& p : patches) {
         cudaGraphNodeType ty;
-        if (!patchable || cudaGraphNodeGetType(p.node, &ty) != cudaSuccess || ty != cudaGraphNodeTypeKernel ||
+        if (cudaGraphNodeGetType(p.node, &ty) != cudaSuccess || ty != cudaGraphNodeTypeKernel ||
             cudaGraphKernelNodeGetParams(p.node, &p.np) != cudaSuccess || p.np.kernelParams == nullptr) {
             cudaGetLastError();
-            patchable = false;
-            break;
+            cudaGraphDestroy(graph);
+            return fail(B2_ECUDA, "launch %s was not captured as a kernel node", plan->launches[size_t(p.launch)].name.c_str());
         }
         p.params.assign(p.np.kernelParams, p.np.kernelParams + p.n_params);
-    }
-    if (!patchable) {
-        cudaGraphDestroy(graph);
-        return B2_OK;
     }
     cudaGraphExec_t exec = nullptr;
     ce = cudaGraphInstantiate(&exec, graph, 0);
@@ -2648,7 +2523,6 @@ int b2_context_create(b2_engine* e, b2_context** out) {
     c->force_fuse = env_int("B2_FORCE_FUSE", 0);
     c->pdl_trigger = env_int("B2_PDL_TRIGGER", 1);
     c->autotune = env_int("B2_AUTOTUNE", 4);
-    c->fork = env_int("B2_FORK", 0);
     c->fuse_tail = env_int("B2_FUSE_TAIL", 1);
     c->input_ctas = env_int("B2_INPUT_CTAS", 0);
     c->i8_bn = env_int("B2_I8_BN", 0);
@@ -2675,9 +2549,6 @@ void b2_context_destroy(b2_context* c) {
     if (!c) return;
     drop_cached(c);
     if (c->d_counters) cudaFree(c->d_counters);
-    if (c->side) cudaStreamDestroy(c->side);
-    if (c->fork_ev) cudaEventDestroy(c->fork_ev);
-    if (c->join_ev) cudaEventDestroy(c->join_ev);
     delete c;
 }
 
@@ -2694,9 +2565,12 @@ int b2_context_set_option(b2_context* c, const char* key, int value) {
     if (!c || !key) return fail(B2_EINVAL, "null context or key");
     const std::string k(key);
     if (k == "graph") {
+        if (value != 0 && value != 1) return fail(B2_EINVAL, "option graph takes 0 or 1, not %d", value);
         c->use_graph = value;
         return B2_OK;
     }
+    // every launch runs on the request's stream: callers that explicitly ask for that (fork = 0) keep working
+    if (k == "fork") return value == 0 ? B2_OK : fail(B2_EINVAL, "option fork takes only 0: every launch runs on the request's stream");
     if (k == "pdl") {
         b2k::set_pdl(value != 0);  // process-wide
         value = 0;
@@ -2710,7 +2584,6 @@ int b2_context_set_option(b2_context* c, const char* key, int value) {
     else if (k == "cn") c->force_cn = value;
     else if (k == "halo") c->force_halo = value;
     else if (k == "fuse") c->force_fuse = value;
-    else if (k == "fork") c->fork = value;
     else if (k == "fuse_tail") c->fuse_tail = value;
     else if (k == "i8_bn") c->i8_bn = value;
     else if (k == "i8_stages") c->i8_stages = value;
@@ -2878,7 +2751,7 @@ int b2_engine_refine_tactics(b2_engine* e, int streams, int passes, double* gain
             // of SMs; splitting K shortens the link and puts more SMs on it.  The per-layer tuner rejects it (more total
             // work), the chain-bound whole-network rate is where it can pay.  (The split factor fixes the fp32 summation
             // order; it is chosen here, at max batch, and shared by every batch size.)
-            if (env_int("B2_TUNE_SPLITK", 0) != 0 && !(op.side_join >= 0) && op.groups == 1 && cur.splits == 1 && !cur.halo) {  // opt-in: changes bits
+            if (env_int("B2_TUNE_SPLITK", 0) != 0 && op.groups == 1 && cur.splits == 1 && !cur.halo) {  // opt-in: changes bits
                 const int m_tiles = (batch * int(e->tensors[r.out].h * e->tensors[r.out].w) + 127) / 128;
                 for (int sp : {2, 4}) {
                     const int tiles = m_tiles * (int(r.cout_phys) / cur.bn);
@@ -2940,8 +2813,8 @@ int b2_engine_get_tactics(const b2_engine* e, uint32_t* out, int cap) {
     return n;
 }
 
-// Builds the launch plan of `batch` for the context's current arena and instantiates its graph segments, so that the
-// first request at this batch size pays neither.  `stream` is only used to record the capture.
+// Builds the launch plan of `batch` for the context's current arena and instantiates its graph, so that the first
+// request at this batch size pays neither.  `stream` is only used to record the capture.
 int b2_context_prepare(b2_context* c, int batch, b2_stream_t stream_) {
     if (!c) return fail(B2_EINVAL, "null context");
     if (batch < 1 || batch > c->e->max_batch) return fail(B2_EINVAL, "batch %d outside [1, %d]", batch, c->e->max_batch);
@@ -2957,13 +2830,7 @@ int b2_context_prepare(b2_context* c, int batch, b2_stream_t stream_) {
     }
     // placeholder binding pointers: a capture only RECORDS launches, and every request re-points the nodes that use them
     std::vector<void*> dummy(c->e->bindings.size(), reinterpret_cast<void*>(uintptr_t(256)));
-    if (c->use_graph != 3 && !plan->exec && !plan->graph_failed) {
-        rc = instantiate_plan_graph(c, plan, dummy.data(), stream);
-        plan->graph_failed = !rc && plan->exec == nullptr;
-    }
-    if (!rc && !plan->exec)
-        for (Segment& sg : plan->segments)
-            if (sg.graphable && !sg.exec && (rc = instantiate_segment(c, plan, &sg, dummy.data(), stream))) break;
+    if (!plan->exec) rc = instantiate_plan_graph(c, plan, dummy.data(), stream);
     if (own) cudaStreamDestroy(own);
     return rc;
 }
@@ -2978,25 +2845,11 @@ int b2_context_enqueue(b2_context* c, int batch, void* const* bindings, b2_strea
     B2_CUDA(cudaStreamIsCapturing(stream, &cap));
     // Inside a caller's capture (the reference graphs enqueueV2 itself, workspace.cc:51-56) or with graphs off: plain launches.
     if (cap != cudaStreamCaptureStatusNone || !c->use_graph) {
-        if ((rc = run_all(c, *plan, bindings, stream))) return rc;
-    } else {
-        if (c->use_graph != 3 && !plan->exec && !plan->graph_failed) {
-            if ((rc = instantiate_plan_graph(c, plan, bindings, stream))) return rc;
-            plan->graph_failed = plan->exec == nullptr;
-        }
-        if (plan->exec) {  // one graph for the whole forward pass, re-pointed at this request's bindings
-            if ((rc = patch_plan_graph(plan, bindings))) return rc;
-            B2_CUDA(cudaGraphLaunch(plan->exec, stream));
-        } else {
-            for (Segment& sg : plan->segments) {
-                if (!sg.graphable) {
-                    if ((rc = run_range(c, *plan, size_t(sg.begin), size_t(sg.end), bindings, stream))) return rc;
-                    continue;
-                }
-                if (!sg.exec && (rc = instantiate_segment(c, plan, &sg, bindings, stream))) return rc;
-                B2_CUDA(cudaGraphLaunch(sg.exec, stream));
-            }
-        }
+        if ((rc = run_all(c->e, *plan, bindings, stream))) return rc;
+    } else {  // one graph for the whole forward pass, re-pointed at this request's bindings
+        if (!plan->exec && (rc = instantiate_plan_graph(c, plan, bindings, stream))) return rc;
+        if ((rc = patch_plan_graph(plan, bindings))) return rc;
+        B2_CUDA(cudaGraphLaunch(plan->exec, stream));
     }
     if (consumed) B2_CUDA(cudaEventRecord(static_cast<cudaEvent_t>(consumed), stream));
     return B2_OK;
@@ -3106,7 +2959,6 @@ const char* b2_context_launch_name(b2_context* c, int batch, int i) {
              (L->i8.group_mode ? " span=" + std::to_string(L->i8.args.group_span) + " mode=" +
                                      (L->i8.group_mode == 128 ? std::string("dense") : std::to_string(L->i8.group_mode))
                                : std::string());
-    if (L->side_join >= 0) s += " side";
     return s.c_str();
 }
 double b2_context_launch_flops(b2_context* c, int batch, int i) {

@@ -79,7 +79,6 @@ class Case(NamedTuple):
     relu2: bool = True       # ReLU after the residual sum
     res: str = "identity"    # identity (the block input), projection ("short", a 1x1 of the block input), input ("a")
     a: bool = True           # a 1x1 "a" in front of the 3x3
-    fork: int = 0            # the projection shortcut on a forked side stream
     max_batch: Optional[int] = None
     seed: int = 0
 
@@ -113,7 +112,7 @@ def case_id(c):
     s = f"ci{c.cin3}-c{c.c3}-co{c.cout2}-{c.h}x{c.w}-n{c.batch}"
     if c.max_batch:
         s += f"of{c.max_batch}"
-    s += f"-{c.res}" + (f"-fork{c.fork}" if c.fork else "") + ("" if c.a else "-noa")
+    s += f"-{c.res}" + ("" if c.a else "-noa")
     s += ("" if c.relu3 else "-lin3") + ("" if c.relu2 else "-lin2")
     return s + ("" if c.fused else "-refused")
 
@@ -225,7 +224,7 @@ WIDTH_CASES = [
     Case(64, 64, 64, 14, 14, res="projection", seed=1),
     Case(192, 64, 192, 14, 14, res="input", seed=2),
     Case(64, 64, 320, 14, 14, seed=3),
-    Case(64, 128, 320, 14, 14, res="projection", fork=1, seed=4),
+    Case(64, 128, 320, 14, 14, res="projection", seed=4),
     Case(128, 128, 512, 14, 14, seed=5),
     Case(64, 64, 2048, 14, 14, seed=6),
 ]
@@ -257,7 +256,7 @@ EPILOGUE_CASES = [
     Case(64, 64, 256, 14, 14, relu2=False, seed=21),
     Case(64, 64, 256, 14, 14, relu3=False, relu2=False, seed=22),
     Case(64, 128, 256, 12, 12, relu2=False, res="projection", seed=23),
-    Case(64, 128, 256, 12, 12, relu3=False, relu2=False, res="projection", fork=1, seed=24),
+    Case(64, 128, 256, 12, 12, relu3=False, relu2=False, res="projection", seed=24),
     Case(192, 128, 192, 12, 12, relu2=False, res="input", seed=25),
     Case(256, 64, 256, 12, 12, relu3=False, a=False, seed=26),   # no "a": the identity residual is the 3x3's input too
 ]
@@ -331,7 +330,7 @@ def test_fused_block(gpu, case):
     low = lowered(block_net(case), case.seed)
     x = block_input(case)
     n = x.shape[0]
-    got = helpers.run_engine(low, x, FP16, {"fuse": 1, "fork": case.fork}, max_batch=case.max_batch)["sum"]
+    got = helpers.run_engine(low, x, FP16, {"fuse": 1}, max_batch=case.max_batch)["sum"]
     names = list(helpers.LAST_LAUNCH_NAMES)
     if case.fused:
         assert_fused(names, [("b", "c", phys(case.c3))])
@@ -340,7 +339,7 @@ def test_fused_block(gpu, case):
         if halo_rows(case.h, case.w) == 0:
             assert not any(" halo" in nm for nm in names), names
     # the unfused pair, every operator read back through a tap (a tapped 3x3 output never fuses)
-    out = helpers.run_engine(low, x, FP16, {"fuse": -1, "fork": case.fork}, outputs=taps(case), max_batch=case.max_batch)
+    out = helpers.run_engine(low, x, FP16, {"fuse": -1}, outputs=taps(case), max_batch=case.max_batch)
     assert_unfused(helpers.LAST_LAUNCH_NAMES, ["b", "c"])
     assert got.tobytes() == out["sum"].tobytes()
     check_block_ops(low, x, case, out)

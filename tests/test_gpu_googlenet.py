@@ -1,6 +1,6 @@
 """GoogLeNet on the H100: convolutions that store into their channel slice of a concatenated tensor, under every tactic
 the rule admits; lrn_h8_kernel against float64; the whole fp16 network against the fp32 and fp16-emulating oracles; and
-the invariances every plan keeps (batch position, partial batch, replay, contexts, tuning, InferenceManager, forks)."""
+the invariances every plan keeps (batch position, partial batch, replay, contexts, tuning, InferenceManager)."""
 from __future__ import annotations
 
 import copy
@@ -254,11 +254,6 @@ def test_googlenet_invariance(googlenet):
         other = s2.infer(x)["prob"]
     finally:
         s2.close()
-    s3 = capi.Session(eng, {"fork": 1})
-    try:
-        forked = s3.infer(x)["prob"]
-    finally:
-        s3.close()
     assert eng.tune(4) > 0
     tuned_blob = builder.attach_tactics(blob, eng.tactics())
     eng.destroy()
@@ -267,7 +262,6 @@ def test_googlenet_invariance(googlenet):
     assert np.array_equal(permuted, full[perm])
     assert np.array_equal(part, full[:5])
     assert np.array_equal(other, full)
-    assert np.array_equal(forked, full)
     assert np.array_equal(tuned["prob"], full)
     m = capi.InferenceManager(max_exec_concurrency=1)
     try:

@@ -164,30 +164,6 @@ def test_fp16_input_binding_matches_fp32_binding(rn50, rn50_session):
         mgr.close()
 
 
-def test_side_branches_run_forked_and_change_nothing(rn50, rn50_session):
-    """The shortcut convolutions of the four "a" blocks run on a forked stream (a parallel branch of the captured graph)
-    while branch2a/2b execute; results are bit-identical to the linear schedule, with and without graph replay."""
-    eng = capi.Engine(rn50_session["blob"])
-    outs = {}
-    try:
-        for fork, graph_ in ((1, 1), (0, 1), (1, 0)):
-            sess = capi.Session(eng, {"fork": fork, "graph": graph_})
-            try:
-                outs[(fork, graph_)] = sess.infer(rn50["x"])["prob"]
-                for _ in range(3):
-                    np.testing.assert_array_equal(sess.infer(rn50["x"])["prob"], outs[(fork, graph_)])
-                n = sess.nb_launches(8)
-                names = [capi.load().b2_context_launch_name(sess.ctx, 8, i).decode() for i in range(n)]
-                assert sum(1 for s_ in names if s_.endswith(" side")) == 4
-            finally:
-                sess.close()
-    finally:
-        eng.destroy()
-    np.testing.assert_array_equal(outs[(1, 1)], outs[(0, 1)])
-    np.testing.assert_array_equal(outs[(1, 0)], outs[(0, 1)])
-    np.testing.assert_array_equal(outs[(1, 1)], rn50_session["sess"].infer(rn50["x"])["prob"])
-
-
 def test_four_contexts_share_the_gpu(rn50, rn50_session):
     """BASELINE configs[1]: four ExecutionContexts on four streams, driven from four threads at once."""
     eng = rn50_session["eng"]
@@ -214,10 +190,11 @@ def test_four_contexts_share_the_gpu(rn50, rn50_session):
             s.close()
 
 
-def test_removed_network_kernel_options_are_rejected(rn50_session):
-    for key in ("net", "net_ctas", "net_bn", "net_stages"):
+def test_removed_options_are_rejected(rn50_session):
+    for key, value in (("net", 1), ("net_ctas", 1), ("net_bn", 1), ("net_stages", 1), ("fork", 1), ("graph", 3), ("graph", 2)):
         with pytest.raises(capi.B2Error):
-            rn50_session["sess"].set_option(key, 1)
+            rn50_session["sess"].set_option(key, value)
+    rn50_session["sess"].set_option("fork", 0)  # the one schedule there is
 
 
 def test_dynamic_batching_runner(rn50, rn50_session):

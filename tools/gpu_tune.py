@@ -42,7 +42,7 @@ def main():
     x = weights.synthetic_input(8)
     ring = weights.synthetic_input(8, ring=8)
     env_keys = {"bn": "B2_FORCE_BN", "stages": "B2_FORCE_STAGES", "splits": "B2_FORCE_SPLITS", "pdl": "B2_PDL",
-                "pdl_trigger": "B2_PDL_TRIGGER", "graph": "B2_GRAPH", "autotune": "B2_AUTOTUNE", "sps": "B2_FORCE_SPS", "ws": "B2_FORCE_WS", "fork": "B2_FORK", "halo": "B2_FORCE_HALO", "cn": "B2_FORCE_CN"}
+                "pdl_trigger": "B2_PDL_TRIGGER", "graph": "B2_GRAPH", "autotune": "B2_AUTOTUNE", "sps": "B2_FORCE_SPS", "ws": "B2_FORCE_WS", "halo": "B2_FORCE_HALO", "cn": "B2_FORCE_CN"}
     for cfg in configs:
         sess = capi.Session(eng, cfg)
         sess.infer(x)
