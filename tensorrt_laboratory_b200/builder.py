@@ -21,6 +21,7 @@ OP_PATCHIFY, OP_TOKENS, OP_CLS_HEAD = range(12, 15)                  # Vision Tr
 OP_LRN = 15                                                          # local response normalisation (version-4 plans)
 CONV_RELU, CONV_PACKED, CONV_INT8, CONV_GELU = 1, 2, 4, 8            # OpRec.relu bits of a convolution
 CONV_PREACT = 16  # OpRec.relu bit of a convolution or average pool: BatchNorm + ReLU input prologue (version-4 plans)
+FC_STREAM = 32    # OpRec.relu bit of an FC: streaming tensor-core FC layer, packed weights (version-4 fp16 plans; bit 0 = ReLU)
 FLAG_ROWS_OUT, FLAG_PACKED = 1, 2  # OpRecV3.flags: channels-last output cast; op on packed (padding-free) rows
 T_ACT, T_VEC = 0, 1
 MAGIC = b"B2ENGINE"
@@ -188,7 +189,16 @@ def build_plan(lowered: dict, precision: int = PREC_FP16, max_batch: int = 8,
         raise ValueError("a graph with a Concat or LRN layer builds in fp16 only: channel concatenation and LRN have no fp32, "
                          "INT8 or FP8 kernels")
     shapes: Dict[str, tuple] = dict(lowered["tensors"])
-    vec_tensors = {op["output"] for op in lowered["ops"] if op["type"] in (G.OP_FC, G.OP_SOFTMAX)}
+    fcs = [op for op in lowered["ops"] if op["type"] == G.OP_FC]
+    for op in fcs:
+        if op.get("relu") and precision != PREC_FP16:
+            raise ValueError(f"fc {op['name']}: an InnerProduct with a fused ReLU builds in fp16 only: hidden fully-connected "
+                             "layers have no fp32, INT8 or FP8 kernels")
+    # a plan with a hidden FC (or an FC with a fused ReLU) runs every FC on the streaming tensor-core kernel; hidden FC
+    # outputs are fp16 activations
+    fc_stream = precision == PREC_FP16 and any(op.get("hidden") or op.get("relu") for op in fcs)
+    hidden = {op["output"] for op in fcs if fc_stream and op.get("hidden")}
+    vec_tensors = {op["output"] for op in lowered["ops"] if op["type"] in (G.OP_FC, G.OP_SOFTMAX)} - hidden
 
     tensors: List[dict] = []
     tindex: Dict[str, int] = {}
@@ -199,6 +209,8 @@ def build_plan(lowered: dict, precision: int = PREC_FP16, max_batch: int = 8,
         c, h, w = shapes[tname]
         if tname in vec_tensors:
             rec = dict(name=tname, kind=T_VEC, h=1, w=1, c=c * h * w, c_phys=c * h * w, binding=-1)
+        elif tname in hidden:  # [1, 1, C]: the reader's K is c_phys, a multiple of 64
+            rec = dict(name=tname, kind=T_ACT, h=1, w=1, c=c, c_phys=_roundup(c, 64), binding=-1)
         elif tname in tscale:  # 1-byte activations: one 128-byte swizzle row = 128 channels
             rec = dict(name=tname, kind=T_ACT, h=h, w=w, c=c, c_phys=_roundup(c, 128), binding=-1, scale=float(np.float32(tscale[tname])))
         else:
@@ -381,6 +393,19 @@ def build_plan(lowered: dict, precision: int = PREC_FP16, max_batch: int = 8,
             if tensors[to]["h"] != 1 or tensors[to]["w"] != 1:
                 raise ValueError(f"avgpool {op['name']}: a windowed average pool runs only with a BatchNorm + ReLU input prologue")
             rec.update(type=OP_AVGPOOL, k=op["k"], stride=op["stride"])
+        elif t == G.OP_FC and fc_stream:  # weights pack_weights_sw128 [cout_phys, K], bias [cout_phys]; plan_format.h kFcStream
+            c, h, w = op["in_chw"]
+            c_phys = tensors[ti]["c_phys"]
+            if tensors[ti]["kind"] != T_ACT or (h * w * c_phys) % 64:
+                raise ValueError(f"fc {op['name']}: a streaming FC layer reads an fp16 activation whose h * w * c_phys is a multiple of "
+                                 f"64 (here {h} * {w} * {c_phys})")
+            cout_phys = _roundup(op["cout"], 128)
+            Wf = np.zeros((cout_phys, h * w, c_phys), dtype=np.float32)
+            Wf[:op["cout"], :, :c] = op["W"].reshape(op["cout"], h * w, c)
+            w_off, w_bytes = add_payload(pack_weights_sw128(Wf.astype(np.float16).reshape(cout_phys, h * w * c_phys)))
+            b_off, b_bytes = add_payload(_pad_vec(op["bias"], cout_phys))
+            rec.update(type=OP_FC, relu=int(bool(op.get("relu"))) | FC_STREAM, cin=op["cin"], cout=op["cout"], cin_phys=h * w * c_phys,
+                       cout_phys=cout_phys, w_off=w_off, w_bytes=w_bytes, b_off=b_off, b_bytes=b_bytes)
         elif t == G.OP_FC:
             c, h, w = op["in_chw"]
             c_phys = tensors[ti]["c_phys"]
@@ -422,7 +447,8 @@ def _serialize(tensors: List[dict], ops: List[dict], bindings: List[dict], paylo
     # version 1 unless a convolution is grouped (2) or the plan has transformer ops / GELU (3): every plan without them
     # stays byte-identical to what older builders wrote
     # version 4 when a convolution writes a channel slice or an op is an LRN
-    concat = any(o["type"] == OP_LRN or "out_cw" in o for o in ops)
+    # (and when an FC streams: kFcStream)
+    concat = any(o["type"] == OP_LRN or "out_cw" in o or (o["type"] == OP_FC and o.get("relu", 0) & FC_STREAM) for o in ops)
     transformer = any(OP_EMBED_LN <= o["type"] <= OP_CLS_HEAD or (o["type"] == OP_CONV and o.get("relu", 0) & CONV_GELU) for o in ops)
     if concat and transformer:
         raise ValueError("a plan holds channel slices / LRN or transformer ops, not both")
@@ -742,6 +768,17 @@ def build_densenet_plan(depth: int = 121, max_batch: int = 8, seed: int = 0, wei
     net = G.densenet_caffe(depth)
     low = G.lower(net, weights if weights is not None else Wt.random_weights(net, seed))
     return build_plan(low, precision, max_batch, input_dtype=input_dtype)
+
+
+def build_vgg_plan(depth: int = 16, max_batch: int = 8, seed: int = 0, weights: Optional[dict] = None,
+                   input_dtype: str = "f32") -> bytes:
+    """Convenience: generated VGG-{16,19} (:func:`graph.vgg_caffe`) + deterministic (or given, Caffe-named:
+    ``weights.random_weights``, ``caffemodel``, ``vgg.load_weights``) weights -> fp16 plan (version 4).  fc6 and fc7 fuse
+    their ReLUs and write fp16 activations; fc6, fc7 and fc8 run on the streaming tensor-core FC kernel."""
+    from . import weights as Wt
+    net = G.vgg_caffe(depth)
+    low = G.lower(net, weights if weights is not None else Wt.random_weights(net, seed))
+    return build_plan(low, PREC_FP16, max_batch, input_dtype=input_dtype)
 
 
 def build_resnet_plan(depth: int = 50, precision: int = PREC_FP16, max_batch: int = 8, seed: int = 0,

@@ -87,6 +87,35 @@ size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 constexpr size_t kSplitWorkspaceBytes = 12u << 20;  // bounds tiles*splits*128*BN*4 (see pick_conv_config)
 constexpr int kMaxSplitTiles = 4096;                 // tile counters per context
 constexpr int kSmemLimit = 227 * 1024;               // dynamic shared memory one CTA may opt in to on sm_90
+constexpr int kFcStreamSms = 132;                    // SMs of an H100 SXM: the CTA count a streaming FC's split count aims at
+
+// Geometry of a kFcStream FC (plan_format.h), fixed per plan from max batch: NB batch columns per CTA, round8(min(max
+// batch, 64)), and the split count.  The split count is a closed-form function of the shapes -- never timed, since it
+// changes the summation order and so the bits -- and every batch size reuses it, so an image's result does not depend on
+// the batch it travels in.  Among S in [lo, 2 lo], lo = the least S whose tiles x chunks x S CTAs cover every SM, it
+// takes the S with the fewest CTA waves per unit of K (ties: the smaller S, fewer partial tiles), and no split gets
+// fewer than 4 of the 64-K blocks.
+struct FcStreamGeom {
+    int nb, tiles, chunks, splits;
+};
+FcStreamGeom fc_stream_geom(int max_batch, int cout_phys, int nkb) {
+    FcStreamGeom g;
+    g.nb = std::min((max_batch + 7) / 8 * 8, 64);
+    g.tiles = cout_phys / 128;
+    g.chunks = (max_batch + g.nb - 1) / g.nb;
+    const int T = g.tiles * g.chunks;
+    const int lo = (kFcStreamSms + T - 1) / T, cap = std::max(1, nkb / 4);
+    g.splits = std::min(lo, cap);
+    double best = 1e30;
+    for (int sp = lo; sp <= std::min(2 * lo, cap); ++sp) {
+        const double cost = double((T * sp + kFcStreamSms - 1) / kFcStreamSms) / sp;
+        if (cost < best - 1e-12) best = cost, g.splits = sp;
+    }
+    return g;
+}
+size_t fc_stream_workspace_bytes(const FcStreamGeom& g) {
+    return g.splits > 1 ? size_t(g.tiles) * g.chunks * g.splits * 128 * g.nb * 4 : 0;
+}
 
 int env_int(const char* name, int dflt) {
     const char* v = getenv(name);
@@ -146,7 +175,7 @@ struct Binding {
 
 enum LKind { L_INPUT_CAST, L_CONV_TC, L_CONV_SIMT, L_MAXPOOL, L_AVGPOOL, L_FC, L_SOFTMAX, L_OUTPUT_CAST, L_TAIL, L_QUANTIZE, L_CONV_I8, L_AVGPOOL_I8, L_OUTPUT_CAST_I8,
              L_EMBED_LN, L_LAYERNORM, L_ATTENTION, L_POOLER, L_OUTPUT_ROWS, L_OUTPUT_UNPACK, L_QUANTIZE_F8, L_CONV_F8, L_AVGPOOL_F8,
-             L_OUTPUT_CAST_F8, L_PATCHIFY, L_TOKENS, L_CLS_HEAD, L_LRN, L_AVGPOOL_PRE };
+             L_OUTPUT_CAST_F8, L_PATCHIFY, L_TOKENS, L_CLS_HEAD, L_LRN, L_AVGPOOL_PRE, L_FC_STREAM };
 
 // Attention kernel of a packed plan's S tokens: the smallest instantiated sequence length S_k >= S (the variable-length
 // kernels attend each item over its own rows, so the rows S ... S_k - 1 of an item's tile are never used)
@@ -183,6 +212,7 @@ struct Launch {
     int c0 = 0, cw = 0;                       // L_CONV_TC / L_MAXPOOL of a slice writer: its output channels (Op::c0, Op::cw)
     int out_pitch = 0;                        // L_MAXPOOL of a slice writer: channels per pixel of its output tensor
     float alpha = 0.f, beta = 0.f, kk = 0.f;  // L_LRN (k = n)
+    b2k::FcStreamLaunch fc{};                 // L_FC_STREAM
 };
 
 // One kernel node of the plan's graph that reads or writes a binding: its pointer argument is re-pointed at the caller's
@@ -795,8 +825,33 @@ int parse_blob(const void* blob, size_t nbytes, b2_engine* e, const uint8_t** pa
             e->flops_per_item += 2.0 * ho * wo * r.cout * op.algo_k();
         } else if (r.type == OP_FC) {
             const Tensor& ti = e->tensors[r.in];
+            const Tensor& to = e->tensors[r.out];
             const size_t K = size_t(ti.h) * ti.w * ti.c_phys;
-            if (r.w_bytes != size_t(r.cout) * K * elt || r.b_bytes != size_t(r.cout) * 4)
+            const char* nm = op.name.c_str();
+            if (r.relu & ~(kConvRelu | kFcStream)) return fail(B2_EINVAL, "plan: fc %s: unknown flags 0x%x", nm, r.relu);
+            if ((r.relu & kConvRelu) && !(r.relu & kFcStream))
+                return fail(B2_EINVAL, "plan: fc %s: a fused ReLU exists on streaming (kFcStream) FC layers only", nm);
+            if (r.relu & kFcStream) {  // plan_format.h, kFcStream
+                if (!v4 || h.precision != B2_PREC_FP16)
+                    return fail(B2_EINVAL, "plan: fc %s: a streaming FC layer needs a version-4 fp16 plan", nm);
+                if (ti.kind != T_ACT || ti.scale != 0.f || ti.binding >= 0)
+                    return fail(B2_EINVAL, "plan: fc %s: a streaming FC layer reads an fp16 activation", nm);
+                if (K == 0 || K % 64)
+                    return fail(B2_EINVAL, "plan: fc %s: K = h * w * c_phys = %zu of its input is not a multiple of 64", nm, K);
+                const uint32_t cout_phys = (r.cout + 127) / 128 * 128;
+                if (r.cout == 0 || r.cout_phys != cout_phys || r.w_bytes != size_t(cout_phys) * K * 2 || r.b_bytes != size_t(cout_phys) * 4)
+                    return fail(B2_EINVAL, "plan: fc %s: weights must be %u x %zu fp16 and the bias %u fp32 (cout_phys = cout %u rounded up to "
+                                "128, record says %u)", nm, cout_phys, K, cout_phys, r.cout, r.cout_phys);
+                if (to.kind == T_ACT ? (to.h != 1 || to.w != 1 || to.c != r.cout || to.c_phys != (r.cout + 63) / 64 * 64 || to.scale != 0.f ||
+                                        to.binding >= 0 || r.in == r.out)
+                                     : to.c != r.cout)
+                    return fail(B2_EINVAL, "plan: fc %s: the output is an fp32 [%u] vector or an fp16 [1, 1, %u] arena activation with c_phys "
+                                "%u", nm, r.cout, r.cout, (r.cout + 63) / 64 * 64);
+                const FcStreamGeom g = fc_stream_geom(int(h.max_batch), int(cout_phys), int(K / 64));
+                if (g.tiles * g.chunks > kMaxSplitTiles)
+                    return fail(B2_EINVAL, "plan: fc %s: %d output tiles at max batch, more than the %d arrival counters", nm,
+                                g.tiles * g.chunks, kMaxSplitTiles);
+            } else if (r.w_bytes != size_t(r.cout) * K * elt || r.b_bytes != size_t(r.cout) * 4)
                 return fail(B2_EINVAL, "plan: fc %s weight size mismatch", op.name.c_str());
             e->flops_per_item += 2.0 * ti.h * ti.w * ti.c * r.cout;
         } else if (r.type == OP_LRN) {
@@ -948,8 +1003,16 @@ void plan_arena(b2_engine* e) {
         top = std::max(top, off + size);
     }
     e->act_bytes = align_up(std::max<size_t>(top, 1024), 1024);
-    // fp16 engines reserve a fixed split-K workspace behind the activations (partial fp32 tiles)
-    e->arena_bytes = e->act_bytes + (e->half() ? kSplitWorkspaceBytes : 0);
+    // fp16 engines reserve a fixed split-K workspace behind the activations (partial fp32 tiles), grown where a streaming
+    // FC layer's partial tiles need more
+    size_t ws = e->half() ? kSplitWorkspaceBytes : 0;
+    for (const Op& op : e->ops)
+        if (op.r.type == b2plan::OP_FC && (op.r.relu & b2plan::kFcStream)) {
+            const Tensor& ti = e->tensors[size_t(op.r.in)];
+            const FcStreamGeom g = fc_stream_geom(e->max_batch, int(op.r.cout_phys), int(size_t(ti.h) * ti.w * ti.c_phys / 64));
+            ws = std::max(ws, align_up(fc_stream_workspace_bytes(g), 1024));
+        }
+    e->arena_bytes = e->act_bytes + ws;
 }
 
 // ---- tensor maps ------------------------------------------------------------------------------
@@ -1998,6 +2061,32 @@ int build_plan(b2_context* c, int batch, Plan** out) {
             case b2plan::OP_FC: {
                 const Tensor& ti = e->tensors[r.in];
                 const Tensor& to = e->tensors[r.out];
+                if (r.relu & b2plan::kFcStream) {
+                    const int K = int(ti.h * ti.w * ti.c_phys);
+                    const FcStreamGeom g = fc_stream_geom(e->max_batch, int(r.cout_phys), K / 64);
+                    b2k::FcStreamLaunch& f = L.fc;
+                    L.kind = L_FC_STREAM;
+                    L.out_binding = to.kind == b2plan::T_VEC ? to.binding : -1;
+                    L.out = tptr(r.out);
+                    L.K = K, L.Cout = int(r.cout);
+                    f.nb = g.nb, f.tiles = g.tiles, f.chunks = (batch + g.nb - 1) / g.nb;
+                    if (!b2k::fc_stream_smem_bytes(f.nb)) return fail(B2_EINVAL, "fc %s: no kernel for %d batch columns", op.name.c_str(), f.nb);
+                    int rc = make_map_2d(&f.mapX, tptr(r.in), uint64_t(K), uint64_t(batch), 64, uint32_t(g.nb), CU_TENSOR_MAP_SWIZZLE_128B);
+                    if (rc) return rc;
+                    f.w = e->d_payload + r.w_off;
+                    f.out = L.out;
+                    f.workspace = reinterpret_cast<float*>(c->scratch + e->act_bytes);
+                    f.counters = c->d_counters;
+                    b2k::FcStreamArgs& a = f.args;
+                    a.bias = reinterpret_cast<const float*>(e->d_payload + r.b_off);
+                    a.N = batch, a.Cout = int(r.cout), a.cout_phys = int(r.cout_phys);
+                    a.out_half = to.kind == b2plan::T_ACT, a.out_pitch = a.out_half ? int(to.c_phys) : int(r.cout);
+                    a.relu = int(r.relu & b2plan::kConvRelu);
+                    a.splits = g.splits, a.num_kblocks = K / 64;
+                    L.flops = 2.0 * batch * ti.h * ti.w * ti.c * r.cout;
+                    L.bytes = double(r.w_bytes) + double(batch) * (ti.item_bytes + to.item_bytes);
+                    break;
+                }
                 L.kind = L_FC;
                 L.in = tptr(r.in);
                 L.out = tptr(r.out);
@@ -2217,6 +2306,11 @@ int run_launch(const b2_engine* e, const Launch& L, void* const* bindings, cudaS
         case L_CLS_HEAD:
             return b2k::launch_cls_head(static_cast<const __half*>(in), static_cast<const __half*>(L.w), L.bias, static_cast<float*>(out), L.N,
                                         L.W, L.C, L.Cout, L.eps, L.pos_map, s);
+        case L_FC_STREAM: {
+            b2k::FcStreamLaunch f = L.fc;
+            f.out = out;
+            return b2k::launch_fc_stream(f, s);
+        }
     }
     return int(cudaErrorInvalidValue);
 }
@@ -2275,6 +2369,9 @@ bool patch_layout(const b2_engine* e, const Launch& L, BindPatch* p) {
             return true;
         case L_CLS_HEAD:                                                    // cls_head_kernel(x, w, gbb, out, N, S, C, classes, eps, pos_map)
             p->n_params = 10, p->slots = {{3, L.out_binding}};
+            return true;
+        case L_FC_STREAM:                                                   // fc_stream_f16_wgmma(mapX, w, out, workspace, counters, args)
+            p->n_params = 6, p->slots = {{2, L.out_binding}};
             return true;
         default:
             return false;
@@ -2935,8 +3032,8 @@ const char* b2_context_launch_name(b2_context* c, int batch, int i) {
     static const char* kinds[] = {"input_cast", "conv_tcgen05", "conv_simt", "maxpool", "avgpool", "fc", "softmax", "output_cast", "tail_pool_fc_softmax",
                                   "quantize", "conv_i8_tcgen05", "avgpool_i8", "output_cast_i8", "embed_ln", "layernorm", "attention_f16_wgmma",
                                   "pooler", "output_cast_rows", "output_unpack_rows", "quantize_f8", "conv_f8_tcgen05", "avgpool_f8",
-                                  "output_cast_f8", "patchify", "tokens", "cls_head", "lrn", "avgpool_bnrelu"};
-    static_assert(sizeof(kinds) / sizeof(kinds[0]) == L_AVGPOOL_PRE + 1, "kinds[] is indexed by LKind");
+                                  "output_cast_f8", "patchify", "tokens", "cls_head", "lrn", "avgpool_bnrelu", "fc_stream_f16_wgmma"};
+    static_assert(sizeof(kinds) / sizeof(kinds[0]) == L_FC_STREAM + 1, "kinds[] is indexed by LKind");
     s = std::string(kinds[L->kind]) + (L->kind == L_ATTENTION && L->attn.S > 128 ? "_ks" : "") +  // key-split kernel
         (L->kind == L_ATTENTION && L->attn.seq_off ? "_varlen" : "") + ":" + L->name;         // variable-length kernel
     if (L->kind == L_ATTENTION && L->attn.S != L->W) s += " sk=" + std::to_string(L->attn.S);  // kernel of a longer sequence
@@ -2953,6 +3050,7 @@ const char* b2_context_launch_name(b2_context* c, int batch, int i) {
              ((L->conv.args.relu & b2plan::kConvGelu) ? " gelu" : "") + (L->conv.args.live ? " live" : "") +
              (L->conv.args.pre ? " pre" : "") +
              (L->cw ? " c0=" + std::to_string(L->c0) + " cw=" + std::to_string(L->cw) : std::string());
+    if (L->kind == L_FC_STREAM) s += " splits=" + std::to_string(L->fc.args.splits) + " nb=" + std::to_string(L->fc.nb);
     if (L->kind == L_CONV_I8 || L->kind == L_CONV_F8)
         s += " bn=" + std::to_string(L->i8.bn) + " st=" + std::to_string(L->i8.stages) + (L->i8.args.a_mode == b2k::A_TILED ? " tiled" : " im2col") + " grid=" +
              std::to_string(L->i8.grid_n) + "x" + std::to_string(L->i8.grid_m) + " kblk=" + std::to_string(L->i8.args.num_kblocks) +

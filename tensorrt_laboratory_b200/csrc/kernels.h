@@ -211,6 +211,32 @@ int launch_fc(const void* in, const void* w, const float* bias, float* out, int 
               bool half_storage, cudaStream_t stream);
 int launch_softmax(const float* in, float* out, int N, int C, cudaStream_t stream);
 
+// Weight-streaming split-K FC on the tensor cores (fc_kernels.cu, plan_format.h kFcStream): out[n][o] = act(b[o] +
+// sum_k W[o][k] x[n][k]) for 128 neurons x NB batch columns per CTA (grid: Cout_phys/128 x splits x column chunks)
+constexpr int kFcStages = 8;  // shared-memory ring depth (16 KiB of weights + NB x 128 B of x per stage)
+struct FcStreamArgs {
+    const float* bias;  // [cout_phys] fp32
+    int N;              // batch rows of x (rows >= N are zero-filled by the map and never stored)
+    int Cout;           // real output neurons (fp32 output row pitch)
+    int cout_phys;      // weight rows, a multiple of 128
+    int out_pitch;      // fp16 output: channels per row (c_phys; rows [Cout, c_phys) are written as 0)
+    int out_half;       // 1: fp16 activation output, 0: fp32 vector
+    int relu;
+    int splits;         // split-K factor (gridDim.y); split s covers 64-K blocks [s num_kblocks / splits, (s + 1) ...)
+    int num_kblocks;    // K / 64
+};
+struct FcStreamLaunch {
+    CUtensorMap mapX;   // x as 2-D tiled [N rows, K], box 64 x NB, SWIZZLE_128B
+    const uint8_t* w;   // pack_weights_sw128 blocks [K/64][cout_phys/32][32][128 B]
+    void* out;
+    float* workspace;   // splits > 1: [tile][split][128][NB] fp32 partial tiles
+    int* counters;      // splits > 1: one arrival counter per (column chunk, tile), zero between launches
+    FcStreamArgs args;
+    int nb, tiles, chunks;  // NB (8 ... 64, step 8), cout_phys / 128, ceil(N / NB)
+};
+int fc_stream_smem_bytes(int nb);  // 0: no instantiation for this NB
+int launch_fc_stream(const FcStreamLaunch& L, cudaStream_t stream);
+
 // global average pool + FC + bias + softmax in one launch (fp16 engines; tail_f16_kernel in kernels.cu)
 struct TailArgs {
     const __half* in;     // [N][HW][C] NHWC activations

@@ -24,7 +24,7 @@ enum OpType : uint32_t {
     OP_CONV = 1,         // conv + folded BN/Scale bias (+ residual) (+ ReLU)
     OP_MAXPOOL = 2,
     OP_AVGPOOL = 3,      // global average pool (version 4: also k x k / stride k, with a BatchNorm + ReLU prologue)
-    OP_FC = 4,           // inner product -> fp32 vector
+    OP_FC = 4,           // inner product -> fp32 vector (version 4, kFcStream: also -> fp16 activation [1, 1, cout])
     OP_SOFTMAX = 5,      // fp32 vector -> fp32 vector
     OP_OUTPUT_CAST = 6,  // NHWC activation tensor -> fp32 NCHW binding (dequantised when the tensor is int8 / e4m3)
     OP_QUANTIZE = 7,     // fp16 NHWC tensor -> 1-byte NHWC tensor (INT8 / FP8 engines: in front of the first 1-byte convolution)
@@ -194,6 +194,17 @@ struct OpRecV3 {  // 224 bytes
     uint8_t reserved[8];
 };
 enum : uint32_t { kConvRelu = 1, kConvPacked = 2, kConvInt8 = 4, kConvGelu = 8, kConvPreAct = 16 };
+// kFcStream (`relu` bit 5, OP_FC, version-4 fp16 plans): a streaming FC layer on the tensor cores (fc_stream_f16_wgmma).
+//   Input: an fp16 arena activation, K = h * w * c_phys a multiple of 64, read in (h, w, c) order.  w = fp16 [cout_phys, K]
+//   laid out by builder.pack_weights_sw128 (blocks [K/64][cout_phys/32][32 rows][128 B]), cout_phys = cout rounded up to
+//   128, rows >= cout zero; b = fp32 [cout_phys], zeros past cout.  `relu` bit 0 (kConvRelu) = fused ReLU, legal only with
+//   this flag.  Output: an fp32 T_VEC [cout] (logits), or an fp16 arena T_ACT h = w = 1, c = cout, c_phys = cout rounded up
+//   to 64, whose channels [cout, c_phys) are written as 0.
+//   Numerics: fp16 operands, fp32 tensor-core accumulation in K order within a split; the splits' fp32 partials added in
+//   split order; then + bias, then ReLU, in fp32; one rounding (fp16 for a T_ACT output).  The split count is a function
+//   of the shapes at max batch (engine.cu, fc_stream_geom) and is the same at every batch size.
+//   Any other `relu` bit of an FC is refused, and so is bit 0 without kFcStream.
+enum : uint32_t { kFcStream = 32 };
 enum : uint32_t { kOpRowsOut = 1, kOpPacked = 2 };  // OpRecV3::flags
 struct BindingRec {  // 128 bytes
     char name[64];

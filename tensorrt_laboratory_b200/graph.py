@@ -381,6 +381,40 @@ def densenet_caffe(depth: int = 121) -> dict:
     return {"name": f"DenseNet-{depth}", "input": "data", "input_dims": [1, 3, 224, 224], "layers": L}
 
 
+# VGG (Simonyan and Zisserman, "Very Deep Convolutional Networks for Large-Scale Image Recognition", configurations D
+# and E): 3x3 convolutions per block, each block followed by a 2x2 / 2 max pool
+_VGG_BLOCKS = {16: (2, 2, 3, 3, 3), 19: (2, 2, 4, 4, 4)}
+_VGG_WIDTHS = (64, 128, 256, 512, 512)
+
+
+def vgg_caffe(depth: int = 16) -> dict:
+    """The raw layer list of VGG-{16,19}'s Caffe deploy net (``VGG_ILSVRC_{16,19}_layers_deploy.prototxt``) under its layer
+    names, so that ``VGG_ILSVRC_{16,19}_layers.caffemodel`` loads by name: ``conv{b}_{l}`` (3x3, pad 1, stride 1, bias)
+    with ``relu{b}_{l}`` in place, ``pool{b}`` (MAX 2x2 / 2) after each block, then ``fc6`` (4096), ``relu6``, ``drop6``,
+    ``fc7`` (4096), ``relu7``, ``drop7``, ``fc8`` (1000) and ``prob``.  Input 3 x 224 x 224."""
+    if depth not in _VGG_BLOCKS:
+        raise ValueError(f"unsupported VGG depth {depth} (16 or 19)")
+    L: List[dict] = []
+    prev = "data"
+    for b, (n, c) in enumerate(zip(_VGG_BLOCKS[depth], _VGG_WIDTHS), 1):
+        for l in range(1, n + 1):
+            name = f"conv{b}_{l}"
+            L.append(dict(name=name, type="Convolution", bottoms=[prev], tops=[name], num_output=c, kernel_size=3, pad=1, stride=1,
+                          bias_term=True))
+            L.append(dict(name=f"relu{b}_{l}", type="ReLU", bottoms=[name], tops=[name]))
+            prev = name
+        L.append(dict(name=f"pool{b}", type="Pooling", bottoms=[prev], tops=[f"pool{b}"], pool="MAX", kernel_size=2, stride=2, pad=0))
+        prev = f"pool{b}"
+    for i, c in ((6, 4096), (7, 4096), (8, 1000)):
+        L.append(dict(name=f"fc{i}", type="InnerProduct", bottoms=[prev], tops=[f"fc{i}"], num_output=c, bias_term=True))
+        prev = f"fc{i}"
+        if i < 8:
+            L.append(dict(name=f"relu{i}", type="ReLU", bottoms=[prev], tops=[prev]))
+            L.append(dict(name=f"drop{i}", type="Dropout", bottoms=[prev], tops=[prev]))
+    L.append(dict(name="prob", type="Softmax", bottoms=[prev], tops=["prob"]))
+    return {"name": f"VGG_ILSVRC_{depth}_layers", "input": "data", "input_dims": [1, 3, 224, 224], "layers": L}
+
+
 # --------------------------------------------------------------------------------------------------
 # shape inference on raw layers
 # --------------------------------------------------------------------------------------------------
@@ -589,14 +623,21 @@ def lower(net: dict, weights: Optional[dict] = None) -> dict:
             preact[L["bottoms"][0]]["relu"] = True
         elif t == "ReLU":
             op = producer[L["bottoms"][0]]
-            if op["type"] != OP_CONV:
+            if op["type"] == OP_SOFTMAX:
+                raise ValueError(f"ReLU {name}: a ReLU on the output of Softmax {op['name']} is not supported")
+            if op["type"] not in (OP_CONV, OP_FC):
                 raise ValueError(f"ReLU {name}: only conv-fused ReLU is supported")
+            if op["type"] == OP_FC and op.get("_sealed"):
+                raise ValueError(f"ReLU {name}: InnerProduct {op['name']} already has a fused ReLU")
             op["relu"] = True
             op["_sealed"] = True
         elif t == "Eltwise":
             if L.get("operation", "SUM") != "SUM" or len(L["bottoms"]) != 2:
                 raise ValueError(f"Eltwise {name}: only 2-input SUM is supported")
             a, b = L["bottoms"]
+            for x in (a, b):
+                if producer.get(x, {}).get("type") == OP_FC:
+                    raise ValueError(f"Eltwise {name}: InnerProduct {producer[x]['name']} cannot take a residual")
             # fuse into whichever input was produced LAST by a conv that nobody else has read yet
             cand = [x for x in (a, b) if producer.get(x, {}).get("type") == OP_CONV
                     and not producer[x].get("_sealed") and x not in consumed_by_eltwise]
@@ -656,7 +697,7 @@ def lower(net: dict, weights: Optional[dict] = None) -> dict:
         elif t == "InnerProduct":
             c, h, w = tensors[L["bottoms"][0]]
             op = dict(type=OP_FC, name=name, input=L["bottoms"][0], output=L["tops"][0],
-                      cin=c * h * w, cout=L["num_output"], in_chw=(c, h, w))
+                      cin=c * h * w, cout=L["num_output"], in_chw=(c, h, w), relu=False)
             if weights is not None:
                 W = np.asarray(weights[name]["W"], dtype=np.float64).reshape(L["num_output"], c, h, w)
                 # Caffe flattens C,H,W; the engine keeps activations NHWC -> permute K to (h, w, c)
@@ -751,6 +792,12 @@ def lower(net: dict, weights: Optional[dict] = None) -> dict:
             op["output"] = phys(op["output"])
     for b in grown:
         tensors.pop(b, None)
+    # an FC whose output another FC reads is a hidden layer: an fp16 activation [C, 1, 1] in fp16 plans (the reader's K
+    # order (h, w, c) is then the channel order); the last FC stays an fp32 vector
+    fc_inputs = {op["input"] for op in ops if op["type"] == OP_FC}
+    for op in ops:
+        if op["type"] == OP_FC:
+            op["hidden"] = op["output"] in fc_inputs
     for op in ops:
         if op["type"] == OP_CONV and "_w" in op:
             op["W"] = np.ascontiguousarray(op.pop("_w").transpose(0, 2, 3, 1)).astype(np.float32)  # OHWI

@@ -129,6 +129,9 @@ def quantize_lowered(lowered: dict, calib_inputs: np.ndarray, amax: Optional[Dic
     qmax = E4M3_MAX if fp8 else QMAX
     from .builder import grouped_1byte_span
     for op in lowered["ops"]:
+        if op["type"] == G.OP_FC and op.get("relu"):
+            raise ValueError(f"fc {op['name']}: an InnerProduct with a fused ReLU builds in fp16 only; {name} hidden "
+                             "fully-connected layers are not supported")
         if "out_c0" in op or op["type"] == G.OP_LRN:
             raise ValueError(f"{op['name']}: a graph with a Concat or LRN layer builds in fp16 only; {name} channel "
                              "concatenation and LRN are not supported")

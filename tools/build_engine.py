@@ -16,6 +16,8 @@ examples/ONNX/resnet50/build.py:35-67).
   python tools/build_engine.py --model googlenet --batch 8 [--caffemodel bvlc_googlenet.caffemodel] --tune -o googlenet.plan  (fp16)
   python tools/build_engine.py --model densenet121 --batch 8 [--caffemodel F | --weights tv.npz] --tune -o densenet.plan  (fp16;
       also densenet169 / densenet201; --weights: a torchvision densenetNNN state_dict saved as .npz)
+  python tools/build_engine.py --model vgg16 --batch 8 [--caffemodel VGG_ILSVRC_16_layers.caffemodel | --weights tv.npz] --tune
+      -o vgg16.plan  (fp16; also vgg19; --weights: a torchvision vggNN state_dict saved as .npz)
 Weights: deterministic synthetic weights (the reference's benchmark engines are weightless too, models/README.md:6-7),
 unless --caffemodel names a binary NetParameter (trtexec --model=...); MNIST and --onnx carry their own weights.
 --precision int8 / fp8: post-training quantization (fp8: E4M3), max-abs calibration on --calib (an .npy [N,C,H,W] fp32) or on
@@ -35,10 +37,10 @@ from tensorrt_laboratory_b200 import builder, graph, weights  # noqa: E402
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--model", choices=["resnet50", "resnet152", "resnext50", "mnist", "bert-base", "vit-b16", "vit-b32", "vit-l16", "googlenet",
-                                        "densenet121", "densenet169", "densenet201"])
+                                        "densenet121", "densenet169", "densenet201", "vgg16", "vgg19"])
     ap.add_argument("--seq", type=int, default=128, help="bert-base: the sequence length of the plan (64, 128, 256, 384 or 512)")
     ap.add_argument("--weights", help="bert-base / vit-*: .npz of Hugging Face BertModel / ViTForImageClassification parameters; "
-                                        "densenet*: .npz of a torchvision state_dict (default: seeded weights)")
+                                        "densenet* / vgg*: .npz of a torchvision state_dict (default: seeded weights)")
     ap.add_argument("--remove-padding", action="store_true",
                     help="bert-base: a packed plan that computes only the tokens with input_mask != 0 (same bindings)")
     ap.add_argument("--prototxt")
@@ -92,6 +94,15 @@ def main():
         if a.weights:
             from tensorrt_laboratory_b200 import densenet
             wts = densenet.load_weights(a.weights, int(a.model[8:]))
+        else:
+            wts = weights_for(net)
+    elif a.model in ("vgg16", "vgg19"):  # hidden FC layers on the streaming tensor-core FC kernel, fp16 only
+        net = graph.vgg_caffe(int(a.model[3:]))
+        if prec != builder.PREC_FP16:
+            raise SystemExit("VGG builds in fp16 only")
+        if a.weights:
+            from tensorrt_laboratory_b200 import vgg
+            wts = vgg.load_weights(a.weights, int(a.model[3:]))
         else:
             wts = weights_for(net)
     elif a.model == "resnext50":  # 32x4d: grouped 3x3 convolutions, cpg 4 ... 32 (every precision)
