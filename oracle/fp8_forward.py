@@ -10,7 +10,8 @@ itself continues from the exact ``A``.
 Rounding contract (every ``fl`` / ``fma`` is one IEEE fp32 operation, round-to-nearest-even; ``e4m3`` rounds to nearest
 even and saturates to +-448):
     quantize   q = e4m3(fl(h * inv_s))                                           h: the fp16 value as fp32
-    conv       t = fma(fl32(acc), m[c], b[c]);  t = fma(float(q_res), r, t);  t = max(t, 0);  q = e4m3(t)
+    conv       t = fma(fl32(acc), m[c], b[c]);  t = fma(float(q_res), r, t);  t = fmax(t, 0);  q = e4m3(t)
+               (fmax under ReLU only: it takes 0 for a NaN t, which without ReLU stays NaN and becomes a NaN code)
     avg pool   h = fp16(fl(sum * k)),  the values summed in fp32 in pixel order
     output     y = fl(float(q) * s)                                              (FP8 tensor exposed as fp32 binding)
 """
@@ -61,7 +62,7 @@ def requant(acc: np.ndarray, op: dict, res_q: Optional[np.ndarray]) -> np.ndarra
     if res_q is not None:
         t = fma32(value(res_q), np.broadcast_to(f32(op["r"]), acc.shape), t)
     if op["relu"]:
-        t = np.maximum(t, f32(0))
+        t = np.fmax(t, f32(0))  # CUDA's fmaxf: NaN -> 0
     return e4m3(t)
 
 

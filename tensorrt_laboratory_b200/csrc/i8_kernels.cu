@@ -18,7 +18,8 @@
 //
 // FP8 (E4M3) kernels, the same layouts with E4M3 codes in place of int8 values:
 //  * conv_f8_tcgen05<BN> -- the same kernel body (conv_1byte_tile<F8 = true>): wgmma 64 x BN x 32 e4m3 x e4m3 -> f32, then
-//        t = fma(acc, m[c], b[c]);  t = fma(float(q_res), r, t);  t = max(t, 0);  q = e4m3(t)  (RNE, saturating to +-448)
+//        t = fma(acc, m[c], b[c]);  t = fma(float(q_res), r, t);  t = fmax(t, 0) under ReLU only;  q = e4m3(t)  (RNE,
+//        saturating to +-448; a NaN accumulator stays NaN without ReLU)
 //  * quantize_h_to_f8_kernel, avgpool_f8_kernel (fp32 sums in pixel order), output_cast_f8_kernel
 #include <cmath>
 #include <type_traits>
@@ -230,9 +231,10 @@ __device__ __forceinline__ void conv_1byte_tile(const CUtensorMap& mapA, const C
         if (has_res) mbar_wait(res_bar, 0);
         const int row0 = 64 * ((warp - 4) >> 2) + 16 * ((warp - 4) & 3) + (lane >> 2);
         const float r = p.r;
-        // q = clip(rint(max(t, relu ? 0 : -inf)), -127, 127): the lower clamp and the ReLU are ONE fp32 max before the
-        // conversion (rint is monotonic and rint(-127) = -127).  FP8 has no lower clamp before its saturating conversion.
-        const float lo = p.relu != 0 ? 0.0f : (F8 ? -INFINITY : -127.0f);
+        // q = clip(rint(max(t, relu ? 0 : -127)), -127, 127): the lower clamp and the ReLU are ONE fp32 max before the
+        // conversion (rint is monotonic and rint(-127) = -127).  FP8 has no lower clamp before its saturating conversion:
+        // without ReLU its bound is NaN, which fmaxf ignores, so a NaN t stays NaN (a bound of -inf would make it -448).
+        const float lo = p.relu != 0 ? 0.0f : (F8 ? __int_as_float(0x7fffffff) : -127.0f);
 #pragma unroll
         for (int j = 0; j < BN / 8; ++j) {
 #pragma unroll
@@ -242,7 +244,8 @@ __device__ __forceinline__ void conv_1byte_tile(const CUtensorMap& mapA, const C
                 const uint32_t so = static_cast<uint32_t>((col >> 7) * (128 * 128)) + swz_off<128>(row, (col & 127) >> 4) + (col & 15);
                 uint16_t packed = 0;  // padding channels (col >= nv): zero by construction
                 if constexpr (F8) {
-                    // t = fma(acc, m[c], b[c]);  t = fma(float(q_res), r, t);  t = max(t, 0);  q = e4m3(t), satfinite RNE.
+                    // t = fma(acc, m[c], b[c]);  t = fma(float(q_res), r, t);  [t = fmax(t, 0)];  q = e4m3(t), satfinite
+                    // RNE (NaN -> NaN, |t| >= 464 -> +-448).
                     if (col < nv) {
                         float2 rf = make_float2(0.f, 0.f);
                         if (has_res) rf = e4m3x2_to_float2(*reinterpret_cast<const uint16_t*>(sRes + so));

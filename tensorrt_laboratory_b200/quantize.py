@@ -32,8 +32,12 @@ subnormals kept, largest value 448) in place of int8 values.  ``e4m3()`` is roun
   * epilogue: INT8's, except for the last step
         t = fma(acc, m[c], b[c])                      m[c] = fl(s_in * s_w[c] / s_out),  b[c] = fl(bias[c] / s_out)
         t = fma(float(q_res), r, t)                   r = fl(s_res / s_out)                      (fused residual)
-        t = max(t, 0)                                                                           (fused ReLU)
+        t = fmax(t, 0)                                                                          (fused ReLU)
         q_out = e4m3(t)                               padding output channels are code 0x00
+    The max is taken under ReLU only: without it a NaN t stays NaN and becomes a NaN code (0x7F / 0xFF), with it
+    fmax gives 0, as CUDA's fmaxf does in every fp16 epilogue.  The quantize op maps NaN to a NaN code and +-inf to
+    +-448.  Measured on an H100: the e4m3 tensor-core MMA gives NaN for NaN x 0 and keeps subnormal operands, so a NaN
+    input reaches every output whose window holds it (tests/test_gpu_fp8_values.py);
   * average pool: each code converted to fp32 and summed in fp32 in pixel order, ``h = fp16(fl(sum * fl(s / HW)))`` (the
     sum is exact for HW < 73: E4M3 values are multiples of 2^-9 and at most 448);
   * output cast of an FP8 tensor to an fp32 binding: ``y = fl(float(q) * s)``.

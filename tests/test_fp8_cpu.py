@@ -77,8 +77,8 @@ def test_e4m3_matches_a_bit_level_encoder():
 
 
 def test_epilogue_contract_on_chosen_accumulators():
-    """t = fma(fl32(acc), m, b); t = fma(value(q_res), r, t); t = max(t, 0); q = e4m3(t): ties, saturation, ReLU, the
-    residual, and accumulators above 2^24 (rounded to fp32 before the multiply-add)."""
+    """t = fma(fl32(acc), m, b); t = fma(value(q_res), r, t); t = fmax(t, 0) under ReLU; q = e4m3(t): ties, saturation,
+    ReLU, the residual, accumulators above 2^24 (rounded to fp32 before the multiply-add), and NaN."""
     f = np.float32
     op = dict(m=np.array([1.0, 1.0, 1.0, 2.0 ** -20, 1.0], f), b=np.array([0.0, 0.0, -1000.0, 0.0, 0.0], f), r=f(0.5), relu=False)
     #           1.0625 (tie -> 1.0), 1.1875 (tie -> 1.25), saturates at -448, 2^25 + 1 -> fp32 2^25 -> 32, 500 -> 448
@@ -89,6 +89,13 @@ def test_epilogue_contract_on_chosen_accumulators():
     op["relu"] = True
     np.testing.assert_array_equal(O8.value(O8.requant(-acc, op, None)).ravel(), [0.0, 0.0, 0.0, 0.0, 0.0])
     np.testing.assert_array_equal(O8.value(O8.requant(-acc, op, res)).ravel(), [0.0, 0.0, 0.0, 0.0, 0.0])
+    # NaN: kept without ReLU (a NaN code), 0 with it (fmaxf takes the number)
+    nan = np.full((1, 5, 1, 1), np.nan)
+    op["relu"] = False
+    assert (O8.requant(nan, op, None) & 0x7F == 0x7F).all() and (O8.requant(nan, op, res) & 0x7F == 0x7F).all()
+    op["relu"] = True
+    np.testing.assert_array_equal(O8.value(O8.requant(nan, op, None)).ravel(), [0.0] * 5)
+    np.testing.assert_array_equal(O8.value(O8.requant(nan, op, res)).ravel(), [0.0] * 5)
 
 
 def test_avgpool_contract():
