@@ -14,6 +14,8 @@ Semantics restated (Caffe, as consumed by the reference through ``models/ResNet-
     windows are clipped to the image (-inf padding)                                   (prototxt lines 48-58: 3x3/2)
   * Pooling AVE, global 7x7: arithmetic mean over the window                          (prototxt lines 2292-2302)
   * Eltwise SUM, ReLU, InnerProduct, Softmax over channels.
+  * GoogLeNet's LRN (ACROSS_CHANNELS):    y_c = x_c (k + alpha / n sum_{|j - c| <= (n - 1) / 2} x_j^2)^(-beta);
+    Concat over channels; Dropout as the identity.
 """
 from __future__ import annotations
 
@@ -81,6 +83,18 @@ def avgpool_global(x):
     return x.astype(np.float64).sum(axis=(2, 3), keepdims=True) / float(x.shape[2] * x.shape[3])
 
 
+def lrn(x, n, alpha, beta, k):
+    """Caffe ACROSS_CHANNELS LRN: the n-channel window zero-padded at the channel edges, the divisor always n."""
+    h = (n - 1) // 2
+    c = x.shape[1]
+    sq = np.zeros((x.shape[0], c + 2 * h) + x.shape[2:], np.float64)
+    sq[:, h:h + c] = x.astype(np.float64) ** 2
+    s = np.zeros_like(x, dtype=np.float64)
+    for ch in range(c):
+        s[:, ch] = sq[:, ch:ch + n].sum(axis=1)
+    return x * (k + alpha / n * s) ** (-beta)
+
+
 def eltwise_sum(*xs):
     y = xs[0].astype(np.float64)
     for t in xs[1:]:
@@ -121,6 +135,12 @@ def forward(net: dict, weights: dict, x: np.ndarray):
                 if L["kernel_size"] != a.shape[2] or a.shape[2] != a.shape[3] or L["pad"]:
                     raise ValueError("numpy oracle: only global AVE pooling is restated")
                 y = avgpool_global(a)
+        elif t == "LRN":
+            y = lrn(a, L["local_size"], L["alpha"], L["beta"], L["k"])
+        elif t == "Concat":
+            y = np.concatenate([blobs[b] for b in L["bottoms"]], axis=1)
+        elif t == "Dropout":
+            y = a
         elif t == "Eltwise":
             y = eltwise_sum(a, *[blobs[b] for b in L["bottoms"][1:]])
         elif t == "InnerProduct":

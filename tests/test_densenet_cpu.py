@@ -9,8 +9,9 @@ import re
 import numpy as np
 import pytest
 
+from oracle.caffe_forward import caffe_forward, lowered_forward_f16emu
 from tensorrt_laboratory_b200 import builder, caffemodel, capi, densenet, graph, weights
-from tests import densenet_oracle as DO
+from tests.cnn_nets import dense_net
 from tests.test_googlenet_cpu import _records
 
 
@@ -105,7 +106,7 @@ def test_prologue_parameters_are_folded_in_float64():
 
 
 def _edit_net(fn):
-    net = DO.dense_net(layers=2)
+    net = dense_net(layers=2)
     layers = [dict(L) for L in net["layers"]]
     fn(layers)
     return dict(net, layers=layers)
@@ -186,7 +187,7 @@ def test_plan_records():
 
 
 def _mutations():
-    net = DO.dense_net(layers=3)
+    net = dense_net(layers=3)
     blob = builder.build_plan(graph.lower(net, weights.random_weights(net, 0)), builder.PREC_FP16, max_batch=2)
     _, _, ops, base = _records(blob)
     idx = {o[0].rstrip(b"\0").decode(): i for i, o in enumerate(ops)}
@@ -272,7 +273,7 @@ def test_load_weights_matches_torchvision():
     model = model.float().double()
     with torch.no_grad():
         ref = torch.softmax(model(torch.from_numpy(x)), 1).numpy()
-    got = DO.caffe_forward(net, wts, x)
+    got = caffe_forward(net, wts, x, dtype=torch.float64)
     assert float(np.abs(got - ref).max() / np.abs(ref).max()) <= 1e-10
     bad = dict(sd)
     del bad["features.denseblock3.denselayer7.norm2.running_var"]
@@ -284,12 +285,13 @@ def test_load_weights_matches_torchvision():
 
 
 def test_emulation_against_float64():
-    net = DO.dense_net(layers=3)
+    import torch
+    net = dense_net(layers=3)
     wts = weights.random_weights(net, 1)
     low = graph.lower(net, wts)
     x = weights.synthetic_input(2, chw=(3, 16, 16), seed=9)
-    ref = DO.caffe_forward(net, wts, x, logits=True)
-    emu = DO.lowered_forward_f16emu(low, x, logits=True)
+    ref = caffe_forward(net, wts, x, dtype=torch.float64, logits=True)
+    emu = lowered_forward_f16emu(low, x, logits=True)
     rel = float(np.abs(emu - ref).max() / np.abs(ref).max())
     assert 1e-5 < rel <= 3e-3, rel  # fp16 storage matters, and only that much
     assert np.array_equal(np.argmax(ref, 1), np.argmax(emu, 1))

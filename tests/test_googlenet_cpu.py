@@ -10,8 +10,10 @@ import struct
 import numpy as np
 import pytest
 
+from oracle import numpy_ops
+from oracle.caffe_forward import caffe_forward
 from tensorrt_laboratory_b200 import builder, caffemodel, capi, graph, onnx_import, onnx_lite, quantize, weights
-from tests import googlenet_oracle as GO
+from tests.cnn_nets import inception_net
 
 PROTOTXT = """
 name: "mini"
@@ -79,7 +81,7 @@ def test_concat_refusals_name_the_layer():
 
 
 def test_precisions_other_than_fp16_are_refused():
-    net = GO.inception_net(hw=7)
+    net = inception_net(hw=7)
     low = graph.lower(net, weights.random_weights(net, 0))
     for prec in (builder.PREC_FP32,):
         with pytest.raises(ValueError, match="fp16 only"):
@@ -160,7 +162,7 @@ def test_existing_plans_keep_their_bytes():
 
 # ---- hand-corrupted plans ----------------------------------------------------------------------------------------------
 def _mutations():
-    net = GO.inception_net(hw=7, widths=(16, 32, 48, 112), lrn=dict(local_size=5, alpha=1e-4, beta=0.75, k=1.0))
+    net = inception_net(hw=7, widths=(16, 32, 48, 112), lrn=dict(local_size=5, alpha=1e-4, beta=0.75, k=1.0))
     blob = builder.build_plan(graph.lower(net, weights.random_weights(net, 0)), builder.PREC_FP16, max_batch=2)
     _, _, ops, base = _records(blob)
     idx = {o[0].rstrip(b"\0").decode(): i for i, o in enumerate(ops)}
@@ -200,13 +202,13 @@ def test_corrupted_plans_are_refused():
 # ---- oracles and round trips --------------------------------------------------------------------------------------------
 def test_torch_oracle_and_numpy_witness_agree():
     import torch
-    net = GO.inception_net(cin=16, hw=9, widths=(8, 16, 8, 8), reduce=(8, 8), lrn=dict(local_size=5, alpha=0.05, beta=0.75, k=2.0))
+    net = inception_net(cin=16, hw=9, widths=(8, 16, 8, 8), reduce=(8, 8), lrn=dict(local_size=5, alpha=0.05, beta=0.75, k=2.0))
     wts = weights.random_weights(net, 4)
     x = np.random.default_rng(0).standard_normal((2, 16, 9, 9)) * 3
-    a = GO.caffe_forward(net, wts, x, dtype=torch.float64)
-    b = GO.numpy_forward(net, wts, x)
+    a = caffe_forward(net, wts, x, dtype=torch.float64)
+    b = numpy_ops.forward(net, wts, x)
     assert float(np.abs(a - b).max() / np.abs(b).max()) <= 1e-10
-    assert float(np.abs(GO.lrn_numpy(x, 5, 0.05, 0.75, 2.0) - x).max()) > 0.1  # the normalisation matters at this scale
+    assert float(np.abs(numpy_ops.lrn(x, 5, 0.05, 0.75, 2.0) - x).max()) > 0.1  # the normalisation matters at this scale
 
 
 def test_caffemodel_round_trip_gives_the_same_plan():
@@ -217,9 +219,9 @@ def test_caffemodel_round_trip_gives_the_same_plan():
 
 
 def test_onnx_round_trip_gives_the_same_oracle_outputs():
-    net = GO.inception_net(cin=16, hw=9, widths=(8, 16, 8, 8), reduce=(8, 8), lrn=dict(local_size=3, alpha=0.05, beta=0.5, k=2.0))
+    net = inception_net(cin=16, hw=9, widths=(8, 16, 8, 8), reduce=(8, 8), lrn=dict(local_size=3, alpha=0.05, beta=0.5, k=2.0))
     wts = weights.random_weights(net, 6)
     x = np.random.default_rng(1).standard_normal((2, 16, 9, 9)).astype(np.float32) * 3
     net2, wts2 = onnx_import.import_onnx(onnx_lite.parse_model(onnx_import.export_onnx(net, wts)))
-    assert np.allclose(GO.numpy_forward(net2, wts2, x), GO.numpy_forward(net, wts, x), rtol=1e-6, atol=1e-7)
+    assert np.allclose(numpy_ops.forward(net2, wts2, x), numpy_ops.forward(net, wts, x), rtol=1e-6, atol=1e-7)
     assert [L["type"] for L in net2["layers"]].count("Concat") == 1 and [L["type"] for L in net2["layers"]].count("LRN") == 1

@@ -11,8 +11,9 @@ import numpy as np
 import pytest
 import torch
 
+from oracle.caffe_forward import avgpool_pre_ref, conv_pre_emu, prologue_f32, r16
 from tensorrt_laboratory_b200 import builder, capi, graph, weights
-from tests import densenet_oracle as DO
+from tests.cnn_nets import dense_net
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -47,8 +48,8 @@ def _ulp16(v):
 
 def _terms(op, a):
     """sum |w| |a'| + |bias| of a prologue 1x1 on fp16 values a: the scale of its fp32 accumulation error."""
-    pa = DO._r16(DO.prologue_f32(a[:, :op["cin"]], op["pre_scale"], op["pre_shift"]))
-    w = DO._r16(torch.from_numpy(op["W"]).double()).permute(0, 3, 1, 2).abs()
+    pa = r16(prologue_f32(a[:, :op["cin"]], op["pre_scale"], op["pre_shift"]))
+    w = r16(torch.from_numpy(op["W"]).double()).permute(0, 3, 1, 2).abs()
     return (torch.nn.functional.conv2d(pa.abs(), w) + torch.from_numpy(op["bias"]).double().abs().view(1, -1, 1, 1)).numpy()
 
 
@@ -60,7 +61,7 @@ OPTIONS = [None, {"bn": 64}, {"bn": 128}, {"bn": 32, "stages": 2}, {"sps": 2}, {
 # 180 rows, ragged against the 128-row tile
 @pytest.mark.parametrize("cin, layers, hw, batch", [(64, 4, 16, 3), (960, 2, 12, 5)])
 def test_prologue_conv_against_the_emulation(gpu, cin, layers, hw, batch):
-    net = DO.dense_net(cin=cin, hw=hw, layers=layers)
+    net = dense_net(cin=cin, hw=hw, layers=layers)
     low = graph.lower(net, weights.random_weights(net, cin + layers))
     block = f"concat_2_{layers}"
     x1 = [o for o in low["ops"] if o.get("pre") and o["type"] == graph.OP_CONV and o["input"] == block]
@@ -72,7 +73,7 @@ def test_prologue_conv_against_the_emulation(gpu, cin, layers, hw, batch):
         out, names = _run(blob, x, opt)
         a = torch.from_numpy(out[block].astype(np.float64))
         for op in x1:
-            ref = DO.conv_pre_emu(op, a).numpy()
+            ref = conv_pre_emu(op, a).numpy()
             got = out[op["output"]]
             # 2 fp16 ulp of the result plus the worst case of K fp32 additions, K 2^-24 sum |w a| (a sum that cancels to
             # almost nothing has an error relative to its terms, not to itself)
@@ -87,7 +88,7 @@ def test_stale_channels_never_leak_into_a_prefix_read(gpu):
     # conv2_2/x1 reads [0, 96) of the block tensor (cin_phys 128); conv2_2/x2 writes [96, 128) after it.  With that slice's
     # weights overflowing to +-Inf, the second pass finds non-finite values in the channels the reader's 64-channel block
     # spans.
-    net = DO.dense_net(cin=64, hw=16, layers=3)
+    net = dense_net(cin=64, hw=16, layers=3)
     wts = weights.random_weights(net, 3)
     hot = {k: dict(v) for k, v in wts.items()}
     hot["conv2_2/x2"]["W"] = wts["conv2_2/x2"]["W"] * 1e6
@@ -108,7 +109,7 @@ def test_stale_channels_never_leak_into_a_prefix_read(gpu):
 
 @pytest.mark.parametrize("cin, layers, hw, pool, c", [(64, 3, 16, "conv2_blk/pool", 160), (128, 2, 28, "pool5", 160)])
 def test_prologue_pools_are_bit_exact(gpu, cin, layers, hw, pool, c):
-    net = DO.dense_net(cin=cin, hw=hw, layers=layers)
+    net = dense_net(cin=cin, hw=hw, layers=layers)
     low = graph.lower(net, weights.random_weights(net, 7))
     op = next(o for o in low["ops"] if o["output"] == pool)
     assert op["type"] == graph.OP_AVGPOOL and op.get("pre") and low["tensors"][op["input"]][0] == c and c % 64 == 32
@@ -117,14 +118,14 @@ def test_prologue_pools_are_bit_exact(gpu, cin, layers, hw, pool, c):
     out, names = _run(blob, x)
     src = torch.from_numpy(out[op["input"]].astype(np.float64))
     k = op["k"] if pool != "pool5" else src.shape[2]
-    ref = DO.avgpool_pre_ref(src, op["pre_scale"], op["pre_shift"], k).numpy()
+    ref = avgpool_pre_ref(src, op["pre_scale"], op["pre_shift"], k).numpy()
     assert np.array_equal(out[pool].reshape(ref.shape), ref)
     assert any(n.startswith(f"avgpool_bnrelu:{op['name']}") for n in names), names
     assert not any(n.startswith("tail_pool_fc_softmax") for n in names)
 
 
 def test_pitched_max_pool_equals_the_unpitched_one(gpu):
-    net = DO.dense_net(cin=64, hw=20, layers=2)
+    net = dense_net(cin=64, hw=20, layers=2)
     wts = weights.random_weights(net, 5)
     low = graph.lower(net, wts)
     blob = builder.build_plan(low, builder.PREC_FP16, max_batch=2, outputs=["prob", "concat_2_2"])
@@ -143,10 +144,10 @@ def _oracles(tmp_path, depth, batch):
     """float64 oracle and fp16 emulation (probabilities) of the seeded DenseNet, in a child process: their
     activations and torch's CPU thread pool should not stay in the process that times the engine later."""
     code = ("import sys, numpy as np; sys.path.insert(0, sys.argv[1]);"
-            "from tensorrt_laboratory_b200 import graph, weights; from tests import densenet_oracle as DO;"
+            "from tensorrt_laboratory_b200 import graph, weights; import torch; from oracle.caffe_forward import caffe_forward, lowered_forward_f16emu;"
             "d, b = int(sys.argv[3]), int(sys.argv[4]); net = graph.densenet_caffe(d); wts = weights.random_weights(net, 0);"
             "x = weights.synthetic_input(b, seed=77); low = graph.lower(net, wts);"
-            "np.savez(sys.argv[2], ref=DO.caffe_forward(net, wts, x), emu=DO.lowered_forward_f16emu(low, x))")
+            "np.savez(sys.argv[2], ref=caffe_forward(net, wts, x, dtype=torch.float64), emu=lowered_forward_f16emu(low, x))")
     out = tmp_path / f"oracles{depth}.npz"
     subprocess.run([sys.executable, "-c", code, ROOT, str(out), str(depth), str(batch)], check=True, timeout=1800)
     z = np.load(out)

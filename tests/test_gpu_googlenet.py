@@ -11,8 +11,10 @@ import sys
 import numpy as np
 import pytest
 
+from oracle.caffe_forward import lrn_f16emu
+from oracle.numpy_ops import lrn as lrn_numpy
 from tensorrt_laboratory_b200 import builder, capi, graph, weights
-from tests import googlenet_oracle as GO
+from tests.cnn_nets import inception_net
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -68,7 +70,7 @@ def _emu_conv(op, a):
 @pytest.mark.parametrize("widths", WIDTHS, ids=lambda w: "-".join(map(str, w)))
 @pytest.mark.parametrize("hw, batch", GEOMS, ids=lambda v: str(v))
 def test_slices_equal_the_host_concatenation(gpu, widths, hw, batch):
-    net = GO.inception_net(cin=64, hw=hw, widths=widths)
+    net = inception_net(cin=64, hw=hw, widths=widths)
     wts = weights.random_weights(net, seed=hw + batch)
     low = graph.lower(net, wts)
     split, branches = _split_net(net)
@@ -96,7 +98,7 @@ def test_slices_equal_the_host_concatenation(gpu, widths, hw, batch):
 
 
 def test_slice_launch_names_and_tactics(gpu):
-    net = GO.inception_net(cin=64, hw=14, widths=(16, 32, 48, 112))
+    net = inception_net(cin=64, hw=14, widths=(16, 32, 48, 112))
     low = graph.lower(net, weights.random_weights(net, 3))
     x = np.random.default_rng(0).standard_normal((2, 64, 14, 14)).astype(np.float32)
     blob = builder.build_plan(low, builder.PREC_FP16, max_batch=2)
@@ -112,7 +114,7 @@ def test_slice_launch_names_and_tactics(gpu):
 
 
 def test_refused_table_entry_falls_back_to_the_cost_model(gpu):
-    net = GO.inception_net(cin=64, hw=14, widths=(16, 32, 48, 112))
+    net = inception_net(cin=64, hw=14, widths=(16, 32, 48, 112))
     low = graph.lower(net, weights.random_weights(net, 5))
     x = np.random.default_rng(1).standard_normal((2, 64, 14, 14)).astype(np.float32)
     blob = builder.build_plan(low, builder.PREC_FP16, max_batch=2)
@@ -129,7 +131,7 @@ def test_refused_table_entry_falls_back_to_the_cost_model(gpu):
 def test_tail_padding_is_rewritten_every_pass(gpu):
     """c = 208, c_phys = 256: a consumer reads the padding channels 208 ... 255 (with zero weights).  An overflowing request
     leaves NaN there (0 x inf); the next request must rewrite them, or the consumer's sums stay NaN."""
-    net = GO.inception_net(cin=64, hw=7, widths=(16, 32, 48, 112))
+    net = inception_net(cin=64, hw=7, widths=(16, 32, 48, 112))
     net["layers"].append(dict(name="after", type="Convolution", bottoms=["b/output"], tops=["after"], num_output=64, kernel_size=1,
                               pad=0, stride=1, bias_term=True))
     low = graph.lower(net, weights.random_weights(net, 9))
@@ -165,12 +167,12 @@ def test_lrn_against_float64(gpu, c, n, k, beta):
     y = out["norm"]
     assert any(nm.startswith("lrn:norm") for nm in names), names
     x16 = x.astype(np.float16).astype(np.float64)
-    ref = GO.lrn_numpy(x16, n, alpha, beta, k)
+    ref = lrn_numpy(x16, n, alpha, beta, k)
     assert float(np.abs(ref - x16).max()) > 1.0  # the normalisation changes the values
     # fp16 output rounding (2^-11) plus the fp32 sum and powf: within 1.5 fp16 ulp of the float64 value, edges included
     err = np.abs(y - ref) / _ulp16(ref)
     assert float(err.max()) <= 1.5, float(err.max())
-    emu = GO.lrn_f16emu(__import__("torch").from_numpy(x16), n, alpha, beta, k).numpy()
+    emu = lrn_f16emu(__import__("torch").from_numpy(x16), n, alpha, beta, k).numpy()
     assert float((np.abs(y - emu) / _ulp16(emu)).max()) <= 1.0
 
 
@@ -180,9 +182,9 @@ def _googlenet_oracles(tmp_path):
     passes hold several GB of float64 activations and start torch's CPU thread pool, none of which should stay in the
     process that goes on to time the engine."""
     code = ("import sys, numpy as np; sys.path.insert(0, sys.argv[1]);"
-            "from tensorrt_laboratory_b200 import graph, weights; from tests import googlenet_oracle as GO;"
+            "from tensorrt_laboratory_b200 import graph, weights; from oracle.caffe_forward import caffe_forward, lowered_forward_f16emu;"
             "net = graph.googlenet_caffe(); wts = weights.random_weights(net, 0); x = weights.synthetic_input(8, seed=77);"
-            "np.savez(sys.argv[2], ref=GO.caffe_forward(net, wts, x), emu=GO.lowered_forward_f16emu(graph.lower(net, wts), x))")
+            "np.savez(sys.argv[2], ref=caffe_forward(net, wts, x), emu=lowered_forward_f16emu(graph.lower(net, wts), x))")
     out = tmp_path / "oracles.npz"
     subprocess.run([sys.executable, "-c", code, ROOT, str(out)], check=True, timeout=900)
     z = np.load(out)

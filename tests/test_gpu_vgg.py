@@ -12,8 +12,9 @@ import numpy as np
 import pytest
 import torch
 
+from oracle.caffe_forward import fc_ref
 from tensorrt_laboratory_b200 import builder, capi, graph, weights
-from tests import vgg_oracle as VO
+from tests.cnn_nets import fc_net
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -40,7 +41,7 @@ def _names(s, batch):
 
 def _check_fc(op, x16, got, hidden):
     """got within 2 fp16 ulp plus the fp32 accumulation bound K 2^-23 sum |w| |x| of the float64 reference."""
-    ref, terms = VO.fc_ref(op, x16)
+    ref, terms = fc_ref(op, x16)
     err = np.abs(got - ref) / (2 * _ulp16(ref) + x16.shape[1] * 2.0 ** -23 * terms)
     assert float(err.max()) <= 1, (op["name"], float(err.max()))
     if hidden:  # fp16 values
@@ -63,13 +64,13 @@ def test_fc_stream_against_float64(gpu, chw, cout, relu):
     """Two-FC plan: fc1 (hidden, fp16 out, ReLU on or off) -> fc2 (fp32 logits, 64 neurons); single-FC plan with a ReLU
     (fp32 out).  Every batch size from one engine of max batch 64, the same bits at each batch position."""
     k = int(np.prod(chw))
-    net2 = VO.fc_net(chw, [cout, 64], [relu, False])
+    net2 = fc_net(chw, [cout, 64], [relu, False])
     low2 = graph.lower(net2, weights.random_weights(net2, k + cout))
     fc1, fc2 = low2["ops"]
     assert fc1["hidden"] and not fc2["hidden"]
     blobs = [(builder.build_plan(low2, builder.PREC_FP16, max_batch=64, outputs=["fc1", "fc2"]), True)]
     if relu:
-        net1 = VO.fc_net(chw, [cout], [True])
+        net1 = fc_net(chw, [cout], [True])
         low1 = graph.lower(net1, weights.random_weights(net1, k + cout))
         blobs.append((builder.build_plan(low1, builder.PREC_FP16, max_batch=64, outputs=["fc1"]), False))
     x = weights.synthetic_input(64, chw=chw, seed=k % 97)
@@ -111,7 +112,7 @@ def test_fc_stream_against_float64(gpu, chw, cout, relu):
 def test_fc_stream_beyond_64_columns(gpu):
     """max batch 80: NB = 64 columns per CTA and a second column chunk along the grid; every batch gives the bits of the
     full one."""
-    net = VO.fc_net((512, 7, 7), [1000, 100], [True, False])
+    net = fc_net((512, 7, 7), [1000, 100], [True, False])
     low = graph.lower(net, weights.random_weights(net, 5))
     blob = builder.build_plan(low, builder.PREC_FP16, max_batch=80, outputs=["fc1", "fc2"])
     x = weights.synthetic_input(80, chw=(512, 7, 7), seed=9)
@@ -147,10 +148,10 @@ def _oracles(tmp_path, depth, batch):
     """float64 oracle and fp16 emulation (probabilities) of the seeded VGG, in a child process: their activations and
     torch's CPU thread pool should not stay in the process that times the engine later."""
     code = ("import sys, numpy as np; sys.path.insert(0, sys.argv[1]);"
-            "from tensorrt_laboratory_b200 import graph, weights; from tests import vgg_oracle as VO;"
+            "from tensorrt_laboratory_b200 import graph, weights; import torch; from oracle.caffe_forward import caffe_forward, lowered_forward_f16emu;"
             "d, b = int(sys.argv[3]), int(sys.argv[4]); net = graph.vgg_caffe(d); wts = weights.random_weights(net, 0);"
             "x = weights.synthetic_input(b, seed=77); low = graph.lower(net, wts);"
-            "np.savez(sys.argv[2], ref=VO.caffe_forward(net, wts, x), emu=VO.lowered_forward_f16emu(low, x))")
+            "np.savez(sys.argv[2], ref=caffe_forward(net, wts, x, dtype=torch.float64), emu=lowered_forward_f16emu(low, x))")
     out = tmp_path / f"oracles{depth}.npz"
     subprocess.run([sys.executable, "-c", code, ROOT, str(out), str(depth), str(batch)], check=True, timeout=1800)
     z = np.load(out)

@@ -58,6 +58,15 @@ def test_f16_emulation_is_close_to_fp32():
     assert 0 < helpers.rel_err(emu, ref) < 5e-3
 
 
+def test_f16_emulation_refuses_a_grouped_conv():
+    """The emulation restates dense convolutions only; a grouped one raises instead of running as if dense."""
+    _, _, low = helpers.conv_case(64, 8, 8, 64, 3, 1, 1, relu=True)
+    op = low["ops"][0]
+    grouped = dict(low, ops=[dict(op, groups=2, W=op["W"][..., :32])])
+    with pytest.raises(ValueError, match="has 2 groups"):
+        lowered_forward_f16emu(grouped, np.zeros((1, 64, 8, 8), np.float32))
+
+
 def test_caffe_ceil_pooling_matches_definition():
     net = {"name": "p", "input": "data", "input_dims": [1, 1, 6, 6],
            "layers": [dict(name="pool", type="Pooling", bottoms=["data"], tops=["pool"], pool="MAX",

@@ -11,8 +11,9 @@ import numpy as np
 import pytest
 import torch
 
+from oracle.caffe_forward import caffe_forward, lowered_forward_f16emu
 from tensorrt_laboratory_b200 import bert, builder, capi, graph, onnx_import, onnx_lite, quantize, vgg, vit, weights
-from tests import vgg_oracle as VO
+from tests.cnn_nets import fc_net
 
 
 def _records(blob):
@@ -57,7 +58,7 @@ def test_fc_relu_fuses_and_hidden_outputs_are_fp16():
     assert [(fcs[n]["relu"], fcs[n]["hidden"]) for n in ("fc6", "fc7", "fc8")] == [(True, True), (True, True), (False, False)]
     assert fcs["fc7"]["in_chw"] == (4096, 1, 1) and fcs["fc8"]["in_chw"] == (4096, 1, 1)
     assert len(low["ops"]) == 22 and not any(o["type"] == "relu" for o in low["ops"])
-    net = VO.fc_net((64, 2, 2), [100, 10], [True, False])
+    net = fc_net((64, 2, 2), [100, 10], [True, False])
     blob = builder.build_plan(graph.lower(net, weights.random_weights(net, 1)), builder.PREC_FP16, max_batch=4)
     version, tensors, ops, _ = _records(blob)
     t = {r[0].rstrip(b"\0").decode(): r for r in tensors}
@@ -68,9 +69,9 @@ def test_fc_relu_fuses_and_hidden_outputs_are_fp16():
     assert [o[9] for o in fc] == [builder.FC_STREAM | 1, builder.FC_STREAM]
     assert [(o[11], o[12], o[13], o[14]) for o in fc] == [(256, 100, 256, 128), (100, 10, 128, 128)]  # cin, cout, K, cout_phys
     # one FC with a fused ReLU also streams; one FC without stays on the old path (and its plan's version)
-    one = VO.fc_net((64, 2, 2), [100], [True])
+    one = fc_net((64, 2, 2), [100], [True])
     assert _records(builder.build_plan(graph.lower(one, weights.random_weights(one, 1)), builder.PREC_FP16, 4))[2][1][9] == 33
-    plain = VO.fc_net((64, 2, 2), [100], [False])
+    plain = fc_net((64, 2, 2), [100], [False])
     version, _, ops, _ = _records(builder.build_plan(graph.lower(plain, weights.random_weights(plain, 1)), builder.PREC_FP16, 4))
     assert version == 1 and ops[1][9] == 0
 
@@ -83,12 +84,12 @@ def test_refusals_name_the_layer():
     for fmt in ("int8", "e4m3"):
         with pytest.raises(ValueError, match="fc fc6: an InnerProduct with a fused ReLU builds in fp16 only"):
             quantize.quantize_lowered(low, weights.synthetic_input(1, seed=1), fmt=fmt)
-    soft = VO.fc_net((64, 1, 1), [10], [False])
+    soft = fc_net((64, 1, 1), [10], [False])
     soft["layers"] += [dict(name="prob", type="Softmax", bottoms=["fc1"], tops=["prob"]),
                        dict(name="relu_prob", type="ReLU", bottoms=["prob"], tops=["prob"])]
     with pytest.raises(ValueError, match="ReLU relu_prob: a ReLU on the output of Softmax prob"):
         graph.lower(soft)
-    res = VO.fc_net((64, 1, 1), [64, 64], [True, False])
+    res = fc_net((64, 1, 1), [64, 64], [True, False])
     res["layers"].append(dict(name="sum", type="Eltwise", bottoms=["fc1", "fc2"], tops=["sum"], operation="SUM"))
     with pytest.raises(ValueError, match="Eltwise sum: InnerProduct fc1 cannot take a residual"):
         graph.lower(res)
@@ -128,7 +129,7 @@ def test_prototxt_generator_and_onnx_lower_alike():
     assert [(L["name"], L["type"]) for L in parsed["layers"]] == [(L["name"], L["type"]) for L in net["layers"]]
     _same_ops(graph.lower(parsed), graph.lower(net))
     # ONNX: Gemm -> Relu, and Flatten / Dropout between Gemms, lower to the same ops (small VGG-style head for speed)
-    small = VO.fc_net((32, 4, 4), [48, 40], [True, False])
+    small = fc_net((32, 4, 4), [48, 40], [True, False])
     small["layers"].insert(2, dict(name="drop1", type="Dropout", bottoms=["fc1"], tops=["fc1"]))
     small["layers"].append(dict(name="prob", type="Softmax", bottoms=["fc2"], tops=["prob"]))
     w = weights.random_weights(small, 3)
@@ -148,7 +149,7 @@ def test_float64_oracle_matches_torchvision(depth):
     x = weights.synthetic_input(2, seed=depth)
     with torch.no_grad():
         want = torch.softmax(model(torch.from_numpy(x).double()), dim=1).numpy()
-    got = VO.caffe_forward(graph.vgg_caffe(depth), wts, x)
+    got = caffe_forward(graph.vgg_caffe(depth), wts, x, dtype=torch.float64)
     assert float(np.abs(got - want).max()) <= 1e-10
     with pytest.raises(ValueError, match="224 x 224 only"):
         vgg.load_weights(sd, depth, image=256)
@@ -165,8 +166,8 @@ def test_emulation_tracks_the_float64_oracle():
     net["layers"] = [dict(L, num_output=64) if L["name"] in ("fc6", "fc7") else L for L in net["layers"]]
     wts = weights.random_weights(net, 2)
     x = weights.synthetic_input(2, chw=(3, 32, 32), seed=2)
-    ref = VO.caffe_forward(net, wts, x)
-    emu = VO.lowered_forward_f16emu(graph.lower(net, wts), x)
+    ref = caffe_forward(net, wts, x, dtype=torch.float64)
+    emu = lowered_forward_f16emu(graph.lower(net, wts), x)
     assert float(np.abs(emu - ref).max()) <= 1e-3 and np.array_equal(emu.argmax(1), ref.argmax(1))
 
 
@@ -198,7 +199,7 @@ def test_plans_without_hidden_fc_keep_their_bytes():
 # ---- plan refusals of the streaming FC record (plan_format.h, kFcStream) ---------------------------------------------------
 def fc_mutations():
     """A two-FC streaming plan and (what, mutated blob, message) triples, one per refusal; used on the GPU too."""
-    net = VO.fc_net((64, 1, 1), [100, 10], [True, False])
+    net = fc_net((64, 1, 1), [100, 10], [True, False])
     blob = builder.build_plan(graph.lower(net, weights.random_weights(net, 0)), builder.PREC_FP16, max_batch=2)
     version, tensors, ops, base = _records(blob)
     assert version == 4
